@@ -1,7 +1,7 @@
-"""ddstore_b200 -- B200-native distributed in-memory sample store with ORNL/DDStore's surface.
+"""ddstore_b200 -- H100-native distributed in-memory sample store with ORNL/DDStore's surface.
 
 Only the get() hot path and what it needs (SURVEY.md section 8):
-  csrc/            CUDA kernels (sm_100a) + host C++ + the C-ABI  -> libddstore_b200.so
+  csrc/            CUDA kernels (sm_90a) + host C++ + the C-ABI  -> libddstore_b200.so
   _capi.py         ctypes binding of include/ddstore_b200.h
   store.py         PyDDStore: the reference's Python surface (src/pyddstore.pyx:58-131) + get_batch
   comm.py          communicator adapters (self / shm / torch.distributed / mpi4py-like)

@@ -1,4 +1,4 @@
-// ddstore_b200/csrc/kernels.cu -- the get() hot path as hand-written sm_100a CUDA.
+// ddstore_b200/csrc/kernels.cu -- the get() hot path as hand-written sm_90a CUDA.
 //
 // What the reference does per sample (include/ddstore.hpp:197-238 + src/ddstore.cxx:5-17):
 //   owner = sortedsearch(lenlist, start); offset = lenlist[owner-1] (or 0); two range checks;
@@ -74,7 +74,7 @@ std::atomic<unsigned long long> g_launches{0};
     } while (0)
 
 // ------------------------------------------------------------------------------------------------
-// PTX helpers (sm_100a): mbarrier, 1-D TMA bulk copies, shared-memory vector access
+// PTX helpers (sm_90a): mbarrier, 1-D TMA bulk copies, shared-memory vector access
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -673,7 +673,7 @@ __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, ui
 // ------------------------------------------------------------------------------------------------
 // Plan in shared memory (variable counts, <= PCAP requests): EVERY CTA computes the whole plan -- lookup + checks +
 // exclusive scan of the request sizes -- for itself. The index arrays are a few tens of KB that stay in L2 after
-// the first CTA touched them, so the redundancy costs ~1 us, and it removes every inter-CTA dependency the plan
+// the first CTA touched them, so the redundancy is cheap, and it removes every inter-CTA dependency the plan
 // used to have (tile tickets, look-back, a grid-wide "all tiles written" wait) as well as the L2 round trips of the
 // walk's searches and descriptor loads. Warp w owns a contiguous run of requests; loads are coalesced (lane-strided).
 // Returns the packed total T (exact, int64); the shared copy keeps 32-bit offsets (the launcher uses this path only
@@ -946,8 +946,8 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         // A claim is one atomic (requested ahead of need) + a division (FIXED), a shared-memory search (VAR, plan in
         // shared memory) or one global load (VAR, plan in global scratch). Small segments (8 per warp) keep the tail
         // short; variable-count segments are multiples of SEG_GRAIN when the segment table is in use.
-        // (push fetch: finer segments were measured WORSE -- 304 vs 270 us per step at N=2 -- because every claim costs a
-        // window of index reads from the requester's list over NVLink)
+        // (push fetch: finer segments were slower, because every claim costs a window of index reads from the
+        // requester's list over NVLink)
         int64_t target = w.T / (nwarps * 8);
         const int64_t unit = (!FIXED && PCAP == 0) ? SEG_GRAIN : (int64_t)CH;
         target = max((int64_t)a.min_seg_chunks * CH, min(target, (int64_t)1 << 20));
@@ -1127,7 +1127,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
 
 // ------------------------------------------------------------------------------------------------
 // dds_small_get_kernel: ONE request, ONE CTA -- the legacy one-get()-per-sample loop (include/ddstore.hpp:197-238
-// driven by examples/vae/distdataset.py:79-92). A 148-CTA persistent launch costs ~6 us of ramp/retire for a few KB;
+// driven by examples/vae/distdataset.py:79-92). A one-CTA-per-SM persistent launch costs more in ramp/retire than a few KB are worth;
 // this one is a plain copy loop that also does the reference's checks, writes the payload (device memory, or pinned
 // host memory zero-copy) and then a completion word the host spins on -- no stream synchronize in the call.
 // flag[0] = status word ((bad << 8) | code, or DDSK_STATUS_OK), flag[1] = bytes, flag[2] = ticket (written last).
@@ -1186,8 +1186,8 @@ struct PlanProto { // overlap protocol as the plan kernel sees it (all zero: ord
 // tiles before it (words tagged with a per-launch tag, so no memset), and writes source addresses, packed offsets and
 // the segment table (which request covers every SEG_GRAIN boundary of the packed buffer -- a segment claim of the
 // gather is then one load instead of a search). The chain of DEPENDENT memory round trips is what this kernel costs
-// when it runs under the previous batch's gather (each one takes 2-3 us in a saturated memory system -- measured,
-// profiles/r2_queue_timeline.md), so there are as few as possible: index loads (+ the sample-table gather) and the
+// when it runs under the previous batch's gather (each one takes microseconds in a saturated memory system), so
+// there are as few as possible: index loads (+ the sample-table gather) and the
 // slot / gate polls in parallel, one look-back, one finish count.
 // tile_state word: [63:42] tag (22 bits) | [41:40] flag (1 = tile aggregate, 2 = inclusive prefix) | [39:0] bytes
 __device__ __forceinline__ unsigned long long tile_pack(unsigned int tag, unsigned int flag, int64_t v) {
@@ -1350,8 +1350,8 @@ __global__ void dds_verify_kernel(const __grid_constant__ ddsk_var_t var, const 
 // calls keep coming (it leaves by itself after `idle_ns` without one, so a device-wide synchronize never waits longer
 // than that) and polls a mailbox in mapped pinned host memory: the host writes the request fields, then a sequence
 // number; the kernel does the reference's checks, copies the rows (to device memory, or zero-copy to a pinned bounce
-// buffer) and answers with ONE word, (sequence << 8) | code. A launch + completion costs ~14 us on this box, a
-// mailbox round trip ~5 (measured: profiles/r2_latency.md).
+// buffer) and answers with ONE word, (sequence << 8) | code. A mailbox round trip is a fraction of the cost of a
+// kernel launch + completion.
 // Exit protocol: the kernel's last action is to write its generation number to mb->exit_gen; it never touches the
 // mailbox afterwards. A host that finds exit_gen == the generation it believes alive while its request is still
 // unanswered launches a fresh kernel (which starts by looking for an unserved request), so no request is lost or
@@ -1462,13 +1462,14 @@ constexpr int kNumGeoms = (int)(sizeof(kGeoms) / sizeof(kGeoms[0]));
 constexpr Geometry kGeomsS[] = {{12, 3, 4096, 4096}, {12, 3, 3072, 8192}, {16, 3, 2048, 8192}, {16, 3, 3072, 4096}, {8, 4, 4096, 4096}};
 constexpr int kNumGeomsS = (int)(sizeof(kGeomsS) / sizeof(kGeomsS[0]));
 constexpr int64_t kPlanSmemMax = 8192;
-// Measured (profiles/r2_timing_probe.md): the redundant plan costs 8.6 us at 4096 requests (19 us with sample-index
-// lookups: 148 SMs hammer the same lines), the plan kernels ~11 us serialised but ~0 when they run under the previous
-// batch's gather -- so by default only small batches, where one launch beats three, plan in shared memory.
+// The redundant plan grows with the batch (every SM reads the same index lines), while the plan kernels cost ~0 when
+// they run under the previous batch's gather -- so by default only small batches, where one launch beats three, plan
+// in shared memory.
 int64_t g_plan_smem_default = 1024; // DDS_SMEM_PLAN_MAX
 
-// Measured on B200 (profiles/r1_configs.md): 12 warps x 4 stages is as fast as 8 x 4 on 4 KiB+ rows and clearly
-// faster on the instruction-heavier variable / re-phase path; rows under 2 KiB want even more warps (16 x 3).
+// On an H100 SXM (400 W limit) config 2 (4 KiB rows) is HBM-bound with every fixed-count variant: 0-4 and 7 are within
+// 0.3 % of each other, so 12 warps x 4 stages (also used for the instruction-heavier variable / re-phase path) stays
+// the default; rows under 2 KiB take more warps (16 x 3) to keep more small copies in flight.
 constexpr int kGeomLarge = 4, kGeomSmall = 2, kGeomVar = 4;
 
 int g_geom_fixed_env = -1; // DDS_GATHER_GEOM      (tuning: force one variant for the fixed-count entry)
@@ -1631,8 +1632,8 @@ void fill_overlap(GatherArgs &a, const ddsk_scratch_t *scr, int flags) {
     a.seq = scr->ovl_seq;
     a.ovl = scr->ovl;
     // segment tickets: the store's word for ordinary launches. Overlap launches: none for the fixed-count entry (plain
-    // striding -- measured: slot tickets cost 3 % on config 2, 1776 warps x 8 claims on one word per 85 us launch, and did
-    // not help a queue that shares the GPU either); the variable-count entries set the slot's own word below (their CTAs
+    // striding -- slot tickets put every warp's claims on one word per launch and did not help a queue that shares the
+    // GPU either); the variable-count entries set the slot's own word below (their CTAs
     // may start late, behind the plan kernel, and must not keep a fixed share of the work).
     a.tickets = a.overlap ? nullptr : scr->counters;
 }
@@ -1863,7 +1864,7 @@ int ddsk_l2_warm(const void *base_dev, size_t bytes, void *stream) {
     g_l2_base = base_dev;
     g_l2_bytes = bytes;
     const size_t n = bytes / 16;
-    const int blocks = (int)std::min<size_t>((n + 255) / 256, 148 * 8);
+    const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)g_sms * 8);
     return launch_pdl(dds_touch_kernel, dim3(blocks), dim3(256), (cudaStream_t)stream, (const uint4 *)base_dev, n, (unsigned int *)nullptr);
 }
 
@@ -1881,7 +1882,8 @@ int ddsk_synth_fill(void *base_dev, int64_t first_global_row, int64_t nrows, int
     uint64_t nelem = (uint64_t)nrows * (uint64_t)disp;
     uint64_t first = (uint64_t)first_global_row * (uint64_t)disp;
     if (nelem == 0) return 0;
-    int blocks = (int)((nelem + 255) / 256 < 148 * 16 ? (nelem + 255) / 256 : 148 * 16);
+    if (int rc = pick_geometry()) return rc;
+    int blocks = (int)std::min<uint64_t>((nelem + 255) / 256, (uint64_t)g_sms * 16);
     switch (itemsize) {
     case 1: dds_synth_kernel<uint8_t><<<blocks, 256, 0, st>>>((uint8_t *)base_dev, first, nelem, seed); break;
     case 2: dds_synth_kernel<uint16_t><<<blocks, 256, 0, st>>>((uint16_t *)base_dev, first, nelem, seed); break;
@@ -1901,7 +1903,8 @@ int ddsk_synth_verify(const ddsk_var_t *var, const void *packed_dev, const int64
                       uint64_t seed, unsigned long long *out_dev, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if (nreq <= 0) return 0;
-    const int blocks = 148 * 8;
+    if (int rc = pick_geometry()) return rc;
+    const int blocks = g_sms * 8;
     const unsigned char *pk = (const unsigned char *)packed_dev;
     switch (itemsize) {
     case 1: dds_verify_kernel<uint8_t><<<blocks, 256, 0, st>>>(*var, pk, starts_dev, counts_dev_or_null, fixed_count, offsets_dev_or_null, nreq, disp, seed, out_dev); break;

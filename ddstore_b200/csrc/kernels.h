@@ -58,7 +58,7 @@ typedef struct ddsk_scratch {
 /* `flags` of the launchers */
 #define DDSK_F_RESET 1      /* reset the status word first */
 #define DDSK_F_MIRROR 2     /* the kernel's last warp mirrors status + total into scr->host_mirror (synchronous calls;
-                               costs ~2 us at the kernel's end, so async queues skip it) */
+                               costs time at the kernel's end, so async queues skip it) */
 #define DDSK_F_OVERLAP 4    /* independent batch: static segment striding, overlap protocol (see kernels.cu) */
 #define DDSK_F_SKIP_WAIT 16 /* ... and the launch right before it in the stream was one too: skip griddepcontrol.wait */
 #define DDSK_F_PREV1 32     /* overlap launch ovl_seq-1 belongs to the same run (retire after it) */

@@ -1,5 +1,5 @@
 // ddstore_b200/csrc/store.cpp -- host side of the store: the reference's `class DDStore`
-// (/root/reference/include/ddstore.hpp:26-258, src/ddstore.cxx:19-96) re-built for B200:
+// (/root/reference/include/ddstore.hpp:26-258, src/ddstore.cxx:19-96) re-built for H100:
 //   * a variable's shard is a CUDA VMM block of this rank's HBM (reference: MPI_Alloc_mem + memcpy,
 //     ddstore.hpp:44-49);
 //   * the "window" is the table of every rank's shard base mapped into this process (VMM handle passed as a file
@@ -40,7 +40,7 @@
 
 namespace {
 
-constexpr int64_t kSmallIdx = 8;          // requests whose host indices are read zero-copy (measured: slower than an H2D copy from ~32 on)
+constexpr int64_t kSmallIdx = 8;          // requests whose host indices are read zero-copy (more go through an H2D copy)
 constexpr int64_t kSmallOut = 64 * 1024;  // host destinations up to this size are written zero-copy
 
 thread_local std::string g_err;
@@ -138,7 +138,7 @@ struct Var {
 } // namespace
 
 // Streaming ingest (SURVEY.md 8f rank 3): a few worker threads copy slices of a pageable source chunk into a pinned
-// staging buffer in parallel (one thread's memcpy tops out around 12-15 GB/s, a PCIe Gen5 x16 link wants ~55), while
+// staging buffer in parallel (one thread's memcpy cannot keep a PCIe Gen5 x16 link busy), while
 // the copy engine moves the previous staging buffer into the shard.
 struct IngestPool {
     static constexpr size_t kStage = 16u << 20; // bytes per staging buffer
@@ -960,7 +960,7 @@ int dds_ingest(dds_store_t *s, const char *name, const void *host_rows, int64_t 
 
 // A packed batch from the store's HBM staging buffer into a PAGEABLE host destination (the reference's np.zeros
 // contract, examples/vae/distdataset.py:80-85): cudaMemcpyAsync into pageable memory is staged by the driver through
-// one thread (20.7 GB/s measured); here the copy engine fills the pool's pinned buffers chunk by chunk while the
+// one thread; here the copy engine fills the pool's pinned buffers chunk by chunk while the
 // worker threads copy the previous chunk out. `st` has the gather queued; synchronous.
 static int d2h_pageable(dds_store_t *s, void *dst, const void *d_src, size_t bytes, cudaStream_t st) {
     if (int rc = ensure_pool(s)) return rc;
@@ -1216,7 +1216,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     void *d_dst = dst;
     int64_t cap = dst_capacity;
     // (Large pinned destinations still go through an HBM staging buffer + one D2H copy: letting the kernel's bulk
-    // stores write over PCIe directly was measured slower, 52.3 vs 55.8 GB/s on config 2.)
+    // stores write over PCIe directly was slower.)
     bool small_out = false;
     if (!dst_dev) {
         int64_t need = upper >= 0 ? std::min(upper, dst_capacity) : dst_capacity;
@@ -1349,8 +1349,8 @@ int dds_set_sample_index(dds_store_t *s, const char *name, const int64_t *row_st
         for (auto &x : s->vars) want += (size_t)x.second.nsamples * 16;
         int maxp = 0;
         if (cudaDeviceGetAttribute(&maxp, cudaDevAttrMaxPersistingL2CacheSize, s->device) != cudaSuccess) maxp = 0;
-        // (at most 32 MiB -- a quarter of the B200's L2 -- is set aside: the rest of the process shares this cache)
-        maxp = (int)std::min<size_t>((size_t)std::max(maxp, 0), (size_t)32 << 20);
+        // (at most 12 MiB -- a quarter of the H100's 50 MB L2 -- is set aside: the rest of the process shares this cache)
+        maxp = (int)std::min<size_t>((size_t)std::max(maxp, 0), (size_t)12 << 20);
         if (maxp > 0) (void)cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, std::min(want, (size_t)maxp));
         (void)cudaGetLastError();
         if (maxp > 0 && (size_t)nsamples * 16 <= (size_t)maxp) { // warm it now: every later lookup hits L2
@@ -1477,7 +1477,7 @@ int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index) {
     s->run_len = 0;
     CU(cudaSetDevice(s->device));
     cudaStream_t st = s->pending_stream;
-    // queued launches skip the host mirror (it costs ~2 us at the end of every kernel): read the words back here
+    // queued launches skip the host mirror (it costs time at the end of every kernel): read the words back here
     CU(cudaMemcpyAsync(&s->h_status[0], s->scr.status, 8, cudaMemcpyDeviceToHost, st));
     if (s->pending_fixed_total < 0 && s->pending_total_ptr)
         CU(cudaMemcpyAsync(&s->h_status[1], s->pending_total_ptr, 8, cudaMemcpyDeviceToHost, st));

@@ -3,9 +3,9 @@
 // The reference exposes a shard with MPI_Win_create (include/ddstore.hpp:56-61). Here the shard is physical
 // HBM created with the CUDA virtual-memory-management API (cuMemCreate, 2 MiB granularity), exported as a POSIX
 // file descriptor, passed to the other ranks of the box over an abstract AF_UNIX datagram socket (SCM_RIGHTS) and
-// mapped there with cuMemImportFromShareableHandle + cuMemMap. Measured on 2xB200 (scripts/probes/mix_probe.py):
-// random 4 KiB peer reads through a legacy cudaIpcOpenMemHandle mapping reach only ~240 GB/s, the same reads
-// through a same-process peer mapping reach 755 GB/s -- hence VMM, with legacy IPC kept as the fallback.
+// mapped there with cuMemImportFromShareableHandle + cuMemMap. Random 4 KiB peer reads through a legacy
+// cudaIpcOpenMemHandle mapping were found to be several times slower than the same reads through a same-process
+// peer mapping (not re-measured on H100) -- hence VMM, with legacy IPC kept as the fallback.
 //
 // The driver entry points are resolved at run time with cudaGetDriverEntryPoint, so the library has no link-time
 // dependency on libcuda and still loads (and fails loudly in dds_create) on a machine without a GPU.

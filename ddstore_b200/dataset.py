@@ -214,7 +214,7 @@ class PrefetchLoader:
 
     dataset: a DistDataset; sampler: iterable of sample indices (e.g. DistributedSampler); yields (vals, labels)
     device tensors that stay valid until the next-but-one FETCH (depth = 2 buffer sets).
-    group: small batches are launch-bound (a 2 MB batch costs ~8 us of launch + ramp for ~0.6 us of HBM time), so
+    group: small batches are launch-bound (a 2 MB batch costs more in launch + ramp than in HBM time), so
     `group` consecutive batches are fetched by ONE launch (one request list of group x batch_size ids, one packed buffer
     sliced back into the batches) -- a queue of small batches served by one kernel.
     """

@@ -1,4 +1,4 @@
-/* include/ddstore_b200.h -- the drop-in boundary: a C-ABI over a B200-native distributed sample
+/* include/ddstore_b200.h -- the drop-in boundary: a C-ABI over an H100-native distributed sample
  * store with the behaviour of ORNL/DDStore's `DDStore` class.
  *
  * The reference's FFI for this path is Cython binding the C++ class (src/pyddstore.pyx:34-50 ->
@@ -8,7 +8,7 @@
  * ddstore_b200/pyddstore.pyx wraps that class with the reference's Python surface.
  *
  * Data plane: each rank's shard lives in its GPU's HBM (cudaMalloc); peers map it through CUDA IPC
- * (the analogue of MPI_Win_create, ddstore.hpp:56-61); get() is a batched-gather sm_100a kernel
+ * (the analogue of MPI_Win_create, ddstore.hpp:56-61); get() is a batched-gather sm_90a kernel
  * reading the owner's HBM directly (local or over NVLink/NVSwitch). There is NO CPU data path:
  * without a CUDA device every data-plane call fails with DDS_ERR_NO_DEVICE.
  */
@@ -173,8 +173,8 @@ int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, c
 
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite
- * flow (1.31 link bytes per payload byte, counters in profiles/r2_nvlink_counters.md). When all ranks fetch in the same
- * step anyway -- a DDP loader -- the owners can push instead (posted writes, +6 % payload per link): each rank
+ * flow. When all ranks fetch in the same
+ * step anyway -- a DDP loader -- the owners can push instead (posted writes, less link overhead per payload byte): each rank
  * publishes its start rows in its WINDOW, every owner sends the rows it owns straight into the requesters' windows and
  * signals arrival; the call's kernel ends when this rank's batch is complete. dds_push_setup allocates and maps the
  * windows (room for max_requests start rows and max_bytes of packed rows, twice: results alternate between two

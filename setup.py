@@ -2,7 +2,7 @@
 
 Packaging only (the reference's own build is setup.py:18-41: one Cython extension over ddstore.cxx + common.cxx with
 mpicc/mpicxx and libfabric). Here the native pieces are built in-tree by __graft_entry__.build(): nvcc
-(-gencode arch=compute_100a,code=sm_100a) + g++ -> ddstore_b200/libddstore_b200.so, Cython -> the `pyddstore` module.
+(-gencode arch=compute_90a,code=sm_90a) + g++ -> ddstore_b200/libddstore_b200.so, Cython -> the `pyddstore` module.
 """
 import os
 import sys
@@ -24,7 +24,7 @@ class BuildNative(build_py):
 setup(
     name="ddstore_b200",
     version="0.1.0",
-    description="B200-native distributed in-memory sample store with ORNL/DDStore's surface (get() hot path)",
+    description="H100-native distributed in-memory sample store with ORNL/DDStore's surface (get() hot path)",
     packages=find_packages(include=["ddstore_b200", "ddstore_b200.*"]),
     package_data={"ddstore_b200": ["libddstore_b200.so", "cython/pyddstore*.so"]},
     cmdclass={"build_py": BuildNative},

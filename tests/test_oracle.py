@@ -2,15 +2,21 @@
 (oracle/oracle.py) against
   (1) the committed golden vectors the unmodified reference produced (tests/golden/golden.json),
   (2) the reference's own known answers (test/demo.cxx:20-37, test/demo.py:55-56, test/test.py:157-159),
-  (3) the verbatim-compiled reference itself (oracle/_ref) on seeded random worlds, when it is built.
+  (3) the verbatim-compiled reference itself (oracle/_ref) on seeded random worlds: live when it is built, else
+      what it returned there (tests/golden/ref_worlds.json).
 CPU only."""
+import json
+import os
+
 import numpy as np
 import pytest
 
 from oracle import oracle as O
-from tests.helpers import (golden_world_shards, load_golden, random_valid_requests, random_world, sha)
+from tests.helpers import (HERE, golden_world_shards, load_golden, random_valid_requests, random_world, sha)
 
 G = load_golden()
+with open(os.path.join(HERE, "golden", "ref_worlds.json")) as _f:
+    REF_WORLDS = json.load(_f)
 
 
 def test_sortedsearch_golden(coracle):
@@ -108,44 +114,63 @@ def test_synth_generator_c_vs_numpy(coracle):
     assert np.isnan(f).any()  # payload deliberately contains NaN bit patterns
 
 
-@pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not built (needs /root/reference at build time)")
 @pytest.mark.parametrize("dtype,disp,P", [(np.float32, 1, 4), (np.float32, 16, 8), (np.int64, 2, 3),
                                           (np.uint8, 7, 2), (np.float64, 5, 1), (np.int32, 3, 5), (np.bool_, 3, 2)])
 def test_c_oracle_vs_compiled_reference(coracle, dtype, disp, P):
+    """against the compiled reference itself when oracle/_ref is built, else against what it returned on the same seeded
+    worlds (tests/golden/ref_worlds.json, generator tests/golden/make_ref_worlds.py)"""
     rng = np.random.default_rng(1000 + disp * 31 + P)
     nrows, shards = random_world(rng, P, dtype, disp)
-    w = O.RefWorld(P)
+    rec = REF_WORLDS[f"{np.dtype(dtype).name}-{disp}-{P}"]
+    w = O.RefWorld(P) if O.have_ref() else None
     try:
-        w.add("v", shards)
-        it, dp, ll = w.query(0, "v")
+        if w:
+            w.add("v", shards)
+            it, dp, ll = w.query(0, "v")
+            assert [it, dp, ll.tolist()] == [rec["itemsize"], rec["disp"], rec["lenlist"]]
+        else:
+            it, dp, ll = rec["itemsize"], rec["disp"], np.array(rec["lenlist"], np.int64)
         assert ll.tolist() == O.np_lenlist(nrows).tolist() and dp == disp and it == np.dtype(dtype).itemsize
         starts, counts = random_valid_requests(rng, ll, 300)
-        ref_out, bad, err, _ = w.get_batch(P - 1, "v", starts, counts)
+        if w:
+            ref_out, bad, err, _ = w.get_batch(P - 1, "v", starts, counts)
+            ref_sha = sha(ref_out.tobytes())
+            assert ref_sha == rec["batch_sha256"] and bad == rec["bad"]
+        else:
+            ref_sha, bad = rec["batch_sha256"], rec["bad"]
         assert bad == -1
         c_out, c_offs, cbad, rc = coracle.get_batch(shards, starts, counts)
         n_out, n_offs, nbad, nrc = O.np_get_batch(shards, starts, counts)
         assert cbad == nbad == -1
-        assert ref_out.tobytes() == c_out.tobytes() == n_out.tobytes()
+        assert ref_sha == sha(c_out.tobytes()) and c_out.tobytes() == n_out.tobytes()
         assert c_offs.tolist() == n_offs.tolist()
         # error classification agrees request by request on arbitrary (mostly invalid) requests
         total = int(ll[-1])
-        for _ in range(400):
+        served = []
+        for code in rec["codes"]:
             s = int(rng.integers(-5, total + 5))
             c = int(rng.integers(0, 60))
-            buf = np.zeros((c, disp), dtype)
-            try:
-                w.get(0, "v", buf, s)
-                ref_err = None
-            except ValueError as e:
-                ref_err = str(e)
+            ref_err = O.ERR_TEXT[code] if code else None
+            if w:
+                buf = np.zeros((c, disp), dtype)
+                try:
+                    w.get(0, "v", buf, s)
+                    live_err = None
+                except ValueError as e:
+                    live_err = str(e)
+                assert live_err == ref_err
             t, off, rc = coracle.locate(ll, s, c)
             assert (O.ERR_TEXT[rc] if rc else None) == ref_err
             assert O.np_locate(ll, s, c)[2] == rc
             if not rc:
                 o2, _, _, _ = coracle.get_batch(shards, [s], [c])
-                assert o2.tobytes() == buf.tobytes()
+                if w:
+                    assert o2.tobytes() == buf.tobytes()
+                served.append(o2.tobytes())
+        assert sha(b"".join(served)) == rec["served_sha256"]
     finally:
-        w.close()
+        if w:
+            w.close()
 
 
 @pytest.mark.skipif(not O.have_ref(), reason="oracle/_ref not built")
