@@ -155,7 +155,8 @@ __device__ __forceinline__ int dev_locate(const ddsk_var_t &v, int64_t start, in
     int t = dev_sortedsearch(v, start);
     int64_t off = t > 0 ? v.lenlist[t - 1] : 0;
     if (start < off) return DDSK_CODE_START;
-    if (count < 0 || start + count > v.lenlist[t]) return DDSK_CODE_COUNT; /* count<0 is UB in the reference */
+    // (count < 0 is UB in the reference; start + count could wrap: start >= off >= 0 here, so the difference cannot)
+    if (count < 0 || count > v.lenlist[t] - start) return DDSK_CODE_COUNT;
     *src = (uint64_t)v.bases[t] + (uint64_t)(start - off) * (uint64_t)v.row_bytes; /* ddstore.hpp:229-236 */
     return 0;
 }
@@ -166,13 +167,15 @@ __device__ __forceinline__ int dev_locate_owner(const ddsk_var_t &v, int64_t sta
     *owner = t;
     int64_t off = t > 0 ? v.lenlist[t - 1] : 0;
     if (start < off) return DDSK_CODE_START;
-    if (count < 0 || start + count > v.lenlist[t]) return DDSK_CODE_COUNT;
+    if (count < 0 || count > v.lenlist[t] - start) return DDSK_CODE_COUNT;
     *src = (uint64_t)v.bases[t] + (uint64_t)(start - off) * (uint64_t)v.row_bytes;
     return 0;
 }
 
-__device__ __forceinline__ void report(unsigned long long *status, int64_t req, int code) {
-    atomicMin(status, ((unsigned long long)req << 8) | (unsigned long long)code);
+// Status word: (launch ordinal in its queue << 48) | (request << 8) | code; the lowest report wins. `tag` is the ordinal
+// part (DDSK_STATUS_ORD_SHIFT), so an error of an earlier batch of a queue beats any error of a later one.
+__device__ __forceinline__ void report(unsigned long long *status, unsigned long long tag, int64_t req, int code) {
+    atomicMin(status, tag | ((unsigned long long)req << 8) | (unsigned long long)code);
 }
 
 // a few more PTX helpers used below
@@ -250,7 +253,8 @@ __device__ __forceinline__ longlong2 ldg_pair(const longlong2 *p) { return __ldg
 // `limit`: requests idx >= limit are not this thread's business (dead lanes).
 template <int K>
 __device__ __forceinline__ void plan_many(const ddsk_var_t &var, const PlanSrc &p, const int64_t (&idx)[K], int64_t limit,
-                                          unsigned long long *status, uint64_t (&src)[K], int64_t (&nbytes)[K]) {
+                                          unsigned long long *status, unsigned long long tag, uint64_t (&src)[K],
+                                          int64_t (&nbytes)[K]) {
     int64_t start[K], count[K];
     bool live[K], badid[K];
     const ddsk_var_t *vp[K];
@@ -304,13 +308,13 @@ __device__ __forceinline__ void plan_many(const ddsk_var_t &var, const PlanSrc &
         nbytes[k] = 0;
         if (!live[k]) continue;
         if (badid[k]) {
-            report(status, idx[k], DDSK_CODE_SAMPLE);
+            report(status, tag, idx[k], DDSK_CODE_SAMPLE);
             continue;
         }
         uint64_t s = 0;
         const int code = dev_locate(*vp[k], start[k], count[k], &s);
         if (code) {
-            report(status, idx[k], code);
+            report(status, tag, idx[k], code);
             continue;
         }
         src[k] = s;
@@ -348,6 +352,7 @@ struct GatherArgs {
     int64_t dst_cap;
     int64_t *offsets_out; // optional [nreq+1]
     unsigned long long *status;
+    unsigned long long status_tag; // this launch's ordinal in its queue, as OR-ed into every status report
     unsigned int *counters; // [0] segment ticket, [1] finished warps -- self-resetting, ticketed launches only
     // multi-array batches (plan.nvars > 1): the packed result of variable v goes to mdst[v]
     char *mdst[DDSK_MAX_MULTI];
@@ -468,8 +473,8 @@ struct ChunkWalker {
             } else if (FIXED) {
                 uint64_t s = 0;
                 int code = dev_locate(a.var, a.starts[idx], a.count, &s);
-                if (code) report(a.status, idx, code); // the reference's two checks; every request with bytes to
-                                                       // fetch passes through some warp's window at least once
+                // the reference's two checks; every request with bytes to fetch passes through some warp's window at least once
+                if (code) report(a.status, a.status_tag, idx, code);
                 w_src = code ? 0 : s; // invalid request: keep its slot in the packed layout, copy nothing
                 w_dst = idx * nb;
                 w_n = nb;
@@ -691,7 +696,7 @@ __device__ __forceinline__ int64_t plan_in_smem(const GatherArgs &a, const PlanV
         uint64_t sv[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) idx[k] = b + k * 32 + lane;
-        plan_many<4>(a.var, a.plan, idx, w1, a.status, sv, nb);
+        plan_many<4>(a.var, a.plan, idx, w1, a.status, a.status_tag, sv, nb);
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             if (idx[k] < w1) {
@@ -736,12 +741,13 @@ struct PieceDesc {
 };
 
 // wait until overlap launch q has retired (its done word carries a sequence number >= q)
-__device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigned int q, unsigned long long *status, int64_t nreq) {
+__device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigned int q, unsigned long long *status,
+                                                unsigned long long tag, int64_t nreq) {
     const uint64_t t0 = globaltimer_ns();
     while ((int)(ld_acquire_u32(&ovl[4 + (q & 3u)]) - q) < 0) {
         __nanosleep(100);
         if (globaltimer_ns() - t0 > 4000000000ull) { // never expected; do not hang the box
-            report(status, nreq, DDSK_CODE_WATCHDOG);
+            report(status, tag, nreq, DDSK_CODE_WATCHDOG);
             __trap();
         }
     }
@@ -784,7 +790,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     bool gate_open = !(a.overlap && a.wait2_valid);
     auto pass_gate = [&]() {
         if (!gate_open) {
-            if (lane == 0) spin_until_done(a.ovl, a.seq - 2u, a.status, a.nreq);
+            if (lane == 0) spin_until_done(a.ovl, a.seq - 2u, a.status, a.status_tag, a.nreq);
             __syncwarp();
             gate_open = true;
         }
@@ -821,7 +827,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                     if (__all_sync(0xffffffffu, ok)) break;
                     __nanosleep(100);
                     if (globaltimer_ns() - t0 > 4000000000ull) {
-                        report(a.status, a.nreq, DDSK_CODE_WATCHDOG);
+                        report(a.status, a.status_tag, a.nreq, DDSK_CODE_WATCHDOG);
                         __trap();
                     }
                 }
@@ -864,7 +870,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             while (r < P && ld_acquire_sys_u64((const unsigned long long *)ps->win[r]) < a.push_step) {
                 __nanosleep(200);
                 if (globaltimer_ns() - t0 > 30000000000ull) { // 30 s: a rank that never launched must not hang the box
-                    report(a.status, a.nreq, DDSK_CODE_WATCHDOG);
+                    report(a.status, a.status_tag, a.nreq, DDSK_CODE_WATCHDOG);
                     __trap();
                 }
             }
@@ -900,7 +906,9 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     w.nwarps = nwarps;
     w.static_claims = a.tickets == nullptr;
     w.gate_ok = gate_open; // (variable-count overlap launches opened it together with the plan word)
-    w.nb = FIXED ? a.count * a.var.row_bytes : 0;
+    // (a fixed count above the variable's row total is invalid for every request, and count * row_bytes need not even
+    //  fit in 64 bits: nothing to walk, the check pass below reports the first request)
+    w.nb = (FIXED && a.count <= a.var.lenlist[a.var.nranks - 1]) ? a.count * a.var.row_bytes : 0;
     w.nreq = (FIXED && push) ? push_rbase[w.push_n] : a.nreq;
     if (FIXED) w.T = w.nb * w.nreq;
     bool over = w.T > a.dst_cap;
@@ -959,7 +967,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         w.nseg = w.T > 0 ? (w.T + w.seg_bytes - 1) / w.seg_bytes : 0;
     }
     if (over) {
-        if (gwarp == 0 && lane == 0) report(a.status, a.nreq, DDSK_CODE_CAPACITY);
+        if (gwarp == 0 && lane == 0) report(a.status, a.status_tag, a.nreq, DDSK_CODE_CAPACITY);
         w.nseg = 0;
     }
 
@@ -969,7 +977,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         for (int64_t i = gwarp * 32 + lane; i < a.nreq; i += nwarps * 32) {
             uint64_t s;
             int code = dev_locate(a.var, a.starts[i], a.count, &s);
-            if (code) report(a.status, i, code);
+            if (code) report(a.status, a.status_tag, i, code);
         }
     }
 
@@ -1011,7 +1019,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             const uint64_t t0 = globaltimer_ns();
             while (!mbar_try_wait(bar, parity)) {
                 if (globaltimer_ns() - t0 > 4000000000ull) { // 4 s: a lost TMA completion must not hang the box
-                    report(a.status, a.nreq, DDSK_CODE_WATCHDOG);
+                    report(a.status, a.status_tag, a.nreq, DDSK_CODE_WATCHDOG);
                     __trap();
                 }
             }
@@ -1083,7 +1091,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 a.ovl[slot] = 0;
                 a.ovl[8 + slot] = 0;
                 if (a.wait_plan) a.plan_word[slot] = 0; // (every CTA has read the total long ago)
-                if (a.wait1_valid) spin_until_done(a.ovl, a.seq - 1u, a.status, a.nreq);
+                if (a.wait1_valid) spin_until_done(a.ovl, a.seq - 1u, a.status, a.status_tag, a.nreq);
                 __threadfence();
                 st_release_u32(&a.ovl[4 + slot], a.seq);
             }
@@ -1107,13 +1115,13 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                     while (ld_acquire_sys_u64(&hdr[8 + r]) < a.push_step) {
                         __nanosleep(200);
                         if (globaltimer_ns() - t0 > 30000000000ull) {
-                            report(a.status, a.nreq, DDSK_CODE_WATCHDOG);
+                            report(a.status, a.status_tag, a.nreq, DDSK_CODE_WATCHDOG);
                             __trap();
                         }
                     }
                 // errors the owners found in MY requests sit in my window's status word
                 const unsigned long long st = *(volatile const unsigned long long *)&hdr[3];
-                if (st != DDSK_STATUS_OK) atomicMin(a.status, st);
+                if (st != DDSK_STATUS_OK) atomicMin(a.status, st | a.status_tag);
             }
             if (a.host_mirror) { // the last warp publishes status + total straight into pinned host memory: the host
                                  // reads them after the stream sync, no D2H copy in the call
@@ -1200,7 +1208,8 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
                                                                 uint64_t *__restrict__ req_src, int64_t *__restrict__ req_dst,
                                                                 unsigned long long *tile_state, unsigned int tag,
                                                                 int64_t *__restrict__ offsets_out, uint32_t *__restrict__ seg_tab,
-                                                                int64_t seg_cap, unsigned long long *status, PlanProto pr) {
+                                                                int64_t seg_cap, unsigned long long *status,
+                                                                unsigned long long status_tag, PlanProto pr) {
     __shared__ int64_t warp_tot[PLAN_THREADS / 32];
     __shared__ int64_t tile_excl_s;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -1214,7 +1223,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
     uint64_t sv[PLAN_ITEMS];
 #pragma unroll
     for (int k = 0; k < PLAN_ITEMS; k++) idx[k] = base + k;
-    plan_many<PLAN_ITEMS>(var, p, idx, nreq, status, sv, nb); // (only reads: may run before the slot is known to be free)
+    plan_many<PLAN_ITEMS>(var, p, idx, nreq, status, status_tag, sv, nb); // (only reads: may run before the slot is known to be free)
     int64_t mine = 0;
 #pragma unroll
     for (int k = 0; k < PLAN_ITEMS; k++) mine += nb[k];
@@ -1224,8 +1233,8 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
     // offsets are caller-visible, so launch seq-2 must have retired too (it implies seq-4): one poll, issued with the
     // index loads above in flight
     if (threadIdx.x == 0) {
-        if (pr.wait2_valid && offsets_out) spin_until_done(pr.ovl, pr.seq - 2u, status, nreq);
-        else if (pr.wait4_valid) spin_until_done(pr.ovl, pr.seq - 4u, status, nreq);
+        if (pr.wait2_valid && offsets_out) spin_until_done(pr.ovl, pr.seq - 2u, status, status_tag, nreq);
+        else if (pr.wait4_valid) spin_until_done(pr.ovl, pr.seq - 4u, status, status_tag, nreq);
     }
     __syncthreads();
     int64_t wbase = 0, agg = 0;
@@ -1249,7 +1258,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
                     do {
                         wv = ld_acquire_u64(&tile_state[t]);
                         if (globaltimer_ns() - t0 > 4000000000ull) { // never expected; do not hang the box
-                            report(status, nreq, DDSK_CODE_WATCHDOG);
+                            report(status, status_tag, nreq, DDSK_CODE_WATCHDOG);
                             __trap();
                         }
                     } while ((unsigned int)(wv >> 42) != (tag & 0x3FFFFFu) || ((wv >> 40) & 3u) == 0);
@@ -1603,7 +1612,9 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
 
 template <bool FIXED>
 int launch_gather(const GatherArgs &args, cudaStream_t stream) {
-    switch (geometry_for(FIXED, FIXED ? args.count * args.var.row_bytes : 0)) {
+    // (the request size only picks a variant: a count too large to multiply safely counts as large)
+    const int64_t request_bytes = args.count < ((int64_t)1 << 20) ? args.count * args.var.row_bytes : INT64_MAX;
+    switch (geometry_for(FIXED, FIXED ? request_bytes : 0)) {
     case 1: return launch_gather_t<FIXED, 8, 6, 4096, 0>(args, stream);
     case 2: return launch_gather_t<FIXED, 16, 3, 4096, 0>(args, stream);
     case 3: return launch_gather_t<FIXED, 4, 4, 8192, 0>(args, stream);
@@ -1685,6 +1696,7 @@ int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t 
     a.dst_cap = dst_capacity;
     a.offsets_out = offsets_dev_or_null;
     a.status = scr->status;
+    a.status_tag = scr->status_tag;
     a.counters = scr->counters;
     a.min_seg_chunks = 1;
     fill_overlap(a, scr, flags);
@@ -1705,6 +1717,7 @@ int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const 
     a.dst = nullptr;
     a.dst_cap = INT64_MAX;
     a.status = scr->status;
+    a.status_tag = scr->status_tag;
     a.counters = scr->counters;
     a.tickets = scr->counters;
     a.min_seg_chunks = 1;
@@ -1722,6 +1735,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
                            int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, cudaStream_t st) {
     a.nreq = nreq;
     a.status = scr->status;
+    a.status_tag = scr->status_tag;
     a.counters = scr->counters;
     a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
@@ -1762,7 +1776,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     }
     if (int rc = launch_pdl(dds_plan_kernel, dim3(tiles), dim3(PLAN_THREADS), st, *var, p, nreq, scr->req_src, scr->req_dst,
                             (unsigned long long *)scr->tile_sums, scr->plan_tag, offsets_dev_or_null, scr->seg_tab, scr->seg_cap,
-                            scr->status, pr))
+                            scr->status, scr->status_tag, pr))
         return rc;
     a.req_src = scr->req_src;
     a.req_dst = scr->req_dst;

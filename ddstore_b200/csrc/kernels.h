@@ -24,8 +24,13 @@ typedef struct ddsk_var {
     int32_t pad_;
 } ddsk_var_t;
 
-/* status word written by the kernels: 0xFFFF... = ok, else (first_bad_request << 8) | code */
+/* status word written by the kernels: 0xFFFF... = ok, else (ordinal << 48) | (first_bad_request << 8) | code, where
+ * ordinal is the launch's position in its queue of DDS_NO_SYNC batches (0 for a synchronous call; saturates at 0xFFFF).
+ * Kernels only atomicMin into it, so the word holds the first error in queue order, and inside that batch the
+ * lowest-index one. Request indices stay below 2^40. */
 #define DDSK_STATUS_OK 0xFFFFFFFFFFFFFFFFull
+#define DDSK_STATUS_ORD_SHIFT 48
+#define DDSK_STATUS_REQ_MASK 0xFFFFFFFFFFull /* (word >> 8) & this = request index */
 #define DDSK_CODE_START 2
 #define DDSK_CODE_COUNT 3
 #define DDSK_CODE_CAPACITY 12
@@ -43,6 +48,7 @@ typedef struct ddsk_scratch {
     unsigned long long *plan_word; /* 8 words: [0..3] per slot (sequence number & 0xFFFFFF) << 40 | packed total ("plan
                                       ready"), [4..7] per slot the packed total parked by the plan kernel's last tile */
     unsigned int ovl_seq;       /* sequence number the NEXT overlap launch carries (host side, set by the caller) */
+    unsigned long long status_tag; /* ordinal << DDSK_STATUS_ORD_SHIFT of the NEXT launch (host side, set by the caller) */
     /* plan in global memory (variable-count batches above ddsk_plan_smem_max() requests, or >= 4 GiB destinations) */
     uint64_t *req_src;          /* [cap_req]   planned source address per request (0 = skip) */
     int64_t *req_dst;           /* [cap_req+1] exclusive scan of request bytes */

@@ -231,6 +231,7 @@ struct dds_store {
     // row were chained on the pending stream right before it (0: the next one starts a new run)
     unsigned int ovl_seq = 1;
     int run_len = 0;
+    unsigned int queue_len = 0; // launches in the current queue of DDS_NO_SYNC batches (saturates at 0xFFFF)
     // plan scratch slots of overlapped variable-count batches: launch q plans into slot q & 3, so its plan kernels can
     // run while the gather of launch q-1 is still reading slot (q-1) & 3
     struct Slot {
@@ -692,13 +693,32 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     return brc;
 }
 
+// nonnegative a * b and a + b, INT64_MAX when the exact result does not fit
+int64_t sat_mul(int64_t a, int64_t b) {
+    int64_t r;
+    return __builtin_mul_overflow(a, b, &r) ? INT64_MAX : r;
+}
+int64_t sat_add(int64_t a, int64_t b) {
+    int64_t r;
+    return __builtin_add_overflow(a, b, &r) ? INT64_MAX : r;
+}
+
+// The kernels tag every status report with the launch's position in its queue of DDS_NO_SYNC batches (0 for a
+// synchronous call or the first of a queue), so the sticky word ends up holding the first failing batch in queue order.
+// `chain`: the launch goes behind batches still pending on the same stream.
+void tag_launch(dds_store *s, bool chain) {
+    const unsigned int ord = chain ? s->queue_len : 0u;
+    s->queue_len = std::min(ord + 1u, 0xFFFFu);
+    s->scr.status_tag = (unsigned long long)ord << DDSK_STATUS_ORD_SHIFT;
+}
+
 int decode_status_word(unsigned long long st, int64_t *bad_index) {
     if (st == DDSK_STATUS_OK) {
         if (bad_index) *bad_index = -1;
         return DDS_OK;
     }
     int code = (int)(st & 0xFFull);
-    if (bad_index) *bad_index = (int64_t)(st >> 8);
+    if (bad_index) *bad_index = (int64_t)((st >> 8) & DDSK_STATUS_REQ_MASK);
     switch (code) {
     case DDSK_CODE_START: return fail(DDS_ERR_START);
     case DDSK_CODE_COUNT: return fail(DDS_ERR_COUNT);
@@ -747,7 +767,8 @@ int dds_locate(const int64_t *lenlist, int nranks, int64_t start, int64_t count,
     if (owner) *owner = t;
     if (offset) *offset = off;
     if (start < off) return fail(DDS_ERR_START);
-    if (count < 0 || start + count > lenlist[t]) return fail(DDS_ERR_COUNT);
+    // (start >= off >= 0 here: lenlist[t] - start cannot wrap, where start + count could)
+    if (count < 0 || count > lenlist[t] - start) return fail(DDS_ERR_COUNT);
     return DDS_OK;
 }
 
@@ -1149,14 +1170,20 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     if (no_sync && !(idx_dev && dst_dev)) return fail(DDS_ERR_ARG, "async batches need device indices and a device destination");
     CU(cudaSetDevice(s->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    // Async batches may queue up behind each other on ONE stream (the status word is then sticky: the first
-    // error of the whole queue is what dds_batch_wait reports). Anything else drains the queue first.
+    // Async batches may queue up behind each other on ONE stream (the status word is then sticky, and every launch tags
+    // its reports with its position in the queue: dds_batch_wait reports the first failing batch of the queue, with that
+    // batch's first invalid request). Anything else drains the queue first.
     const bool chain = s->pending && no_sync && st == s->pending_stream;
     if (s->pending && !chain) {
         if (int rc = dds_batch_wait(s, nullptr, nullptr)) return rc;
     }
     const int64_t R = v->kv.row_bytes;
     const bool fixed = !by_sample && counts == nullptr;
+    // A count above the variable's row total cannot be valid for any start (and count * R may not fit in 64 bits):
+    // such requests pack nothing. Every product below is then bounded by the variable's size, every sum saturates.
+    const int64_t rows = v->lenlist.empty() ? 0 : v->lenlist.back();
+    auto req_bytes = [&](int64_t c) { return c > 0 && c <= rows ? c * R : (int64_t)0; };
+    const int64_t nb_fixed = fixed ? req_bytes(fixed_count) : 0;
 
     if (nreq == 0) {
         if (dst_offsets) {
@@ -1170,7 +1197,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
 
     // ---- the legacy per-sample call: one request, host indices, synchronous, small result -> 1-CTA kernel
     if (fixed && nreq == 1 && !idx_dev && !no_sync && !cuda_stream && !dst_offsets) {
-        const int64_t need = fixed_count > 0 ? fixed_count * R : 0;
+        const int64_t need = nb_fixed;
         if (need <= (dst_dev ? (int64_t)(1 << 20) : kSmallOut) && (dst || need == 0))
             return small_get(s, v, starts[0], fixed_count, dst, dst_dev ? dst_capacity : std::min(dst_capacity, kSmallOut), dst_dev,
                              total_bytes, bad_index);
@@ -1200,15 +1227,15 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     // ---- packed size as far as the host can know it
     int64_t upper = -1; // upper bound of the packed bytes (== total when every request is valid)
     if (fixed)
-        upper = fixed_count > 0 ? nreq * fixed_count * R : 0;
+        upper = sat_mul(nreq, nb_fixed);
     else if (!idx_dev && !by_sample) {
         upper = 0;
-        for (int64_t i = 0; i < nreq; i++) upper += counts[i] > 0 ? counts[i] * R : 0;
+        for (int64_t i = 0; i < nreq; i++) upper = sat_add(upper, req_bytes(counts[i]));
     } else if (!idx_dev && by_sample && !v->h_tab_count.empty()) {
         upper = 0;
         for (int64_t i = 0; i < nreq; i++) {
             const int64_t id = starts[i];
-            if (id >= 0 && id < v->nsamples) upper += v->h_tab_count[(size_t)id] > 0 ? v->h_tab_count[(size_t)id] * R : 0;
+            if (id >= 0 && id < v->nsamples) upper = sat_add(upper, req_bytes(v->h_tab_count[(size_t)id]));
         }
     }
 
@@ -1240,10 +1267,12 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
 
     // ---- launch
     int64_t *d_offsets = dst_dev ? dst_offsets : nullptr;
-    if (!dst_dev && dst_offsets && !fixed) { // byte offsets for a host caller: staged on the device, copied back below
+    if (!dst_dev && !fixed) { // byte offsets for a host destination: staged on the device (the caller's, and the length of
+                              // the prefix to copy back on an error), copied back below
         if (int rc = ensure_offs(s, nreq + 1)) return rc;
         d_offsets = s->d_offs;
     }
+    tag_launch(s, chain);
     const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
     int krc;
@@ -1275,29 +1304,40 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     }
     // status + total arrive in the pinned mirror words with the end of the kernel (no D2H copy)
 
-    // ---- results back to a host destination
+    // ---- results back to a host destination: exactly what the serial get() loop would have left there. The status
+    // comes first: after an invalid request only the requests before it are copied, after a capacity error nothing --
+    // the rest of the staging buffer holds whatever an earlier batch left in it.
     if (!dst_dev) {
+        CU(cudaStreamSynchronize(st));
+        const unsigned long long stw = s->h_status[0];
+        const int64_t total = fixed ? upper : (int64_t)s->h_status[1];
+        int64_t n = total; // bytes the caller receives
+        if (stw != DDSK_STATUS_OK) {
+            const int code = (int)(stw & 0xFFull);
+            const int64_t bad = (int64_t)((stw >> 8) & DDSK_STATUS_REQ_MASK);
+            const bool invalid = code == DDSK_CODE_START || code == DDSK_CODE_COUNT || code == DDSK_CODE_SAMPLE;
+            if (total > cap || !invalid || bad >= nreq)
+                n = 0; // the batch did not fit (whatever else was wrong): nothing was packed
+            else if (fixed)
+                n = bad * nb_fixed;
+            else { // the packed offset of the first invalid request
+                CU(cudaMemcpyAsync(&n, d_offsets + bad, 8, cudaMemcpyDeviceToHost, st));
+                CU(cudaStreamSynchronize(st));
+            }
+        }
+        if (n > 0) {
+            if (small_out) {
+                memcpy(dst, s->h_small + kSmallIdx * 16, (size_t)n); // pinned bounce -> the caller's buffer
+            } else if (n >= (int64_t)(4u << 20) && is_pageable(dst)) {
+                if (int rc = d2h_pageable(s, dst, d_dst, (size_t)n, st)) return rc;
+            } else {
+                CU(cudaMemcpyAsync(dst, d_dst, (size_t)n, cudaMemcpyDeviceToHost, st));
+            }
+        }
         if (dst_offsets && !fixed)
             CU(cudaMemcpyAsync(dst_offsets, d_offsets, (size_t)(nreq + 1) * 8, cudaMemcpyDeviceToHost, st));
-        if (small_out) {
-            CU(cudaStreamSynchronize(st));
-            int64_t tot = fixed ? upper : (int64_t)s->h_status[1];
-            if (tot > cap) tot = cap;
-            if (tot > 0) memcpy(dst, s->h_small + kSmallIdx * 16, (size_t)tot); // pinned bounce -> the caller's buffer
-        } else if (upper >= 0) {
-            if (cap >= (int64_t)(4u << 20) && is_pageable(dst)) {
-                if (int rc = d2h_pageable(s, dst, d_dst, (size_t)cap, st)) return rc;
-            } else if (cap > 0) {
-                CU(cudaMemcpyAsync(dst, d_dst, (size_t)cap, cudaMemcpyDeviceToHost, st));
-            }
-        } else {
-            CU(cudaStreamSynchronize(st)); // device-resident counts: the size is only known on the device
-            int64_t tot = (int64_t)s->h_status[1];
-            if (s->h_status[0] == DDSK_STATUS_OK && tot > 0 && tot <= cap)
-                CU(cudaMemcpyAsync(dst, d_dst, (size_t)tot, cudaMemcpyDeviceToHost, st));
-        }
         if (dst_offsets && fixed)
-            for (int64_t i = 0; i <= nreq; i++) dst_offsets[i] = i * (fixed_count > 0 ? fixed_count * R : 0);
+            for (int64_t i = 0; i <= nreq; i++) dst_offsets[i] = i * nb_fixed;
     }
     CU(cudaStreamSynchronize(st));
     if (total_bytes) *total_bytes = fixed ? upper : (int64_t)s->h_status[1];
@@ -1445,6 +1485,7 @@ int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, c
         m.cap[v] = dst_capacities[v];
         m.offsets[v] = dst_offsets && dst_offsets[v] ? dst_offsets[v] : (stage_offs ? s->d_offs + (int64_t)v * (nreq + 1) : nullptr);
     }
+    tag_launch(s, chain);
     const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
     const int mrc = ddsk_gather_multi(&m, d_ids, nreq, &scr, kflags, st);
@@ -1495,7 +1536,9 @@ int dds_get(dds_store_t *s, const char *name, int64_t start, int64_t count, int 
         clear_error();
         return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
     }
-    int64_t cap = count > 0 ? count * v->kv.row_bytes : 0;
+    // (a count above the variable's row total is invalid whatever the start: no room is needed for it)
+    const int64_t rows = v->lenlist.empty() ? 0 : v->lenlist.back();
+    const int64_t cap = count > 0 && count <= rows ? count * v->kv.row_bytes : 0;
     return dds_get_batch(s, name, &start, nullptr, count, 1, itemsize, buffer, cap, nullptr,
                          buffer_on_device ? DDS_DST_ON_DEVICE : 0u, nullptr, nullptr, nullptr);
 }
@@ -1575,6 +1618,7 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
         if (int rc = dds_batch_wait(s, nullptr, nullptr)) return rc;
     }
     s->run_len = 0;
+    tag_launch(s, s->pending);
     const unsigned long long step = ++s->push.step;
     if (ddsk_gather_push(&v->kv, &s->push.table, s->push.d_table, starts_dev, fixed_count, nreq, step, &s->scr, st))
         return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());

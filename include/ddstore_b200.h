@@ -133,7 +133,13 @@ int dds_get(dds_store_t *s, const char *name, int64_t start, int64_t count, int 
  * (the loader loop, examples/vae/distdataset.py:79-89). counts == NULL means every request fetches
  * `fixed_count` rows. dst_offsets (nullable) receives nreq+1 byte offsets (exclusive scan).
  * On the first (lowest-index) invalid request returns its DDS_ERR_START/COUNT and its index in
- * *bad_index; requests before it are delivered, like the serial loop that stops at the exception. */
+ * *bad_index; requests before it are delivered, like the serial loop that stops at the exception. A host dst
+ * receives exactly those bytes and nothing else; a device dst may also receive later VALID requests, each at the
+ * offset the batch packs it to (an invalid request packs as zero bytes; with a fixed count it keeps its slot),
+ * never anything else. A negative count, and a count for which start + count overflows, are "Invalid count on
+ * target". If the packed batch does not fit dst_capacity, nothing is written: DDS_ERR_CAPACITY (*bad_index = -1),
+ * unless a request is invalid -- then that request's error wins, as in the loop that raises before it runs out of
+ * room. */
 /* cuda_stream: a cudaStream_t to enqueue on; NULL selects the store's own stream (pass cudaStreamLegacy,
  * (void*)0x1, for CUDA's legacy default stream). */
 #define DDS_IDX_ON_DEVICE 1u /* starts / counts are device pointers */
@@ -166,7 +172,9 @@ int dds_get_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
 /* Multi-array samples (BASELINE config 4: node_feat + edge_index per graph): the rows of the SAME nreq samples in
  * nvars (1..4) variables that each have a sample index, in ONE launch. dsts[v] (device) receives variable v's packed
  * rows, dst_offsets[v] (nullable, device, nreq+1 entries) its per-sample byte offsets, total_bytes[v] its packed size.
- * Needs DDS_DST_ON_DEVICE. bad_index is the position in sample_ids of the first failing request. */
+ * Needs DDS_DST_ON_DEVICE. The reported request is the first invalid one in variable order, then sample order: the
+ * lowest variable with an invalid request, and in it the lowest one (the loop over variables of a loop over samples);
+ * *bad_index is its position in sample_ids. Variables before it are delivered whole, that variable up to the sample. */
 int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids, int64_t nreq,
                           void *const *dsts, const int64_t *dst_capacities, int64_t *const *dst_offsets, unsigned flags,
                           void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
@@ -185,7 +193,8 @@ int dds_push_setup(dds_store_t *s, int64_t max_requests, int64_t max_bytes);
 int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_dev, int64_t fixed_count, int64_t nreq,
                        int itemsize, void **dst_out, void *cuda_stream);
 
-/* Completes the batch issued with DDS_NO_SYNC (stream sync + status decode). */
+/* Completes the batches issued with DDS_NO_SYNC (stream sync + status decode). Of a queue of several, the earliest
+ * failing batch in queue order is reported, with that batch's first invalid request in *bad_index. */
 int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index);
 
 /* void query(string name, VarInfo_t&), ddstore.cxx:46-49 */

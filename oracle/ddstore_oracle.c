@@ -59,7 +59,10 @@ int orc_locate(const long *lenlist, int nranks, long start, long count, int *tar
     *target = t;
     *offset = off;
     if (start < off) return ORC_ERR_START;
-    if (start + count > lenlist[t]) return ORC_ERR_COUNT;
+    /* Two intentional divergences from the reference (DESIGN.md section 5), whose `start + count > lenlist[t]` is UB
+     * for both: a negative count, and a count for which start + count overflows, are "Invalid count on target".
+     * start >= off >= 0 here, so lenlist[t] - start cannot overflow. */
+    if (count < 0 || count > lenlist[t] - start) return ORC_ERR_COUNT;
     return ORC_OK;
 }
 

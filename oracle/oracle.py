@@ -58,12 +58,14 @@ def np_lenlist(nrows):
 
 
 def np_locate(lenlist, start, count):
-    """include/ddstore.hpp:205-214 -> (target, offset, errcode)"""
+    """include/ddstore.hpp:205-214 -> (target, offset, errcode). Python integers do not overflow, so a count for which
+    start + count would overflow int64 is "Invalid count on target" here as in the product; a negative count is too
+    (both intentional divergences from the reference, where they are UB: DESIGN.md section 5)."""
     t = np_sortedsearch(lenlist, start)
     off = int(lenlist[t - 1]) if t > 0 else 0
     if start < off:
         return t, off, 2
-    if start + count > int(lenlist[t]):
+    if count < 0 or start + count > int(lenlist[t]):
         return t, off, 3
     return t, off, 0
 
@@ -153,7 +155,7 @@ class COracle:
         bases = (C.c_void_p * len(shards))(*[s.ctypes.data for s in shards])
         starts = np.ascontiguousarray(starts, dtype=np.int64)
         counts = np.ascontiguousarray(counts, dtype=np.int64)
-        cap = int(np.clip(counts, 0, None).sum()) * disp * itemsize
+        cap = int(np.clip(counts, 0, int(lenlist[-1])).sum()) * disp * itemsize  # (larger counts are invalid)
         out = np.zeros(max(cap, 1), np.uint8)
         offs = np.zeros(len(starts) + 1, np.int64)
         bad = C.c_long(-1)

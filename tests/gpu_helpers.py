@@ -155,3 +155,163 @@ def sample_ids(rng, nbytes, n):
     small = np.nonzero(np.asarray(nbytes) <= 4096)[0]
     ids = np.concatenate([np.arange(len(nbytes)), rng.choice(small, size=max(0, n - len(nbytes)))])
     return rng.permutation(ids)[:n].astype(np.int64)
+
+
+# ------------------------------------------------------------------------------- invalid requests and their expected result
+INT64_MAX = (1 << 63) - 1
+CODE_SAMPLE = 15  # a sample id outside the variable's sample index (no counterpart in the reference)
+
+
+def classify(lenlist, starts, counts):
+    """per-request result of the serial get() loop: 0, 2 ("Invalid start on target") or 3 ("Invalid count on target"),
+    with the documented divergences (negative and overflowing counts are count errors). Vectorised restatement of
+    oracle.np_locate, checked against it on every invalid request and on a sample of the valid ones."""
+    from oracle import oracle as O
+    ll = np.asarray(lenlist, np.int64)
+    s = np.asarray(starts, np.int64)
+    c = np.asarray(counts, np.int64)
+    k = np.searchsorted(ll, s, side="right")  # ll[k-1] <= s < ll[k]: the owner (src/ddstore.cxx:5-17), else owner 0
+    t = np.where((k >= 1) & (k < len(ll)), k, 0)
+    off = np.where(t > 0, ll[np.maximum(t - 1, 0)], 0)
+    with np.errstate(over="ignore"):
+        room = ll[t] - s  # (only used where s >= off >= 0: no wrap there)
+    codes = np.where(s < off, 2, np.where((c < 0) | (c > room), 3, 0)).astype(np.int64)
+    check = np.nonzero(codes)[0].tolist()[:3000] + list(range(0, len(s), max(1, len(s) // 500)))
+    for i in check:
+        assert O.np_locate(ll, int(s[i]), int(c[i]))[2] == codes[i], (int(s[i]), int(c[i]))
+    return codes
+
+
+class Expected:
+    """What a batch must leave behind. codes: per-request oracle result; nbytes: bytes of every request in the store's
+    packed layout (fixed counts keep a slot of count * row bytes for every request, variable counts pack an invalid
+    request as zero bytes); offs: its exclusive scan; lay: the layout with every VALID request's rows in place and
+    `valid` marking those bytes; bad: the first invalid request (-1: none); prefix: bytes the serial loop delivers."""
+
+    def __init__(self, allrows, row, lenlist, starts, counts, fixed, codes=None, shards=None):
+        starts = np.asarray(starts, np.int64)
+        counts = np.asarray(counts, np.int64)
+        total = int(lenlist[-1])
+        self.codes = classify(lenlist, starts, counts) if codes is None else np.asarray(codes, np.int64)
+        ok = self.codes == 0
+        bad = np.nonzero(~ok)[0]
+        self.bad = int(bad[0]) if bad.size else -1
+        self.code = int(self.codes[self.bad]) if bad.size else 0
+        sane = (counts > 0) & (counts <= total)  # (a larger count is invalid for every start, and packs nothing)
+        self.nbytes = np.where(sane & (ok | fixed), counts, 0) * row
+        self.offs = np.concatenate([[0], np.cumsum(self.nbytes)]).astype(np.int64)
+        self.T = int(self.offs[-1])
+        self.prefix = int(self.offs[self.bad]) if self.bad >= 0 else self.T
+        self.lay = np.zeros(self.T, np.uint8)
+        self.valid = np.zeros(self.T, bool)
+        v = np.nonzero(ok & (counts > 0))[0]
+        if v.size:
+            nb = counts[v] * row
+            dst = np.repeat(self.offs[v] - np.concatenate([[0], np.cumsum(nb)[:-1]]), nb) + np.arange(int(nb.sum()))
+            src = np.repeat(starts[v] * row - np.concatenate([[0], np.cumsum(nb)[:-1]]), nb) + np.arange(int(nb.sum()))
+            self.lay[dst] = allrows[src]
+            self.valid[dst] = True
+        n = self.bad if self.bad >= 0 else len(starts)
+        if shards is not None and n <= 20_000:  # the prefix is the oracle's serial loop, byte for byte
+            from oracle import oracle as O
+            pre, pre_offs, pbad, _ = O.np_get_batch(shards, starts[:n], counts[:n])
+            assert pbad == -1 and pre.size == self.prefix and np.array_equal(pre, self.lay[:self.prefix])
+            assert np.array_equal(pre_offs, self.offs[:n + 1])
+
+    def request_of(self, pos):
+        return int(np.searchsorted(self.offs, pos, side="right") - 1)
+
+
+def error_text(code):
+    from oracle import oracle as O
+    return "sample id" if code == CODE_SAMPLE else O.ERR_TEXT[code]
+
+
+def expect_raise(store, call, exp, over, what):
+    """run `call`; it must raise exactly the oracle's first error (an invalid request wins over a capacity error) with
+    last_bad_index = its index, or succeed when there is none"""
+    try:
+        call()
+        got = None
+    except ValueError as e:
+        got = str(e)
+    if exp.bad >= 0:
+        want = error_text(exp.code)
+        assert got is not None and (want in got if exp.code == CODE_SAMPLE else got == want), \
+            f"{what}: raised {got!r}, oracle: {want!r} at request {exp.bad}"
+        assert store.last_bad_index == exp.bad, f"{what}: last_bad_index {store.last_bad_index}, oracle {exp.bad}"
+    elif over:
+        assert got is not None and "too small" in got, f"{what}: raised {got!r}, expected a capacity error"
+        assert store.last_bad_index == -1, f"{what}: last_bad_index {store.last_bad_index} on a capacity error"
+    else:
+        assert got is None, f"{what}: raised {got!r} on a valid batch"
+
+
+class Dest:
+    """A destination of `nbytes` between GUARD-byte sentinel bands: kind 'device' (guarded_buffer), 'pinned' or
+    'pageable' (a numpy view into a larger sentinel-filled host array)"""
+
+    def __init__(self, torch, kind, nbytes, sentinel, off=0):
+        self.torch, self.kind, self.nbytes, self.sentinel, self.off = torch, kind, int(nbytes), sentinel, off
+        n = 2 * GUARD + off + self.nbytes
+        if kind == "device":
+            self.whole, self.view = guarded_buffer(torch, self.nbytes, off, sentinel)
+        else:
+            self.whole = torch.full((n,), sentinel, dtype=torch.uint8).pin_memory().numpy() if kind == "pinned" else \
+                np.full(n, sentinel, np.uint8)
+            self.view = self.whole[GUARD + off:GUARD + off + self.nbytes]
+
+    def reset(self):
+        if self.kind == "device":
+            self.whole.fill_(self.sentinel)
+            self.torch.cuda.synchronize()
+        else:
+            self.whole[:] = self.sentinel
+
+    def host(self):
+        return self.whole.cpu().numpy() if self.kind == "device" else self.whole.copy()
+
+
+def check_dest(dest, exp, over, what, offsets=None):
+    """The destination after a call (see expect_raise): no guard byte written; a capacity error leaves every byte
+    untouched; else bytes [0, prefix) are the oracle's and every later byte is the sentinel -- host destinations, the
+    serial loop's result exactly -- or, on the device, also may be a byte of a VALID request at the offset the store
+    packs it to. offsets (when requested) equal the oracle's up to the first invalid request."""
+    w = dest.host()
+    base, n, s = GUARD + dest.off, dest.nbytes, dest.sentinel
+    pre = np.nonzero(w[:base] != s)[0]
+    assert pre.size == 0, f"{what}: guard byte {int(pre[-1]) - base} (before the destination) was written"
+    post = np.nonzero(w[base + n:] != s)[0]
+    assert post.size == 0, f"{what}: guard byte {int(post[0])} past the destination's end was written"
+    d = w[base:base + n]
+    if over:
+        hit = np.nonzero(d != s)[0]
+        assert hit.size == 0, f"{what}: capacity error, yet byte {int(hit[0])} of the destination was written"
+        return
+    p = exp.prefix
+    diff = np.nonzero(d[:p] != exp.lay[:p])[0]
+    if diff.size:
+        i = int(diff[0])
+        r = exp.request_of(i)
+        raise AssertionError(f"{what}: byte {i} of the delivered prefix (request {r}, packed offset {int(exp.offs[r])}) is "
+                             f"{int(d[i]):#04x}, oracle {int(exp.lay[i]):#04x}")
+    rest = d[p:]
+    lay = np.full(rest.size, s, np.uint8)
+    ok_mask = np.zeros(rest.size, bool)
+    m = min(exp.T, n) - p
+    if dest.kind == "device" and m > 0:
+        ok_mask[:m] = exp.valid[p:p + m]
+        lay[:m] = exp.lay[p:p + m]
+    bad = np.nonzero((rest != s) & ~(ok_mask & (rest == lay)))[0]
+    if bad.size:
+        i = p + int(bad[0])
+        r = exp.request_of(i) if i < exp.T else None
+        where = (f"request {r} (code {int(exp.codes[r])}, packed offset {int(exp.offs[r])})" if r is not None
+                 else "past the packed end")
+        raise AssertionError(f"{what}: byte {i} after the first invalid request ({exp.bad}) was written "
+                             f"({int(rest[bad[0]]):#04x}); it lies in {where}")
+    if offsets is not None:
+        go = offsets.cpu().numpy() if hasattr(offsets, "cpu") else np.asarray(offsets)
+        k = (exp.bad if exp.bad >= 0 else len(exp.offs) - 1) + 1
+        diff = np.nonzero(go[:k] != exp.offs[:k])[0]
+        assert diff.size == 0, f"{what}: offsets[{int(diff[0])}] = {int(go[diff[0]])}, oracle {int(exp.offs[diff[0]])}"

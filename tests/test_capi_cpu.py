@@ -78,6 +78,32 @@ def test_host_locate_vs_oracle(coracle):
                 assert _capi.last_error() == {2: "Invalid start on target", 3: "Invalid count on target"}[rc]
 
 
+INT64_MAX = (1 << 63) - 1
+
+
+def test_host_locate_rejects_counts_whose_end_overflows(coracle):
+    """start + count past INT64_MAX must not wrap into an accepted request: every count from INT64_MAX - start + 1 (the
+    first whose end overflows) to INT64_MAX is "Invalid count on target", for starts in every owner and on the owner
+    boundaries; counts that end on or one row past an owner's end keep their old answers"""
+    for ll in ([10, 20], [7], [0, 5, 5, 12], [3, 3, 9]):
+        total = ll[-1]
+        for start in range(0, total):
+            for count in sorted({INT64_MAX - start + 1, INT64_MAX - start + 2, INT64_MAX // 2 + 1, INT64_MAX - 1,
+                                 INT64_MAX}):
+                t, off, rc = _locate(ll, start, count)
+                assert rc == _capi.ERR_COUNT, (ll, start, count, rc)
+                assert _capi.last_error() == "Invalid count on target"
+                assert coracle.locate(ll, start, count) == (t, off, rc)
+            t, off, rc = _locate(ll, start, 0)
+            assert rc == 0 and (t, off) == coracle.locate(ll, start, 0)[:2]
+            end = ll[t] - start  # the largest count that fits in the owner
+            assert _locate(ll, start, end)[2] == 0 and _locate(ll, start, end + 1)[2] == _capi.ERR_COUNT
+    # a start past the end falls back to owner 0: still a count error, also for overflowing counts
+    assert _locate([10, 20], 25, INT64_MAX)[2] == _capi.ERR_COUNT
+    assert _locate([10, 20], -1, INT64_MAX)[2] == _capi.ERR_START
+    assert _locate([10, 20], 1, -INT64_MAX - 1)[2] == _capi.ERR_COUNT
+
+
 def test_golden_request_errors_host_side():
     for w in G["worlds"]:
         for r in w["requests"]:

@@ -826,8 +826,9 @@ def test_large_pageable_destination_and_ingest(coracle):
 
 def test_doorbell_kernel_lifecycle():
     """the resident CTA behind get(): it leaves by itself when idle and a later get() starts a fresh one without losing
-    or repeating a request; a device-wide synchronize, an async batch and a free() in between all work; DDS_DOORBELL=0
-    semantics (1-CTA launch per call) are covered by the plan-variant subprocess tests' get() calls"""
+    or repeating a request; a device-wide synchronize, an async batch and a free() in between all work. (Without the
+    resident kernel -- DDS_DOORBELL=0, or a store's variables past the 256th -- every get() launches
+    dds_small_get_kernel: tests/test_gpu_errors.py runs both.)"""
     import time
     torch = _torch()
     rng = np.random.default_rng(9)

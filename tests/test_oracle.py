@@ -94,6 +94,23 @@ def test_demo_py_mean_property(coracle, dt):
         assert float(np.mean(out.view(dt))) == mean == idx // rec["num"] + 1
 
 
+def test_overflowing_and_negative_counts_c_vs_numpy(coracle):
+    """the two restatements agree where the reference is UB: a count whose end start + count overflows int64, and a
+    negative count, are both "Invalid count on target" (NumPy's Python integers cannot wrap; the C oracle must not)"""
+    imax = (1 << 63) - 1
+    for ll in ([10, 20], [7], [0, 5, 5, 12], [4, 0, 9]):
+        for start in (-3, -1, 0, 1, 3, 4, 5, ll[-1] - 1, ll[-1], ll[-1] + 2):
+            for count in (imax - start + 1 if start > 0 else imax, imax - 1, imax, imax // 2 + 1, -1, -imax - 1):
+                got = coracle.locate(ll, start, count)
+                assert got == O.np_locate(ll, start, count), (ll, start, count, got)
+                assert got[2] == (2 if start < 0 else 3), (ll, start, count, got)
+    # ... and a batch stops there, with the requests before it delivered
+    shards = [np.arange(20, dtype=np.int64).reshape(10, 2), np.arange(20, 40, dtype=np.int64).reshape(10, 2)]
+    for impl in (coracle.get_batch, O.np_get_batch):
+        out, offs, bad, rc = impl(shards, [0, 12, 1, 2], [2, 1, imax, 1])
+        assert (bad, rc) == (2, 3) and out.view(np.int64).tolist() == [0, 1, 2, 3, 24, 25]
+
+
 def test_dtype_mismatch(coracle):
     shards = [np.zeros((4, 2), np.float32)]
     out, offs, bad, rc = coracle.get_batch(shards, [0], [1], req_itemsize=8)
