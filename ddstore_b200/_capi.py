@@ -26,6 +26,14 @@ class VarInfo(C.Structure):
                 ("local_base", C.c_void_p)]
 
 
+# conversions of the converting batch entries (DDS_CVT_*)
+CVT_NONE, CVT_F32_BF16, CVT_F32_F16, CVT_F64_F32, CVT_U8_LUT16, CVT_U8_LUT32 = 0, 1, 2, 3, 4, 5
+
+
+class Convert(C.Structure):  # dds_convert_t
+    _fields_ = [("code", C.c_int32), ("lut", C.c_void_p)]
+
+
 # every symbol include/ddstore_b200.h declares: name -> (restype, argtypes)
 I64P = C.POINTER(C.c_int64)
 SIGNATURES = {
@@ -57,6 +65,14 @@ SIGNATURES = {
     "dds_get_samples_multi": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.c_void_p, C.c_int64,
                                         C.POINTER(C.c_void_p), I64P, C.POINTER(C.c_void_p), C.c_uint, C.c_void_p, I64P,
                                         I64P]),
+    "dds_get_batch_convert": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                        C.c_void_p, C.c_int64, C.c_void_p, C.c_uint, C.c_void_p, C.POINTER(Convert),
+                                        I64P, I64P]),
+    "dds_get_samples_convert": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                          C.c_void_p, C.c_uint, C.c_void_p, C.POINTER(Convert), I64P, I64P]),
+    "dds_get_samples_multi_convert": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.c_void_p, C.c_int64,
+                                                C.POINTER(C.c_void_p), I64P, C.POINTER(C.c_void_p), C.c_uint,
+                                                C.c_void_p, C.POINTER(Convert), I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_get_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,

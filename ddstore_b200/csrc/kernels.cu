@@ -55,6 +55,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <type_traits>
 
 #include "kernels.h"
 
@@ -423,7 +424,10 @@ struct PlanView<0> {
     __device__ __forceinline__ int64_t d(int64_t i) const { return __ldcg(&dst[i]); }
 };
 
-template <bool FIXED, int CH, int PCAP>
+// VALIGN (converting multi-array launches): segment boundaries are aligned down to 8 bytes relative to the variable
+// they fall in (vb[]: the variables' starts in the concatenated packed space), so that no segment cuts a source element
+// of a variable that starts at an odd offset
+template <bool FIXED, int CH, int PCAP, bool VALIGN = false>
 struct ChunkWalker {
     // warp-uniform state
     int64_t seg_pos = 0, seg_end = 0, T = 0, seg_bytes = 0, nseg = 0, nb = 0;
@@ -441,6 +445,8 @@ struct ChunkWalker {
     const uint64_t *push_win = nullptr;   // shared memory: [push_n] window of requester p
     int64_t push_idx_off = 0;
     PlanView<PCAP> pv;
+    bool valign = false;
+    int64_t vb[VALIGN ? DDSK_MAX_MULTI : 1];
     // per-lane window of 32 request descriptors
     uint64_t w_src = 0;
     int64_t w_dst = 0, w_n = 0;
@@ -486,8 +492,23 @@ struct ChunkWalker {
         }
     }
 
+    __device__ __forceinline__ int64_t align_to_var(int64_t pos) const {
+        int64_t b = vb[0];
+#pragma unroll
+        for (int k = 1; k < (VALIGN ? DDSK_MAX_MULTI : 1); k++)
+            if (pos >= vb[k]) b = vb[k];
+        return b + ((pos - b) & ~(int64_t)7);
+    }
+
     // largest r in [0, nreq) with dst[r] <= pos
     __device__ __forceinline__ int64_t locate_var(const GatherArgs &a, int64_t pos, int lane) {
+        if constexpr (VALIGN && PCAP == 0) {
+            if (valign) { // pos lies at most 7 bytes below a SEG_GRAIN boundary (that of the segment's nominal start)
+                int64_t r0 = (int64_t)__ldcg(&a.seg_tab[(pos + 7) / SEG_GRAIN]);
+                while (r0 > 0 && pv.d(r0) > pos) r0--;
+                return r0;
+            }
+        }
         if (PCAP == 0) {
             // plan in global memory: the plan kernels left the answer for every SEG_GRAIN boundary (one load)
             int64_t r0 = (int64_t)__ldcg(&a.seg_tab[pos / SEG_GRAIN]);
@@ -543,6 +564,13 @@ struct ChunkWalker {
                 if (seg >= nseg) return 0;
                 seg_pos = seg * seg_bytes;
                 seg_end = min(T, seg_pos + seg_bytes);
+                if constexpr (VALIGN) {
+                    if (valign) {
+                        seg_pos = align_to_var(seg_pos);
+                        if (seg_end < T) seg_end = align_to_var(seg_end);
+                        if (seg_pos >= seg_end) continue; // (an empty segment)
+                    }
+                }
                 r = FIXED ? seg_pos / nb : locate_var(a, seg_pos, lane);
             }
             if (r >= nreq) { // defensive: cannot happen while seg_pos < T
@@ -676,6 +704,155 @@ __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, ui
 }
 
 // ------------------------------------------------------------------------------------------------
+// Converting drain (DDSK_CVT_*): the load side of the walk is unchanged, the staged SOURCE elements are converted on the
+// way out of shared memory. Source byte p of a variable's packed rows goes to output byte (p >> IL) << OL; the ratio is
+// a power of two, so every position is a shift.
+// Invariant relied on here: a staged piece never cuts a source element. The walk cuts only at request boundaries
+// (multiples of the row size, itself a multiple of the itemsize), at segment boundaries (multiples of CH, SEG_GRAIN or
+// of a whole fixed-count request) and at CH bytes -- CH and SEG_GRAIN are multiples of 8, and itemsizes are 1, 4 or 8.
+// Source elements are therefore also aligned to their size in shared memory (stage offsets are 16-byte aligned and
+// source rows start at itemsize-aligned addresses).
+// ------------------------------------------------------------------------------------------------
+__host__ __device__ constexpr int cvt_in_log2(int code) { return code == DDSK_CVT_F64_F32 ? 3 : (code == DDSK_CVT_F32_BF16 || code == DDSK_CVT_F32_F16) ? 2 : 0; }
+__host__ __device__ constexpr int cvt_out_log2(int code) {
+    return code == DDSK_CVT_NONE ? 0 : (code == DDSK_CVT_F64_F32 || code == DDSK_CVT_U8_LUT32) ? 2 : 1;
+}
+__device__ __forceinline__ int64_t cvt_scale(int64_t p, int code) { return (p >> cvt_in_log2(code)) << cvt_out_log2(code); }
+
+__device__ __forceinline__ uint32_t cvt2_bf16(float lo, float hi) { // packs (lo, hi) -> [15:0] lo, [31:16] hi
+    uint32_t d;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
+    return d;
+}
+__device__ __forceinline__ uint32_t cvt2_f16(float lo, float hi) {
+    uint32_t d;
+    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
+    return d;
+}
+__device__ __forceinline__ uint32_t cvt_f32_of_f64(uint64_t bits) {
+    float f;
+    asm("cvt.rn.f32.f64 %0, %1;" : "=f"(f) : "d"(__longlong_as_double((long long)bits)));
+    return __float_as_uint(f);
+}
+__device__ __forceinline__ uint32_t lds16(uint32_t addr) {
+    uint16_t v;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ uint32_t lut16(uint32_t lut, uint32_t b) { return lds16(lut + (b << 1)); }
+__device__ __forceinline__ uint32_t lut32(uint32_t lut, uint32_t b) { return lds32(lut + (b << 2)); }
+
+// one element: source at shared address s, output at d
+template <int CODE>
+__device__ __forceinline__ void cvt_one(uint32_t s, char *d, uint32_t lut) {
+    if constexpr (CODE == DDSK_CVT_F32_BF16 || CODE == DDSK_CVT_F32_F16) {
+        const float f = __uint_as_float(lds32(s));
+        const uint32_t w = CODE == DDSK_CVT_F32_BF16 ? cvt2_bf16(f, 0.0f) : cvt2_f16(f, 0.0f);
+        *(uint16_t *)d = (uint16_t)(w & 0xFFFFu);
+    } else if constexpr (CODE == DDSK_CVT_F64_F32) {
+        *(uint32_t *)d = cvt_f32_of_f64(lds64(s));
+    } else if constexpr (CODE == DDSK_CVT_U8_LUT16) {
+        *(uint16_t *)d = (uint16_t)lut16(lut, lds8(s));
+    } else {
+        *(uint32_t *)d = lut32(lut, lds8(s));
+    }
+}
+
+// one 16-byte output vector from the source elements at shared address s (VEC: s is aligned for vector loads)
+template <int CODE, bool VEC>
+__device__ __forceinline__ uint4 cvt_vec(uint32_t s, uint32_t lut) {
+    uint4 o;
+    if constexpr (CODE == DDSK_CVT_F32_BF16 || CODE == DDSK_CVT_F32_F16) { // 8 floats (32 B) -> 8 halves
+        uint32_t w[8];
+        if (VEC) {
+            const uint4 a = lds128(s), b = lds128(s + 16);
+            w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; k++) w[k] = lds32(s + 4u * k);
+        }
+        uint32_t r[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+            r[k] = CODE == DDSK_CVT_F32_BF16 ? cvt2_bf16(__uint_as_float(w[2 * k]), __uint_as_float(w[2 * k + 1]))
+                                             : cvt2_f16(__uint_as_float(w[2 * k]), __uint_as_float(w[2 * k + 1]));
+        o = make_uint4(r[0], r[1], r[2], r[3]);
+    } else if constexpr (CODE == DDSK_CVT_F64_F32) { // 4 doubles (32 B) -> 4 floats
+        uint64_t q[4];
+        if (VEC) {
+            const uint4 a = lds128(s), b = lds128(s + 16);
+            q[0] = (uint64_t)a.y << 32 | a.x; q[1] = (uint64_t)a.w << 32 | a.z;
+            q[2] = (uint64_t)b.y << 32 | b.x; q[3] = (uint64_t)b.w << 32 | b.z;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) q[k] = lds64(s + 8u * k);
+        }
+        o = make_uint4(cvt_f32_of_f64(q[0]), cvt_f32_of_f64(q[1]), cvt_f32_of_f64(q[2]), cvt_f32_of_f64(q[3]));
+    } else if constexpr (CODE == DDSK_CVT_U8_LUT16) { // 8 bytes -> 8 table entries of 2 bytes
+        uint32_t b[8];
+        if (VEC) {
+            const uint64_t v = lds64(s);
+#pragma unroll
+            for (int k = 0; k < 8; k++) b[k] = (uint32_t)(v >> (8 * k)) & 0xFFu;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; k++) b[k] = lds8(s + k);
+        }
+        uint32_t r[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) r[k] = lut16(lut, b[2 * k]) | (lut16(lut, b[2 * k + 1]) << 16);
+        o = make_uint4(r[0], r[1], r[2], r[3]);
+    } else { // LUT32: 4 bytes -> 4 table entries of 4 bytes
+        uint32_t b[4];
+        if (VEC) {
+            const uint32_t v = lds32(s);
+#pragma unroll
+            for (int k = 0; k < 4; k++) b[k] = (v >> (8 * k)) & 0xFFu;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) b[k] = lds8(s + k);
+        }
+        o = make_uint4(lut32(lut, b[0]), lut32(lut, b[1]), lut32(lut, b[2]), lut32(lut, b[3]));
+    }
+    return o;
+}
+
+// Drain one staged piece converted: n source bytes at shared address s0 (whole elements) go to d (aligned to the output
+// itemsize). Element-wise head up to the first 16-byte boundary of d, aligned 128-bit stores, element-wise tail.
+template <int CODE>
+__device__ __forceinline__ void cvt_drain(uint32_t s0, char *d, uint32_t n, uint32_t lut, int lane) {
+    constexpr int IL = cvt_in_log2(CODE), OL = cvt_out_log2(CODE);
+    constexpr uint32_t E = 16u >> OL;                              // elements per output vector
+    constexpr uint32_t VA = (E << IL) < 16u ? (E << IL) : 16u;     // source alignment of the vector loads
+    const uint32_t ne = n >> IL;
+    uint32_t head = ((16u - (uint32_t)((uint64_t)d & 15u)) & 15u) >> OL;
+    if (head > ne) head = ne;
+    const uint32_t nv = (ne - head) / E;
+    const uint32_t tail = ne - head - nv * E;
+    const uint32_t sb = s0 + (head << IL);
+    char *dv = d + (head << OL);
+    if ((sb & (VA - 1u)) == 0) { // warp-uniform
+#pragma unroll 2
+        for (uint32_t j = (uint32_t)lane; j < nv; j += 32) stg128(dv + ((size_t)j << 4), cvt_vec<CODE, true>(sb + j * (E << IL), lut));
+    } else {
+#pragma unroll 2
+        for (uint32_t j = (uint32_t)lane; j < nv; j += 32) stg128(dv + ((size_t)j << 4), cvt_vec<CODE, false>(sb + j * (E << IL), lut));
+    }
+    if ((uint32_t)lane < head) cvt_one<CODE>(s0 + ((uint32_t)lane << IL), d + ((uint32_t)lane << OL), lut);
+    if ((uint32_t)lane < tail) {
+        const uint32_t k = head + nv * E + (uint32_t)lane;
+        cvt_one<CODE>(s0 + (k << IL), d + ((size_t)k << OL), lut);
+    }
+}
+
+// the kernel parameter carrying a launch's conversion: ddsk_cvt_t, or nothing at all for raw launches
+struct NoCvt {
+    int32_t unused_;
+};
+template <bool CVT>
+using CvtParam = typename std::conditional<CVT, ddsk_cvt_t, NoCvt>::type;
+
+// ------------------------------------------------------------------------------------------------
 // Plan in shared memory (variable counts, <= PCAP requests): EVERY CTA computes the whole plan -- lookup + checks +
 // exclusive scan of the request sizes -- for itself. The index arrays are a few tens of KB that stay in L2 after
 // the first CTA touched them, so the redundancy is cheap, and it removes every inter-CTA dependency the plan
@@ -684,9 +861,14 @@ __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, ui
 // Returns the packed total T (exact, int64); the shared copy keeps 32-bit offsets (the launcher uses this path only
 // when the destination capacity is below 4 GiB, so T > 2^32 is a capacity error and nothing is copied).
 // ------------------------------------------------------------------------------------------------
-template <int NW, int PCAP>
+// (CVT: the offsets the caller sees are in output bytes of conversion `code`; the plan itself stays in source bytes)
+template <int NW, int PCAP, bool CVT = false>
 __device__ __forceinline__ int64_t plan_in_smem(const GatherArgs &a, const PlanView<PCAP> &pv, int64_t *wtot, int warp,
-                                                int lane, bool writer) {
+                                                int lane, bool writer, int code = 0) {
+    auto out = [&](int64_t x) -> int64_t {
+        if constexpr (CVT) return cvt_scale(x, code);
+        else return x;
+    };
     const int64_t nreq = a.nreq;
     const int64_t per_warp = ((nreq + NW * 128 - 1) / (NW * 128)) * 128;
     const int64_t w0 = min(nreq, (int64_t)warp * per_warp), w1 = min(nreq, w0 + per_warp);
@@ -720,15 +902,15 @@ __device__ __forceinline__ int64_t plan_in_smem(const GatherArgs &a, const PlanV
         const int64_t incl = warp_incl_scan(v, lane);
         if (i < w1) {
             sts32(pv.dst_s + (uint32_t)i * 4u, (uint32_t)(run + incl - v));
-            if (writer && a.offsets_out) a.offsets_out[i] = run + incl - v;
+            if (writer && a.offsets_out) a.offsets_out[i] = out(run + incl - v);
         }
         run += __shfl_sync(0xffffffffu, incl, 31);
     }
     if (warp == 0 && lane == 0) {
         sts32(pv.dst_s + (uint32_t)nreq * 4u, (uint32_t)min(T, (int64_t)0xFFFFFFFFll));
         if (writer) {
-            if (a.offsets_out) a.offsets_out[nreq] = T;
-            if (a.total_out) *a.total_out = T;
+            if (a.offsets_out) a.offsets_out[nreq] = out(T);
+            if (a.total_out) *a.total_out = T; // (source bytes: the host scales the total it reports)
         }
     }
     __syncthreads();
@@ -753,15 +935,20 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
     }
 }
 
-template <bool FIXED, int NW, int S, int CH, int PCAP>
-__global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a) {
+// CVT: the converting form (DDSK_CVT_*, `c` carries the codes and tables). Everything on the load side -- walk over the
+// packed SOURCE byte space, rings, plan, checks, overlap protocol -- is the raw kernel's; only the drain and the
+// caller-visible offsets differ. Converting launches have no push fetch.
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false>
+__global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
+                                                                const __grid_constant__ CvtParam<CVT> c) {
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
+    constexpr bool PUSH = FIXED && !CVT;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
     __shared__ __align__(8) uint64_t full_bar[NW][S];
     __shared__ __align__(16) PieceDesc desc[NW][S][32];
     __shared__ int64_t wtot[PCAP > 0 ? NW : 1];
-    __shared__ int64_t push_rbase[FIXED ? DDSK_MAX_RANKS + 1 : 1];
-    __shared__ uint64_t push_win[FIXED ? DDSK_MAX_RANKS : 1];
+    __shared__ int64_t push_rbase[PUSH ? DDSK_MAX_RANKS + 1 : 1];
+    __shared__ uint64_t push_win[PUSH ? DDSK_MAX_RANKS : 1];
 
     const int lane = threadIdx.x & 31;
     const int warp = threadIdx.x >> 5;
@@ -773,6 +960,15 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         for (int s = 0; s < S; s++) mbar_init(smem_u32(&full_bar[warp][s]), 1);
         fence_mbar_init();
     }
+    // the launch's tables, copied from the parameter into shared memory behind the rings and the plan
+    uint32_t lut_s = 0;
+    if constexpr (CVT) {
+        lut_s = smem_u32(smem_dyn) + (uint32_t)(NW * S * STAGE + (PCAP ? PCAP * 12 + 16 : 0));
+        for (int i = threadIdx.x; i < c.lut_bytes / 4; i += NW * 32) sts32(lut_s + 4u * (uint32_t)i, c.lut[i]);
+        __syncthreads();
+    }
+    int code0 = 0; // the conversion of a single-variable launch
+    if constexpr (CVT) code0 = c.code[0];
     if (a.dbg && threadIdx.x == 0) a.dbg[blockIdx.x * 4 + 0] = globaltimer_ns();
     // Programmatic dependent launch: let the NEXT kernel of the stream start launching early (its CTAs take over each
     // SM as ours retire), and do not touch global memory before the PREVIOUS kernel (which may have produced our
@@ -797,14 +993,14 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     };
 
     // ---- the plan (variable counts) ------------------------------------------------------------
-    ChunkWalker<FIXED, CH, PCAP> w;
+    ChunkWalker<FIXED, CH, PCAP, CVT> w;
     if (!FIXED) {
         if constexpr (PCAP > 0) {
             w.pv.src_s = smem_u32(smem_dyn) + (uint32_t)(NW * S * STAGE);
             w.pv.dst_s = w.pv.src_s + (uint32_t)PCAP * 8u;
             const bool writer = blockIdx.x == 0;
             if (writer) pass_gate(); // CTA 0 writes the offsets / the total for the caller
-            w.T = plan_in_smem<NW, PCAP>(a, w.pv, wtot, warp, lane, writer);
+            w.T = plan_in_smem<NW, PCAP, CVT>(a, w.pv, wtot, warp, lane, writer, code0);
         } else {
             w.pv.src = a.req_src;
             w.pv.dst = a.req_dst;
@@ -853,7 +1049,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     // ended, i.e. after every owner finished reading list t (they signalled arrival after their last read).
     // CTA 0 never waits for another CTA of its own grid, and CTAs are dispatched in index order, so the only waits are
     // on other GPUs' kernels -- which every rank launches (the call is collective).
-    const bool push = FIXED && a.push != nullptr;
+    const bool push = PUSH && a.push != nullptr;
     if (FIXED && push) {
         const ddsk_push_t *ps = a.push;
         const int P = ps->nranks, me = ps->me, par = (int)(a.push_step & 1ull);
@@ -931,6 +1127,11 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 over |= endv - vbase[v] > a.mcap[v];
             }
         if (PCAP > 0) over |= w.T > 0xFFFFFFFFll; // 32-bit shared offsets
+        if constexpr (CVT) {
+            w.valign = true;
+#pragma unroll
+            for (int v = 0; v < DDSK_MAX_MULTI; v++) w.vb[v] = vbase[v];
+        }
     }
     auto dst_of = [&](int64_t dpos) -> char * {
         if (FIXED && push) { // the requester's window, found from the position in the concatenated packed space
@@ -949,6 +1150,33 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 d = a.mdst[k];
             }
         return d + (dpos - b);
+    };
+    // converting launches: the OUTPUT address of packed source position dpos, the conversion of its variable and the
+    // shared address of that variable's table
+    auto out_of = [&](int64_t dpos, int &code, uint32_t &lut) -> char * {
+        if constexpr (CVT) {
+            if (!multi) {
+                code = code0;
+                lut = lut_s + (uint32_t)c.lut_off[0];
+                return a.dst + cvt_scale(dpos, code0);
+            }
+            int64_t b = vbase[0];
+            char *d = a.mdst[0];
+            int cd = c.code[0], lo = c.lut_off[0];
+#pragma unroll
+            for (int k = 1; k < DDSK_MAX_MULTI; k++)
+                if (dpos >= vbase[k]) {
+                    b = vbase[k];
+                    d = a.mdst[k];
+                    cd = c.code[k];
+                    lo = c.lut_off[k];
+                }
+            code = cd;
+            lut = lut_s + (uint32_t)lo;
+            return d + cvt_scale(dpos - b, cd);
+        } else {
+            return nullptr; // (never called)
+        }
     };
     {
         // A claim is one atomic (requested ahead of need) + a division (FIXED), a shared-memory search (VAR, plan in
@@ -1037,6 +1265,35 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         const int64_t my_dpos = desc[warp][st][lane].dpos;
         const uint32_t my_n = desc[warp][st][lane].n;
         const uint32_t my_pack = desc[warp][st][lane].pack;
+        if constexpr (CVT) {
+            // converting launch: a converted piece is always drained cooperatively; the raw variables of a multi-array
+            // batch (code 0) keep the raw paths below
+            int my_code;
+            uint32_t my_lut;
+            char *const my_dst = out_of(my_dpos, my_code, my_lut);
+            const bool direct = my_code == 0 && my_n != 0 && (((uint32_t)(uint64_t)my_dst | my_n | (my_pack >> 16)) & 15u) == 0;
+            if (direct) tma_store_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n);
+            unsigned todo = __ballot_sync(0xffffffffu, my_n != 0 && !direct);
+            while (todo) {
+                const int j = __ffs(todo) - 1;
+                todo &= todo - 1;
+                const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
+                const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
+                const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
+                int code;
+                uint32_t lut;
+                char *const d = out_of(dpos, code, lut);
+                const uint32_t s0 = ring + st * STAGE + (pk & 0xffffu); // + source misalignment = first payload byte
+                switch (code) { // warp-uniform
+                case DDSK_CVT_F32_BF16: cvt_drain<DDSK_CVT_F32_BF16>(s0 + (pk >> 16), d, n, lut, lane); break;
+                case DDSK_CVT_F32_F16: cvt_drain<DDSK_CVT_F32_F16>(s0 + (pk >> 16), d, n, lut, lane); break;
+                case DDSK_CVT_F64_F32: cvt_drain<DDSK_CVT_F64_F32>(s0 + (pk >> 16), d, n, lut, lane); break;
+                case DDSK_CVT_U8_LUT16: cvt_drain<DDSK_CVT_U8_LUT16>(s0 + (pk >> 16), d, n, lut, lane); break;
+                case DDSK_CVT_U8_LUT32: cvt_drain<DDSK_CVT_U8_LUT32>(s0 + (pk >> 16), d, n, lut, lane); break;
+                default: drain_chunk<CH>(s0, pk >> 16, d, n, lane); break;
+                }
+            }
+        } else {
         // Pieces whose staged bytes, destination and size are all 16-byte aligned (every piece of an aligned
         // fixed-stride batch) are stored by their own lane, all lanes at once: one TMA bulk store each, no loop.
         char *const my_dst = dst_of(my_dpos);
@@ -1052,6 +1309,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
             drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, dst_of(dpos), n, lane);
         }
+        } // (raw drain: the same code as before converting launches existed)
         bulk_commit(); // every lane: one (possibly empty) bulk group per drained stage
         __syncwarp();  // all lanes are done reading the stage before it is refilled
         consumed++;
@@ -1072,12 +1330,26 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             if (v < a.plan.nvars && a.moffsets[v]) {
                 const int64_t basev = w.pv.d((int64_t)v * a.plan.per_var); // == vbase[v]; re-read so that vbase[] is
                 int64_t e = (v * a.plan.per_var + j == a.nreq) ? w.T : w.pv.d((int64_t)v * a.plan.per_var + j);
-                a.moffsets[v][j] = e - basev;                                // never indexed dynamically
+                if constexpr (CVT) a.moffsets[v][j] = cvt_scale(e - basev, c.code[v]); // (output bytes)
+                else a.moffsets[v][j] = e - basev;                                     // never indexed dynamically
+            }
+        }
+        if constexpr (CVT) { // the batch's total in output bytes (the sum over the variables' conversions)
+            if (gwarp == 0 && lane == 0 && a.total_out) {
+                int64_t t = 0;
+#pragma unroll
+                for (int v = 0; v < DDSK_MAX_MULTI; v++)
+                    if (v < a.plan.nvars) t += cvt_scale((v + 1 < a.plan.nvars ? vbase[v + 1] : w.T) - vbase[v], c.code[v]);
+                *a.total_out = t;
             }
         }
     }
     if (FIXED && a.offsets_out && !push) { // arithmetic offsets, written off the critical path
-        for (int64_t i = gwarp * 32 + lane; i <= a.nreq; i += nwarps * 32) a.offsets_out[i] = i * w.nb;
+        if constexpr (CVT) {
+            for (int64_t i = gwarp * 32 + lane; i <= a.nreq; i += nwarps * 32) a.offsets_out[i] = cvt_scale(i * w.nb, code0);
+        } else {
+            for (int64_t i = gwarp * 32 + lane; i <= a.nreq; i += nwarps * 32) a.offsets_out[i] = i * w.nb;
+        }
     }
 
     if (a.dbg && lane == 0) atomicMax(&a.dbg[blockIdx.x * 4 + 3], (unsigned long long)globaltimer_ns());
@@ -1209,7 +1481,8 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
                                                                 unsigned long long *tile_state, unsigned int tag,
                                                                 int64_t *__restrict__ offsets_out, uint32_t *__restrict__ seg_tab,
                                                                 int64_t seg_cap, unsigned long long *status,
-                                                                unsigned long long status_tag, PlanProto pr) {
+                                                                unsigned long long status_tag, PlanProto pr,
+                                                                int cvt_code) { // offsets_out in output bytes of this conversion
     __shared__ int64_t warp_tot[PLAN_THREADS / 32];
     __shared__ int64_t tile_excl_s;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -1283,7 +1556,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
             const int64_t d0 = run, d1 = run + nb[k];
             req_src[idx[k]] = sv[k];
             req_dst[idx[k]] = d0;
-            if (offsets_out) offsets_out[idx[k]] = d0;
+            if (offsets_out) offsets_out[idx[k]] = cvt_scale(d0, cvt_code);
             for (int64_t g = (d0 + SEG_GRAIN - 1) / SEG_GRAIN; g * SEG_GRAIN < d1 && g < seg_cap; g++) seg_tab[g] = (uint32_t)idx[k];
             run = d1;
         }
@@ -1292,7 +1565,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
     const int64_t T = tile_excl_s + agg;
     if (last_tile && threadIdx.x == 0) {
         req_dst[nreq] = T;
-        if (offsets_out) offsets_out[nreq] = T;
+        if (offsets_out) offsets_out[nreq] = cvt_scale(T, cvt_code);
     }
     if (pr.dbg && threadIdx.x == 0) atomicMax(&pr.dbg[4096 + 1], (unsigned long long)globaltimer_ns());
     if (pr.ovl) {
@@ -1547,14 +1820,25 @@ int ctas_per_sm_for(int nw, int s, int ch, int pcap) {
     return per_sm;
 }
 
-template <bool FIXED, int NW, int S, int CH, int PCAP>
-int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream) {
-    constexpr int smem = smem_bytes_of(NW, S, CH, PCAP);
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false>
+int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
+    // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan)
+    const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP>;
+    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
-    if (dev >= 64 || !(configured.load() & (1ull << dev))) {
+    if (CVT) { // the most a converting launch can ask for: every table at its widest
+        if (dev >= 64 || !(configured.load() & (1ull << dev))) {
+            cudaFuncAttributes fa;
+            int optin = 0;
+            CUDA_TRY(cudaFuncGetAttributes(&fa, kern));
+            CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+            const int most = std::min(smem_bytes_of(NW, S, CH, PCAP) + DDSK_MAX_MULTI * 1024, optin - (int)fa.sharedSizeBytes);
+            CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+            if (dev < 64) configured.fetch_or(1ull << dev);
+        }
+    } else if (dev >= 64 || !(configured.load() & (1ull << dev))) {
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         if (dev < 64) configured.fetch_or(1ull << dev);
     }
@@ -1571,9 +1855,27 @@ int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream) {
     attr[0].val.programmaticStreamSerializationAllowed = g_pdl ? 1 : 0;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, args));
+    if constexpr (CVT) {
+        CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, args, *cvt));
+    } else {
+        CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, args, NoCvt{0}));
+    }
     g_launches++;
     return 0;
+}
+
+// Does a converting launch of shared-memory-plan variant g with `lut_bytes` of tables fit in shared memory? (With four
+// 1 KiB tables the 8192-request variant does not: such batches plan in global memory instead.)
+template <int NW, int S, int CH, int PCAP>
+bool cvt_s_fits_t(int lut_bytes) {
+    cudaFuncAttributes fa;
+    int dev = 0, optin = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaFuncGetAttributes(&fa, dds_gather_kernel<false, NW, S, CH, PCAP, true>) != cudaSuccess ||
+        cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return false;
+    }
+    return smem_bytes_of(NW, S, CH, PCAP) + lut_bytes + (int)fa.sharedSizeBytes <= optin;
 }
 
 // launch with the programmatic-dependent-launch attribute (the kernels call griddepcontrol.wait themselves)
@@ -1611,7 +1913,9 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
 }
 
 template <bool FIXED>
-int launch_gather(const GatherArgs &args, cudaStream_t stream) {
+int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
+    // converting launches: the default variant of each entry (kGeomLarge = kGeomVar), whatever DDS_GATHER_GEOM* say
+    if (cvt) return launch_gather_t<FIXED, 12, 4, 4096, 0, true>(args, stream, cvt);
     // (the request size only picks a variant: a count too large to multiply safely counts as large)
     const int64_t request_bytes = args.count < ((int64_t)1 << 20) ? args.count * args.var.row_bytes : INT64_MAX;
     switch (geometry_for(FIXED, FIXED ? request_bytes : 0)) {
@@ -1625,7 +1929,9 @@ int launch_gather(const GatherArgs &args, cudaStream_t stream) {
     default: return launch_gather_t<FIXED, 8, 4, 4096, 0>(args, stream);
     }
 }
-int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream) {
+int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
+    if (cvt) return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, true>(args, stream, cvt)
+                           : launch_gather_t<false, 12, 3, 4096, 4096, true>(args, stream, cvt);
     switch (g) {
     case 1: return launch_gather_t<false, 12, 3, 3072, 8192>(args, stream);
     case 2: return launch_gather_t<false, 16, 3, 2048, 8192>(args, stream);
@@ -1633,6 +1939,16 @@ int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream) {
     case 4: return launch_gather_t<false, 8, 4, 4096, 4096>(args, stream);
     default: return launch_gather_t<false, 12, 3, 4096, 4096>(args, stream);
     }
+}
+
+// The shared-memory-plan variant for a batch of nreq requests into cap bytes (-1: the plan kernels). Converting launches
+// use the default variants only (DDS_GATHER_GEOM_S applies to raw batches), and need room for their tables.
+int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt) {
+    if (!g_smem_plan || cap >= ((int64_t)1 << 32)) return -1;
+    if (!cvt) return geometry_s_for(nreq);
+    if (nreq > kPlanSmemMax || nreq > g_plan_smem_default) return -1;
+    if (nreq <= 4096) return cvt_s_fits_t<12, 3, 4096, 4096>(cvt->lut_bytes) ? 0 : -1;
+    return cvt_s_fits_t<12, 3, 3072, 8192>(cvt->lut_bytes) ? 1 : -1;
 }
 
 void fill_overlap(GatherArgs &a, const ddsk_scratch_t *scr, int flags) {
@@ -1681,7 +1997,7 @@ void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk
 
 int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t count, int64_t nreq, void *dst_dev,
                       int64_t dst_capacity, int64_t *offsets_dev_or_null, const ddsk_scratch_t *scr, int flags,
-                      void *stream) {
+                      const ddsk_cvt_t *cvt, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
     if (nreq <= 0) return 0;
@@ -1701,7 +2017,7 @@ int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t 
     a.min_seg_chunks = 1;
     fill_overlap(a, scr, flags);
     a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
-    return launch_gather<true>(a, st);
+    return launch_gather<true>(a, st, cvt);
 }
 
 int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const ddsk_push_t *push_dev,
@@ -1727,12 +2043,13 @@ int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const 
                                  cudaMemcpyDeviceToDevice, st));
     a.push_nreq = nreq;
     a.push_step = step;
-    return launch_gather<true>(a, st);
+    return launch_gather<true>(a, st, nullptr);
 }
 
 // shared by ddsk_gather_var / ddsk_gather_multi: plan (in the launch, or by the two plan kernels) + gather
 static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq, int64_t cap_total, GatherArgs &a,
-                           int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, cudaStream_t st) {
+                           int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt,
+                           cudaStream_t st) {
     a.nreq = nreq;
     a.status = scr->status;
     a.status_tag = scr->status_tag;
@@ -1740,13 +2057,13 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
-    const int gs = (g_smem_plan && cap_total < ((int64_t)1 << 32)) ? geometry_s_for(nreq) : -1;
+    const int gs = select_s(nreq, cap_total, cvt);
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
         fill_overlap(a, scr, flags); // no scratch is shared between launches: independent batches may overlap
         if (a.overlap) a.tickets = scr->ovl + 8 + (a.seq & 3u);
-        return launch_gather_s(gs, a, st);
+        return launch_gather_s(gs, a, st, cvt);
     }
     if (nreq > scr->cap_req || cap_total / SEG_GRAIN + 2 > scr->seg_cap) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_gather_var: scratch too small (%lld requests > %lld, or %lld segments > %lld)",
@@ -1776,12 +2093,13 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     }
     if (int rc = launch_pdl(dds_plan_kernel, dim3(tiles), dim3(PLAN_THREADS), st, *var, p, nreq, scr->req_src, scr->req_dst,
                             (unsigned long long *)scr->tile_sums, scr->plan_tag, offsets_dev_or_null, scr->seg_tab, scr->seg_cap,
-                            scr->status, scr->status_tag, pr))
+                            scr->status, scr->status_tag, pr, cvt && p.nvars <= 1 ? (int)cvt->code[0] : 0))
         return rc;
     a.req_src = scr->req_src;
     a.req_dst = scr->req_dst;
     a.seg_tab = scr->seg_tab;
-    a.total_out = nullptr;
+    // (a converting multi-array batch has no single source total: its gather writes the output total here)
+    a.total_out = (cvt && p.nvars > 1) ? scr->total : nullptr;
     a.min_seg_chunks = g_min_seg_var;
     fill_overlap(a, scr, flags);
     if (a.overlap) {
@@ -1790,16 +2108,16 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
         a.plan_word = scr->plan_word;
         a.plan_tiles = tiles;
     }
-    return launch_gather<false>(a, st);
+    return launch_gather<false>(a, st, cvt);
 }
 
-int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity) {
+int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt) {
     if (pick_geometry()) return 1;
-    return !(g_smem_plan && dst_capacity < ((int64_t)1 << 32) && geometry_s_for(nreq) >= 0);
+    return select_s(nreq, dst_capacity, cvt) < 0;
 }
 
 int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, void *dst_dev, int64_t dst_capacity,
-                    int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, void *stream) {
+                    int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
     if (nreq <= 0) return 0;
@@ -1816,11 +2134,11 @@ int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nr
     a.var = *var;
     a.dst = (char *)dst_dev;
     a.dst_cap = dst_capacity;
-    return plan_and_gather(var, p, nreq, dst_capacity, a, offsets_dev_or_null, scr, flags, st);
+    return plan_and_gather(var, p, nreq, dst_capacity, a, offsets_dev_or_null, scr, flags, cvt, st);
 }
 
 int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int64_t nreq, ddsk_scratch_t *scr, int flags,
-                      void *stream) {
+                      const ddsk_cvt_t *cvt, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
     if (nreq <= 0 || m->nvars <= 0) return 0;
@@ -1853,7 +2171,7 @@ int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int6
         a.mcap[v] = m->cap[v];
         a.moffsets[v] = m->offsets[v];
     }
-    return plan_and_gather(&dummy, p, nreq * m->nvars, cap_total, a, nullptr, scr, flags, st);
+    return plan_and_gather(&dummy, p, nreq * m->nvars, cap_total, a, nullptr, scr, flags, cvt, st);
 }
 
 int ddsk_small_get(const ddsk_var_t *var, int64_t start, int64_t count, void *dst, int64_t dst_capacity,

@@ -71,11 +71,34 @@ typedef struct ddsk_scratch {
 #define DDSK_F_PREV2 64     /* overlap launch ovl_seq-2 belongs to the same run (do not write before it retired) */
 #define DDSK_F_PREV4 128    /* overlap launch ovl_seq-4 belongs to the same run (it used the same plan scratch slot) */
 
+/* Element conversion inside the gather (same values as DDS_CVT_* in include/ddstore_b200.h). Source byte p of a
+ * variable's packed rows goes to output byte (p >> in_log2) << out_log2. */
+#define DDSK_CVT_NONE 0      /* raw bytes (a variable of a multi-array batch that is not converted) */
+#define DDSK_CVT_F32_BF16 1  /* 4 -> 2 bytes, cvt.rn.bf16.f32 */
+#define DDSK_CVT_F32_F16 2   /* 4 -> 2 bytes, cvt.rn.f16.f32 */
+#define DDSK_CVT_F64_F32 3   /* 8 -> 4 bytes, cvt.rn.f32.f64 */
+#define DDSK_CVT_U8_LUT16 4  /* 1 -> 2 bytes, out = lut[in] */
+#define DDSK_CVT_U8_LUT32 5  /* 1 -> 4 bytes, out = lut[in] */
+#define DDSK_CVT_MAX 5
+/* The conversion of one launch, passed BY VALUE as a kernel parameter (so every queued launch carries its own tables).
+ * code[v] is variable v's conversion; the tables of the variables with a LUT code are packed into lut[] (lut_off[v]
+ * bytes in, 256 entries of the output itemsize) and copied to shared memory by every CTA. */
+typedef struct ddsk_cvt {
+    int32_t code[DDSK_MAX_MULTI];
+    int32_t lut_off[DDSK_MAX_MULTI];
+    int32_t lut_bytes; /* bytes of lut[] in use (0..4096) */
+    int32_t pad_;
+    uint32_t lut[DDSK_MAX_MULTI * 256];
+} ddsk_cvt_t;
+
 /* Fixed-count batch: every request fetches `count` rows; offsets are i*count*row_bytes.
- * One launch: validate + owner lookup + gather + pack. */
+ * One launch: validate + owner lookup + gather + pack.
+ * cvt (nullable): convert the elements on the way; dst_capacity is then in SOURCE bytes (the caller's output capacity
+ * rounded down to whole elements, scaled), while offsets_dev_or_null receives OUTPUT byte offsets. The same holds for
+ * ddsk_gather_var and ddsk_gather_multi (per variable). */
 int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t count, int64_t nreq, void *dst_dev,
                       int64_t dst_capacity, int64_t *offsets_dev_or_null, const ddsk_scratch_t *scr, int flags,
-                      void *stream);
+                      const ddsk_cvt_t *cvt, void *stream);
 
 /* Where the (start row, row count) of request i comes from (all device pointers): explicit arrays, or -- when
  * sample_ids is set -- the per-sample table of the variable: {start, count} = table[sample_ids[i]] (int64 pairs). */
@@ -92,8 +115,9 @@ typedef struct ddsk_index {
  * of the launch's own (slot = ovl_seq & 3): the plan then runs under the previous batch's gather. */
 int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, void *dst_dev,
                     int64_t dst_capacity, int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags,
-                    void *stream);
-int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity);
+                    const ddsk_cvt_t *cvt, void *stream);
+/* (cvt: the conversion the launch will carry, or NULL; its tables take shared memory from the in-launch plan) */
+int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt);
 int64_t ddsk_plan_smem_max(void);
 
 /* Multi-array batch: the rows of the SAME nreq sample ids in nvars (<= DDSK_MAX_MULTI) variables, one launch. vars_dev =
@@ -109,7 +133,7 @@ typedef struct ddsk_multi {
     int64_t *offsets[DDSK_MAX_MULTI];
 } ddsk_multi_t;
 int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int64_t nreq, ddsk_scratch_t *scr, int flags,
-                      void *stream);
+                      const ddsk_cvt_t *cvt, void *stream);
 
 /* Collective owner-push fetch (fixed-count batches, every rank on its own GPU). Each rank owns a WINDOW -- a peer-mapped
  * block of the store -- holding a header, two index lists and two destination buffers (alternating by step parity).

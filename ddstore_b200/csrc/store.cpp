@@ -225,6 +225,7 @@ struct dds_store {
     int64_t pending_fixed_total = -1;
     int64_t pending_nreq = 0;
     const int64_t *pending_total_ptr = nullptr; // device word holding the packed total of the last queued launch
+    int pending_cvt = 0;                        // that word is in source bytes of this conversion (DDSK_CVT_*)
     ddsk_var_t *d_multi_vars = nullptr; // device copy of the windows of the last multi-array combination
     std::string multi_key;
     // overlap protocol (DDS_OVERLAP): sequence number of the next overlap launch, and how many overlap launches in a
@@ -703,6 +704,18 @@ int64_t sat_add(int64_t a, int64_t b) {
     return __builtin_add_overflow(a, b, &r) ? INT64_MAX : r;
 }
 
+// ---- converting batches: source itemsize / output itemsize of a DDSK_CVT_* code, as log2
+int cvt_in_log2(int code) { return code == DDSK_CVT_F64_F32 ? 3 : (code == DDSK_CVT_F32_BF16 || code == DDSK_CVT_F32_F16) ? 2 : 0; }
+int cvt_out_log2(int code) { return code == DDSK_CVT_NONE ? 0 : (code == DDSK_CVT_F64_F32 || code == DDSK_CVT_U8_LUT32) ? 2 : 1; }
+// source bytes (whole elements) -> output bytes; saturates
+int64_t cvt_to_out(int64_t p, int code) {
+    if (p == INT64_MAX) return p;
+    return sat_mul(p >> cvt_in_log2(code), (int64_t)1 << cvt_out_log2(code));
+}
+// output capacity -> the source bytes it holds: whole output elements, scaled (exact, since every packed total is a whole
+// number of elements); saturates
+int64_t cvt_cap_to_src(int64_t cap, int code) { return sat_mul(cap >> cvt_out_log2(code), (int64_t)1 << cvt_in_log2(code)); }
+
 // The kernels tag every status report with the launch's position in its queue of DDS_NO_SYNC batches (0 for a
 // synchronous call or the first of a queue), so the sticky word ends up holding the first failing batch in queue order.
 // `chain`: the launch goes behind batches still pending on the same stream.
@@ -1160,9 +1173,12 @@ static int small_get(dds_store_t *s, Var *v, int64_t start, int64_t count, void 
 // The one batched path behind dds_get_batch / dds_get_samples / dds_get.
 //   by_sample == false: request i = (starts[i], counts ? counts[i] : fixed_count)
 //   by_sample == true : request i = the rows of sample starts[i] (= sample id) in v's per-sample index
+//   cvt != NULL: a converting batch (checked by the caller: device destination); dst_capacity, dst_offsets and the
+//   totals are in output bytes, the kernels get the capacity in source bytes
 static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
                       int64_t fixed_count, int64_t nreq, void *dst, int64_t dst_capacity, int64_t *dst_offsets,
-                      unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+                      unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index,
+                      const ddsk_cvt_t *cvt = nullptr) {
     if (nreq < 0 || dst_capacity < 0) return fail(DDS_ERR_ARG, "negative nreq or capacity");
     if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
     const bool idx_dev = flags & DDS_IDX_ON_DEVICE, dst_dev = flags & DDS_DST_ON_DEVICE;
@@ -1196,7 +1212,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     }
 
     // ---- the legacy per-sample call: one request, host indices, synchronous, small result -> 1-CTA kernel
-    if (fixed && nreq == 1 && !idx_dev && !no_sync && !cuda_stream && !dst_offsets) {
+    if (fixed && nreq == 1 && !idx_dev && !no_sync && !cuda_stream && !dst_offsets && !cvt) {
         const int64_t need = nb_fixed;
         if (need <= (dst_dev ? (int64_t)(1 << 20) : kSmallOut) && (dst || need == 0))
             return small_get(s, v, starts[0], fixed_count, dst, dst_dev ? dst_capacity : std::min(dst_capacity, kSmallOut), dst_dev,
@@ -1256,10 +1272,12 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
         }
         cap = need;
     }
+    const int code = cvt ? cvt->code[0] : DDSK_CVT_NONE;
+    if (cvt) cap = cvt_cap_to_src(dst_capacity, code);
     if (!d_dst && cap > 0) return fail(DDS_ERR_ARG, "null destination");
     // DDS_OVERLAP: declared independent of the batch queued right before it (see the protocol in kernels.cu)
     const bool ovl = no_sync && (flags & DDS_OVERLAP);
-    const bool uses_scratch = !fixed && ddsk_var_uses_scratch(nreq, cap);
+    const bool uses_scratch = !fixed && ddsk_var_uses_scratch(nreq, cap, cvt);
     if (uses_scratch) {
         if (int rc = renew_plan_tags(s)) return rc;
         if (int rc = ovl ? ensure_slots(s, nreq, cap) : ensure_scratch(s, nreq, cap)) return rc;
@@ -1277,7 +1295,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
     int krc;
     if (fixed) {
-        krc = ddsk_gather_fixed(&v->kv, d_starts, fixed_count, nreq, d_dst, cap, d_offsets, &scr, kflags, st);
+        krc = ddsk_gather_fixed(&v->kv, d_starts, fixed_count, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, st);
     } else {
         ddsk_index_t ix;
         memset(&ix, 0, sizeof(ix));
@@ -1289,13 +1307,14 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
             ix.starts = d_starts;
             ix.counts = d_counts;
         }
-        krc = ddsk_gather_var(&v->kv, &ix, nreq, d_dst, cap, d_offsets, &scr, kflags, st);
+        krc = ddsk_gather_var(&v->kv, &ix, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, st);
         s->scr.plan_tag = scr.plan_tag;
         s->pending_total_ptr = uses_scratch ? &scr.req_dst[nreq] : s->scr.total;
     }
     if (krc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
 
-    s->pending_fixed_total = fixed ? upper : -1;
+    s->pending_fixed_total = fixed ? cvt_to_out(upper, code) : -1;
+    s->pending_cvt = code; // (the device word of a variable-count total is in source bytes)
     s->pending_nreq = nreq;
     if (no_sync) { // nothing but the kernel(s) goes on the stream; the status word is read back in dds_batch_wait
         s->pending = true;
@@ -1340,8 +1359,58 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
             for (int64_t i = 0; i <= nreq; i++) dst_offsets[i] = i * nb_fixed;
     }
     CU(cudaStreamSynchronize(st));
-    if (total_bytes) *total_bytes = fixed ? upper : (int64_t)s->h_status[1];
+    if (total_bytes) *total_bytes = cvt_to_out(fixed ? upper : (int64_t)s->h_status[1], code);
     return decode_status(s, st, s->h_status[0], bad_index);
+}
+
+// Validate the conversions of a converting call (one per variable) and pack them, tables included, into the launch's
+// parameter. `none_ok`: DDS_CVT_NONE is allowed (a raw variable of a multi-array batch).
+static int make_cvt(Var *const *vars, const dds_convert_t *cv, int nvars, bool none_ok, ddsk_cvt_t *out) {
+    memset(out, 0, sizeof(*out));
+    if (!cv) return fail(DDS_ERR_ARG, "null conversion");
+    int off = 0;
+    for (int v = 0; v < nvars; v++) {
+        const int code = cv[v].code;
+        if (code < (none_ok ? DDS_CVT_NONE : DDS_CVT_F32_BF16) || code > DDSK_CVT_MAX)
+            return fail(DDS_ERR_ARG, "unknown conversion code " + std::to_string(code));
+        if (code != DDS_CVT_NONE && vars[v]->itemsize != (1 << cvt_in_log2(code))) return fail(DDS_ERR_DTYPE);
+        out->code[v] = code;
+        if (code == DDS_CVT_U8_LUT16 || code == DDS_CVT_U8_LUT32) {
+            if (!cv[v].lut) return fail(DDS_ERR_ARG, "a LUT conversion needs a table");
+            const int bytes = 256 << cvt_out_log2(code);
+            memcpy((char *)out->lut + off, cv[v].lut, (size_t)bytes); // copied now: the caller may free it on return
+            out->lut_off[v] = off;
+            off += bytes;
+        }
+    }
+    out->lut_bytes = off;
+    return DDS_OK;
+}
+
+// the argument checks the converting single-variable entries share
+static int convert_args(Var *v, const dds_convert_t *cvt, void *dst, const int64_t *dst_offsets, unsigned flags,
+                        ddsk_cvt_t *kc) {
+    if (int rc = make_cvt(&v, cvt, 1, false, kc)) return rc;
+    if (!(flags & DDS_DST_ON_DEVICE)) return fail(DDS_ERR_ARG, "converting batches deliver into device memory");
+    if ((uint64_t)dst % (uint64_t)(1 << cvt_out_log2(kc->code[0])) || (uint64_t)dst_offsets % 8u)
+        return fail(DDS_ERR_ARG, "destination not aligned to the output itemsize (or offsets to 8 bytes)");
+    return DDS_OK;
+}
+
+int dds_get_batch_convert(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                          int64_t fixed_count, int64_t nreq, void *dst, int64_t dst_capacity, int64_t *dst_offsets,
+                          unsigned flags, void *cuda_stream, const dds_convert_t *cvt, int64_t *total_bytes,
+                          int64_t *bad_index) {
+    clear_error();
+    if (bad_index) *bad_index = -1;
+    if (total_bytes) *total_bytes = 0;
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    Var *v = find_var(s, name);
+    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    ddsk_cvt_t kc;
+    if (int rc = convert_args(v, cvt, dst, dst_offsets, flags, &kc)) return rc;
+    return batch_impl(s, v, false, starts, counts, fixed_count, nreq, dst, dst_capacity, dst_offsets, flags, cuda_stream,
+                      total_bytes, bad_index, &kc);
 }
 
 int dds_get_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
@@ -1417,9 +1486,27 @@ int dds_get_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
                       total_bytes, bad_index);
 }
 
-int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids, int64_t nreq,
-                          void *const *dsts, const int64_t *dst_capacities, int64_t *const *dst_offsets, unsigned flags,
-                          void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+int dds_get_samples_convert(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, void *dst,
+                            int64_t dst_capacity, int64_t *dst_offsets, unsigned flags, void *cuda_stream,
+                            const dds_convert_t *cvt, int64_t *total_bytes, int64_t *bad_index) {
+    clear_error();
+    if (bad_index) *bad_index = -1;
+    if (total_bytes) *total_bytes = 0;
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    Var *v = find_var(s, name);
+    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    ddsk_cvt_t kc;
+    if (int rc = convert_args(v, cvt, dst, dst_offsets, flags, &kc)) return rc;
+    if (!v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
+    return batch_impl(s, v, true, sample_ids, nullptr, 0, nreq, dst, dst_capacity, dst_offsets, flags, cuda_stream,
+                      total_bytes, bad_index, &kc);
+}
+
+// The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,
+// or NULL for raw bytes)
+static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids, int64_t nreq,
+                      void *const *dsts, const int64_t *dst_capacities, int64_t *const *dst_offsets, unsigned flags,
+                      void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, const dds_convert_t *cvts) {
     clear_error();
     if (bad_index) *bad_index = -1;
     if (!s || !names || !dsts || !dst_capacities) return fail(DDS_ERR_ARG, "null argument");
@@ -1434,9 +1521,22 @@ int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, c
         if (!vv[v]) return fail(DDS_ERR_UNKNOWN_VAR, names[v] ? names[v] : "(null)");
         if (!vv[v]->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
         if (dst_capacities[v] < 0) return fail(DDS_ERR_ARG, "negative capacity");
-        cap_total += dst_capacities[v];
         key += vv[v]->name;
         key += '\n';
+    }
+    ddsk_cvt_t kc;
+    const ddsk_cvt_t *kcp = nullptr;
+    int64_t cap_src[DDSK_MAX_MULTI]; // the kernels check capacities in source bytes
+    if (cvts) {
+        if (int rc = make_cvt(vv, cvts, nvars, true, &kc)) return rc;
+        for (int v = 0; v < nvars; v++)
+            if ((uint64_t)dsts[v] % (uint64_t)(1 << cvt_out_log2(kc.code[v])) || (dst_offsets && (uint64_t)dst_offsets[v] % 8u))
+                return fail(DDS_ERR_ARG, "destination not aligned to the output itemsize (or offsets to 8 bytes)");
+        kcp = &kc;
+    }
+    for (int v = 0; v < nvars; v++) {
+        cap_src[v] = kcp ? cvt_cap_to_src(dst_capacities[v], kc.code[v]) : dst_capacities[v];
+        cap_total += cap_src[v];
     }
     const bool idx_dev = flags & DDS_IDX_ON_DEVICE, no_sync = flags & DDS_NO_SYNC;
     if (no_sync && !idx_dev) return fail(DDS_ERR_ARG, "async batches need device indices and a device destination");
@@ -1463,7 +1563,7 @@ int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, c
         d_ids = s->d_starts;
     }
     const bool ovl = no_sync && (flags & DDS_OVERLAP);
-    const bool uses_scratch = ddsk_var_uses_scratch(nreq * nvars, cap_total);
+    const bool uses_scratch = ddsk_var_uses_scratch(nreq * nvars, cap_total, kcp);
     if (uses_scratch) {
         if (int rc = renew_plan_tags(s)) return rc;
         if (int rc = ovl ? ensure_slots(s, nreq * nvars, cap_total) : ensure_scratch(s, nreq * nvars, cap_total)) return rc;
@@ -1482,18 +1582,20 @@ int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, c
         m.table[v] = vv[v]->d_tab;
         m.nsamples[v] = vv[v]->nsamples;
         m.dst[v] = dsts[v];
-        m.cap[v] = dst_capacities[v];
+        m.cap[v] = cap_src[v];
         m.offsets[v] = dst_offsets && dst_offsets[v] ? dst_offsets[v] : (stage_offs ? s->d_offs + (int64_t)v * (nreq + 1) : nullptr);
     }
     tag_launch(s, chain);
     const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
-    const int mrc = ddsk_gather_multi(&m, d_ids, nreq, &scr, kflags, st);
+    const int mrc = ddsk_gather_multi(&m, d_ids, nreq, &scr, kflags, kcp, st);
     s->scr.plan_tag = scr.plan_tag;
     if (mrc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
     s->pending_fixed_total = -1;
     s->pending_nreq = nreq * nvars;
-    s->pending_total_ptr = uses_scratch ? &scr.req_dst[nreq * nvars] : s->scr.total;
+    // (a converting launch writes its total in output bytes to the store's total word, whichever plan it used)
+    s->pending_total_ptr = (uses_scratch && !kcp) ? &scr.req_dst[nreq * nvars] : s->scr.total;
+    s->pending_cvt = DDSK_CVT_NONE;
     if (no_sync) {
         s->pending = true;
         s->pending_stream = st;
@@ -1510,6 +1612,26 @@ int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, c
     return rc;
 }
 
+int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids, int64_t nreq,
+                          void *const *dsts, const int64_t *dst_capacities, int64_t *const *dst_offsets, unsigned flags,
+                          void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    return multi_impl(s, nvars, names, sample_ids, nreq, dsts, dst_capacities, dst_offsets, flags, cuda_stream, total_bytes,
+                      bad_index, nullptr);
+}
+
+int dds_get_samples_multi_convert(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids,
+                                  int64_t nreq, void *const *dsts, const int64_t *dst_capacities,
+                                  int64_t *const *dst_offsets, unsigned flags, void *cuda_stream,
+                                  const dds_convert_t *cvts, int64_t *total_bytes, int64_t *bad_index) {
+    if (!cvts) {
+        clear_error();
+        if (bad_index) *bad_index = -1;
+        return fail(DDS_ERR_ARG, "null conversion");
+    }
+    return multi_impl(s, nvars, names, sample_ids, nreq, dsts, dst_capacities, dst_offsets, flags, cuda_stream, total_bytes,
+                      bad_index, cvts);
+}
+
 // completes a batch issued with DDS_NO_SYNC
 int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index) {
     if (!s) return fail(DDS_ERR_ARG, "null store");
@@ -1523,7 +1645,8 @@ int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index) {
     if (s->pending_fixed_total < 0 && s->pending_total_ptr)
         CU(cudaMemcpyAsync(&s->h_status[1], s->pending_total_ptr, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    if (total_bytes) *total_bytes = s->pending_fixed_total >= 0 ? s->pending_fixed_total : (int64_t)s->h_status[1];
+    if (total_bytes)
+        *total_bytes = s->pending_fixed_total >= 0 ? s->pending_fixed_total : cvt_to_out((int64_t)s->h_status[1], s->pending_cvt);
     return decode_status(s, st, s->h_status[0], bad_index);
 }
 

@@ -17,7 +17,7 @@ from libcpp cimport bool as cbool
 import numpy as np
 
 from ddstore_b200.comm import as_dds_comm
-from ddstore_b200.store import _Buf, _i64
+from ddstore_b200.store import _Buf, _conversion, _i64
 
 cdef extern from *:
     """
@@ -45,6 +45,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
         void get_device[T](string name, long start, long count, T* buffer) except +dds_translate_exception
         long get_batch[T](string name, const long* starts, const long* counts, long fixed_count, long nreq, T* dst,
                           long cap, long* offsets, cbool on_device, void* stream) except +dds_translate_exception
+        long get_batch_convert(string name, const long* starts, const long* counts, long fixed_count, long nreq,
+                               void* dst, long cap, int code, const void* lut, long* offsets, cbool idx_on_device,
+                               void* stream) except +dds_translate_exception
         void epoch_begin() except +dds_translate_exception
         void epoch_end() except +dds_translate_exception
         void free() except +dds_translate_exception
@@ -115,13 +118,20 @@ cdef class PyDDStore:
                 elif w == 4: self.c_ddstore.get[int](nm, start, count, <int*> p)
                 else: self.c_ddstore.get[long](nm, start, count, <long*> p)
 
-    def get_batch(self, str name, starts, counts=None, out=None, count=None, offsets=None, stream=None):
+    def get_batch(self, str name, starts, counts=None, out=None, count=None, offsets=None, stream=None, src_dtype=None,
+                  lut=None):
         """one kernel launch for len(starts) requests, packed in request order into `out`; see
-        ddstore_b200.store.PyDDStore.get_batch. `out` decides the element width checked against the variable."""
+        ddstore_b200.store.PyDDStore.get_batch. `out` decides the element width checked against the variable.
+        src_dtype / lut: deliver the rows converted to out.dtype (a CUDA tensor), as in ddstore_b200's get_batch."""
         if out is None:
             raise ValueError("get_batch needs an `out` buffer")
-        ob = _Buf(out, writable=True)
+        cv = None
+        if src_dtype is not None:
+            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut)
+        ob = _Buf(out, writable=True, half_ok=cv is not None)
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        if cv is not None:
+            return self._get_batch_convert(name, starts, counts, ob, count, offsets, stream, cv, lut_keep, bool(s_dev))
         if bool(s_dev) != bool(ob.on_device):
             raise ValueError("the Cython get_batch wants indices and out on the same side (both host or both device)")
         cdef size_t sp, cp = 0, op = 0, dp = ob.ptr
@@ -155,6 +165,37 @@ cdef class PyDDStore:
           else:
             total = self.c_ddstore.get_batch[long](nm, <const long*> sp, <const long*> cp, fixed, nreq, <long*> dp, cap, <long*> op, dev, <void*> st)
         del keep
+        return total
+
+    def _get_batch_convert(self, str name, starts, counts, ob, count, offsets, stream, cv, lut_keep, s_dev):
+        cdef size_t sp, cp = 0, op = 0, dp = ob.ptr, lp = cv.lut or 0
+        cdef long nreq
+        if s_dev:
+            nreq = starts.numel(); sp = starts.data_ptr()
+            if counts is not None: cp = counts.data_ptr()
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
+            ca = _i64(counts) if counts is not None else None
+            if ca is not None: cp = ca.ctypes.data
+            keep = (sa, ca)
+        if offsets is not None:
+            op = _Buf(offsets, writable=True).ptr
+        cdef long fixed = 1 if count is None else int(count)
+        cdef long cap = ob.nbytes
+        cdef size_t st = 0
+        if stream is not None:
+            st = int(stream) if int(stream) != 0 else 1
+        cdef string nm = name.encode()
+        cdef int code = cv.code
+        cdef cbool idx_dev = s_dev
+        cdef long total
+        if not ob.on_device:
+            raise ValueError("converting batches deliver into device memory")
+        with nogil:
+            total = self.c_ddstore.get_batch_convert(nm, <const long*> sp, <const long*> cp, fixed, nreq, <void*> dp, cap,
+                                                     code, <const void*> lp, <long*> op, idx_dev, <void*> st)
+        del keep, lut_keep
         return total
 
     def epoch_begin(self):

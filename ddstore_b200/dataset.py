@@ -19,7 +19,7 @@ from torch.utils.data import DataLoader, Dataset
 from torch.utils.data.distributed import DistributedSampler
 
 from .comm import as_dds_comm
-from .store import PyDDStore
+from .store import PyDDStore, _conversion
 
 
 def nsplit(a, n):
@@ -33,9 +33,13 @@ class DistDataset(Dataset):
 
     data: sequence of (tensor/ndarray, label) pairs -- every rank passes the same sequence (like the reference) and
     keeps only its block; or pass `local_only=True` when `data` already is this rank's block.
+    out_dtype / lut: batches (__getitems__, PrefetchLoader) deliver the samples converted to `out_dtype` inside the
+    gather (float32 -> bfloat16 / float16, float64 -> float32, uint8 -> bfloat16 / float16 / float32 through `lut`, 256
+    entries of out_dtype, default the plain value cast); the labels are never converted. The per-sample get() keeps
+    the stored dtype.
     """
 
-    def __init__(self, data, label, comm=None, ddstore_width=None, device=None, local_only=False):
+    def __init__(self, data, label, comm=None, ddstore_width=None, device=None, local_only=False, out_dtype=None, lut=None):
         super().__init__()
         self.label = label
         self.comm = as_dds_comm(comm)
@@ -69,6 +73,12 @@ class DistDataset(Dataset):
         self.sample_size = arr.shape[1]
         self.dtype = torch.from_numpy(arr[:0]).dtype
         self._np_dtype = arr.dtype
+        # batch dtype: the stored one, or out_dtype converted in the gather (src_dtype = what the gather converts from)
+        self.src_dtype = self.dtype if out_dtype is not None else None
+        self.out_dtype = out_dtype if out_dtype is not None else self.dtype
+        self.lut = lut
+        if self.src_dtype is not None:
+            _conversion(self.src_dtype, self.out_dtype, lut)  # an unsupported pair fails here, not at the first batch
         self.ddstore.add(f"{self.label}data", np.ascontiguousarray(arr))
         self.ddstore.add(f"{self.label}labels", np.ascontiguousarray(np.array(labels, dtype=np.int32).reshape(-1, 1)))
 
@@ -97,12 +107,12 @@ class DistDataset(Dataset):
     def __getitems__(self, indices):
         B = len(indices)
         idx = np.asarray(indices, dtype=np.int64)
-        vals = torch.empty((B, self.sample_size), dtype=self.dtype, device=self.device)
+        vals = torch.empty((B, self.sample_size), dtype=self.out_dtype, device=self.device)
         labs = torch.empty((B, 1), dtype=torch.int32, device=self.device)
         # on torch's CURRENT stream: the output tensors come from its caching allocator, whose blocks may still be in use
         # by work queued there, and the index copy + the gather are then ordered with everything the caller queued before
         st = torch.cuda.current_stream(self.device).cuda_stream
-        self.ddstore.get_batch(f"{self.label}data", idx, out=vals, count=1, stream=st)
+        self.ddstore.get_batch(f"{self.label}data", idx, out=vals, count=1, stream=st, src_dtype=self.src_dtype, lut=self.lut)
         self.ddstore.get_batch(f"{self.label}labels", idx, out=labs, count=1, stream=st)
         return vals.view((B,) + self.sample_shape), labs.view(B)
 
@@ -127,8 +137,11 @@ class RaggedDataset(Dataset):
     reference's get(name, arr, start) with count = arr.shape[0] implies (src/pyddstore.pyx:84-87).
     The (start, count) tables of ALL samples are kept on the device, so a batch needs only the sample ids."""
 
-    def __init__(self, local_arrays, local_counts, comm=None, device=None):
-        """local_arrays: {name: 2-D ndarray of this rank's rows}; local_counts: {name: int64[n_local_samples]}"""
+    def __init__(self, local_arrays, local_counts, comm=None, device=None, out_dtypes=None, luts=None):
+        """local_arrays: {name: 2-D ndarray of this rank's rows}; local_counts: {name: int64[n_local_samples]}
+        out_dtypes / luts: {name: dtype} / {name: 256-entry table}: those variables' batches are delivered converted in
+        the gather (see DistDataset); their row offsets count rows as always."""
+        out_dtypes, luts = dict(out_dtypes or {}), dict(luts or {})
         super().__init__()
         self.comm = as_dds_comm(comm)
         self.rank, self.comm_size = self.comm.Get_rank(), self.comm.Get_size()
@@ -160,6 +173,15 @@ class RaggedDataset(Dataset):
             self.row_bytes[name] = arr.dtype.itemsize * int(np.prod(arr.shape[1:], dtype=np.int64))
             self.dtypes[name] = torch.from_numpy(arr[:0]).dtype
             self.widths[name] = arr.shape[1:]
+        # what the batches deliver: out_dtypes[name] converted from the stored dtype, else the stored bytes
+        self.src_dtypes = {n: (self.dtypes[n] if n in out_dtypes else None) for n in self.names}
+        self.out_dtypes = {n: out_dtypes.get(n, self.dtypes[n]) for n in self.names}
+        self.luts = {n: luts.get(n) for n in self.names}
+        self.out_row_bytes = {}
+        for n in self.names:
+            if self.src_dtypes[n] is not None:
+                _conversion(self.src_dtypes[n], self.out_dtypes[n], self.luts[n])  # an unsupported pair fails here
+            self.out_row_bytes[n] = self.row_bytes[n] // self.dtypes[n].itemsize * self.out_dtypes[n].itemsize
         self.total_ns = int(len(self.counts[self.names[0]]))
 
     def __len__(self):
@@ -179,16 +201,19 @@ class RaggedDataset(Dataset):
         for name in self.names:
             r = int(self.counts[name][ids].sum())  # host-side size of the packed result (sizes only, no data)
             rows.append(r)
-            bufs.append(torch.empty((max(r, 1),) + tuple(self.widths[name]), dtype=self.dtypes[name], device=self.device))
+            bufs.append(torch.empty((max(r, 1),) + tuple(self.widths[name]), dtype=self.out_dtypes[name], device=self.device))
             offs.append(torch.empty(len(ids) + 1, dtype=torch.int64, device=self.device))
+        conv = any(d is not None for d in self.src_dtypes.values())
         if len(self.names) <= 4:
             # every variable of the batch in ONE launch (dds_get_samples_multi)
-            self.ddstore.get_samples_multi(self.names, ids, bufs, offsets=offs, stream=st)
+            kw = dict(src_dtypes=[self.src_dtypes[n] for n in self.names], luts=[self.luts[n] for n in self.names]) if conv else {}
+            self.ddstore.get_samples_multi(self.names, ids, bufs, offsets=offs, stream=st, **kw)
         else:
             for name, buf, off in zip(self.names, bufs, offs):
-                self.ddstore.get_samples(name, ids, out=buf, offsets=off, stream=st)
+                self.ddstore.get_samples(name, ids, out=buf, offsets=off, stream=st, src_dtype=self.src_dtypes[name],
+                                         lut=self.luts[name])
         for name, buf, off, r in zip(self.names, bufs, offs, rows):
-            out[name] = (buf[:r], off // self.row_bytes[name])
+            out[name] = (buf[:r], off // self.out_row_bytes[name])
         return out
 
     collate = staticmethod(lambda batch: batch)
@@ -225,7 +250,7 @@ class PrefetchLoader:
         dev = dataset.device
         self.stream = torch.cuda.Stream(device=dev)
         rows = batch_size * self.group
-        self.bufs = [(torch.empty((rows, dataset.sample_size), dtype=dataset.dtype, device=dev),
+        self.bufs = [(torch.empty((rows, dataset.sample_size), dtype=dataset.out_dtype, device=dev),
                       torch.empty((rows, 1), dtype=torch.int32, device=dev),
                       torch.empty(rows, dtype=torch.int64, device=dev)) for _ in range(self.depth)]
         self.events = [torch.cuda.Event() for _ in range(self.depth)]
@@ -260,7 +285,7 @@ class PrefetchLoader:
             st = self.stream.cuda_stream
             # independent batches into alternating buffer sets: let consecutive launches overlap (DDS_OVERLAP)
             self.ds.ddstore.get_batch(f"{self.ds.label}data", ids, out=vals[:n], count=1, stream=st, wait=False,
-                                      overlap=True)
+                                      overlap=True, src_dtype=self.ds.src_dtype, lut=self.ds.lut)
             self.ds.ddstore.get_batch(f"{self.ds.label}labels", ids, out=labs[:n], count=1, stream=st, wait=False,
                                       overlap=True)
             self.events[slot].record(self.stream)
@@ -345,16 +370,21 @@ class RaggedPrefetchLoader:
         ds = self.ds
         ids = np.asarray(idx, dtype=np.int64)
         rows = [int(ds.counts[name][ids].sum()) for name in ds.names]  # host-side sizes only
-        need = [max(r, 1) * ds.row_bytes[name] for r, name in zip(rows, ds.names)]
+        need = [max(r, 1) * ds.out_row_bytes[name] for r, name in zip(rows, ds.names)]
         if self.bufs[slot] is None or any(b.numel() < n for b, n in zip(self.bufs[slot], need)):
             # (grown rarely; a fresh buffer cannot still be in use by an earlier fetch)
-            self.bufs[slot] = [torch.empty(int(n * 1.25) + 64, dtype=torch.uint8, device=ds.device) for n in need]
+            # (whole 8-byte words, so a converting fetch can view them in its output dtype)
+            self.bufs[slot] = [torch.empty((int(n * 1.25) + 64 + 7) // 8 * 8, dtype=torch.uint8, device=ds.device) for n in need]
         keep = torch.from_numpy(ids).pin_memory()
         n = len(ids)
         with torch.cuda.stream(self.stream):
             self.d_ids[slot][:n].copy_(keep, non_blocking=True)
-            ds.ddstore.get_samples_multi(ds.names, self.d_ids[slot][:n], self.bufs[slot], offsets=[o[:n + 1] for o in self.offs[slot]],
-                                         stream=self.stream.cuda_stream, wait=False, overlap=True)
+            kw = {}
+            if any(d is not None for d in ds.src_dtypes.values()):  # (the uint8 buffers are viewed as out_dtypes)
+                kw = dict(src_dtypes=[ds.src_dtypes[m] for m in ds.names], luts=[ds.luts[m] for m in ds.names])
+            bufs = [b.view(ds.out_dtypes[m]) if kw else b for b, m in zip(self.bufs[slot], ds.names)]
+            ds.ddstore.get_samples_multi(ds.names, self.d_ids[slot][:n], bufs, offsets=[o[:n + 1] for o in self.offs[slot]],
+                                         stream=self.stream.cuda_stream, wait=False, overlap=True, **kw)
             self.events[slot].record(self.stream)
         return n, rows, keep
 
@@ -376,9 +406,9 @@ class RaggedPrefetchLoader:
         consumer.wait_event(self.events[slot])
         ds, out = self.ds, {}
         for k, name in enumerate(ds.names):
-            nb = rows[k] * ds.row_bytes[name]
-            buf = self.bufs[slot][k][:nb].view(ds.dtypes[name]).view((rows[k],) + tuple(ds.widths[name]))
-            out[name] = (buf, self.offs[slot][k][:n + 1] // ds.row_bytes[name])
+            nb = rows[k] * ds.out_row_bytes[name]
+            buf = self.bufs[slot][k][:nb].view(ds.out_dtypes[name]).view((rows[k],) + tuple(ds.widths[name]))
+            out[name] = (buf, self.offs[slot][k][:n + 1] // ds.out_row_bytes[name])
         return out
 
 

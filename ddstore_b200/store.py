@@ -16,13 +16,63 @@ from .comm import as_dds_comm
 _NP_OK = {np.dtype(np.int32), np.dtype(np.int64), np.dtype(np.uint8), np.dtype(np.float32),
           np.dtype(np.float64), np.dtype(np.bool_)}
 _TORCH_OK = {"torch.int32", "torch.int64", "torch.uint8", "torch.float32", "torch.float64", "torch.bool"}
+# output dtypes only a converting batch delivers (the store keeps no 2-byte floats)
+_TORCH_HALF = {"torch.bfloat16", "torch.float16"}
+
+# converting batches: (source dtype, output dtype) -> DDS_CVT_* code
+_CVT_CODES = {("float32", "bfloat16"): _capi.CVT_F32_BF16, ("float32", "float16"): _capi.CVT_F32_F16,
+              ("float64", "float32"): _capi.CVT_F64_F32, ("uint8", "bfloat16"): _capi.CVT_U8_LUT16,
+              ("uint8", "float16"): _capi.CVT_U8_LUT16, ("uint8", "float32"): _capi.CVT_U8_LUT32}
+_default_luts = {}  # output dtype name -> host table of the plain value cast, torch.arange(256).to(dtype)
+
+
+def _dtype_name(dt):
+    """'float32', 'bfloat16', ... of a torch dtype, a NumPy dtype or a name"""
+    s = str(dt)
+    if s.startswith("torch."):
+        return s[len("torch."):]
+    if s in ("bfloat16", "float16"):
+        return s
+    return str(np.dtype(dt))
+
+
+def _conversion(src_dtype, out_dtype, lut):
+    """-> (dds_convert_t, keepalive) of a converting batch from `src_dtype` rows into an `out_dtype` buffer. A uint8 source
+    takes `lut` (256 entries of the output dtype; default: the plain value cast torch.arange(256).to(out_dtype))."""
+    import torch
+    key = (_dtype_name(src_dtype), _dtype_name(out_dtype))
+    code = _CVT_CODES.get(key)
+    if code is None:
+        raise ValueError(f"unsupported conversion {key[0]} -> {key[1]}")
+    if code not in (_capi.CVT_U8_LUT16, _capi.CVT_U8_LUT32):
+        if lut is not None:
+            raise ValueError("a table (lut) applies to uint8 sources only")
+        return _capi.Convert(code, None), None
+    tdt = getattr(torch, key[1])
+    if lut is None:
+        host = _default_luts.get(key[1])
+        if host is None:
+            host = _default_luts[key[1]] = _lut_bits(torch.arange(256).to(tdt))
+    else:
+        t = torch.as_tensor(lut)
+        if t.dtype != tdt or t.numel() != 256:
+            raise ValueError(f"lut must hold 256 entries of {tdt}")
+        host = _lut_bits(t)
+    return _capi.Convert(code, host.ctypes.data), host
+
+
+def _lut_bits(t):
+    """a 256-entry torch table as a host int16 / int32 array of its bits"""
+    import torch
+    t = t.detach().reshape(-1).cpu().contiguous()
+    return t.view(torch.int16 if t.element_size() == 2 else torch.int32).numpy().copy()
 
 
 class _Buf:
     """pointer / shape / itemsize / residency of an ndarray, a CUDA tensor or a CAI object"""
 
-    def __init__(self, arr, writable=False):  # `writable` documents intent at the call sites; nothing is copied
-        self.keep = arr
+    def __init__(self, arr, writable=False, half_ok=False):  # `writable` documents intent at the call sites; nothing is
+        self.keep = arr                                          # copied. half_ok: bf16/f16 tensors (converting batches)
         if isinstance(arr, np.ndarray):
             assert arr.flags.c_contiguous  # src/pyddstore.pyx:66,85,116
             if arr.dtype not in _NP_OK:
@@ -31,7 +81,7 @@ class _Buf:
             self.shape, self.itemsize, self.size = arr.shape, arr.dtype.itemsize, arr.size
         elif hasattr(arr, "data_ptr") and hasattr(arr, "element_size"):  # torch.Tensor
             assert arr.is_contiguous()
-            if str(arr.dtype) not in _TORCH_OK:
+            if str(arr.dtype) not in _TORCH_OK and not (half_ok and str(arr.dtype) in _TORCH_HALF):
                 raise NotImplementedError
             self.ptr, self.on_device = arr.data_ptr(), 1 if arr.is_cuda else 0
             self.shape, self.itemsize, self.size = tuple(arr.shape), arr.element_size(), arr.numel()
@@ -139,7 +189,7 @@ class PyDDStore:
 
     # ---------------------------------------------------------------- the batched hot path
     def get_batch(self, name, starts, counts=None, out=None, count=None, offsets=None, stream=None, wait=True,
-                  overlap=False):
+                  overlap=False, src_dtype=None, lut=None):
         """Fetch len(starts) requests in ONE kernel launch, packed back to back in request order.
 
         starts/counts: int64 index arrays (host ndarray/list, or CUDA int64 tensors). counts=None means
@@ -158,13 +208,21 @@ class PyDDStore:
         e.g. produced by a synchronous copy. When they were produced or are consumed on torch's current stream, pass
         stream=torch.cuda.current_stream().cuda_stream.
         Raises the reference's ValueError for the first invalid request (requests before it are delivered).
+        src_dtype (with a CUDA `out`): deliver the rows converted from `src_dtype` (the variable's element type) to
+        out.dtype inside the gather: float32 -> bfloat16 / float16, float64 -> float32, uint8 -> bfloat16 / float16 /
+        float32 through `lut` (256 entries of out.dtype; default torch.arange(256).to(out.dtype)). The capacity, the
+        offsets and the returned size are then in bytes of `out`.
         """
-        itemsize = self._itemsize.get(name)
-        if itemsize is None:
-            itemsize = self._itemsize[name] = self.query(name)["itemsize"]
         if out is None:
             raise ValueError("get_batch needs an `out` buffer (like get(), it never allocates)")
-        ob = _Buf(out, writable=True)
+        cv = lut_keep = None
+        if src_dtype is not None:
+            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut)
+        else:
+            itemsize = self._itemsize.get(name)
+            if itemsize is None:
+                itemsize = self._itemsize[name] = self.query(name)["itemsize"]
+        ob = _Buf(out, writable=True, half_ok=cv is not None)
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
         if s_dev:
             nreq = starts.numel()
@@ -188,10 +246,15 @@ class PyDDStore:
                 raise ValueError("offsets must be int64[len(starts)+1] with the same residency as out")
             op = fb.ptr
         total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_get_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
-                                   itemsize, ob.ptr, ob.nbytes, op, flags,
-                                   self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep
+        if cv is None:
+            rc = self._L.dds_get_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
+                                       itemsize, ob.ptr, ob.nbytes, op, flags,
+                                       self._stream_arg(stream), C.byref(total), C.byref(bad))
+        else:
+            rc = self._L.dds_get_batch_convert(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
+                                               ob.ptr, ob.nbytes, op, flags, self._stream_arg(stream), C.byref(cv),
+                                               C.byref(total), C.byref(bad))
+        del keep, lut_keep
         self.last_bad_index = bad.value
         _capi.raise_for(rc)
         return total.value
@@ -233,13 +296,18 @@ class PyDDStore:
         _capi.raise_for(self._L.dds_set_sample_index(self._h, name.encode(), sp, cp, n, 1 if dev else 0))
         del keep
 
-    def get_samples(self, name, sample_ids, out, offsets=None, stream=None, wait=True, overlap=False):
+    def get_samples(self, name, sample_ids, out, offsets=None, stream=None, wait=True, overlap=False, src_dtype=None,
+                    lut=None):
         """get_batch by SAMPLE ID: the id -> (start, count) lookup runs inside the launch, against the index
-        registered with set_sample_index. Same packing / offsets / error behaviour as get_batch."""
-        itemsize = self._itemsize.get(name)
-        if itemsize is None:
-            itemsize = self._itemsize[name] = self.query(name)["itemsize"]
-        ob = _Buf(out, writable=True)
+        registered with set_sample_index. Same packing / offsets / error behaviour, and conversions, as get_batch."""
+        cv = lut_keep = None
+        if src_dtype is not None:
+            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut)
+        else:
+            itemsize = self._itemsize.get(name)
+            if itemsize is None:
+                itemsize = self._itemsize[name] = self.query(name)["itemsize"]
+        ob = _Buf(out, writable=True, half_ok=cv is not None)
         s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
         if s_dev:
             nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
@@ -256,19 +324,35 @@ class PyDDStore:
                 raise ValueError("offsets must be int64[len(sample_ids)+1] with the same residency as out")
             op = fb.ptr
         total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_get_samples(self._h, name.encode(), sp, nreq, itemsize, ob.ptr, ob.nbytes, op, flags,
-                                     self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep
+        if cv is None:
+            rc = self._L.dds_get_samples(self._h, name.encode(), sp, nreq, itemsize, ob.ptr, ob.nbytes, op, flags,
+                                         self._stream_arg(stream), C.byref(total), C.byref(bad))
+        else:
+            rc = self._L.dds_get_samples_convert(self._h, name.encode(), sp, nreq, ob.ptr, ob.nbytes, op, flags,
+                                                 self._stream_arg(stream), C.byref(cv), C.byref(total), C.byref(bad))
+        del keep, lut_keep
         self.last_bad_index = bad.value
         _capi.raise_for(rc)
         return total.value
 
-    def get_samples_multi(self, names, sample_ids, outs, offsets=None, stream=None, wait=True, overlap=False):
+    def get_samples_multi(self, names, sample_ids, outs, offsets=None, stream=None, wait=True, overlap=False,
+                          src_dtypes=None, luts=None):
         """The rows of the same samples in several variables (<= 4, each with a sample index) in ONE launch:
         outs[v] (CUDA tensors) receive variable names[v]'s packed rows, offsets[v] (optional int64 CUDA tensors of
-        len(ids)+1) the per-sample byte offsets. Returns the list of packed sizes (None when wait=False)."""
+        len(ids)+1) the per-sample byte offsets. Returns the list of packed sizes (None when wait=False).
+        src_dtypes[v] / luts[v]: variable v delivered converted to outs[v].dtype, as in get_batch (None: raw bytes);
+        its offsets and size are then in bytes of outs[v]."""
         nv = len(names)
-        obs = [_Buf(o, writable=True) for o in outs]
+        cvs = None
+        if src_dtypes is not None:
+            luts = [None] * nv if luts is None else list(luts)
+            if len(src_dtypes) != nv or len(luts) != nv:
+                raise ValueError("src_dtypes / luts need one entry per variable")
+            pairs = [(_capi.Convert(_capi.CVT_NONE, None), None) if sd is None else _conversion(sd, getattr(o, "dtype", None), lt)
+                     for sd, o, lt in zip(src_dtypes, outs, luts)]
+            cvs = (_capi.Convert * nv)(*[c for c, _ in pairs])
+            lut_keep = [k for _, k in pairs]
+        obs = [_Buf(o, writable=True, half_ok=cvs is not None and src_dtypes[v] is not None) for v, o in enumerate(outs)]
         if not all(o.on_device for o in obs):
             raise ValueError("get_samples_multi delivers into device buffers")
         s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
@@ -289,8 +373,13 @@ class PyDDStore:
             c_offs = (C.c_void_p * nv)(*[f.ptr for f in fbs])
         totals = (C.c_int64 * nv)()
         bad = C.c_int64(-1)
-        rc = self._L.dds_get_samples_multi(self._h, nv, c_names, sp, nreq, c_dsts, c_caps, c_offs, flags,
-                                           self._stream_arg(stream), totals, C.byref(bad))
+        if cvs is None:
+            rc = self._L.dds_get_samples_multi(self._h, nv, c_names, sp, nreq, c_dsts, c_caps, c_offs, flags,
+                                               self._stream_arg(stream), totals, C.byref(bad))
+        else:
+            rc = self._L.dds_get_samples_multi_convert(self._h, nv, c_names, sp, nreq, c_dsts, c_caps, c_offs, flags,
+                                                       self._stream_arg(stream), cvs, totals, C.byref(bad))
+            del lut_keep
         del keep
         self.last_bad_index = bad.value
         _capi.raise_for(rc)

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define DDS_VERSION 100
+#define DDS_VERSION 110 /* 110: converting batches (dds_get_batch_convert & co.) */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -178,6 +178,45 @@ int dds_get_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
 int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids, int64_t nreq,
                           void *const *dsts, const int64_t *dst_capacities, int64_t *const *dst_offsets, unsigned flags,
                           void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+
+/* ---- converting batches: rows delivered in the training dtype, converted inside the gather ----------------------
+ * The store only knows a variable's itemsize; the code names the source type. Element rules:
+ *   DDS_CVT_F32_BF16  4 -> 2 bytes  round to nearest even (cvt.rn.bf16.f32)
+ *   DDS_CVT_F32_F16   4 -> 2 bytes  round to nearest even, overflow to +-inf, f16 subnormals kept (cvt.rn.f16.f32)
+ *   DDS_CVT_F64_F32   8 -> 4 bytes  cvt.rn.f32.f64
+ *   DDS_CVT_U8_LUT16  1 -> 2 bytes  out = lut[in], 256 two-byte entries (bf16 or f16 bits)
+ *   DDS_CVT_U8_LUT32  1 -> 4 bytes  out = lut[in], 256 four-byte entries (f32 bits)
+ * NaN inputs of the float rules give the quiet NaN of cvt.rn, which is what torch's CUDA .to(dtype) gives. A table makes
+ * a uint8 normalisation bit-exact with whatever expression built it. `lut` is a host pointer, copied when the call is
+ * made (the caller may free it on return; every queued batch keeps its own tables).
+ * Request i is located, validated and ordered exactly as in the raw entry, then written converted: it sits at output
+ * byte sum_{j<i} count_j * disp * out_itemsize. The capacity, dst_offsets and the reported totals are all in OUTPUT
+ * bytes, and the error rules are those of dds_get_batch with sizes in output bytes. The entries take the raw entries'
+ * arguments and flags minus `itemsize`, and require DDS_DST_ON_DEVICE (host indices are fine). Argument errors: the
+ * variable's itemsize is not the code's source itemsize -> DDS_ERR_DTYPE; an unknown code, a LUT code without a table,
+ * a host destination, or dst / dst_offsets not aligned to the output itemsize / 8 bytes -> DDS_ERR_ARG. */
+#define DDS_CVT_NONE 0 /* raw bytes: valid only for a variable of dds_get_samples_multi_convert */
+#define DDS_CVT_F32_BF16 1
+#define DDS_CVT_F32_F16 2
+#define DDS_CVT_F64_F32 3
+#define DDS_CVT_U8_LUT16 4
+#define DDS_CVT_U8_LUT32 5
+typedef struct {
+    int32_t code;    /* DDS_CVT_* */
+    const void *lut; /* host pointer to 256 table entries (LUT codes only) */
+} dds_convert_t;
+int dds_get_batch_convert(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                          int64_t fixed_count, int64_t nreq, void *dst, int64_t dst_capacity, int64_t *dst_offsets,
+                          unsigned flags, void *cuda_stream, const dds_convert_t *cvt, int64_t *total_bytes,
+                          int64_t *bad_index);
+int dds_get_samples_convert(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, void *dst,
+                            int64_t dst_capacity, int64_t *dst_offsets, unsigned flags, void *cuda_stream,
+                            const dds_convert_t *cvt, int64_t *total_bytes, int64_t *bad_index);
+/* cvts[v]: variable v's conversion; DDS_CVT_NONE delivers that variable's bytes unchanged in the same launch. */
+int dds_get_samples_multi_convert(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids,
+                                  int64_t nreq, void *const *dsts, const int64_t *dst_capacities,
+                                  int64_t *const *dst_offsets, unsigned flags, void *cuda_stream,
+                                  const dds_convert_t *cvts, int64_t *total_bytes, int64_t *bad_index);
 
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite

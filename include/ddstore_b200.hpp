@@ -99,6 +99,20 @@ class DDStore {
                             &bad));
         return (long)total;
     }
+    // The same batch delivered converted (dds_get_batch_convert): `code` is a DDS_CVT_* code, `lut` a host table of 256
+    // entries for the LUT codes (copied by the call). dst / dst_offsets are device memory; the capacity, the offsets and
+    // the result are in OUTPUT bytes. idx_on_device: starts / counts are device pointers.
+    long get_batch_convert(std::string name, const long *starts, const long *counts, long fixed_count, long nreq,
+                           void *dst, long dst_capacity_bytes, int code, const void *lut = nullptr,
+                           long *dst_offsets = nullptr, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const dds_convert_t cvt = {code, lut};
+        const unsigned flags = DDS_DST_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_get_batch_convert(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts, fixed_count,
+                                    nreq, dst, dst_capacity_bytes, (int64_t *)dst_offsets, flags, cuda_stream, &cvt,
+                                    &total, &bad));
+        return (long)total;
+    }
     // device-pointer variants of add/get for callers that already hold the data in HBM
     template <typename T>
     void add_device(std::string name, const T *dev_buffer, long nrows, int disp) {
