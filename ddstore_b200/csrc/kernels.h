@@ -40,7 +40,8 @@ typedef struct ddsk_var {
 /* scratch a store owns for the batched path (all device memory) */
 typedef struct ddsk_scratch {
     unsigned long long *status; /* 1 word, sticky (kernels only atomicMin into it) */
-    int64_t *total;             /* 1 word: packed total of the last variable-count launch planned in shared memory */
+    int64_t *total;             /* 1 word: packed total of the last variable-count launch planned in shared memory (and of
+                                   a converting multi-array launch); an overlap launch gets the word of its slot */
     unsigned int *counters;     /* 2 words: [0] segment ticket, [1] finished warps -- self-resetting */
     unsigned int *ovl;          /* 24 words of the overlap protocol, one of each kind per slot (sequence number & 3):
                                    finished-warp counters, done words, segment tickets, lookup tiles done, scan tiles

@@ -391,6 +391,13 @@ ddsk_scratch_t scratch_view(dds_store *s, bool slot) {
     return v;
 }
 
+// The device word an overlap launch reports its packed total in, one per slot (sequence number & 3), behind the plan
+// words. The store's single total word cannot serve an overlapped run: a launch planned in shared memory writes it
+// at its start, a converting multi-array launch at the end of its walk, and launch q may start before launch q-1 has
+// retired, so q-1 could overwrite q's total. Slot q & 3 is next written by launch q+4, which writes nothing before
+// launch q+2 -- and so q -- has retired.
+int64_t *ovl_total_word(dds_store *s) { return (int64_t *)(s->scr.counters + 48) + (s->scr.ovl_seq & 3u); }
+
 int ensure_offs(dds_store *s, int64_t n) {
     if (n <= s->offs_cap) return DDS_OK;
     int64_t cap = std::max<int64_t>(4096, s->offs_cap);
@@ -837,7 +844,8 @@ dds_store_t *dds_create(dds_comm_t *comm, int device, int method) {
     bool ok = cudaSetDevice(device) == cudaSuccess &&
               cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) == cudaSuccess &&
               cudaMalloc((void **)&s->scr.status, 16) == cudaSuccess && // [0] sticky status, [1] packed total
-              cudaMalloc((void **)&s->scr.counters, 256) == cudaSuccess && // 2 ticket words (+pad), 24 protocol words, 4 plan words
+              cudaMalloc((void **)&s->scr.counters, 256) == cudaSuccess && // 2 ticket words (+pad), 24 protocol words, 8 plan
+                                                                           // words, 4 total words (ovl_total_word)
               cudaMemset(s->scr.counters, 0, 256) == cudaSuccess &&
               cudaMemset(s->scr.status, 0xFF, 8) == cudaSuccess &&
               cudaHostAlloc((void **)&s->h_status, 32, cudaHostAllocMapped) == cudaSuccess &&
@@ -1293,6 +1301,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     tag_launch(s, chain);
     const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
+    if (ovl) scr.total = ovl_total_word(s);
     int krc;
     if (fixed) {
         krc = ddsk_gather_fixed(&v->kv, d_starts, fixed_count, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, st);
@@ -1309,7 +1318,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
         }
         krc = ddsk_gather_var(&v->kv, &ix, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, st);
         s->scr.plan_tag = scr.plan_tag;
-        s->pending_total_ptr = uses_scratch ? &scr.req_dst[nreq] : s->scr.total;
+        s->pending_total_ptr = uses_scratch ? &scr.req_dst[nreq] : scr.total;
     }
     if (krc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
 
@@ -1588,13 +1597,14 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
     tag_launch(s, chain);
     const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
+    if (ovl) scr.total = ovl_total_word(s);
     const int mrc = ddsk_gather_multi(&m, d_ids, nreq, &scr, kflags, kcp, st);
     s->scr.plan_tag = scr.plan_tag;
     if (mrc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
     s->pending_fixed_total = -1;
     s->pending_nreq = nreq * nvars;
-    // (a converting launch writes its total in output bytes to the store's total word, whichever plan it used)
-    s->pending_total_ptr = (uses_scratch && !kcp) ? &scr.req_dst[nreq * nvars] : s->scr.total;
+    // (a converting launch writes its total in output bytes to the total word, whichever plan it used)
+    s->pending_total_ptr = (uses_scratch && !kcp) ? &scr.req_dst[nreq * nvars] : scr.total;
     s->pending_cvt = DDSK_CVT_NONE;
     if (no_sync) {
         s->pending = true;

@@ -30,6 +30,35 @@ def f64_to_f32_bits(bits):
     return np.asarray(bits, dtype=np.uint64).view(np.float64).astype(np.float32).view(np.uint32)
 
 
+# float32 rounding edges for bf16 and f16: ties both ways, overflow, subnormals, -0, inf, NaN
+F32_EDGE_BITS = (0x3F808000, 0x3F818000, 0x3F80FFFF, 0x7F7FFFFF, 0x477FF000, 0x477FEFFF, 0x33800000, 0x33000000,
+                 0x33000001, 0x387FC000, 0x80000000, 0x00000001, 0x7F800000, 0xFF800000, 0x7FC00000, 0x7F800001,
+                 0xFF7FFFFF, 0x00800000)
+
+
+def f64_edge_bits():
+    """float64 bit patterns at the edges of the f64 -> f32 rounding (round to nearest even), each with its sign flipped
+    too: ties at the f32 half-ulp with an even and an odd last kept bit, one f64 ulp either side of them; the largest
+    value that rounds to FLT_MAX and the smallest that rounds to inf; results in the f32 subnormal range, the smallest
+    subnormal's half (a tie to 0) and 1.5 of it (a tie to 2 units), the largest subnormal's tie into the normal range;
+    f64 subnormals, 0, inf; NaNs whose payload lies only in the 29 bits the cast drops (quiet NaN, not inf)"""
+    pos = [0x3FF0000010000000, 0x3FF0000030000000,                          # 1 + 2^-24 (down to even), 1 + 3*2^-24 (up)
+           0x3FF000000FFFFFFF, 0x3FF0000010000001, 0x3FF000002FFFFFFF, 0x3FF0000030000001,
+           0x4123456790000000, 0x4123456770000000,                          # ties in another binade, even / odd kept bit
+           0x47EFFFFFE0000000, 0x47EFFFFFEFFFFFFF,                          # FLT_MAX, the largest that rounds to it
+           0x47EFFFFFF0000000, 0x47F0000000000000,                          # the smallest that rounds to inf, 2^128
+           0x3810000000000000, 0x380FFFFFC0000000,                          # FLT_MIN, the largest f32 subnormal,
+           0x380FFFFFE0000000, 0x380FFFFFDFFFFFFF,                          # its tie up to FLT_MIN, just below it
+           0x37D0000000000000, 0x36A0000000000000, 0x36A8000000000000,      # 2^-130, 2^-149, 1.5 * 2^-149
+           0x3690000000000000, 0x3690000000000001, 0x368FFFFFFFFFFFFF,      # 2^-150 (tie to 0) and either side
+           0x36B4000000000000, 0x36B2000000000000,                          # 2.5 units (tie to 2), 2.25 units
+           0x0000000000000001, 0x000FFFFFFFFFFFFF, 0x0000000000000000,      # f64 subnormals, 0
+           0x7FF0000000000000, 0x7FF0000000000001, 0x7FF000001FFFFFFF,      # inf, NaNs with low payload only
+           0x7FF0000010000000, 0x7FF8000000000000]
+    pos = np.array(pos, np.uint64)
+    return np.concatenate([pos, pos | np.uint64(1 << 63)])
+
+
 def convert_bytes(src, code, lut=None):
     """packed source bytes (uint8, whole elements) -> packed output bytes of conversion `code`"""
     src = np.ascontiguousarray(src, dtype=np.uint8)

@@ -59,6 +59,29 @@ def test_f64_rule_matches_torch_cpu_cast():
     assert np.array_equal(co.f64_to_f32_bits(bits), exp)
 
 
+def test_f64_edge_patterns_match_torch_cpu_cast():
+    """the f64 -> f32 rounding edges the converting sweep stores in its float64 variables: the oracle's rule is torch's
+    CPU cast on every one, and the edges land where their names say"""
+    bits = co.f64_edge_bits()
+    f = bits.view(np.float64)
+    got = co.f64_to_f32_bits(bits)
+    nan = np.isnan(f)
+    exp = torch.from_numpy(f.copy()).to(torch.float32).numpy().view(np.uint32)
+    bad = np.flatnonzero(~nan & (got != exp))
+    assert bad.size == 0, f"{bits[bad[0]]:#018x}: oracle {got[bad[0]]:#010x}, torch {exp[bad[0]]:#010x}"
+    # NaN stays NaN, also when its payload lies only in the 29 bits the cast drops (a truncation would give inf)
+    assert nan.sum() == 8 and (np.isnan(got[nan].view(np.float32))).all() and (np.isnan(exp[nan].view(np.float32))).all()
+    want = {0x3FF0000010000000: 0x3F800000, 0x3FF0000030000000: 0x3F800002, 0x3FF000000FFFFFFF: 0x3F800000,
+            0x3FF0000010000001: 0x3F800001, 0x4123456790000000: 0x491A2B3C, 0x4123456770000000: 0x491A2B3C,
+            0x47EFFFFFEFFFFFFF: 0x7F7FFFFF, 0x47EFFFFFF0000000: 0x7F800000, 0x380FFFFFC0000000: 0x007FFFFF,
+            0x380FFFFFE0000000: 0x00800000, 0x380FFFFFDFFFFFFF: 0x007FFFFF, 0x36A0000000000000: 0x00000001, 0x36A8000000000000: 0x00000002,
+            0x3690000000000000: 0x00000000, 0x3690000000000001: 0x00000001, 0x36B4000000000000: 0x00000002,
+            0x0000000000000001: 0x00000000, 0x800FFFFFFFFFFFFF: 0x80000000, 0xB690000000000000: 0x80000000,
+            0xFFF0000000000000: 0xFF800000}
+    lut = dict(zip(bits.tolist(), got.tolist()))
+    assert {k: lut[k] for k in want} == want
+
+
 @pytest.mark.parametrize("out_dtype", [torch.bfloat16, torch.float16, torch.float32])
 def test_table_rules(out_dtype):
     from ddstore_b200.store import _conversion

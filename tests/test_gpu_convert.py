@@ -47,9 +47,7 @@ CASE_IDS = [c[0] for c in CASES]
 
 def _edge_rows(disp):
     """float32 rounding edges for bf16 and f16: ties both ways, overflow, subnormals, -0, inf, NaN"""
-    vals = np.array([0x3F808000, 0x3F818000, 0x3F80FFFF, 0x7F7FFFFF, 0x477FF000, 0x477FEFFF, 0x33800000, 0x33000000,
-                     0x33000001, 0x387FC000, 0x80000000, 0x00000001, 0x7F800000, 0xFF800000, 0x7FC00000, 0x7F800001,
-                     0xFF7FFFFF, 0x00800000], np.uint32)
+    vals = np.array(co.F32_EDGE_BITS, np.uint32)
     n = (len(vals) * 4 + disp - 1) // disp
     return np.resize(vals, n * disp).reshape(n, disp).view(np.float32)
 
@@ -383,6 +381,37 @@ def test_overlapped_queues(env, contention):
             assert torch.equal(bufs[k][:exp[k].numel()], exp[k]), f"{mode} contention={contention}: batch {k}"
 
 
+def test_wait_total_after_a_converting_multi_array_batch_in_an_overlapped_queue():
+    """regression: wait() reports the total of the LAST queued batch. A converting multi-array batch writes its total
+    at the end of its walk, a batch planned in shared memory at its start; while an overlapped run shared one total
+    word, the multi-array batch, still running, overwrote the total of the small batch queued behind it"""
+    from ddstore_b200 import PyDDStore
+    store = PyDDStore(device=0)
+    try:
+        rows, disp = 8192, 1024
+        for nm in ("a", "b"):
+            store.init(nm, rows, disp, 4)
+            store.synth_fill(nm, 3)
+            store.set_sample_index(nm, np.arange(0, rows, 8, dtype=np.int64), np.full(rows // 8, 8, np.int64))
+        rng = np.random.default_rng(5)
+        ids = torch.from_numpy(rng.integers(0, rows // 8, 2000)).to(DEV)  # 4000 requests: the plan kernels
+        starts = torch.from_numpy(rng.integers(0, rows, 100)).to(DEV)     # 100 requests: the shared-memory plan
+        counts = torch.ones(100, dtype=torch.int64, device=DEV)
+        big = [torch.empty(2000 * 8 * disp, dtype=torch.bfloat16, device=DEV) for _ in range(2)]
+        small = torch.empty(100 * disp, dtype=torch.bfloat16, device=DEV)
+        side = torch.cuda.Stream(device=DEV)
+        torch.cuda.synchronize()
+        store.get_samples_multi(["a", "b"], ids, big, stream=side.cuda_stream, wait=False, overlap=True,
+                                src_dtypes=[torch.float32, torch.float32])
+        store.get_batch("a", starts, counts, out=small, stream=side.cuda_stream, wait=False, overlap=True,
+                        src_dtype=torch.float32)
+        assert store.wait() == small.numel() * 2
+        torch.cuda.synchronize()
+    finally:
+        store.free()
+        store.close()
+
+
 def test_u8_to_f32_beyond_4gib(env):
     """a uint8 source below 4 GiB whose float32 output is above it: fixed count and explicit counts"""
     from ddstore_b200 import PyDDStore
@@ -422,11 +451,12 @@ def test_u8_to_f32_beyond_4gib(env):
         store.close()
 
 
-def test_multi_owner_world():
+def _multi_owner_world(P, devices=None):
     from tests.gpu_helpers import run_world
-    P, per, disp = 3, 5000, 24
+    per, disp = 5000, 24
 
     def body(store, r):
+        DEV = torch.device("cuda", devices[r] if devices else 0)
         rng = np.random.default_rng(r)
         shard = rng.integers(0, 2 ** 32, size=(per + 100 * r, disp), dtype=np.uint32).view(np.float32)
         store.add("w", shard)
@@ -442,7 +472,19 @@ def test_multi_owner_world():
         assert torch.equal(o.view(torch.int16), raw.to(torch.float16).view(torch.int16)), f"rank {r}"
         return True
 
-    assert all(run_world(P, body))
+    assert all(run_world(P, body, devices=devices))
+
+
+def test_multi_owner_world():
+    _multi_owner_world(3)
+
+
+def test_multi_owner_world_peer_devices():
+    """every rank on its own GPU: converting batches read the other owners' HBM through the peer mappings"""
+    P = min(3, torch.cuda.device_count())
+    if P < 2:
+        pytest.skip("needs two or more GPUs")
+    _multi_owner_world(P, devices=list(range(P)))
 
 
 def test_loaders(env):
