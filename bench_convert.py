@@ -9,6 +9,11 @@ raw gather of the same indices, bitwise, NaN also by class):
          that expression
   cfg3   variable-length float32 samples of 100..10000 elements by sample id, B = 16384, overlapped: raw vs f32->bf16
   f64    4 KiB float64 rows (disp 512), B = 65536: raw vs f64->f32
+  norm   the cfg2 shape normalised per feature (1024 channels), (x - mean) / std into bfloat16: fused, also as an
+         overlapped queue, against raw gather + (x - m) / s + .to(bfloat16) on the same stream (and the plain fused
+         f32->bf16 of cfg2)
+  u8norm the u8 images viewed as 3 x 32 x 32 CHW (3 channels of 1024), ToTensor() + Normalize() into bfloat16: fused
+         with the div(255) decode table, against raw gather + .float().div(255).sub(m).div(s).to(bfloat16)
 Reported per workload: ms/batch, samples/s, and the modelled HBM traffic (payload read + output written, and every
 byte a torch cast reads and writes, computed from the shapes here; index reads are left out) over the time, as a
 fraction of the H100 SXM data-sheet 3.35 TB/s. Without a GPU the script fails: there is no fallback.
@@ -88,7 +93,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--batch", type=int, default=65536)
     ap.add_argument("--scale", type=float, default=1.0, help="shrink every store (tests)")
-    ap.add_argument("--workloads", default="cfg2,u8,cfg3,f64")
+    ap.add_argument("--workloads", default="cfg2,norm,u8,u8norm,cfg3,f64")
     args = ap.parse_args()
 
     import torch
@@ -107,7 +112,7 @@ def main():
     out = res["workloads"]
 
     # ---- config-2 shape: 10M x 1024 float32, B rows per batch
-    if "cfg2" in names:
+    if "cfg2" in names or "norm" in names:
         N, D = int(10_000_000 * args.scale), 1024
         store = PyDDStore(device=0)
         store.init("x", N, D, 4)
@@ -116,6 +121,33 @@ def main():
         raw = [torch.empty((B, D), dtype=torch.float32, device=dev) for _ in range(2)]
         half = {dt: [torch.empty((B, D), dtype=dt, device=dev) for _ in range(2)] for dt in (torch.bfloat16, torch.float16)}
         rb = B * D * 4
+    if "norm" in names:
+        g = np.random.default_rng(SEED)
+        mean = torch.from_numpy(g.standard_normal(D).astype(np.float32)).to(dev)
+        std = torch.from_numpy((g.random(D) + 0.1).astype(np.float32)).to(dev)
+        store.set_normalization("x", mean, std)
+        tmp = torch.empty((B, D), dtype=torch.float32, device=dev)
+        nrm = [torch.empty((B, D), dtype=torch.bfloat16, device=dev) for _ in range(2)]
+
+        def gather_norm_cast(i):  # (division by a CUDA tensor: the expression the fused gather is bit-exact with)
+            store.get_batch("x", idx[i & 1], out=raw[i & 1], stream=sh)
+            torch.sub(raw[i & 1], mean, out=tmp)
+            torch.div(tmp, std, out=tmp)
+            nrm[i & 1].copy_(tmp)
+        ms, p = timed(gather_norm_cast, K, W, st)
+        out.append(entry("norm_raw_f32_then_torch_sub_div_bf16", ms, p, B, 2 * rb + 2 * rb + 2 * rb + rb + rb // 2, (None, 0)))
+        for ovl in (False, True):
+            kw = dict(wait=False, overlap=True) if ovl else {}
+            ms, p = timed(lambda i: store.get_batch("x", idx[i & 1], out=nrm[i & 1], stream=sh, src_dtype=torch.float32,
+                                                    normalize=True, **kw), K, W, st)  # noqa: B023
+            if ovl:
+                store.wait()
+            last = (W + K - 1) & 1
+            store.get_batch("x", idx[last], out=raw[0], stream=sh)
+            ver = compare(nrm[last], ((raw[0] - mean) / std).to(torch.bfloat16))
+            out.append(entry("norm_fused_f32_bf16_per_feature" + ("_overlapped" if ovl else ""), ms, p, B, rb + rb // 2, ver))
+        del tmp, nrm
+    if "cfg2" in names:
         ms, p = timed(lambda i: store.get_batch("x", idx[i & 1], out=raw[i & 1], stream=sh), K, W, st)
         out.append(entry("cfg2_raw_f32", ms, p, B, 2 * rb, (None, 0)))
         casted = [torch.empty((B, D), dtype=torch.bfloat16, device=dev) for _ in range(2)]
@@ -139,13 +171,15 @@ def main():
                 store.get_batch("x", idx[last], out=raw[0], stream=sh)
                 ver = compare(bufs[last], raw[0].to(dt))
                 out.append(entry(f"cfg2_fused_f32_{tag}" + ("_overlapped" if ovl else ""), ms, p, B, rb + rb // 2, ver))
+        del casted
+    if "cfg2" in names or "norm" in names:
         store.free()
         store.close()
-        del raw, half, casted
+        del raw, half
         torch.cuda.empty_cache()
 
     # ---- uint8 images: 4M x 3072, normalised to float
-    if "u8" in names:
+    if "u8" in names or "u8norm" in names:
         N, D = int(4_000_000 * args.scale), 3072
         store = PyDDStore(device=0)
         store.init("img", N, D, 1)
@@ -154,6 +188,34 @@ def main():
         raw = torch.empty((B, D), dtype=torch.uint8, device=dev)
         flt = torch.empty((B, D), dtype=torch.float32, device=dev)
         rb = B * D
+    if "u8norm" in names:  # 3 x 32 x 32 CHW images, torchvision's ImageNet mean / std
+        C, HW = 3, D // 3
+        mean = torch.tensor([0.485, 0.456, 0.406], dtype=torch.float32, device=dev)
+        std = torch.tensor([0.229, 0.224, 0.225], dtype=torch.float32, device=dev)
+        store.set_normalization("img", mean, std, HW)
+        m3, s3 = mean.view(1, C, 1), std.view(1, C, 1)
+        table = torch.arange(256, device=dev, dtype=torch.uint8).float().div(255)  # ToTensor()'s expression
+        bf = torch.empty((B, D), dtype=torch.bfloat16, device=dev)
+
+        def gather_totensor_normalize(i):
+            store.get_batch("img", idx[i & 1], out=raw, stream=sh)
+            torch.div(raw.float(), 255, out=flt)
+            v = flt.view(B, C, HW)
+            torch.sub(v, m3, out=v)
+            torch.div(v, s3, out=v)
+            bf.copy_(flt)
+        ms, p = timed(gather_totensor_normalize, K, W, st)
+        out.append(entry("u8norm_raw_then_torch_float_div255_sub_div_bf16", ms, p, B,
+                         2 * rb + (rb + 4 * rb) + 3 * (2 * 4 * rb) + (4 * rb + 2 * rb), (None, 0)))
+        o = torch.empty((B, D), dtype=torch.bfloat16, device=dev)
+        ms, p = timed(lambda i: store.get_batch("img", idx[i & 1], out=o, stream=sh, src_dtype=torch.uint8, lut=table,
+                                                normalize=True), K, W, st)
+        last = (W + K - 1) & 1
+        store.get_batch("img", idx[last], out=raw, stream=sh)
+        ver = compare(o, ((raw.view(B, C, HW).float().div(255) - m3) / s3).to(torch.bfloat16))
+        out.append(entry("u8norm_fused_chw_bf16", ms, p, B, rb + 2 * rb, ver))
+        del o, bf
+    if "u8" in names:
 
         def gather_norm(i):
             store.get_batch("img", idx[i & 1], out=raw, stream=sh)
@@ -170,6 +232,7 @@ def main():
             ver = compare(o, raw.float().div(255).to(dt))
             out.append(entry(f"u8_fused_{tag}", ms, p, B, rb + rb * o.element_size(), ver))
             del o
+    if "u8" in names or "u8norm" in names:
         store.free()
         store.close()
         del raw, flt
@@ -234,6 +297,14 @@ def main():
         res["cfg2_fused_bf16_speedup_vs_raw_f32"] = by["cfg2_fused_f32_bf16"]["samples_per_s"] / by["cfg2_raw_f32"]["samples_per_s"]
         res["cfg2_fused_bf16_speedup_vs_gather_then_cast"] = (by["cfg2_fused_f32_bf16"]["samples_per_s"] /
                                                               by["cfg2_raw_f32_then_torch_bf16"]["samples_per_s"])
+    if "norm_fused_f32_bf16_per_feature" in by:
+        nf = by["norm_fused_f32_bf16_per_feature"]["samples_per_s"]
+        res["norm_fused_speedup_vs_gather_then_sub_div_cast"] = nf / by["norm_raw_f32_then_torch_sub_div_bf16"]["samples_per_s"]
+        if "cfg2_fused_f32_bf16" in by:
+            res["norm_fused_vs_plain_fused_bf16"] = nf / by["cfg2_fused_f32_bf16"]["samples_per_s"]
+    if "u8norm_fused_chw_bf16" in by:
+        res["u8norm_fused_speedup_vs_unfused"] = (by["u8norm_fused_chw_bf16"]["samples_per_s"] /
+                                                  by["u8norm_raw_then_torch_float_div255_sub_div_bf16"]["samples_per_s"])
     res["all_verified"] = all(e["mismatches_nan_by_class"] == 0 for e in out)
     print(json.dumps(res))
 

@@ -28,6 +28,9 @@ class VarInfo(C.Structure):
 
 # conversions of the converting batch entries (DDS_CVT_*)
 CVT_NONE, CVT_F32_BF16, CVT_F32_F16, CVT_F64_F32, CVT_U8_LUT16, CVT_U8_LUT32 = 0, 1, 2, 3, 4, 5
+# normalising conversions ((x - mean[ch]) / std[ch] in f32; dds_set_normalization registers the tables)
+CVT_NORM_F32_F32, CVT_NORM_F32_BF16, CVT_NORM_F32_F16, CVT_NORM_F64_F32 = 6, 7, 8, 9
+CVT_NORM_U8_F32, CVT_NORM_U8_BF16, CVT_NORM_U8_F16 = 10, 11, 12
 
 
 class Convert(C.Structure):  # dds_convert_t
@@ -75,6 +78,8 @@ SIGNATURES = {
                                                 C.c_void_p, C.POINTER(Convert), I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
+    "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                        C.c_int]),
     "dds_get_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
                                   C.c_void_p, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_query": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(VarInfo)]),

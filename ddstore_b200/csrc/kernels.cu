@@ -713,11 +713,19 @@ __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, ui
 // Source elements are therefore also aligned to their size in shared memory (stage offsets are 16-byte aligned and
 // source rows start at itemsize-aligned addresses).
 // ------------------------------------------------------------------------------------------------
-__host__ __device__ constexpr int cvt_in_log2(int code) { return code == DDSK_CVT_F64_F32 ? 3 : (code == DDSK_CVT_F32_BF16 || code == DDSK_CVT_F32_F16) ? 2 : 0; }
-__host__ __device__ constexpr int cvt_out_log2(int code) {
-    return code == DDSK_CVT_NONE ? 0 : (code == DDSK_CVT_F64_F32 || code == DDSK_CVT_U8_LUT32) ? 2 : 1;
+// (NORM: the codes may include the normalising ones; launches without them evaluate the tables of codes 0..5 only)
+template <bool NORM = false>
+__host__ __device__ constexpr int cvt_in_log2(int code) {
+    if constexpr (NORM) return DDSK_CVT_IN_LOG2(code);
+    else return DDSK_CVT_PLAIN_IN_LOG2(code);
 }
-__device__ __forceinline__ int64_t cvt_scale(int64_t p, int code) { return (p >> cvt_in_log2(code)) << cvt_out_log2(code); }
+template <bool NORM = false>
+__host__ __device__ constexpr int cvt_out_log2(int code) {
+    if constexpr (NORM) return DDSK_CVT_OUT_LOG2(code);
+    else return DDSK_CVT_PLAIN_OUT_LOG2(code);
+}
+template <bool NORM = false>
+__device__ __forceinline__ int64_t cvt_scale(int64_t p, int code) { return (p >> cvt_in_log2<NORM>(code)) << cvt_out_log2<NORM>(code); }
 
 __device__ __forceinline__ uint32_t cvt2_bf16(float lo, float hi) { // packs (lo, hi) -> [15:0] lo, [31:16] hi
     uint32_t d;
@@ -845,6 +853,194 @@ __device__ __forceinline__ void cvt_drain(uint32_t s0, char *d, uint32_t n, uint
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Normalising drain (DDSK_CVT_NORM_*): y = __fdiv_rn(__fsub_rn(decode(x), mean[ch]), std[ch]), then encoded -- explicit
+// IEEE roundings, so the result does not depend on contraction flags. Channel of element e of a variable's packed rows:
+// (e mod (nchan * inner)) / inner -- every request starts at a row boundary and nchan * inner divides the row. It is
+// found once per piece (one 64-bit remainder) and per lane (32-bit), then advanced incrementally element by element.
+// The {mean, std} pairs are read with ld.global.nc: nchan * 8 bytes that stay in L1 / L2.
+// ------------------------------------------------------------------------------------------------
+// source (0 f32, 1 f64, 2 uint8 through the f32 table) and output (0 f32, 1 bf16, 2 f16) of a normalising code
+__host__ __device__ constexpr int norm_src(int code) { return code == DDSK_CVT_NORM_F64_F32 ? 1 : code >= DDSK_CVT_NORM_U8_F32 ? 2 : 0; }
+__host__ __device__ constexpr int norm_out(int code) {
+    return (code == DDSK_CVT_NORM_F32_BF16 || code == DDSK_CVT_NORM_U8_BF16) ? 1
+         : (code == DDSK_CVT_NORM_F32_F16 || code == DDSK_CVT_NORM_U8_F16)  ? 2 : 0;
+}
+
+// position inside the channel pattern: channel ch, element in of its run of `inner`
+struct ChanPos {
+    uint32_t ch, in;
+    __device__ __forceinline__ void step(uint32_t nchan, uint32_t inner) {
+        if (++in == inner) {
+            in = 0;
+            if (++ch == nchan) ch = 0;
+        }
+    }
+    // forward by dq * inner + dr elements (dq < nchan, dr < inner)
+    __device__ __forceinline__ void advance(uint32_t dq, uint32_t dr, uint32_t nchan, uint32_t inner) {
+        uint32_t c = ch + dq;
+        in += dr;
+        if (in >= inner) {
+            in -= inner;
+            c++;
+        }
+        ch = c >= nchan ? c - nchan : c;
+    }
+};
+// the position r elements into the pattern (r < nchan * inner)
+__device__ __forceinline__ ChanPos chan_at(uint32_t r, uint32_t inner) {
+    const uint32_t ch = r / inner;
+    return ChanPos{ch, r - ch * inner};
+}
+
+template <int CODE>
+__device__ __forceinline__ float norm_decode1(uint32_t s, uint32_t lut) {
+    if constexpr (norm_src(CODE) == 0) return __uint_as_float(lds32(s));
+    else if constexpr (norm_src(CODE) == 1) return __uint_as_float(cvt_f32_of_f64(lds64(s)));
+    else return __uint_as_float(lut32(lut, lds8(s)));
+}
+__device__ __forceinline__ float norm_apply(float x, const float *tab, uint32_t ch) {
+    const float2 ms = __ldg((const float2 *)tab + ch);
+    return __fdiv_rn(__fsub_rn(x, ms.x), ms.y);
+}
+
+// one element: source at shared address s, output at d, channel ch
+template <int CODE>
+__device__ __forceinline__ void norm_one(uint32_t s, char *d, uint32_t lut, const float *tab, uint32_t ch) {
+    const float y = norm_apply(norm_decode1<CODE>(s, lut), tab, ch);
+    if constexpr (norm_out(CODE) == 0) *(uint32_t *)d = __float_as_uint(y);
+    else *(uint16_t *)d = (uint16_t)((norm_out(CODE) == 1 ? cvt2_bf16(y, 0.0f) : cvt2_f16(y, 0.0f)) & 0xFFFFu);
+}
+
+// one 16-byte output vector (E elements) from the source elements at shared address s; p = channel of the first
+template <int CODE, bool VEC>
+__device__ __forceinline__ uint4 norm_vec(uint32_t s, uint32_t lut, const float *tab, ChanPos p, uint32_t nchan, uint32_t inner) {
+    constexpr int E = norm_out(CODE) == 0 ? 4 : 8;
+    float x[E];
+    if constexpr (norm_src(CODE) == 0) { // 4 or 8 floats
+        if (VEC) {
+#pragma unroll
+            for (int k = 0; k < E; k += 4) {
+                const uint4 a = lds128(s + 4u * k);
+                x[k] = __uint_as_float(a.x); x[k + 1] = __uint_as_float(a.y); x[k + 2] = __uint_as_float(a.z); x[k + 3] = __uint_as_float(a.w);
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < E; k++) x[k] = __uint_as_float(lds32(s + 4u * k));
+        }
+    } else if constexpr (norm_src(CODE) == 1) { // 4 doubles
+        uint64_t q[4];
+        if (VEC) {
+            const uint4 a = lds128(s), b = lds128(s + 16);
+            q[0] = (uint64_t)a.y << 32 | a.x; q[1] = (uint64_t)a.w << 32 | a.z;
+            q[2] = (uint64_t)b.y << 32 | b.x; q[3] = (uint64_t)b.w << 32 | b.z;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) q[k] = lds64(s + 8u * k);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; k++) x[k] = __uint_as_float(cvt_f32_of_f64(q[k]));
+    } else { // 4 or 8 bytes through the decode table
+        uint32_t b[E];
+        if (VEC) {
+            const uint64_t v = E == 8 ? lds64(s) : (uint64_t)lds32(s);
+#pragma unroll
+            for (int k = 0; k < E; k++) b[k] = (uint32_t)(v >> (8 * k)) & 0xFFu;
+        } else {
+#pragma unroll
+            for (int k = 0; k < E; k++) b[k] = lds8(s + k);
+        }
+#pragma unroll
+        for (int k = 0; k < E; k++) x[k] = __uint_as_float(lut32(lut, b[k]));
+    }
+#pragma unroll
+    for (int k = 0; k < E; k++) {
+        x[k] = norm_apply(x[k], tab, p.ch);
+        p.step(nchan, inner);
+    }
+    if constexpr (norm_out(CODE) == 0) {
+        return make_uint4(__float_as_uint(x[0]), __float_as_uint(x[1]), __float_as_uint(x[2]), __float_as_uint(x[3]));
+    } else {
+        uint32_t r[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) r[k] = norm_out(CODE) == 1 ? cvt2_bf16(x[2 * k], x[2 * k + 1]) : cvt2_f16(x[2 * k], x[2 * k + 1]);
+        return make_uint4(r[0], r[1], r[2], r[3]);
+    }
+}
+
+// Drain one staged piece normalised: as cvt_drain; `rel` = the piece's first source byte relative to its variable's
+// packed base, tab / nchan / inner = that variable's normalisation.
+template <int CODE>
+__device__ __forceinline__ void norm_drain(uint32_t s0, char *d, uint32_t n, uint32_t lut, int lane, const float *tab,
+                                           int64_t rel, uint32_t nchan, uint32_t inner) {
+    constexpr int IL = cvt_in_log2<true>(CODE), OL = cvt_out_log2<true>(CODE);
+    constexpr uint32_t E = 16u >> OL;                          // elements per output vector
+    constexpr uint32_t VA = (E << IL) < 16u ? (E << IL) : 16u; // source alignment of the vector loads
+    const uint32_t ne = n >> IL;
+    uint32_t head = ((16u - (uint32_t)((uint64_t)d & 15u)) & 15u) >> OL;
+    if (head > ne) head = ne;
+    const uint32_t nv = (ne - head) / E;
+    const uint32_t tail = ne - head - nv * E;
+    const uint32_t sb = s0 + (head << IL);
+    char *dv = d + (head << OL);
+    const uint32_t period = nchan * inner;
+    const uint32_t r0 = (uint32_t)((rel >> IL) % (int64_t)period); // pattern position of the piece's first element
+    // (r0 + k < 2^32: the pattern is below 2^31 elements, a piece below 2^16)
+    ChanPos p = chan_at((r0 + head + (uint32_t)lane * E) % period, inner);
+    const uint32_t dq = ((32u * E) / inner) % nchan, dr = (32u * E) % inner; // one round of the warp: 32 vectors
+    if ((sb & (VA - 1u)) == 0) { // warp-uniform
+#pragma unroll 2
+        for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
+            stg128(dv + ((size_t)j << 4), norm_vec<CODE, true>(sb + j * (E << IL), lut, tab, p, nchan, inner));
+            p.advance(dq, dr, nchan, inner);
+        }
+    } else {
+#pragma unroll 2
+        for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
+            stg128(dv + ((size_t)j << 4), norm_vec<CODE, false>(sb + j * (E << IL), lut, tab, p, nchan, inner));
+            p.advance(dq, dr, nchan, inner);
+        }
+    }
+    if ((uint32_t)lane < head) {
+        const uint32_t k = (uint32_t)lane;
+        norm_one<CODE>(s0 + (k << IL), d + (k << OL), lut, tab, chan_at((r0 + k) % period, inner).ch);
+    }
+    if ((uint32_t)lane < tail) {
+        const uint32_t k = head + nv * E + (uint32_t)lane;
+        norm_one<CODE>(s0 + (k << IL), d + ((size_t)k << OL), lut, tab, chan_at((r0 + k) % period, inner).ch);
+    }
+}
+
+// a normalising launch drains one piece of a variable with a normalising code (its position relative to the variable's
+// packed base gives the channels; vbase: the variables' starts in a multi-array launch)
+__device__ __forceinline__ void norm_piece(const ddsk_cvt_t &c, bool multi, const int64_t (&vbase)[DDSK_MAX_MULTI + 1],
+                                           int64_t dpos, int code, uint32_t lut, char *d, uint32_t s, uint32_t n, int lane) {
+    int64_t b = 0;
+    const float *tab = c.norm[0];
+    uint32_t nc = (uint32_t)c.nchan[0], inr = (uint32_t)c.inner[0];
+    if (multi) {
+        b = vbase[0];
+#pragma unroll
+        for (int k = 1; k < DDSK_MAX_MULTI; k++)
+            if (dpos >= vbase[k]) {
+                b = vbase[k];
+                tab = c.norm[k];
+                nc = (uint32_t)c.nchan[k];
+                inr = (uint32_t)c.inner[k];
+            }
+    }
+    const int64_t rel = dpos - b;
+    switch (code) { // warp-uniform
+    case DDSK_CVT_NORM_F32_F32: norm_drain<DDSK_CVT_NORM_F32_F32>(s, d, n, lut, lane, tab, rel, nc, inr); break;
+    case DDSK_CVT_NORM_F32_BF16: norm_drain<DDSK_CVT_NORM_F32_BF16>(s, d, n, lut, lane, tab, rel, nc, inr); break;
+    case DDSK_CVT_NORM_F32_F16: norm_drain<DDSK_CVT_NORM_F32_F16>(s, d, n, lut, lane, tab, rel, nc, inr); break;
+    case DDSK_CVT_NORM_F64_F32: norm_drain<DDSK_CVT_NORM_F64_F32>(s, d, n, lut, lane, tab, rel, nc, inr); break;
+    case DDSK_CVT_NORM_U8_F32: norm_drain<DDSK_CVT_NORM_U8_F32>(s, d, n, lut, lane, tab, rel, nc, inr); break;
+    case DDSK_CVT_NORM_U8_BF16: norm_drain<DDSK_CVT_NORM_U8_BF16>(s, d, n, lut, lane, tab, rel, nc, inr); break;
+    default: norm_drain<DDSK_CVT_NORM_U8_F16>(s, d, n, lut, lane, tab, rel, nc, inr); break;
+    }
+}
+
 // the kernel parameter carrying a launch's conversion: ddsk_cvt_t, or nothing at all for raw launches
 struct NoCvt {
     int32_t unused_;
@@ -862,11 +1058,11 @@ using CvtParam = typename std::conditional<CVT, ddsk_cvt_t, NoCvt>::type;
 // when the destination capacity is below 4 GiB, so T > 2^32 is a capacity error and nothing is copied).
 // ------------------------------------------------------------------------------------------------
 // (CVT: the offsets the caller sees are in output bytes of conversion `code`; the plan itself stays in source bytes)
-template <int NW, int PCAP, bool CVT = false>
+template <int NW, int PCAP, bool CVT = false, bool NORM = false>
 __device__ __forceinline__ int64_t plan_in_smem(const GatherArgs &a, const PlanView<PCAP> &pv, int64_t *wtot, int warp,
                                                 int lane, bool writer, int code = 0) {
     auto out = [&](int64_t x) -> int64_t {
-        if constexpr (CVT) return cvt_scale(x, code);
+        if constexpr (CVT) return cvt_scale<NORM>(x, code);
         else return x;
     };
     const int64_t nreq = a.nreq;
@@ -938,9 +1134,12 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // CVT: the converting form (DDSK_CVT_*, `c` carries the codes and tables). Everything on the load side -- walk over the
 // packed SOURCE byte space, rings, plan, checks, overlap protocol -- is the raw kernel's; only the drain and the
 // caller-visible offsets differ. Converting launches have no push fetch.
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false>
+// NORM (with CVT): the form of launches that carry a normalising code (DDSK_CVT_NORM_*); its drain handles every code,
+// since a multi-array launch may mix normalised, plainly converted and raw variables.
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
                                                                 const __grid_constant__ CvtParam<CVT> c) {
+    static_assert(CVT || !NORM, "a normalising launch is a converting one");
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
     constexpr bool PUSH = FIXED && !CVT;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
@@ -1000,7 +1199,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             w.pv.dst_s = w.pv.src_s + (uint32_t)PCAP * 8u;
             const bool writer = blockIdx.x == 0;
             if (writer) pass_gate(); // CTA 0 writes the offsets / the total for the caller
-            w.T = plan_in_smem<NW, PCAP, CVT>(a, w.pv, wtot, warp, lane, writer, code0);
+            w.T = plan_in_smem<NW, PCAP, CVT, NORM>(a, w.pv, wtot, warp, lane, writer, code0);
         } else {
             w.pv.src = a.req_src;
             w.pv.dst = a.req_dst;
@@ -1158,7 +1357,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             if (!multi) {
                 code = code0;
                 lut = lut_s + (uint32_t)c.lut_off[0];
-                return a.dst + cvt_scale(dpos, code0);
+                return a.dst + cvt_scale<NORM>(dpos, code0);
             }
             int64_t b = vbase[0];
             char *d = a.mdst[0];
@@ -1173,7 +1372,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 }
             code = cd;
             lut = lut_s + (uint32_t)lo;
-            return d + cvt_scale(dpos - b, cd);
+            return d + cvt_scale<NORM>(dpos - b, cd);
         } else {
             return nullptr; // (never called)
         }
@@ -1284,6 +1483,12 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 uint32_t lut;
                 char *const d = out_of(dpos, code, lut);
                 const uint32_t s0 = ring + st * STAGE + (pk & 0xffffu); // + source misalignment = first payload byte
+                if constexpr (NORM) {
+                    if (DDSK_CVT_IS_NORM(code)) {
+                        norm_piece(c, multi, vbase, dpos, code, lut, d, s0 + (pk >> 16), n, lane);
+                        continue;
+                    }
+                }
                 switch (code) { // warp-uniform
                 case DDSK_CVT_F32_BF16: cvt_drain<DDSK_CVT_F32_BF16>(s0 + (pk >> 16), d, n, lut, lane); break;
                 case DDSK_CVT_F32_F16: cvt_drain<DDSK_CVT_F32_F16>(s0 + (pk >> 16), d, n, lut, lane); break;
@@ -1330,7 +1535,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             if (v < a.plan.nvars && a.moffsets[v]) {
                 const int64_t basev = w.pv.d((int64_t)v * a.plan.per_var); // == vbase[v]; re-read so that vbase[] is
                 int64_t e = (v * a.plan.per_var + j == a.nreq) ? w.T : w.pv.d((int64_t)v * a.plan.per_var + j);
-                if constexpr (CVT) a.moffsets[v][j] = cvt_scale(e - basev, c.code[v]); // (output bytes)
+                if constexpr (CVT) a.moffsets[v][j] = cvt_scale<NORM>(e - basev, c.code[v]); // (output bytes)
                 else a.moffsets[v][j] = e - basev;                                     // never indexed dynamically
             }
         }
@@ -1339,14 +1544,14 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 int64_t t = 0;
 #pragma unroll
                 for (int v = 0; v < DDSK_MAX_MULTI; v++)
-                    if (v < a.plan.nvars) t += cvt_scale((v + 1 < a.plan.nvars ? vbase[v + 1] : w.T) - vbase[v], c.code[v]);
+                    if (v < a.plan.nvars) t += cvt_scale<NORM>((v + 1 < a.plan.nvars ? vbase[v + 1] : w.T) - vbase[v], c.code[v]);
                 *a.total_out = t;
             }
         }
     }
     if (FIXED && a.offsets_out && !push) { // arithmetic offsets, written off the critical path
         if constexpr (CVT) {
-            for (int64_t i = gwarp * 32 + lane; i <= a.nreq; i += nwarps * 32) a.offsets_out[i] = cvt_scale(i * w.nb, code0);
+            for (int64_t i = gwarp * 32 + lane; i <= a.nreq; i += nwarps * 32) a.offsets_out[i] = cvt_scale<NORM>(i * w.nb, code0);
         } else {
             for (int64_t i = gwarp * 32 + lane; i <= a.nreq; i += nwarps * 32) a.offsets_out[i] = i * w.nb;
         }
@@ -1556,7 +1761,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
             const int64_t d0 = run, d1 = run + nb[k];
             req_src[idx[k]] = sv[k];
             req_dst[idx[k]] = d0;
-            if (offsets_out) offsets_out[idx[k]] = cvt_scale(d0, cvt_code);
+            if (offsets_out) offsets_out[idx[k]] = cvt_scale<true>(d0, cvt_code);
             for (int64_t g = (d0 + SEG_GRAIN - 1) / SEG_GRAIN; g * SEG_GRAIN < d1 && g < seg_cap; g++) seg_tab[g] = (uint32_t)idx[k];
             run = d1;
         }
@@ -1565,7 +1770,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
     const int64_t T = tile_excl_s + agg;
     if (last_tile && threadIdx.x == 0) {
         req_dst[nreq] = T;
-        if (offsets_out) offsets_out[nreq] = cvt_scale(T, cvt_code);
+        if (offsets_out) offsets_out[nreq] = cvt_scale<true>(T, cvt_code);
     }
     if (pr.dbg && threadIdx.x == 0) atomicMax(&pr.dbg[4096 + 1], (unsigned long long)globaltimer_ns());
     if (pr.ovl) {
@@ -1820,12 +2025,19 @@ int ctas_per_sm_for(int nw, int s, int ch, int pcap) {
     return per_sm;
 }
 
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false>
+// does a converting launch carry a normalising code? (then it takes the NORM form of the kernel; unused slots are 0)
+bool cvt_has_norm(const ddsk_cvt_t *cvt) {
+    for (int v = 0; v < DDSK_MAX_MULTI; v++)
+        if (DDSK_CVT_IS_NORM(cvt->code[v])) return true;
+    return false;
+}
+
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
     // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan)
     const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT>;
+    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -1915,7 +2127,8 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
 template <bool FIXED>
 int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
     // converting launches: the default variant of each entry (kGeomLarge = kGeomVar), whatever DDS_GATHER_GEOM* say
-    if (cvt) return launch_gather_t<FIXED, 12, 4, 4096, 0, true>(args, stream, cvt);
+    if (cvt) return cvt_has_norm(cvt) ? launch_gather_t<FIXED, 12, 4, 4096, 0, true, true>(args, stream, cvt)
+                                      : launch_gather_t<FIXED, 12, 4, 4096, 0, true>(args, stream, cvt);
     // (the request size only picks a variant: a count too large to multiply safely counts as large)
     const int64_t request_bytes = args.count < ((int64_t)1 << 20) ? args.count * args.var.row_bytes : INT64_MAX;
     switch (geometry_for(FIXED, FIXED ? request_bytes : 0)) {
@@ -1930,6 +2143,9 @@ int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t 
     }
 }
 int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
+    if (cvt && cvt_has_norm(cvt))
+        return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, true, true>(args, stream, cvt)
+                      : launch_gather_t<false, 12, 3, 4096, 4096, true, true>(args, stream, cvt);
     if (cvt) return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, true>(args, stream, cvt)
                            : launch_gather_t<false, 12, 3, 4096, 4096, true>(args, stream, cvt);
     switch (g) {

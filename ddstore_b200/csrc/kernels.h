@@ -80,16 +80,40 @@ typedef struct ddsk_scratch {
 #define DDSK_CVT_F64_F32 3   /* 8 -> 4 bytes, cvt.rn.f32.f64 */
 #define DDSK_CVT_U8_LUT16 4  /* 1 -> 2 bytes, out = lut[in] */
 #define DDSK_CVT_U8_LUT32 5  /* 1 -> 4 bytes, out = lut[in] */
-#define DDSK_CVT_MAX 5
+/* normalising conversions: y = (decode(x) - mean[ch]) / std[ch] in f32 (two IEEE roundings), then encoded */
+#define DDSK_CVT_NORM_F32_F32 6  /* 4 -> 4 bytes */
+#define DDSK_CVT_NORM_F32_BF16 7 /* 4 -> 2 bytes */
+#define DDSK_CVT_NORM_F32_F16 8  /* 4 -> 2 bytes */
+#define DDSK_CVT_NORM_F64_F32 9  /* 8 -> 4 bytes, decode = cvt.rn.f32.f64 */
+#define DDSK_CVT_NORM_U8_F32 10  /* 1 -> 4 bytes, decode = 256-entry f32 table */
+#define DDSK_CVT_NORM_U8_BF16 11 /* 1 -> 2 bytes, decode = 256-entry f32 table */
+#define DDSK_CVT_NORM_U8_F16 12  /* 1 -> 2 bytes, decode = 256-entry f32 table */
+#define DDSK_CVT_MAX 12
+#define DDSK_CVT_IS_NORM(c) ((c) >= DDSK_CVT_NORM_F32_F32)
+/* source / output itemsize of a code, as log2: the one table the host and the kernels share. The _PLAIN forms cover codes
+ * 0..5 only (the launches that carry no normalising code evaluate those). */
+#define DDSK_CVT_PLAIN_IN_LOG2(c) ((c) == DDSK_CVT_F64_F32 ? 3 : ((c) == DDSK_CVT_F32_BF16 || (c) == DDSK_CVT_F32_F16) ? 2 : 0)
+#define DDSK_CVT_PLAIN_OUT_LOG2(c) ((c) == DDSK_CVT_NONE ? 0 : ((c) == DDSK_CVT_F64_F32 || (c) == DDSK_CVT_U8_LUT32) ? 2 : 1)
+#define DDSK_CVT_IN_LOG2(c) \
+    (DDSK_CVT_IS_NORM(c) ? ((c) == DDSK_CVT_NORM_F64_F32 ? 3 : (c) >= DDSK_CVT_NORM_U8_F32 ? 0 : 2) : DDSK_CVT_PLAIN_IN_LOG2(c))
+#define DDSK_CVT_OUT_LOG2(c)                                                                                              \
+    (DDSK_CVT_IS_NORM(c) ? (((c) == DDSK_CVT_NORM_F32_F32 || (c) == DDSK_CVT_NORM_F64_F32 || (c) == DDSK_CVT_NORM_U8_F32) ? 2 : 1) \
+                         : DDSK_CVT_PLAIN_OUT_LOG2(c))
 /* The conversion of one launch, passed BY VALUE as a kernel parameter (so every queued launch carries its own tables).
- * code[v] is variable v's conversion; the tables of the variables with a LUT code are packed into lut[] (lut_off[v]
- * bytes in, 256 entries of the output itemsize) and copied to shared memory by every CTA. */
+ * code[v] is variable v's conversion; the tables of the variables with a LUT code (and the f32 decode tables of the
+ * uint8 normalising codes) are packed into lut[] (lut_off[v] bytes in, 256 entries of the output itemsize -- 4 bytes for
+ * the normalising codes) and copied to shared memory by every CTA. A variable with a normalising code also has norm[v]:
+ * nchan {mean, std} f32 pairs in device memory the store owns (read through the non-coherent cache, never copied), and
+ * element e of a row belongs to channel (e / inner) % nchan. */
 typedef struct ddsk_cvt {
     int32_t code[DDSK_MAX_MULTI];
     int32_t lut_off[DDSK_MAX_MULTI];
     int32_t lut_bytes; /* bytes of lut[] in use (0..4096) */
     int32_t pad_;
     uint32_t lut[DDSK_MAX_MULTI * 256];
+    const float *norm[DDSK_MAX_MULTI]; /* [nchan][2] = {mean, std} */
+    int32_t nchan[DDSK_MAX_MULTI];     /* nchan * inner divides the variable's disp (< 2^31) */
+    int32_t inner[DDSK_MAX_MULTI];
 } ddsk_cvt_t;
 
 /* Fixed-count batch: every request fetches `count` rows; offsets are i*count*row_bytes.

@@ -133,6 +133,9 @@ struct Var {
     int64_t *d_tab = nullptr; // [nsamples][2] = {row_start, row_count}: one 16-byte load per sample id
     int64_t nsamples = 0;
     std::vector<int64_t> h_tab_count;
+    // per-channel normalisation (dds_set_normalization): element e of a row is in channel (e / norm_inner) % norm_nchan
+    float *d_norm = nullptr; // [norm_nchan][2] = {mean, std}: one 8-byte load per element
+    int64_t norm_nchan = 0, norm_inner = 1;
 };
 
 } // namespace
@@ -457,6 +460,9 @@ void release_var(Var &v, int rank) {
 void free_shard(Var &v) {
     if (v.d_tab) cudaFree(v.d_tab);
     v.d_tab = nullptr;
+    if (v.d_norm) cudaFree(v.d_norm);
+    v.d_norm = nullptr;
+    v.norm_nchan = 0;
     if (v.vmm)
         dds_vmm::release(&v.block);
     else if (v.base)
@@ -712,8 +718,8 @@ int64_t sat_add(int64_t a, int64_t b) {
 }
 
 // ---- converting batches: source itemsize / output itemsize of a DDSK_CVT_* code, as log2
-int cvt_in_log2(int code) { return code == DDSK_CVT_F64_F32 ? 3 : (code == DDSK_CVT_F32_BF16 || code == DDSK_CVT_F32_F16) ? 2 : 0; }
-int cvt_out_log2(int code) { return code == DDSK_CVT_NONE ? 0 : (code == DDSK_CVT_F64_F32 || code == DDSK_CVT_U8_LUT32) ? 2 : 1; }
+int cvt_in_log2(int code) { return DDSK_CVT_IN_LOG2(code); }
+int cvt_out_log2(int code) { return DDSK_CVT_OUT_LOG2(code); }
 // source bytes (whole elements) -> output bytes; saturates
 int64_t cvt_to_out(int64_t p, int code) {
     if (p == INT64_MAX) return p;
@@ -1382,17 +1388,56 @@ static int make_cvt(Var *const *vars, const dds_convert_t *cv, int nvars, bool n
         const int code = cv[v].code;
         if (code < (none_ok ? DDS_CVT_NONE : DDS_CVT_F32_BF16) || code > DDSK_CVT_MAX)
             return fail(DDS_ERR_ARG, "unknown conversion code " + std::to_string(code));
+        // (a normalising code needs the variable's tables before anything else: without them it names no conversion)
+        if (DDSK_CVT_IS_NORM(code) && vars[v]->norm_nchan <= 0) // checked at call time: they may have been removed since
+            return fail(DDS_ERR_ARG, "variable has no normalization (call dds_set_normalization first)");
         if (code != DDS_CVT_NONE && vars[v]->itemsize != (1 << cvt_in_log2(code))) return fail(DDS_ERR_DTYPE);
         out->code[v] = code;
-        if (code == DDS_CVT_U8_LUT16 || code == DDS_CVT_U8_LUT32) {
+        const bool u8_norm = code == DDS_CVT_NORM_U8_F32 || code == DDS_CVT_NORM_U8_BF16 || code == DDS_CVT_NORM_U8_F16;
+        if (code == DDS_CVT_U8_LUT16 || code == DDS_CVT_U8_LUT32 || u8_norm) {
             if (!cv[v].lut) return fail(DDS_ERR_ARG, "a LUT conversion needs a table");
-            const int bytes = 256 << cvt_out_log2(code);
+            const int bytes = u8_norm ? 256 * 4 : 256 << cvt_out_log2(code); // (a normalising code decodes through f32)
             memcpy((char *)out->lut + off, cv[v].lut, (size_t)bytes); // copied now: the caller may free it on return
             out->lut_off[v] = off;
             off += bytes;
         }
+        if (DDSK_CVT_IS_NORM(code)) {
+            out->norm[v] = vars[v]->d_norm;
+            out->nchan[v] = (int32_t)vars[v]->norm_nchan;
+            out->inner[v] = (int32_t)vars[v]->norm_inner;
+        }
     }
     out->lut_bytes = off;
+    return DDS_OK;
+}
+
+int dds_set_normalization(dds_store_t *s, const char *name, const float *mean, const float *std, int64_t nchan,
+                          int64_t inner, int tables_on_device) {
+    clear_error();
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    Var *v = find_var(s, name);
+    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    if (nchan < 0 || inner < 1) return fail(DDS_ERR_ARG, "bad normalization layout (nchan >= 0, inner >= 1)");
+    if (nchan > 0 && (!mean || !std)) return fail(DDS_ERR_ARG, "null normalization table");
+    // (both factors are bounded by disp before they are multiplied: no overflow, and the pattern stays below 2^31)
+    if (nchan > 0 && (nchan > v->disp || inner > v->disp || v->disp % (nchan * inner) != 0))
+        return fail(DDS_ERR_ARG, "nchan * inner must divide the row's element count (disp " + std::to_string(v->disp) + ")");
+    CU(cudaSetDevice(s->device));
+    if (s->pending) dds_batch_wait(s, nullptr, nullptr);
+    CU(device_sync(s)); // no queued launch may still be reading the old tables
+    if (v->d_norm) cudaFree(v->d_norm);
+    v->d_norm = nullptr;
+    v->norm_nchan = 0;
+    v->norm_inner = 1;
+    if (nchan == 0) return DDS_OK;
+    // mean and std are interleaved into {mean, std} pairs: an element's channel is ONE 8-byte load
+    CU(cudaMalloc((void **)&v->d_norm, (size_t)nchan * 8));
+    const cudaMemcpyKind kind = tables_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    CU(cudaMemcpy2DAsync(v->d_norm, 8, mean, 4, 4, (size_t)nchan, kind, s->stream));
+    CU(cudaMemcpy2DAsync(v->d_norm + 1, 8, std, 4, 4, (size_t)nchan, kind, s->stream));
+    CU(cudaStreamSynchronize(s->stream));
+    v->norm_nchan = nchan;
+    v->norm_inner = inner;
     return DDS_OK;
 }
 

@@ -17,7 +17,7 @@ from libcpp cimport bool as cbool
 import numpy as np
 
 from ddstore_b200.comm import as_dds_comm
-from ddstore_b200.store import _Buf, _conversion, _i64
+from ddstore_b200.store import _Buf, _conversion, _i64, _norm_tables, _ptr
 
 cdef extern from *:
     """
@@ -48,6 +48,8 @@ cdef extern from "ddstore_b200.hpp" nogil:
         long get_batch_convert(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                                void* dst, long cap, int code, const void* lut, long* offsets, cbool idx_on_device,
                                void* stream) except +dds_translate_exception
+        void set_normalization(string name, const float* mean, const float* std, long nchan, long inner,
+                               cbool tables_on_device) except +dds_translate_exception
         void epoch_begin() except +dds_translate_exception
         void epoch_end() except +dds_translate_exception
         void free() except +dds_translate_exception
@@ -119,15 +121,18 @@ cdef class PyDDStore:
                 else: self.c_ddstore.get[long](nm, start, count, <long*> p)
 
     def get_batch(self, str name, starts, counts=None, out=None, count=None, offsets=None, stream=None, src_dtype=None,
-                  lut=None):
+                  lut=None, normalize=False):
         """one kernel launch for len(starts) requests, packed in request order into `out`; see
         ddstore_b200.store.PyDDStore.get_batch. `out` decides the element width checked against the variable.
-        src_dtype / lut: deliver the rows converted to out.dtype (a CUDA tensor), as in ddstore_b200's get_batch."""
+        src_dtype / lut: deliver the rows converted to out.dtype (a CUDA tensor), as in ddstore_b200's get_batch;
+        normalize=True: normalised with the tables of set_normalization, as there."""
         if out is None:
             raise ValueError("get_batch needs an `out` buffer")
         cv = None
+        if normalize and src_dtype is None:
+            raise ValueError("normalize=True needs src_dtype")
         if src_dtype is not None:
-            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut)
+            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
         ob = _Buf(out, writable=True, half_ok=cv is not None)
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
         if cv is not None:
@@ -197,6 +202,17 @@ cdef class PyDDStore:
                                                      code, <const void*> lp, <long*> op, idx_dev, <void*> st)
         del keep, lut_keep
         return total
+
+    def set_normalization(self, str name, mean, std, long inner=1):
+        """per-channel normalisation of `name` for normalize=True batches; see ddstore_b200.store.PyDDStore.set_normalization"""
+        m, s, n, dev = _norm_tables(mean, std)
+        cdef size_t mp = _ptr(m) if n else 0, sp = _ptr(s) if n else 0
+        cdef long nchan = n
+        cdef cbool on_dev = bool(dev)
+        cdef string nm = name.encode()
+        with nogil:
+            self.c_ddstore.set_normalization(nm, <const float*> mp, <const float*> sp, nchan, inner, on_dev)
+        del m, s
 
     def epoch_begin(self):
         with nogil:

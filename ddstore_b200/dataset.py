@@ -28,6 +28,15 @@ def nsplit(a, n):
     return (a[i * k + min(i, m):(i + 1) * k + min(i + 1, m)] for i in range(n))
 
 
+def _norm_spec(spec):
+    """(mean, std[, inner]) of a dataset's `normalize` -> set_normalization's (mean, std, inner); lists become float32"""
+    if not isinstance(spec, (tuple, list)) or len(spec) not in (2, 3):
+        raise ValueError("normalize takes (mean, std) or (mean, std, inner)")
+    def f32(t):
+        return t if torch.is_tensor(t) or isinstance(t, np.ndarray) else np.asarray(t, dtype=np.float32).reshape(-1)
+    return f32(spec[0]), f32(spec[1]), int(spec[2]) if len(spec) == 3 else 1
+
+
 class DistDataset(Dataset):
     """Fixed-shape samples + integer labels, sharded over the ranks of `comm` by contiguous blocks.
 
@@ -37,9 +46,14 @@ class DistDataset(Dataset):
     gather (float32 -> bfloat16 / float16, float64 -> float32, uint8 -> bfloat16 / float16 / float32 through `lut`, 256
     entries of out_dtype, default the plain value cast); the labels are never converted. The per-sample get() keeps
     the stored dtype.
+    normalize=(mean, std[, inner]): batches deliver (x - mean[ch]) / std[ch] per channel, computed in float32 inside the
+    gather (see PyDDStore.set_normalization for the channel rule), as out_dtype (default float32). A uint8 source is
+    decoded through `lut` (256 float32 entries, default the plain value: pass torch.arange(256).float().div(255) for
+    ToTensor() + Normalize()). The labels are never normalised.
     """
 
-    def __init__(self, data, label, comm=None, ddstore_width=None, device=None, local_only=False, out_dtype=None, lut=None):
+    def __init__(self, data, label, comm=None, ddstore_width=None, device=None, local_only=False, out_dtype=None, lut=None,
+                 normalize=None):
         super().__init__()
         self.label = label
         self.comm = as_dds_comm(comm)
@@ -74,12 +88,15 @@ class DistDataset(Dataset):
         self.dtype = torch.from_numpy(arr[:0]).dtype
         self._np_dtype = arr.dtype
         # batch dtype: the stored one, or out_dtype converted in the gather (src_dtype = what the gather converts from)
-        self.src_dtype = self.dtype if out_dtype is not None else None
-        self.out_dtype = out_dtype if out_dtype is not None else self.dtype
+        self.normalize = normalize is not None
+        self.src_dtype = self.dtype if (out_dtype is not None or self.normalize) else None
+        self.out_dtype = out_dtype if out_dtype is not None else (torch.float32 if self.normalize else self.dtype)
         self.lut = lut
-        if self.src_dtype is not None:
-            _conversion(self.src_dtype, self.out_dtype, lut)  # an unsupported pair fails here, not at the first batch
+        if self.src_dtype is not None:  # an unsupported pair fails here, not at the first batch
+            _conversion(self.src_dtype, self.out_dtype, lut, self.normalize)
         self.ddstore.add(f"{self.label}data", np.ascontiguousarray(arr))
+        if self.normalize:
+            self.ddstore.set_normalization(f"{self.label}data", *_norm_spec(normalize))
         self.ddstore.add(f"{self.label}labels", np.ascontiguousarray(np.array(labels, dtype=np.int32).reshape(-1, 1)))
 
     def _allgather_int(self, v):
@@ -112,7 +129,8 @@ class DistDataset(Dataset):
         # on torch's CURRENT stream: the output tensors come from its caching allocator, whose blocks may still be in use
         # by work queued there, and the index copy + the gather are then ordered with everything the caller queued before
         st = torch.cuda.current_stream(self.device).cuda_stream
-        self.ddstore.get_batch(f"{self.label}data", idx, out=vals, count=1, stream=st, src_dtype=self.src_dtype, lut=self.lut)
+        self.ddstore.get_batch(f"{self.label}data", idx, out=vals, count=1, stream=st, src_dtype=self.src_dtype, lut=self.lut,
+                               normalize=self.normalize)
         self.ddstore.get_batch(f"{self.label}labels", idx, out=labs, count=1, stream=st)
         return vals.view((B,) + self.sample_shape), labs.view(B)
 
@@ -137,11 +155,13 @@ class RaggedDataset(Dataset):
     reference's get(name, arr, start) with count = arr.shape[0] implies (src/pyddstore.pyx:84-87).
     The (start, count) tables of ALL samples are kept on the device, so a batch needs only the sample ids."""
 
-    def __init__(self, local_arrays, local_counts, comm=None, device=None, out_dtypes=None, luts=None):
+    def __init__(self, local_arrays, local_counts, comm=None, device=None, out_dtypes=None, luts=None, normalize=None):
         """local_arrays: {name: 2-D ndarray of this rank's rows}; local_counts: {name: int64[n_local_samples]}
         out_dtypes / luts: {name: dtype} / {name: 256-entry table}: those variables' batches are delivered converted in
-        the gather (see DistDataset); their row offsets count rows as always."""
-        out_dtypes, luts = dict(out_dtypes or {}), dict(luts or {})
+        the gather (see DistDataset); their row offsets count rows as always.
+        normalize: {name: (mean, std[, inner])}: those variables are delivered normalised per channel (see DistDataset),
+        as out_dtypes[name] (default float32)."""
+        out_dtypes, luts, normalize = dict(out_dtypes or {}), dict(luts or {}), dict(normalize or {})
         super().__init__()
         self.comm = as_dds_comm(comm)
         self.rank, self.comm_size = self.comm.Get_rank(), self.comm.Get_size()
@@ -173,14 +193,17 @@ class RaggedDataset(Dataset):
             self.row_bytes[name] = arr.dtype.itemsize * int(np.prod(arr.shape[1:], dtype=np.int64))
             self.dtypes[name] = torch.from_numpy(arr[:0]).dtype
             self.widths[name] = arr.shape[1:]
-        # what the batches deliver: out_dtypes[name] converted from the stored dtype, else the stored bytes
-        self.src_dtypes = {n: (self.dtypes[n] if n in out_dtypes else None) for n in self.names}
-        self.out_dtypes = {n: out_dtypes.get(n, self.dtypes[n]) for n in self.names}
+        # what the batches deliver: out_dtypes[name] converted (or normalised) from the stored dtype, else the stored bytes
+        self.normalize = {n: n in normalize for n in self.names}
+        self.src_dtypes = {n: (self.dtypes[n] if (n in out_dtypes or self.normalize[n]) else None) for n in self.names}
+        self.out_dtypes = {n: out_dtypes.get(n, torch.float32 if self.normalize[n] else self.dtypes[n]) for n in self.names}
         self.luts = {n: luts.get(n) for n in self.names}
         self.out_row_bytes = {}
         for n in self.names:
-            if self.src_dtypes[n] is not None:
-                _conversion(self.src_dtypes[n], self.out_dtypes[n], self.luts[n])  # an unsupported pair fails here
+            if self.src_dtypes[n] is not None:  # an unsupported pair fails here
+                _conversion(self.src_dtypes[n], self.out_dtypes[n], self.luts[n], self.normalize[n])
+            if self.normalize[n]:
+                self.ddstore.set_normalization(n, *_norm_spec(normalize[n]))
             self.out_row_bytes[n] = self.row_bytes[n] // self.dtypes[n].itemsize * self.out_dtypes[n].itemsize
         self.total_ns = int(len(self.counts[self.names[0]]))
 
@@ -206,12 +229,13 @@ class RaggedDataset(Dataset):
         conv = any(d is not None for d in self.src_dtypes.values())
         if len(self.names) <= 4:
             # every variable of the batch in ONE launch (dds_get_samples_multi)
-            kw = dict(src_dtypes=[self.src_dtypes[n] for n in self.names], luts=[self.luts[n] for n in self.names]) if conv else {}
+            kw = dict(src_dtypes=[self.src_dtypes[n] for n in self.names], luts=[self.luts[n] for n in self.names],
+                      normalize=[self.normalize[n] for n in self.names]) if conv else {}
             self.ddstore.get_samples_multi(self.names, ids, bufs, offsets=offs, stream=st, **kw)
         else:
             for name, buf, off in zip(self.names, bufs, offs):
                 self.ddstore.get_samples(name, ids, out=buf, offsets=off, stream=st, src_dtype=self.src_dtypes[name],
-                                         lut=self.luts[name])
+                                         lut=self.luts[name], normalize=self.normalize[name])
         for name, buf, off, r in zip(self.names, bufs, offs, rows):
             out[name] = (buf[:r], off // self.out_row_bytes[name])
         return out
@@ -285,7 +309,7 @@ class PrefetchLoader:
             st = self.stream.cuda_stream
             # independent batches into alternating buffer sets: let consecutive launches overlap (DDS_OVERLAP)
             self.ds.ddstore.get_batch(f"{self.ds.label}data", ids, out=vals[:n], count=1, stream=st, wait=False,
-                                      overlap=True, src_dtype=self.ds.src_dtype, lut=self.ds.lut)
+                                      overlap=True, src_dtype=self.ds.src_dtype, lut=self.ds.lut, normalize=self.ds.normalize)
             self.ds.ddstore.get_batch(f"{self.ds.label}labels", ids, out=labs[:n], count=1, stream=st, wait=False,
                                       overlap=True)
             self.events[slot].record(self.stream)
@@ -381,7 +405,8 @@ class RaggedPrefetchLoader:
             self.d_ids[slot][:n].copy_(keep, non_blocking=True)
             kw = {}
             if any(d is not None for d in ds.src_dtypes.values()):  # (the uint8 buffers are viewed as out_dtypes)
-                kw = dict(src_dtypes=[ds.src_dtypes[m] for m in ds.names], luts=[ds.luts[m] for m in ds.names])
+                kw = dict(src_dtypes=[ds.src_dtypes[m] for m in ds.names], luts=[ds.luts[m] for m in ds.names],
+                          normalize=[ds.normalize[m] for m in ds.names])
             bufs = [b.view(ds.out_dtypes[m]) if kw else b for b, m in zip(self.bufs[slot], ds.names)]
             ds.ddstore.get_samples_multi(ds.names, self.d_ids[slot][:n], bufs, offsets=[o[:n + 1] for o in self.offs[slot]],
                                          stream=self.stream.cuda_stream, wait=False, overlap=True, **kw)

@@ -23,6 +23,12 @@ _TORCH_HALF = {"torch.bfloat16", "torch.float16"}
 _CVT_CODES = {("float32", "bfloat16"): _capi.CVT_F32_BF16, ("float32", "float16"): _capi.CVT_F32_F16,
               ("float64", "float32"): _capi.CVT_F64_F32, ("uint8", "bfloat16"): _capi.CVT_U8_LUT16,
               ("uint8", "float16"): _capi.CVT_U8_LUT16, ("uint8", "float32"): _capi.CVT_U8_LUT32}
+# normalising batches ((x - mean[ch]) / std[ch] in float32, then the output dtype): (source, output) -> DDS_CVT_NORM_*
+_NORM_CODES = {("float32", "float32"): _capi.CVT_NORM_F32_F32, ("float32", "bfloat16"): _capi.CVT_NORM_F32_BF16,
+               ("float32", "float16"): _capi.CVT_NORM_F32_F16, ("float64", "float32"): _capi.CVT_NORM_F64_F32,
+               ("uint8", "float32"): _capi.CVT_NORM_U8_F32, ("uint8", "bfloat16"): _capi.CVT_NORM_U8_BF16,
+               ("uint8", "float16"): _capi.CVT_NORM_U8_F16}
+_U8_NORM = (_capi.CVT_NORM_U8_F32, _capi.CVT_NORM_U8_BF16, _capi.CVT_NORM_U8_F16)
 _default_luts = {}  # output dtype name -> host table of the plain value cast, torch.arange(256).to(dtype)
 
 
@@ -36,19 +42,22 @@ def _dtype_name(dt):
     return str(np.dtype(dt))
 
 
-def _conversion(src_dtype, out_dtype, lut):
+def _conversion(src_dtype, out_dtype, lut, normalize=False):
     """-> (dds_convert_t, keepalive) of a converting batch from `src_dtype` rows into an `out_dtype` buffer. A uint8 source
-    takes `lut` (256 entries of the output dtype; default: the plain value cast torch.arange(256).to(out_dtype))."""
+    takes `lut` (256 entries of the output dtype; default: the plain value cast torch.arange(256).to(out_dtype)).
+    normalize=True: the normalising conversion ((x - mean) / std per channel, see set_normalization); a uint8 source then
+    decodes through 256 float32 entries (default torch.arange(256).float())."""
     import torch
     key = (_dtype_name(src_dtype), _dtype_name(out_dtype))
-    code = _CVT_CODES.get(key)
+    code = (_NORM_CODES if normalize else _CVT_CODES).get(key)
     if code is None:
-        raise ValueError(f"unsupported conversion {key[0]} -> {key[1]}")
-    if code not in (_capi.CVT_U8_LUT16, _capi.CVT_U8_LUT32):
+        raise ValueError(f"unsupported {'normalising ' if normalize else ''}conversion {key[0]} -> {key[1]}")
+    if code not in (_capi.CVT_U8_LUT16, _capi.CVT_U8_LUT32) + _U8_NORM:
         if lut is not None:
             raise ValueError("a table (lut) applies to uint8 sources only")
         return _capi.Convert(code, None), None
-    tdt = getattr(torch, key[1])
+    tdt = torch.float32 if normalize else getattr(torch, key[1])
+    key = (key[0], "float32") if normalize else key
     if lut is None:
         host = _default_luts.get(key[1])
         if host is None:
@@ -59,6 +68,31 @@ def _conversion(src_dtype, out_dtype, lut):
             raise ValueError(f"lut must hold 256 entries of {tdt}")
         host = _lut_bits(t)
     return _capi.Convert(code, host.ctypes.data), host
+
+
+def _norm_tables(mean, std):
+    """(mean, std) of set_normalization -> (mean, std, nchan, on_device), both 1-D float32 of one length and residency"""
+    def info(t, what):
+        if isinstance(t, np.ndarray):
+            if t.dtype != np.float32 or t.ndim != 1:
+                raise ValueError(f"{what} must be a 1-D float32 array")
+            return np.ascontiguousarray(t), t.size, 0
+        if hasattr(t, "data_ptr") and hasattr(t, "element_size"):
+            if str(t.dtype) != "torch.float32" or t.dim() != 1:
+                raise ValueError(f"{what} must be a 1-D float32 tensor")
+            return t.contiguous(), t.numel(), 1 if t.is_cuda else 0
+        raise TypeError(f"{what}: unsupported array type {type(t).__name__}")
+    m, nm, dm = info(mean, "mean")
+    s, ns, ds = info(std, "std")
+    if nm != ns:
+        raise ValueError(f"mean and std differ in length ({nm} != {ns})")
+    if dm != ds:
+        raise ValueError("mean and std must both be on the host or both on the device")
+    return m, s, nm, dm
+
+
+def _ptr(t):
+    return t.ctypes.data if isinstance(t, np.ndarray) else t.data_ptr()
 
 
 def _lut_bits(t):
@@ -189,7 +223,7 @@ class PyDDStore:
 
     # ---------------------------------------------------------------- the batched hot path
     def get_batch(self, name, starts, counts=None, out=None, count=None, offsets=None, stream=None, wait=True,
-                  overlap=False, src_dtype=None, lut=None):
+                  overlap=False, src_dtype=None, lut=None, normalize=False):
         """Fetch len(starts) requests in ONE kernel launch, packed back to back in request order.
 
         starts/counts: int64 index arrays (host ndarray/list, or CUDA int64 tensors). counts=None means
@@ -212,12 +246,17 @@ class PyDDStore:
         out.dtype inside the gather: float32 -> bfloat16 / float16, float64 -> float32, uint8 -> bfloat16 / float16 /
         float32 through `lut` (256 entries of out.dtype; default torch.arange(256).to(out.dtype)). The capacity, the
         offsets and the returned size are then in bytes of `out`.
+        normalize=True (with src_dtype): deliver (x - mean[ch]) / std[ch], computed in float32 with the tables registered
+        by set_normalization, as out.dtype: float32 -> float32 / bfloat16 / float16, float64 -> float32, uint8 -> float32 /
+        bfloat16 / float16 (decoded through `lut`, 256 float32 entries, default torch.arange(256).float()).
         """
         if out is None:
             raise ValueError("get_batch needs an `out` buffer (like get(), it never allocates)")
         cv = lut_keep = None
+        if normalize and src_dtype is None:
+            raise ValueError("normalize=True needs src_dtype")
         if src_dtype is not None:
-            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut)
+            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
         else:
             itemsize = self._itemsize.get(name)
             if itemsize is None:
@@ -296,13 +335,25 @@ class PyDDStore:
         _capi.raise_for(self._L.dds_set_sample_index(self._h, name.encode(), sp, cp, n, 1 if dev else 0))
         del keep
 
+    def set_normalization(self, name, mean, std, inner=1):
+        """Register the per-channel normalisation of variable `name` for batches fetched with normalize=True: element e
+        of a row is in channel (e // inner) % len(mean) and becomes (x - mean[ch]) / std[ch]. mean / std: 1-D float32
+        arrays of one length (ndarray or tensor, host or CUDA), copied. One value: a scalar; disp values with inner=1:
+        per feature; C values with inner=H*W: a CHW image. Empty tables remove the normalisation. Local to this rank."""
+        m, s, n, dev = _norm_tables(mean, std)
+        _capi.raise_for(self._L.dds_set_normalization(self._h, name.encode(), _ptr(m) if n else None,
+                                                      _ptr(s) if n else None, n, int(inner), dev))
+        del m, s
+
     def get_samples(self, name, sample_ids, out, offsets=None, stream=None, wait=True, overlap=False, src_dtype=None,
-                    lut=None):
+                    lut=None, normalize=False):
         """get_batch by SAMPLE ID: the id -> (start, count) lookup runs inside the launch, against the index
         registered with set_sample_index. Same packing / offsets / error behaviour, and conversions, as get_batch."""
         cv = lut_keep = None
+        if normalize and src_dtype is None:
+            raise ValueError("normalize=True needs src_dtype")
         if src_dtype is not None:
-            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut)
+            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
         else:
             itemsize = self._itemsize.get(name)
             if itemsize is None:
@@ -336,20 +387,29 @@ class PyDDStore:
         return total.value
 
     def get_samples_multi(self, names, sample_ids, outs, offsets=None, stream=None, wait=True, overlap=False,
-                          src_dtypes=None, luts=None):
+                          src_dtypes=None, luts=None, normalize=None):
         """The rows of the same samples in several variables (<= 4, each with a sample index) in ONE launch:
         outs[v] (CUDA tensors) receive variable names[v]'s packed rows, offsets[v] (optional int64 CUDA tensors of
         len(ids)+1) the per-sample byte offsets. Returns the list of packed sizes (None when wait=False).
         src_dtypes[v] / luts[v]: variable v delivered converted to outs[v].dtype, as in get_batch (None: raw bytes);
-        its offsets and size are then in bytes of outs[v]."""
+        its offsets and size are then in bytes of outs[v]. normalize[v] (with src_dtypes[v]): variable v normalised, as
+        in get_batch."""
         nv = len(names)
         cvs = None
+        if normalize is not None:
+            normalize = [bool(x) for x in normalize]
+            if len(normalize) != nv:
+                raise ValueError("normalize needs one entry per variable")
+            if any(nz and (src_dtypes is None or src_dtypes[v] is None) for v, nz in enumerate(normalize)):
+                raise ValueError("a normalised variable needs its src_dtypes entry")
+        else:
+            normalize = [False] * nv
         if src_dtypes is not None:
             luts = [None] * nv if luts is None else list(luts)
             if len(src_dtypes) != nv or len(luts) != nv:
                 raise ValueError("src_dtypes / luts need one entry per variable")
-            pairs = [(_capi.Convert(_capi.CVT_NONE, None), None) if sd is None else _conversion(sd, getattr(o, "dtype", None), lt)
-                     for sd, o, lt in zip(src_dtypes, outs, luts)]
+            pairs = [(_capi.Convert(_capi.CVT_NONE, None), None) if sd is None else _conversion(sd, getattr(o, "dtype", None), lt, nz)
+                     for sd, o, lt, nz in zip(src_dtypes, outs, luts, normalize)]
             cvs = (_capi.Convert * nv)(*[c for c, _ in pairs])
             lut_keep = [k for _, k in pairs]
         obs = [_Buf(o, writable=True, half_ok=cvs is not None and src_dtypes[v] is not None) for v, o in enumerate(outs)]

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define DDS_VERSION 110 /* 110: converting batches (dds_get_batch_convert & co.) */
+#define DDS_VERSION 111 /* 110: converting batches (dds_get_batch_convert & co.); 111: normalising conversions */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -201,10 +201,35 @@ int dds_get_samples_multi(dds_store_t *s, int nvars, const char *const *names, c
 #define DDS_CVT_F64_F32 3
 #define DDS_CVT_U8_LUT16 4
 #define DDS_CVT_U8_LUT32 5
+/* Normalising conversions: every element x of a delivered row becomes
+ *   y   = __fdiv_rn(__fsub_rn(decode(x), mean[ch]), std[ch])   (f32, two IEEE roundings, no contraction)
+ *   out = encode(y)                                              (f32 as is, cvt.rn.bf16.f32 or cvt.rn.f16.f32)
+ * with mean / std / the channel rule registered for the variable by dds_set_normalization. decode: f32 as is, f64 by
+ * cvt.rn.f32.f64, uint8 through `lut`, 256 FLOAT32 entries (required; {0, 1, ..., 255} is the plain value, {k / 255.f}
+ * that of ToTensor()). The result is bit-exact with torch's ((x.to(float32) - mean_t) / std_t).to(out_dtype) on CUDA
+ * for CUDA float32 tensors mean_t / std_t laid out by the channel rule. Capacity, offsets, totals and every error rule
+ * are those of the plain conversions with the same itemsizes, plus DDS_ERR_ARG for a variable without a registered
+ * normalisation (checked before the itemsize). They may be mixed with plain and raw variables in dds_get_samples_multi_convert.
+ *   code                     source -> output   table */
+#define DDS_CVT_NORM_F32_F32 6  /* 4 -> 4 */
+#define DDS_CVT_NORM_F32_BF16 7 /* 4 -> 2 */
+#define DDS_CVT_NORM_F32_F16 8  /* 4 -> 2 */
+#define DDS_CVT_NORM_F64_F32 9  /* 8 -> 4 */
+#define DDS_CVT_NORM_U8_F32 10  /* 1 -> 4   256 f32 */
+#define DDS_CVT_NORM_U8_BF16 11 /* 1 -> 2   256 f32 */
+#define DDS_CVT_NORM_U8_F16 12  /* 1 -> 2   256 f32 */
 typedef struct {
     int32_t code;    /* DDS_CVT_* */
-    const void *lut; /* host pointer to 256 table entries (LUT codes only) */
+    const void *lut; /* host pointer to 256 table entries (LUT and uint8 normalising codes only) */
 } dds_convert_t;
+/* The per-channel normalisation of a variable, for the DDS_CVT_NORM_* codes: nchan means and standard deviations
+ * (float32, host or device pointers), copied into device memory the store owns. Element e in [0, disp) of a row is in
+ * channel (e / inner) % nchan: nchan = 1 is one scalar, nchan = disp per feature, (C, 1) channels-last, (C, H*W) CHW.
+ * Local (not collective): the normalisation is applied on the requesting rank. nchan = 0 removes it. Like
+ * dds_set_sample_index it first completes pending batches and synchronises, so no queued batch reads replaced tables.
+ * DDS_ERR_ARG: inner < 1, nchan < 0, nchan * inner not dividing disp, or a null table. */
+int dds_set_normalization(dds_store_t *s, const char *name, const float *mean, const float *std, int64_t nchan,
+                          int64_t inner, int tables_on_device);
 int dds_get_batch_convert(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
                           int64_t fixed_count, int64_t nreq, void *dst, int64_t dst_capacity, int64_t *dst_offsets,
                           unsigned flags, void *cuda_stream, const dds_convert_t *cvt, int64_t *total_bytes,

@@ -99,6 +99,12 @@ class DDStore {
                             &bad));
         return (long)total;
     }
+    // The per-channel normalisation of variable `name` for the DDS_CVT_NORM_* codes (dds_set_normalization): nchan
+    // means and standard deviations, element e of a row in channel (e / inner) % nchan. nchan = 0 removes it.
+    void set_normalization(std::string name, const float *mean, const float *std, long nchan, long inner = 1,
+                           bool tables_on_device = false) {
+        check(dds_set_normalization(store_, name.c_str(), mean, std, nchan, inner, tables_on_device ? 1 : 0));
+    }
     // The same batch delivered converted (dds_get_batch_convert): `code` is a DDS_CVT_* code, `lut` a host table of 256
     // entries for the LUT codes (copied by the call). dst / dst_offsets are device memory; the capacity, the offsets and
     // the result are in OUTPUT bytes. idx_on_device: starts / counts are device pointers.
