@@ -235,7 +235,11 @@ struct dds_store {
     // row were chained on the pending stream right before it (0: the next one starts a new run)
     unsigned int ovl_seq = 1;
     int run_len = 0;
-    unsigned int queue_len = 0; // launches in the current queue of DDS_NO_SYNC batches (saturates at 0xFFFF)
+    unsigned int queue_len = 0; // launches in the current queue of DDS_NO_SYNC batches (< kQueueMax, see tag_launch)
+    // outcome of queues completed by calls other than dds_batch_wait (drain_pending), reported by the next
+    // dds_batch_wait: the first failing status word in queue order, and the total of the last batch queued
+    unsigned long long kept_status = DDSK_STATUS_OK;
+    int64_t kept_total = 0;
     // plan scratch slots of overlapped variable-count batches: launch q plans into slot q & 3, so its plan kernels can
     // run while the gather of launch q-1 is still reading slot (q-1) & 3
     struct Slot {
@@ -729,13 +733,52 @@ int64_t cvt_to_out(int64_t p, int code) {
 // number of elements); saturates
 int64_t cvt_cap_to_src(int64_t cap, int code) { return sat_mul(cap >> cvt_out_log2(code), (int64_t)1 << cvt_in_log2(code)); }
 
+// The device status word is sticky (kernels only atomicMin into it): re-arm it after an error was read.
+void rearm_status(dds_store *s, cudaStream_t stream) {
+    if (s->push.ready) // the owners report errors of a pushed batch into this rank's window
+        cudaMemsetAsync(s->push.table.win[s->push.table.me] + 24, 0xFF, 8, stream);
+    cudaMemsetAsync(s->scr.status, 0xFF, 8, stream);
+    cudaStreamSynchronize(stream);
+}
+
+// Complete the pending queue of DDS_NO_SYNC batches without reporting its outcome: dds_batch_wait alone reports it,
+// once. The queue's first failure is kept unless an earlier one already is (that one is earlier in queue order), and
+// so is the total of its last batch. Every call that must complete a queue before its own work comes through here,
+// and then reports only its own outcome. Returns nothing but a CUDA error of the drain itself.
+int drain_pending(dds_store *s) {
+    if (!s->pending) return DDS_OK;
+    s->pending = false;
+    s->run_len = 0;
+    cudaStream_t st = s->pending_stream;
+    // queued launches skip the host mirror (it costs time at the end of every kernel): read the words back here
+    CU(cudaMemcpyAsync(&s->h_status[0], s->scr.status, 8, cudaMemcpyDeviceToHost, st));
+    if (s->pending_fixed_total < 0 && s->pending_total_ptr)
+        CU(cudaMemcpyAsync(&s->h_status[1], s->pending_total_ptr, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    s->kept_total = s->pending_fixed_total >= 0 ? s->pending_fixed_total : cvt_to_out((int64_t)s->h_status[1], s->pending_cvt);
+    const unsigned long long stw = s->h_status[0];
+    if (stw != DDSK_STATUS_OK) {
+        if (s->kept_status == DDSK_STATUS_OK) s->kept_status = stw;
+        rearm_status(s, st);
+    }
+    return DDS_OK;
+}
+
 // The kernels tag every status report with the launch's position in its queue of DDS_NO_SYNC batches (0 for a
 // synchronous call or the first of a queue), so the sticky word ends up holding the first failing batch in queue order.
+// The tag has 16 bits: a launch that would be the kQueueMax-th of its queue first drains the queue and starts a new one
+// (one stream synchronise per kQueueMax launches), so no two launches of a queue share a tag.
 // `chain`: the launch goes behind batches still pending on the same stream.
-void tag_launch(dds_store *s, bool chain) {
+constexpr unsigned int kQueueMax = 0xFFFF;
+int tag_launch(dds_store *s, bool chain) {
+    if (chain && s->queue_len >= kQueueMax) {
+        if (int rc = drain_pending(s)) return rc;
+        chain = false;
+    }
     const unsigned int ord = chain ? s->queue_len : 0u;
-    s->queue_len = std::min(ord + 1u, 0xFFFFu);
+    s->queue_len = ord + 1u;
     s->scr.status_tag = (unsigned long long)ord << DDSK_STATUS_ORD_SHIFT;
+    return DDS_OK;
 }
 
 int decode_status_word(unsigned long long st, int64_t *bad_index) {
@@ -756,14 +799,8 @@ int decode_status_word(unsigned long long st, int64_t *bad_index) {
     }
 }
 
-// The device status word is sticky (kernels only atomicMin into it): re-arm it after an error was read.
 int decode_status(dds_store *s, cudaStream_t stream, unsigned long long st, int64_t *bad_index) {
-    if (st != DDSK_STATUS_OK) {
-        if (s->push.ready) // the owners report errors of a pushed batch into this rank's window
-            cudaMemsetAsync(s->push.table.win[s->push.table.me] + 24, 0xFF, 8, stream);
-        cudaMemsetAsync(s->scr.status, 0xFF, 8, stream);
-        cudaStreamSynchronize(stream);
-    }
+    if (st != DDSK_STATUS_OK) rearm_status(s, stream);
     return decode_status_word(st, bad_index);
 }
 
@@ -860,6 +897,8 @@ dds_store_t *dds_create(dds_comm_t *comm, int device, int method) {
               cudaHostGetDevicePointer((void **)&s->d_small, s->h_small, 0) == cudaSuccess;
     if (const char *e = getenv("DDS_DOORBELL")) s->db_enabled = atoi(e) != 0;
     if (const char *e = getenv("DDS_DOORBELL_IDLE_US")) s->db_idle_ns = (unsigned long long)std::max(1, atoi(e)) * 1000ull;
+    // test hook: where the 22-bit plan-tag counter starts, so a test can reach its wrap (renew_plan_tags) in a few launches
+    if (const char *e = getenv("DDS_PLAN_TAG_START")) s->scr.plan_tag = (unsigned int)strtoul(e, nullptr, 0) & 0x3FFFFFu;
     if (ok && s->db_enabled) {
         ok = cudaHostAlloc((void **)&s->h_mb, sizeof(ddsk_mailbox_t), cudaHostAllocMapped) == cudaSuccess &&
              cudaHostGetDevicePointer((void **)&s->d_mb, s->h_mb, 0) == cudaSuccess &&
@@ -1205,7 +1244,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     // batch's first invalid request). Anything else drains the queue first.
     const bool chain = s->pending && no_sync && st == s->pending_stream;
     if (s->pending && !chain) {
-        if (int rc = dds_batch_wait(s, nullptr, nullptr)) return rc;
+        if (int rc = drain_pending(s)) return rc;
     }
     const int64_t R = v->kv.row_bytes;
     const bool fixed = !by_sample && counts == nullptr;
@@ -1304,7 +1343,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
         if (int rc = ensure_offs(s, nreq + 1)) return rc;
         d_offsets = s->d_offs;
     }
-    tag_launch(s, chain);
+    if (int rc = tag_launch(s, chain)) return rc;
     const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
     if (ovl) scr.total = ovl_total_word(s);
@@ -1423,7 +1462,7 @@ int dds_set_normalization(dds_store_t *s, const char *name, const float *mean, c
     if (nchan > 0 && (nchan > v->disp || inner > v->disp || v->disp % (nchan * inner) != 0))
         return fail(DDS_ERR_ARG, "nchan * inner must divide the row's element count (disp " + std::to_string(v->disp) + ")");
     CU(cudaSetDevice(s->device));
-    if (s->pending) dds_batch_wait(s, nullptr, nullptr);
+    if (int rc = drain_pending(s)) return rc;
     CU(device_sync(s)); // no queued launch may still be reading the old tables
     if (v->d_norm) cudaFree(v->d_norm);
     v->d_norm = nullptr;
@@ -1490,7 +1529,7 @@ int dds_set_sample_index(dds_store_t *s, const char *name, const int64_t *row_st
     if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
     if (nsamples < 0 || (nsamples > 0 && (!row_start || !row_count))) return fail(DDS_ERR_ARG, "bad sample index");
     CU(cudaSetDevice(s->device));
-    if (s->pending) dds_batch_wait(s, nullptr, nullptr);
+    if (int rc = drain_pending(s)) return rc;
     CU(device_sync(s)); // no queued launch may still be reading the old table
     if (v->d_tab) cudaFree(v->d_tab);
     v->d_tab = nullptr;
@@ -1598,7 +1637,7 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
     const bool chain = s->pending && no_sync && st == s->pending_stream;
     if (s->pending && !chain) {
-        if (int rc = dds_batch_wait(s, nullptr, nullptr)) return rc;
+        if (int rc = drain_pending(s)) return rc;
     }
     if (total_bytes)
         for (int v = 0; v < nvars; v++) total_bytes[v] = 0;
@@ -1639,7 +1678,7 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
         m.cap[v] = cap_src[v];
         m.offsets[v] = dst_offsets && dst_offsets[v] ? dst_offsets[v] : (stage_offs ? s->d_offs + (int64_t)v * (nreq + 1) : nullptr);
     }
-    tag_launch(s, chain);
+    if (int rc = tag_launch(s, chain)) return rc;
     const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
     ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
     if (ovl) scr.total = ovl_total_word(s);
@@ -1687,22 +1726,18 @@ int dds_get_samples_multi_convert(dds_store_t *s, int nvars, const char *const *
                       bad_index, cvts);
 }
 
-// completes a batch issued with DDS_NO_SYNC
+// completes the batches issued with DDS_NO_SYNC, and reports what every queue completed since the last call left
 int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index) {
     if (!s) return fail(DDS_ERR_ARG, "null store");
-    if (!s->pending) return DDS_OK;
-    s->pending = false;
-    s->run_len = 0;
-    CU(cudaSetDevice(s->device));
-    cudaStream_t st = s->pending_stream;
-    // queued launches skip the host mirror (it costs time at the end of every kernel): read the words back here
-    CU(cudaMemcpyAsync(&s->h_status[0], s->scr.status, 8, cudaMemcpyDeviceToHost, st));
-    if (s->pending_fixed_total < 0 && s->pending_total_ptr)
-        CU(cudaMemcpyAsync(&s->h_status[1], s->pending_total_ptr, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (total_bytes)
-        *total_bytes = s->pending_fixed_total >= 0 ? s->pending_fixed_total : cvt_to_out((int64_t)s->h_status[1], s->pending_cvt);
-    return decode_status(s, st, s->h_status[0], bad_index);
+    if (s->pending) {
+        CU(cudaSetDevice(s->device));
+        if (int rc = drain_pending(s)) return rc;
+    }
+    const unsigned long long st = s->kept_status;
+    if (total_bytes) *total_bytes = s->kept_total;
+    s->kept_status = DDSK_STATUS_OK;
+    s->kept_total = 0;
+    return decode_status_word(st, bad_index);
 }
 
 int dds_get(dds_store_t *s, const char *name, int64_t start, int64_t count, int itemsize, void *buffer,
@@ -1793,10 +1828,10 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
     CU(cudaSetDevice(s->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
     if (s->pending && st != s->pending_stream) {
-        if (int rc = dds_batch_wait(s, nullptr, nullptr)) return rc;
+        if (int rc = drain_pending(s)) return rc;
     }
     s->run_len = 0;
-    tag_launch(s, s->pending);
+    if (int rc = tag_launch(s, s->pending)) return rc;
     const unsigned long long step = ++s->push.step;
     if (ddsk_gather_push(&v->kv, &s->push.table, s->push.d_table, starts_dev, fixed_count, nreq, step, &s->scr, st))
         return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
@@ -1846,7 +1881,7 @@ int dds_epoch_end(dds_store_t *s) {
     for (auto &x : s->vars)
         if (!x.second.fence_active) return fail(DDS_ERR_FENCE_INACTIVE);
     CU(cudaSetDevice(s->device));
-    if (s->pending) dds_batch_wait(s, nullptr, nullptr);
+    if (int rc = drain_pending(s)) return rc;
     CU(cudaStreamSynchronize(s->stream));
     if (int rc = drain_update_streams(s)) return rc;
     if (int rc = dds_comm_barrier(s->comm)) return rc;
@@ -1864,7 +1899,7 @@ int dds_free(dds_store_t *s) {
     if (!s) return fail(DDS_ERR_ARG, "null store");
     if (s->vars.empty() && s->zombies.empty() && s->zombie_blocks.empty()) return DDS_OK;
     CU(cudaSetDevice(s->device));
-    if (s->pending) dds_batch_wait(s, nullptr, nullptr);
+    if (int rc = drain_pending(s)) return rc;
     s->update_streams.clear();
     CU(device_sync(s));
     int rc = dds_comm_barrier(s->comm); // nobody is reading any more

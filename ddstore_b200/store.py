@@ -456,7 +456,14 @@ class PyDDStore:
         return C.c_void_p(h if h != 0 else 1)
 
     def wait(self):
-        """complete the batches queued with wait=False; raises like get_batch; returns packed bytes of the last"""
+        """Complete the batches queued with wait=False; raises like get_batch for the earliest failing batch in queue
+        order (last_bad_index: its first invalid request); returns the packed bytes of the last batch queued since the
+        previous wait() (0 if none).
+        wait() alone reports the outcome of queued batches, exactly once. Any other call that meets a pending queue
+        (a synchronous get_batch / get / get_samples / get_samples_multi, a batch on another stream, set_sample_index,
+        set_normalization, epoch_end, free) completes it, keeps its first failure for the next wait(), and raises only
+        for its own requests. A failure kept from earlier wins over later ones; after wait() has raised it, the next
+        wait() is clean. close() drops an outcome no wait() has reported."""
         total, bad = C.c_int64(0), C.c_int64(-1)
         rc = self._L.dds_batch_wait(self._h, C.byref(total), C.byref(bad))
         self.last_bad_index = bad.value

@@ -144,7 +144,8 @@ int dds_get(dds_store_t *s, const char *name, int64_t start, int64_t count, int 
  * (void*)0x1, for CUDA's legacy default stream). */
 #define DDS_IDX_ON_DEVICE 1u /* starts / counts are device pointers */
 #define DDS_DST_ON_DEVICE 2u /* dst / dst_offsets are device pointers */
-#define DDS_NO_SYNC 4u       /* needs both flags above: enqueue on cuda_stream and return; dds_batch_wait() reports */
+#define DDS_NO_SYNC 4u       /* needs both flags above: enqueue on cuda_stream and return; dds_batch_wait() reports,
+                              * and only it: see dds_batch_wait for how a queue of such batches ends */
 #define DDS_OVERLAP 8u       /* with DDS_NO_SYNC: this batch is INDEPENDENT of the ONE batch queued just before it on the
                               * same stream (different destination / offsets buffers; indices not produced by it), so the
                               * two may overlap: the head of this one fills the SMs the tail of the previous one vacates
@@ -258,7 +259,17 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
                        int itemsize, void **dst_out, void *cuda_stream);
 
 /* Completes the batches issued with DDS_NO_SYNC (stream sync + status decode). Of a queue of several, the earliest
- * failing batch in queue order is reported, with that batch's first invalid request in *bad_index. */
+ * failing batch in queue order is reported, with that batch's first invalid request in *bad_index.
+ * The outcome of queued batches is reported here and only here, exactly once. Any other call that meets a pending
+ * queue (a synchronous batch or get(), a batch on another stream, dds_set_sample_index, dds_set_normalization,
+ * dds_epoch_end, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
+ * then does its own work and reports only its own outcome (its error and *bad_index describe its own requests). The
+ * next dds_batch_wait reports the kept failure, with its index and text, after completing any queue still pending; a
+ * failure kept from earlier wins over any failure queued after it, since it is earlier in queue order. After it has
+ * been reported, the next call returns DDS_OK. *total_bytes is the packed size of the last batch queued since the
+ * previous dds_batch_wait, 0 if there was none. A queue reaching 65535 launches is completed the same way before its
+ * next launch (the status word's queue ordinal has 16 bits), so its failures are still reported in queue order.
+ * dds_destroy drops a kept outcome that no dds_batch_wait has reported. */
 int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index);
 
 /* void query(string name, VarInfo_t&), ddstore.cxx:46-49 */
