@@ -37,6 +37,10 @@ class Convert(C.Structure):  # dds_convert_t
     _fields_ = [("code", C.c_int32), ("lut", C.c_void_p)]
 
 
+class Pad(C.Structure):  # dds_pad_t
+    _fields_ = [("max_rows", C.c_int64), ("pad_bits", C.c_uint64), ("lengths", C.c_void_p)]
+
+
 # every symbol include/ddstore_b200.h declares: name -> (restype, argtypes)
 I64P = C.POINTER(C.c_int64)
 SIGNATURES = {
@@ -76,6 +80,11 @@ SIGNATURES = {
     "dds_get_samples_multi_convert": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.c_void_p, C.c_int64,
                                                 C.POINTER(C.c_void_p), I64P, C.POINTER(C.c_void_p), C.c_uint,
                                                 C.c_void_p, C.POINTER(Convert), I64P, I64P]),
+    "dds_get_batch_padded": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
+                                       C.POINTER(Convert), C.POINTER(Pad), C.c_void_p, C.c_int64, C.c_uint, C.c_void_p,
+                                       I64P, I64P]),
+    "dds_get_samples_padded": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(Convert),
+                                         C.POINTER(Pad), C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

@@ -355,10 +355,20 @@ struct GatherArgs {
     unsigned long long *status;
     unsigned long long status_tag; // this launch's ordinal in its queue, as OR-ed into every status report
     unsigned int *counters; // [0] segment ticket, [1] finished warps -- self-resetting, ticketed launches only
-    // multi-array batches (plan.nvars > 1): the packed result of variable v goes to mdst[v]
-    char *mdst[DDSK_MAX_MULTI];
-    int64_t mcap[DDSK_MAX_MULTI];
-    int64_t *moffsets[DDSK_MAX_MULTI]; // optional per-variable [per_var + 1] byte offsets
+    union { // (a launch is never both: the union keeps the parameter block, and the conversion behind it, where they were)
+        struct { // multi-array batches (plan.nvars > 1): the packed result of variable v goes to mdst[v]
+            char *mdst[DDSK_MAX_MULTI];
+            int64_t mcap[DDSK_MAX_MULTI];
+            int64_t *moffsets[DDSK_MAX_MULTI]; // optional per-variable [per_var + 1] byte offsets
+        };
+        struct { // padded batches (PAD). Request i = the plan's (start, count) of index i; its slot is pad_slot source
+                 // bytes (count = max_rows). See ddsk_pad_cut in kernels.h.
+            int64_t pad_slot;
+            uint64_t pad_bits;
+            int pad_log2, pad_in_log2, pad_out_log2; // output element size; source -> output position shifts
+            int64_t *pad_lengths;                    // optional [nreq] delivered row counts
+        };
+    };
     int min_seg_chunks;                // smallest segment, in chunks (claims cost more when the plan is in global memory)
     // ---- overlap protocol (DDS_OVERLAP: a batch declared independent of the ONE batch queued right before it)
     //   * fixed-count launches stride their segments statically; variable-count launches (whose CTAs may start late,
@@ -424,10 +434,57 @@ struct PlanView<0> {
     __device__ __forceinline__ int64_t d(int64_t i) const { return __ldcg(&dst[i]); }
 };
 
+// ---- padded batches: request lookup and padding fill
+// (start, count) of request idx through the plan's index (explicit arrays or the sample table), validated on the FULL
+// count (errors reported); -> source address (0: invalid) and payload bytes min(count, max_rows) * row_bytes
+__device__ __forceinline__ void pad_lookup(const GatherArgs &a, int64_t idx, uint64_t &src, int64_t &payload) {
+    const int64_t ix[1] = {idx};
+    uint64_t s[1];
+    int64_t nbytes[1];
+    plan_many<1>(a.var, a.plan, ix, a.nreq, a.status, a.status_tag, s, nbytes);
+    src = s[0];
+    payload = min(nbytes[0], a.pad_slot);
+}
+
+// the 16-byte pattern of a padding element of 1 << el bytes (dst positions are aligned to the element, so every aligned
+// 16-byte vector of padding holds this pattern)
+__device__ __forceinline__ uint4 pad_pattern(uint64_t bits, int el) {
+    uint32_t lo, hi;
+    if (el == 0) lo = hi = (uint32_t)(bits & 0xFFu) * 0x01010101u;
+    else if (el == 1) lo = hi = (uint32_t)(bits & 0xFFFFu) * 0x00010001u;
+    else if (el == 2) lo = hi = (uint32_t)bits;
+    else {
+        lo = (uint32_t)bits;
+        hi = (uint32_t)(bits >> 32);
+    }
+    return make_uint4(lo, hi, lo, hi);
+}
+__device__ __forceinline__ void pad_store1(char *d, uint64_t bits, int el) {
+    if (el == 0) *(uint8_t *)d = (uint8_t)bits;
+    else if (el == 1) *(uint16_t *)d = (uint16_t)bits;
+    else if (el == 2) *(uint32_t *)d = (uint32_t)bits;
+    else *(uint64_t *)d = bits;
+}
+// the whole warp writes n bytes (whole elements) of padding at d: element-wise head up to the first 16-byte boundary,
+// aligned 128-bit stores, element-wise tail
+__device__ __forceinline__ void pad_fill(char *d, int64_t n, uint64_t bits, int el, int lane) {
+    int64_t head = (16 - (int64_t)((uint64_t)d & 15u)) & 15;
+    if (head > n) head = n;
+    const int64_t nv = (n - head) >> 4;
+    const int64_t tail = n - head - (nv << 4);
+    if ((int64_t)lane < (head >> el)) pad_store1(d + ((int64_t)lane << el), bits, el);
+    const uint4 v = pad_pattern(bits, el);
+    char *dv = d + head;
+    for (int64_t j = lane; j < nv; j += 32) stg128(dv + (j << 4), v);
+    if ((int64_t)lane < (tail >> el)) pad_store1(dv + (nv << 4) + ((int64_t)lane << el), bits, el);
+}
+
 // VALIGN (converting multi-array launches): segment boundaries are aligned down to 8 bytes relative to the variable
 // they fall in (vb[]: the variables' starts in the concatenated packed space), so that no segment cuts a source element
 // of a variable that starts at an odd offset
-template <bool FIXED, int CH, int PCAP, bool VALIGN = false>
+// PAD (padded batches, with FIXED): slot i of the walk holds request i's payload followed by padding; the walk copies the
+// payload and each warp fills the padding of the segments it claims
+template <bool FIXED, int CH, int PCAP, bool VALIGN = false, bool PAD = false>
 struct ChunkWalker {
     // warp-uniform state
     int64_t seg_pos = 0, seg_end = 0, T = 0, seg_bytes = 0, nseg = 0, nb = 0;
@@ -458,7 +515,12 @@ struct ChunkWalker {
         w_dst = 0;
         w_n = 0;
         if (idx < nreq) {
-            if (FIXED && push_n > 0) {
+            if constexpr (PAD) {
+                int64_t payload;
+                pad_lookup(a, idx, w_src, payload);
+                w_dst = idx * nb; // the slot's start in the padded source space
+                w_n = payload;    // (the rest of the slot is padding: no piece covers it)
+            } else if (FIXED && push_n > 0) {
                 // which requester's list does virtual request idx belong to, and which entry of it?
                 int p = 0;
                 for (int k = 1; k < push_n; k++)
@@ -528,6 +590,34 @@ struct ChunkWalker {
         return lo;
     }
 
+    // PAD: write the padding of every slot the new segment [seg_pos, seg_end) covers, clipped to it, 32 slots at a time
+    // (one lookup per lane), each region by the whole warp. Padding is caller-visible: the overlap gate opens first.
+    template <typename Gate>
+    __device__ __forceinline__ void fill_pads(const GatherArgs &a, int lane, Gate &&gate) {
+        const int64_t i_end = min(nreq, (seg_end + nb - 1) / nb);
+        for (int64_t i0 = seg_pos / nb; i0 < i_end; i0 += 32) {
+            const int64_t i = i0 + lane;
+            int64_t pad_dst = 0, pad_len = 0;
+            if (i < i_end) {
+                uint64_t src;
+                int64_t payload;
+                pad_lookup(a, i, src, payload);
+                const ddsk_pad_cut_t c = ddsk_pad_cut(i, payload, nb, max(seg_pos - i * nb, (int64_t)0),
+                                                      min(seg_end - i * nb, nb), a.pad_in_log2, a.pad_out_log2);
+                pad_dst = c.pad_dst;
+                pad_len = c.pad_len;
+            }
+            unsigned todo = __ballot_sync(0xffffffffu, pad_len > 0);
+            if (todo) gate();
+            while (todo) {
+                const int j = __ffs(todo) - 1;
+                todo &= todo - 1;
+                pad_fill(a.dst + __shfl_sync(0xffffffffu, pad_dst, j), __shfl_sync(0xffffffffu, pad_len, j), a.pad_bits,
+                         a.pad_log2, lane);
+            }
+        }
+    }
+
     // Next group of the walk. Returns the bytes to expect in the stage (0: no more work); `pc` is this lane's piece.
     __device__ __forceinline__ void arm(const GatherArgs &a, int lane) { // request the ticket of the NEXT segment
         if (lane == 0) pend = atomicAdd(a.tickets, 1u);
@@ -572,8 +662,10 @@ struct ChunkWalker {
                     }
                 }
                 r = FIXED ? seg_pos / nb : locate_var(a, seg_pos, lane);
+                if constexpr (PAD) fill_pads(a, lane, gate);
             }
-            if (r >= nreq) { // defensive: cannot happen while seg_pos < T
+            // (PAD: the rest of the segment, if any, is the padding fill_pads wrote)
+            if (r >= nreq || (PAD && r * nb >= seg_end)) { // defensive without PAD: cannot happen while seg_pos < T
                 seg_pos = seg_end;
                 continue;
             }
@@ -1136,12 +1228,15 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // caller-visible offsets differ. Converting launches have no push fetch.
 // NORM (with CVT): the form of launches that carry a normalising code (DDSK_CVT_NORM_*); its drain handles every code,
 // since a multi-array launch may mix normalised, plainly converted and raw variables.
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false>
+// PAD (with FIXED): a padded batch -- a fixed-stride walk over slots of a.pad_slot source bytes (see ChunkWalker), the
+// padding filled by the warps that claim it, the lengths written after the walk. No plan, no offsets, no push fetch.
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
                                                                 const __grid_constant__ CvtParam<CVT> c) {
     static_assert(CVT || !NORM, "a normalising launch is a converting one");
+    static_assert(FIXED || !PAD, "a padded batch is a fixed-stride walk");
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
-    constexpr bool PUSH = FIXED && !CVT;
+    constexpr bool PUSH = FIXED && !CVT && !PAD;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
     __shared__ __align__(8) uint64_t full_bar[NW][S];
     __shared__ __align__(16) PieceDesc desc[NW][S][32];
@@ -1192,7 +1287,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     };
 
     // ---- the plan (variable counts) ------------------------------------------------------------
-    ChunkWalker<FIXED, CH, PCAP, CVT> w;
+    ChunkWalker<FIXED, CH, PCAP, CVT, PAD> w;
     if (!FIXED) {
         if constexpr (PCAP > 0) {
             w.pv.src_s = smem_u32(smem_dyn) + (uint32_t)(NW * S * STAGE);
@@ -1303,7 +1398,8 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     w.gate_ok = gate_open; // (variable-count overlap launches opened it together with the plan word)
     // (a fixed count above the variable's row total is invalid for every request, and count * row_bytes need not even
     //  fit in 64 bits: nothing to walk, the check pass below reports the first request)
-    w.nb = (FIXED && a.count <= a.var.lenlist[a.var.nranks - 1]) ? a.count * a.var.row_bytes : 0;
+    if constexpr (PAD) w.nb = a.pad_slot; // (max_rows * row_bytes, checked by the host: nreq * slot fits)
+    else w.nb = (FIXED && a.count <= a.var.lenlist[a.var.nranks - 1]) ? a.count * a.var.row_bytes : 0;
     w.nreq = (FIXED && push) ? push_rbase[w.push_n] : a.nreq;
     if (FIXED) w.T = w.nb * w.nreq;
     bool over = w.T > a.dst_cap;
@@ -1383,6 +1479,9 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         // short; variable-count segments are multiples of SEG_GRAIN when the segment table is in use.
         // (push fetch: finer segments were slower, because every claim costs a window of index reads from the
         // requester's list over NVLink)
+        if constexpr (PAD) {
+            w.seg_bytes = ddsk_fixed_seg_bytes(w.T, w.nb, nwarps, a.min_seg_chunks, CH);
+        } else {
         int64_t target = w.T / (nwarps * 8);
         const int64_t unit = (!FIXED && PCAP == 0) ? SEG_GRAIN : (int64_t)CH;
         target = max((int64_t)a.min_seg_chunks * CH, min(target, (int64_t)1 << 20));
@@ -1391,6 +1490,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             w.seg_bytes = (target / w.nb) * w.nb; // whole requests per segment
         else
             w.seg_bytes = (target / unit) * unit;
+        }
         w.nseg = w.T > 0 ? (w.T + w.seg_bytes - 1) / w.seg_bytes : 0;
     }
     if (over) {
@@ -1400,7 +1500,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
 
     // ---- FIXED with nothing to walk (count <= 0, or the batch does not fit): run the reference's two checks here,
     //      so an invalid request is still the error that gets reported
-    if (FIXED && !push && (w.nb <= 0 || over)) {
+    if (FIXED && !PAD && !push && (w.nb <= 0 || over)) {
         for (int64_t i = gwarp * 32 + lane; i < a.nreq; i += nwarps * 32) {
             uint64_t s;
             int code = dev_locate(a.var, a.starts[i], a.count, &s);
@@ -1546,6 +1646,16 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 for (int v = 0; v < DDSK_MAX_MULTI; v++)
                     if (v < a.plan.nvars) t += cvt_scale<NORM>((v + 1 < a.plan.nvars ? vbase[v + 1] : w.T) - vbase[v], c.code[v]);
                 *a.total_out = t;
+            }
+        }
+    }
+    if constexpr (PAD) { // delivered row counts; with max_rows = 0 nothing was walked, and this pass runs the checks
+        if (a.pad_lengths || w.nb == 0) {
+            for (int64_t i = gwarp * 32 + lane; i < a.nreq; i += nwarps * 32) {
+                uint64_t src;
+                int64_t payload;
+                pad_lookup(a, i, src, payload);
+                if (a.pad_lengths) a.pad_lengths[i] = payload / a.var.row_bytes;
             }
         }
     }
@@ -2032,12 +2142,12 @@ bool cvt_has_norm(const ddsk_cvt_t *cvt) {
     return false;
 }
 
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false>
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
     // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan)
     const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM>;
+    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -2260,6 +2370,43 @@ int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const 
     a.push_nreq = nreq;
     a.push_step = step;
     return launch_gather<true>(a, st, nullptr);
+}
+
+int ddsk_gather_padded(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, int64_t max_rows, uint64_t pad_bits,
+                       int pad_log2, int64_t *lengths, void *dst_dev, const ddsk_scratch_t *scr, int flags,
+                       const ddsk_cvt_t *cvt, void *stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
+    if (nreq <= 0) return 0;
+    if (int rc = pick_geometry()) return rc;
+    GatherArgs a;
+    memset(&a, 0, sizeof(a));
+    a.var = *var;
+    a.plan.starts = index->starts;
+    a.plan.counts = index->counts;
+    a.plan.ids = index->sample_ids;
+    a.plan.tab = (const longlong2 *)index->table;
+    a.plan.nsamples = index->nsamples;
+    a.count = max_rows;
+    a.nreq = nreq;
+    a.dst = (char *)dst_dev;
+    a.pad_slot = max_rows * var->row_bytes;
+    a.dst_cap = nreq * a.pad_slot; // (the host checked the padded size against the caller's capacity)
+    a.pad_bits = pad_bits;
+    a.pad_log2 = pad_log2;
+    a.pad_in_log2 = cvt ? cvt_in_log2<true>(cvt->code[0]) : 0;
+    a.pad_out_log2 = cvt ? cvt_out_log2<true>(cvt->code[0]) : 0;
+    a.pad_lengths = lengths;
+    a.status = scr->status;
+    a.status_tag = scr->status_tag;
+    a.counters = scr->counters;
+    a.min_seg_chunks = 1;
+    fill_overlap(a, scr, flags);
+    a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
+    // the default fixed-count geometry, whatever DDS_GATHER_GEOM says
+    if (!cvt) return launch_gather_t<true, 12, 4, 4096, 0, false, false, true>(a, st);
+    return cvt_has_norm(cvt) ? launch_gather_t<true, 12, 4, 4096, 0, true, true, true>(a, st, cvt)
+                             : launch_gather_t<true, 12, 4, 4096, 0, true, false, true>(a, st, cvt);
 }
 
 // shared by ddsk_gather_var / ddsk_gather_multi: plan (in the launch, or by the two plan kernels) + gather

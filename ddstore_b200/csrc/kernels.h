@@ -145,6 +145,59 @@ int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nr
 int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt);
 int64_t ddsk_plan_smem_max(void);
 
+/* Padded batch: request i owns a slot of max_rows rows. The walk runs over the padded SOURCE byte space [0, nreq * slot)
+ * (slot = max_rows * row_bytes) exactly like a fixed-count batch whose requests are all `slot` bytes long; the first
+ * `payload` = min(count_i, max_rows) * row_bytes bytes of slot i are rows (0 for an invalid request), the rest padding.
+ * Source position p goes to output byte (p >> in_log2) << out_log2 (0 / 0 for raw batches, the conversion's otherwise),
+ * and every padding element of the output is `pad_bits` (its low 1 << pad_log2 bytes), written verbatim. index: explicit
+ * starts AND counts, or sample ids. lengths (nullable, device): nreq delivered row counts. cvt: NULL for raw bytes. */
+int ddsk_gather_padded(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, int64_t max_rows, uint64_t pad_bits,
+                       int pad_log2, int64_t *lengths, void *dst_dev, const ddsk_scratch_t *scr, int flags,
+                       const ddsk_cvt_t *cvt, void *stream);
+
+#if defined(__CUDACC__)
+#define DDSK_HD __host__ __device__
+#else
+#define DDSK_HD
+#endif
+
+/* Segment size of a fixed-stride walk over T bytes of `nb`-byte requests by `nwarps` warps (chunk: CH; min_chunks: the
+ * smallest segment in chunks): about 8 segments per warp, at most 1 MiB, whole requests when one fits, else whole chunks.
+ * Every cut is therefore a request boundary or a multiple of CH. The padded gather uses it (tests/cpp/pad_layout_check.cpp
+ * replays it). */
+static inline DDSK_HD int64_t ddsk_fixed_seg_bytes(int64_t T, int64_t nb, int64_t nwarps, int64_t min_chunks, int64_t ch) {
+    int64_t target = T / (nwarps * 8);
+    if (target > ((int64_t)1 << 20)) target = (int64_t)1 << 20;
+    if (target < min_chunks * ch) target = min_chunks * ch;
+    if (target < ch) target = ch;
+    return (nb > 0 && nb <= target) ? (target / nb) * nb : (target / ch) * ch;
+}
+
+/* The layout of a padded batch, for a source range [lo, hi) of slot i (0 <= lo <= hi <= slot) whose first `payload`
+ * bytes are rows: which of those bytes are payload and where they go, and which OUTPUT bytes are padding. Source and
+ * output positions are absolute (from the batch's start); lengths are in source bytes for the payload, output bytes for
+ * the padding. Every cut the walk makes (slot boundaries, multiples of CH, row boundaries) is element-aligned, so the
+ * shifts are exact. */
+typedef struct ddsk_pad_cut {
+    int64_t pay_src, pay_len; /* source range [pay_src, pay_src + pay_len) of rows */
+    int64_t pay_dst;          /* its output position */
+    int64_t pad_dst, pad_len; /* output range of padding */
+} ddsk_pad_cut_t;
+static inline DDSK_HD ddsk_pad_cut_t ddsk_pad_cut(int64_t i, int64_t payload, int64_t slot, int64_t lo, int64_t hi,
+                                                  int in_log2, int out_log2) {
+    ddsk_pad_cut_t c;
+    const int64_t base = i * slot;
+    const int64_t pe = payload < hi ? payload : hi;
+    const int64_t ps = lo < pe ? lo : pe;
+    const int64_t qs = lo > payload ? lo : payload;
+    c.pay_src = base + ps;
+    c.pay_len = pe - ps;
+    c.pay_dst = ((base + ps) >> in_log2) << out_log2;
+    c.pad_dst = ((base + qs) >> in_log2) << out_log2;
+    c.pad_len = qs < hi ? ((hi - qs) >> in_log2) << out_log2 : 0;
+    return c;
+}
+
 /* Multi-array batch: the rows of the SAME nreq sample ids in nvars (<= DDSK_MAX_MULTI) variables, one launch. vars_dev =
  * device array of the variables' windows; table[v] = sample index of variable v; dst[v]/cap[v]/offsets[v] per variable
  * (offsets[v] nullable, nreq+1 entries). */

@@ -1223,6 +1223,32 @@ static int small_get(dds_store_t *s, Var *v, int64_t start, int64_t count, void 
     return decode_status_word(stw, bad_index);
 }
 
+// The indices of a batch as the kernels read them (counts: NULL when the batch has none of its own). Host indices:
+// few requests are read by the kernel straight from pinned host memory (no H2D copy to wait for), more are copied on
+// `st` into the store's index arrays.
+static int stage_indices(dds_store_t *s, const int64_t *starts, const int64_t *counts, int64_t nreq, bool idx_dev,
+                         cudaStream_t st, const int64_t **d_starts, const int64_t **d_counts) {
+    if (idx_dev) return DDS_OK;
+    if (nreq <= kSmallIdx) {
+        int64_t *hs = (int64_t *)s->h_small, *hc = hs + kSmallIdx;
+        memcpy(hs, starts, (size_t)nreq * 8);
+        *d_starts = (const int64_t *)s->d_small;
+        if (counts) {
+            memcpy(hc, counts, (size_t)nreq * 8);
+            *d_counts = (const int64_t *)s->d_small + kSmallIdx;
+        }
+        return DDS_OK;
+    }
+    if (int rc = ensure_idx(s, nreq)) return rc;
+    CU(cudaMemcpyAsync(s->d_starts, starts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
+    *d_starts = s->d_starts;
+    if (counts) {
+        CU(cudaMemcpyAsync(s->d_counts, counts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
+        *d_counts = s->d_counts;
+    }
+    return DDS_OK;
+}
+
 // The one batched path behind dds_get_batch / dds_get_samples / dds_get.
 //   by_sample == false: request i = (starts[i], counts ? counts[i] : fixed_count)
 //   by_sample == true : request i = the rows of sample starts[i] (= sample id) in v's per-sample index
@@ -1274,24 +1300,8 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
 
     // ---- indices to the device (8-16 B per request)
     const int64_t *d_starts = starts, *d_counts = counts;
-    if (!idx_dev && nreq <= kSmallIdx) {
-        // few requests: the kernel reads the indices straight from pinned host memory (no H2D copy to wait for)
-        int64_t *hs = (int64_t *)s->h_small, *hc = hs + kSmallIdx;
-        memcpy(hs, starts, (size_t)nreq * 8);
-        d_starts = (const int64_t *)s->d_small;
-        if (!fixed && !by_sample) {
-            memcpy(hc, counts, (size_t)nreq * 8);
-            d_counts = (const int64_t *)s->d_small + kSmallIdx;
-        }
-    } else if (!idx_dev) {
-        if (int rc = ensure_idx(s, nreq)) return rc;
-        CU(cudaMemcpyAsync(s->d_starts, starts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
-        d_starts = s->d_starts;
-        if (!fixed && !by_sample) {
-            CU(cudaMemcpyAsync(s->d_counts, counts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
-            d_counts = s->d_counts;
-        }
-    }
+    if (int rc = stage_indices(s, starts, !fixed && !by_sample ? counts : nullptr, nreq, idx_dev, st, &d_starts, &d_counts))
+        return rc;
 
     // ---- packed size as far as the host can know it
     int64_t upper = -1; // upper bound of the packed bytes (== total when every request is valid)
@@ -1593,6 +1603,112 @@ int dds_get_samples_convert(dds_store_t *s, const char *name, const int64_t *sam
     if (!v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
     return batch_impl(s, v, true, sample_ids, nullptr, 0, nreq, dst, dst_capacity, dst_offsets, flags, cuda_stream,
                       total_bytes, bad_index, &kc);
+}
+
+// The padded path behind dds_get_batch_padded / dds_get_samples_padded (by_sample: starts = sample ids, counts unused;
+// cvt: the checked conversion, or NULL for raw bytes). Every argument is checked before anything is enqueued.
+static int padded_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts, int64_t nreq,
+                       const ddsk_cvt_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity, unsigned flags,
+                       void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    if (!pad) return fail(DDS_ERR_ARG, "null padding");
+    if (nreq < 0 || dst_capacity < 0) return fail(DDS_ERR_ARG, "negative nreq or capacity");
+    if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
+    if (!by_sample && nreq > 0 && !counts)
+        return fail(DDS_ERR_ARG, "padded batches need counts (there is no fixed-count form)");
+    if (!(flags & DDS_DST_ON_DEVICE)) return fail(DDS_ERR_ARG, "padded batches deliver into device memory");
+    const bool idx_dev = flags & DDS_IDX_ON_DEVICE, no_sync = flags & DDS_NO_SYNC;
+    if (no_sync && !idx_dev) return fail(DDS_ERR_ARG, "async batches need device indices and a device destination");
+    int out_log2 = cvt ? cvt_out_log2(cvt->code[0]) : -1;
+    if (!cvt)
+        for (int l = 0; l <= 3; l++)
+            if (v->itemsize == 1 << l) out_log2 = l;
+    if (out_log2 < 0) return fail(DDS_ERR_ARG, "padded batches need an itemsize of 1, 2, 4 or 8");
+    if ((uint64_t)dst % (uint64_t)(1 << out_log2) || (uint64_t)pad->lengths % 8u)
+        return fail(DDS_ERR_ARG, "destination not aligned to the output itemsize (or lengths to 8 bytes)");
+    if (pad->max_rows < 0) return fail(DDS_ERR_ARG, "max_rows < 0");
+    // slot sizes in source and output bytes, and the batch in both: the walk runs over nreq * src_slot
+    int64_t slot = 0, src_slot = 0, total = 0, src_total = 0;
+    if (__builtin_mul_overflow(pad->max_rows, (int64_t)v->disp << out_log2, &slot) ||
+        __builtin_mul_overflow(pad->max_rows, v->kv.row_bytes, &src_slot) || __builtin_mul_overflow(nreq, slot, &total) ||
+        __builtin_mul_overflow(nreq, src_slot, &src_total))
+        return fail(DDS_ERR_ARG, "the padded batch's size overflows");
+    if (dst_capacity < total)
+        return fail(DDS_ERR_ARG, "destination holds " + std::to_string(dst_capacity) + " bytes, the padded batch " +
+                                     std::to_string(total));
+    if (total > 0 && !dst) return fail(DDS_ERR_ARG, "null destination");
+    if (by_sample && !v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
+
+    CU(cudaSetDevice(s->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
+    const bool chain = s->pending && no_sync && st == s->pending_stream;
+    if (s->pending && !chain) {
+        if (int rc = drain_pending(s)) return rc;
+    }
+    if (nreq == 0) return DDS_OK;
+    const int64_t *d_starts = starts, *d_counts = counts;
+    if (int rc = stage_indices(s, starts, by_sample ? nullptr : counts, nreq, idx_dev, st, &d_starts, &d_counts)) return rc;
+    ddsk_index_t ix;
+    memset(&ix, 0, sizeof(ix));
+    if (by_sample) {
+        ix.sample_ids = d_starts;
+        ix.table = v->d_tab;
+        ix.nsamples = v->nsamples;
+    } else {
+        ix.starts = d_starts;
+        ix.counts = d_counts;
+    }
+    if (int rc = tag_launch(s, chain)) return rc;
+    const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, no_sync && (flags & DDS_OVERLAP), chain);
+    ddsk_scratch_t scr = scratch_view(s, false);
+    if (ddsk_gather_padded(&v->kv, &ix, nreq, pad->max_rows, pad->pad_bits, out_log2, pad->lengths, dst, &scr, kflags, cvt, st))
+        return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
+    s->pending_fixed_total = total;
+    s->pending_cvt = DDSK_CVT_NONE;
+    s->pending_nreq = nreq;
+    if (total_bytes) *total_bytes = total;
+    if (no_sync) {
+        s->pending = true;
+        s->pending_stream = st;
+        return DDS_OK;
+    }
+    CU(cudaStreamSynchronize(st)); // status arrives in the pinned mirror word with the end of the kernel
+    return decode_status(s, st, s->h_status[0], bad_index);
+}
+
+// the checks the padded entries share with the raw and the converting ones: the itemsize, and the conversion if any
+static int padded_args(Var *v, int itemsize, const dds_convert_t *cvt, ddsk_cvt_t *kc) {
+    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
+    return cvt ? make_cvt(&v, cvt, 1, false, kc) : DDS_OK;
+}
+
+int dds_get_batch_padded(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts, int64_t nreq,
+                         int itemsize, const dds_convert_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity,
+                         unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    clear_error();
+    if (bad_index) *bad_index = -1;
+    if (total_bytes) *total_bytes = 0;
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    Var *v = find_var(s, name);
+    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    ddsk_cvt_t kc;
+    if (int rc = padded_args(v, itemsize, cvt, &kc)) return rc;
+    return padded_impl(s, v, false, starts, counts, nreq, cvt ? &kc : nullptr, pad, dst, dst_capacity, flags, cuda_stream,
+                       total_bytes, bad_index);
+}
+
+int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
+                           const dds_convert_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity, unsigned flags,
+                           void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    clear_error();
+    if (bad_index) *bad_index = -1;
+    if (total_bytes) *total_bytes = 0;
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    Var *v = find_var(s, name);
+    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    ddsk_cvt_t kc;
+    if (int rc = padded_args(v, itemsize, cvt, &kc)) return rc;
+    return padded_impl(s, v, true, sample_ids, nullptr, nreq, cvt ? &kc : nullptr, pad, dst, dst_capacity, flags,
+                       cuda_stream, total_bytes, bad_index);
 }
 
 // The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,

@@ -13,11 +13,12 @@ Differences from the reference binding, all at the edges:
 """
 from libcpp.string cimport string
 from libcpp cimport bool as cbool
+from libc.stdint cimport uint64_t
 
 import numpy as np
 
 from ddstore_b200.comm import as_dds_comm
-from ddstore_b200.store import _Buf, _conversion, _i64, _norm_tables, _ptr
+from ddstore_b200.store import _Buf, _conversion, _dtype_name, _i64, _norm_tables, _pad_bits, _ptr
 
 cdef extern from *:
     """
@@ -48,6 +49,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
         long get_batch_convert(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                                void* dst, long cap, int code, const void* lut, long* offsets, cbool idx_on_device,
                                void* stream) except +dds_translate_exception
+        long get_batch_padded_convert(string name, const long* starts, const long* counts, long nreq, int itemsize,
+                                      int code, const void* lut, long max_rows, uint64_t pad_bits, void* dst, long cap,
+                                      long* lengths, cbool idx_on_device, void* stream) except +dds_translate_exception
         void set_normalization(string name, const float* mean, const float* std, long nchan, long inner,
                                cbool tables_on_device) except +dds_translate_exception
         void epoch_begin() except +dds_translate_exception
@@ -121,20 +125,26 @@ cdef class PyDDStore:
                 else: self.c_ddstore.get[long](nm, start, count, <long*> p)
 
     def get_batch(self, str name, starts, counts=None, out=None, count=None, offsets=None, stream=None, src_dtype=None,
-                  lut=None, normalize=False):
+                  lut=None, normalize=False, pad_rows=None, pad_value=0, lengths=None):
         """one kernel launch for len(starts) requests, packed in request order into `out`; see
         ddstore_b200.store.PyDDStore.get_batch. `out` decides the element width checked against the variable.
         src_dtype / lut: deliver the rows converted to out.dtype (a CUDA tensor), as in ddstore_b200's get_batch;
-        normalize=True: normalised with the tables of set_normalization, as there."""
+        normalize=True: normalised with the tables of set_normalization, as there.
+        pad_rows / pad_value / lengths (with counts and a CUDA tensor `out`): a padded batch, as there."""
         if out is None:
             raise ValueError("get_batch needs an `out` buffer")
-        cv = None
+        cv = lut_keep = None
         if normalize and src_dtype is None:
             raise ValueError("normalize=True needs src_dtype")
+        if pad_rows is not None and (counts is None or count is not None or offsets is not None):
+            raise ValueError("pad_rows needs counts, and takes neither `count` nor `offsets`")
         if src_dtype is not None:
             cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
-        ob = _Buf(out, writable=True, half_ok=cv is not None)
+        ob = _Buf(out, writable=True, half_ok=cv is not None or pad_rows is not None)
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        if pad_rows is not None:
+            return self._get_batch_padded(name, starts, counts, out, ob, stream, src_dtype, cv, lut_keep, bool(s_dev),
+                                          pad_rows, pad_value, lengths)
         if cv is not None:
             return self._get_batch_convert(name, starts, counts, ob, count, offsets, stream, cv, lut_keep, bool(s_dev))
         if bool(s_dev) != bool(ob.on_device):
@@ -200,6 +210,44 @@ cdef class PyDDStore:
         with nogil:
             total = self.c_ddstore.get_batch_convert(nm, <const long*> sp, <const long*> cp, fixed, nreq, <void*> dp, cap,
                                                      code, <const void*> lp, <long*> op, idx_dev, <void*> st)
+        del keep, lut_keep
+        return total
+
+    def _get_batch_padded(self, str name, starts, counts, out, ob, stream, src_dtype, cv, lut_keep, s_dev, pad_rows,
+                          pad_value, lengths):
+        if not (ob.on_device and str(getattr(out, "dtype", "")).startswith("torch.")):
+            raise ValueError("a padded batch delivers into a CUDA tensor")
+        cdef size_t sp, cp, dp = ob.ptr, lp = (cv.lut or 0) if cv is not None else 0, lnp = 0
+        cdef long nreq
+        if s_dev:
+            nreq = starts.numel(); sp = starts.data_ptr(); cp = counts.data_ptr()
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
+            ca = _i64(counts); cp = ca.ctypes.data
+            keep = (sa, ca)
+        if lengths is not None:
+            lb = _Buf(lengths, writable=True)
+            if not lb.on_device or lb.itemsize != 8 or lb.size < nreq:
+                raise ValueError("lengths must be an int64 CUDA tensor of len(starts)")
+            lnp = lb.ptr
+        cdef int itemsize = ob.itemsize if cv is None else np.dtype(_dtype_name(src_dtype)).itemsize
+        cdef int code = 0 if cv is None else cv.code
+        cdef long max_rows = int(pad_rows)
+        if max_rows < 0:
+            raise ValueError("pad_rows must be >= 0")
+        cdef uint64_t bits = _pad_bits(pad_value, out.dtype)
+        cdef long cap = ob.nbytes
+        cdef size_t st = 0
+        if stream is not None:
+            st = int(stream) if int(stream) != 0 else 1
+        cdef string nm = name.encode()
+        cdef cbool idx_dev = s_dev
+        cdef long total
+        with nogil:
+            total = self.c_ddstore.get_batch_padded_convert(nm, <const long*> sp, <const long*> cp, nreq, itemsize, code,
+                                                            <const void*> lp, max_rows, bits, <void*> dp, cap,
+                                                            <long*> lnp, idx_dev, <void*> st)
         del keep, lut_keep
         return total
 

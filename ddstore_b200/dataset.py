@@ -19,7 +19,7 @@ from torch.utils.data import DataLoader, Dataset
 from torch.utils.data.distributed import DistributedSampler
 
 from .comm import as_dds_comm
-from .store import PyDDStore, _conversion
+from .store import PyDDStore, _conversion, _pad_bits
 
 
 def nsplit(a, n):
@@ -155,12 +155,16 @@ class RaggedDataset(Dataset):
     reference's get(name, arr, start) with count = arr.shape[0] implies (src/pyddstore.pyx:84-87).
     The (start, count) tables of ALL samples are kept on the device, so a batch needs only the sample ids."""
 
-    def __init__(self, local_arrays, local_counts, comm=None, device=None, out_dtypes=None, luts=None, normalize=None):
+    def __init__(self, local_arrays, local_counts, comm=None, device=None, out_dtypes=None, luts=None, normalize=None,
+                 pad=None):
         """local_arrays: {name: 2-D ndarray of this rank's rows}; local_counts: {name: int64[n_local_samples]}
         out_dtypes / luts: {name: dtype} / {name: 256-entry table}: those variables' batches are delivered converted in
         the gather (see DistDataset); their row offsets count rows as always.
         normalize: {name: (mean, std[, inner])}: those variables are delivered normalised per channel (see DistDataset),
-        as out_dtypes[name] (default float32)."""
+        as out_dtypes[name] (default float32).
+        pad: {name: max_rows | (max_rows, pad_value)}: those variables are delivered padded, as (tensor [B, max_rows,
+        ...width] in their output dtype, int64 lengths [B]): each sample's first max_rows rows, then pad_value (default
+        0) encoded in the output dtype. The other variables stay packed."""
         out_dtypes, luts, normalize = dict(out_dtypes or {}), dict(luts or {}), dict(normalize or {})
         super().__init__()
         self.comm = as_dds_comm(comm)
@@ -181,11 +185,11 @@ class RaggedDataset(Dataset):
             # every rank learns every sample's (start, count): 16 B per sample per variable
             blobs = self.comm.allgather_bytes(len(cnt).to_bytes(8, "little"))
             sizes = [int.from_bytes(b, "little") for b in blobs]
-            pad = max(sizes)
-            buf = np.zeros((2, pad), np.int64)
+            most = max(sizes)
+            buf = np.zeros((2, most), np.int64)
             buf[0, :len(cnt)], buf[1, :len(cnt)] = local_start, cnt
             parts = self.comm.allgather_bytes(buf.tobytes())
-            tabs = [np.frombuffer(p, np.int64).reshape(2, pad)[:, :n] for p, n in zip(parts, sizes)]
+            tabs = [np.frombuffer(p, np.int64).reshape(2, most)[:, :n] for p, n in zip(parts, sizes)]
             all_start = np.concatenate([t[0] for t in tabs])
             all_count = np.concatenate([t[1] for t in tabs])
             self.ddstore.set_sample_index(name, all_start, all_count)  # device-resident (start, count) of every sample
@@ -205,6 +209,16 @@ class RaggedDataset(Dataset):
             if self.normalize[n]:
                 self.ddstore.set_normalization(n, *_norm_spec(normalize[n]))
             self.out_row_bytes[n] = self.row_bytes[n] // self.dtypes[n].itemsize * self.out_dtypes[n].itemsize
+        self.pad = {}  # name -> (max_rows, pad_value) of the padded variables
+        for n, spec in dict(pad or {}).items():
+            if n not in self.names:
+                raise KeyError(f"pad: no variable {n!r}")
+            m, v = (spec if isinstance(spec, (tuple, list)) else (spec, 0))
+            if int(m) < 0:
+                raise ValueError("pad: max_rows must be >= 0")
+            _pad_bits(v, self.out_dtypes[n])  # (a value the output dtype cannot hold fails here)
+            self.pad[n] = (int(m), v)
+        self.packed_names = [n for n in self.names if n not in self.pad]
         self.total_ns = int(len(self.counts[self.names[0]]))
 
     def __len__(self):
@@ -214,29 +228,41 @@ class RaggedDataset(Dataset):
         return self.__getitems__([idx])
 
     def __getitems__(self, indices):
-        """-> {name: (packed rows tensor [sum(count), ...width], int64 row offsets per sample [B+1])}.
+        """-> {name: (packed rows tensor [sum(count), ...width], int64 row offsets per sample [B+1])}, and for a padded
+        variable {name: (tensor [B, max_rows, ...width], int64 lengths [B])}.
         One launch chain per variable; the sample-id -> (start, count) lookup happens on the device."""
         ids = np.ascontiguousarray(indices, dtype=np.int64)
         # host ids go to the store as they are: it copies them on the stream the gather runs on (torch's current stream:
         # the outputs below come from that stream's allocator), so the kernel can never read them before they landed
         st = torch.cuda.current_stream(self.device).cuda_stream
-        out, bufs, offs, rows = {}, [], [], []
-        for name in self.names:
+        out = {}
+        for name, (m, v) in self.pad.items():  # one padded launch per padded variable
+            buf = torch.empty((len(ids), m) + tuple(self.widths[name]), dtype=self.out_dtypes[name], device=self.device)
+            lengths = torch.empty(len(ids), dtype=torch.int64, device=self.device)
+            self.ddstore.get_samples(name, ids, buf, stream=st, src_dtype=self.src_dtypes[name], lut=self.luts[name],
+                                     normalize=self.normalize[name], pad_rows=m, pad_value=v, lengths=lengths)
+            out[name] = (buf, lengths)
+        names = self.packed_names
+        if not names:
+            return out
+        bufs, offs, rows = [], [], []
+        for name in names:
             r = int(self.counts[name][ids].sum())  # host-side size of the packed result (sizes only, no data)
             rows.append(r)
             bufs.append(torch.empty((max(r, 1),) + tuple(self.widths[name]), dtype=self.out_dtypes[name], device=self.device))
             offs.append(torch.empty(len(ids) + 1, dtype=torch.int64, device=self.device))
-        conv = any(d is not None for d in self.src_dtypes.values())
-        if len(self.names) <= 4:
-            # every variable of the batch in ONE launch (dds_get_samples_multi)
-            kw = dict(src_dtypes=[self.src_dtypes[n] for n in self.names], luts=[self.luts[n] for n in self.names],
-                      normalize=[self.normalize[n] for n in self.names]) if conv else {}
-            self.ddstore.get_samples_multi(self.names, ids, bufs, offsets=offs, stream=st, **kw)
+        conv = any(self.src_dtypes[n] is not None for n in names)
+        if 1 < len(names) <= 4:
+            # every packed variable of the batch in ONE launch (dds_get_samples_multi; a single variable takes
+            # dds_get_samples, which the multi-array launch does not stand in for)
+            kw = dict(src_dtypes=[self.src_dtypes[n] for n in names], luts=[self.luts[n] for n in names],
+                      normalize=[self.normalize[n] for n in names]) if conv else {}
+            self.ddstore.get_samples_multi(names, ids, bufs, offsets=offs, stream=st, **kw)
         else:
-            for name, buf, off in zip(self.names, bufs, offs):
+            for name, buf, off in zip(names, bufs, offs):
                 self.ddstore.get_samples(name, ids, out=buf, offsets=off, stream=st, src_dtype=self.src_dtypes[name],
                                          lut=self.luts[name], normalize=self.normalize[name])
-        for name, buf, off, r in zip(self.names, bufs, offs, rows):
+        for name, buf, off, r in zip(names, bufs, offs, rows):
             out[name] = (buf[:r], off // self.out_row_bytes[name])
         return out
 
@@ -367,7 +393,9 @@ class RaggedPrefetchLoader:
 
     sampler: iterable of sample ids on the host (e.g. DistributedSampler): the packed sizes come from the host copy of
     the row counts. Yields {name: (packed rows tensor [sum(count), ...width], int64 row offsets [B+1])}; a batch stays
-    valid until the next-but-one fetch."""
+    valid until the next-but-one fetch. The dataset's padded variables (RaggedDataset(pad=...)) are queued beside that
+    launch, one padded launch each (also overlap=True), into fixed-size per-slot buffers, and yielded as
+    {name: (tensor [B, max_rows, ...width], int64 lengths [B])}."""
 
     def __init__(self, dataset, sampler, batch_size, drop_last=False, depth=2):
         if len(dataset.names) > 4:
@@ -377,8 +405,11 @@ class RaggedPrefetchLoader:
         self.stream = torch.cuda.Stream(device=dev)
         self.events = [torch.cuda.Event() for _ in range(self.depth)]
         self.bufs = [None] * self.depth   # per slot: {name: uint8 buffer}, grown on demand
-        self.offs = [[torch.empty(batch_size + 1, dtype=torch.int64, device=dev) for _ in dataset.names] for _ in range(self.depth)]
+        self.offs = [[torch.empty(batch_size + 1, dtype=torch.int64, device=dev) for _ in dataset.packed_names] for _ in range(self.depth)]
         self.d_ids = [torch.empty(batch_size, dtype=torch.int64, device=dev) for _ in range(self.depth)]
+        self.pbufs = [{name: (torch.empty((batch_size, m) + tuple(dataset.widths[name]), dtype=dataset.out_dtypes[name],
+                                          device=dev), torch.empty(batch_size, dtype=torch.int64, device=dev))
+                       for name, (m, _) in dataset.pad.items()} for _ in range(self.depth)]
 
     def _batches(self):
         cur = []
@@ -392,9 +423,10 @@ class RaggedPrefetchLoader:
 
     def _issue(self, slot, idx):
         ds = self.ds
+        names = ds.packed_names
         ids = np.asarray(idx, dtype=np.int64)
-        rows = [int(ds.counts[name][ids].sum()) for name in ds.names]  # host-side sizes only
-        need = [max(r, 1) * ds.out_row_bytes[name] for r, name in zip(rows, ds.names)]
+        rows = [int(ds.counts[name][ids].sum()) for name in names]  # host-side sizes only
+        need = [max(r, 1) * ds.out_row_bytes[name] for r, name in zip(rows, names)]
         if self.bufs[slot] is None or any(b.numel() < n for b, n in zip(self.bufs[slot], need)):
             # (grown rarely; a fresh buffer cannot still be in use by an earlier fetch)
             # (whole 8-byte words, so a converting fetch can view them in its output dtype)
@@ -403,13 +435,24 @@ class RaggedPrefetchLoader:
         n = len(ids)
         with torch.cuda.stream(self.stream):
             self.d_ids[slot][:n].copy_(keep, non_blocking=True)
+            for name, (buf, lengths) in self.pbufs[slot].items():
+                m, v = ds.pad[name]
+                ds.ddstore.get_samples(name, self.d_ids[slot][:n], buf[:n], stream=self.stream.cuda_stream, wait=False,
+                                       overlap=True, src_dtype=ds.src_dtypes[name], lut=ds.luts[name],
+                                       normalize=ds.normalize[name], pad_rows=m, pad_value=v, lengths=lengths[:n])
             kw = {}
-            if any(d is not None for d in ds.src_dtypes.values()):  # (the uint8 buffers are viewed as out_dtypes)
-                kw = dict(src_dtypes=[ds.src_dtypes[m] for m in ds.names], luts=[ds.luts[m] for m in ds.names],
-                          normalize=[ds.normalize[m] for m in ds.names])
-            bufs = [b.view(ds.out_dtypes[m]) if kw else b for b, m in zip(self.bufs[slot], ds.names)]
-            ds.ddstore.get_samples_multi(ds.names, self.d_ids[slot][:n], bufs, offsets=[o[:n + 1] for o in self.offs[slot]],
-                                         stream=self.stream.cuda_stream, wait=False, overlap=True, **kw)
+            if any(ds.src_dtypes[m] is not None for m in names):  # (the uint8 buffers are viewed as out_dtypes)
+                kw = dict(src_dtypes=[ds.src_dtypes[m] for m in names], luts=[ds.luts[m] for m in names],
+                          normalize=[ds.normalize[m] for m in names])
+            bufs = [b.view(ds.out_dtypes[m]) if kw else b for b, m in zip(self.bufs[slot], names)]
+            if len(names) > 1:
+                ds.ddstore.get_samples_multi(names, self.d_ids[slot][:n], bufs, offsets=[o[:n + 1] for o in self.offs[slot]],
+                                             stream=self.stream.cuda_stream, wait=False, overlap=True, **kw)
+            elif names:  # (a single packed variable: dds_get_samples)
+                m = names[0]
+                ds.ddstore.get_samples(m, self.d_ids[slot][:n], bufs[0], offsets=self.offs[slot][0][:n + 1],
+                                       stream=self.stream.cuda_stream, wait=False, overlap=True, src_dtype=ds.src_dtypes[m],
+                                       lut=ds.luts[m], normalize=ds.normalize[m])
             self.events[slot].record(self.stream)
         return n, rows, keep
 
@@ -430,7 +473,9 @@ class RaggedPrefetchLoader:
         slot, n, rows, _ = item
         consumer.wait_event(self.events[slot])
         ds, out = self.ds, {}
-        for k, name in enumerate(ds.names):
+        for name, (buf, lengths) in self.pbufs[slot].items():
+            out[name] = (buf[:n], lengths[:n])
+        for k, name in enumerate(ds.packed_names):
             nb = rows[k] * ds.out_row_bytes[name]
             buf = self.bufs[slot][k][:nb].view(ds.out_dtypes[name]).view((rows[k],) + tuple(ds.widths[name]))
             out[name] = (buf, self.offs[slot][k][:n + 1] // ds.out_row_bytes[name])

@@ -95,6 +95,39 @@ def _ptr(t):
     return t.ctypes.data if isinstance(t, np.ndarray) else t.data_ptr()
 
 
+_INT_VIEW = {1: "uint8", 2: "int16", 4: "int32", 8: "int64"}
+
+
+def _pad_bits(value, dtype):
+    """the bits of one `dtype` element holding `value` (a number, or a one-element tensor of `dtype` whose bits are used
+    verbatim, e.g. a NaN with a payload). ValueError for a value `dtype` cannot represent."""
+    import math
+
+    import torch
+    if isinstance(value, torch.Tensor):
+        if value.numel() != 1 or value.dtype != dtype:
+            raise ValueError(f"pad_value must be a number or a one-element {dtype} tensor")
+        t = value.detach().reshape(1).cpu()
+    elif dtype == torch.bool:
+        if value not in (0, 1):
+            raise ValueError(f"pad_value {value!r} is not a bool")
+        t = torch.tensor([bool(value)])
+    elif dtype.is_floating_point:
+        v = float(value)
+        t = torch.tensor([v], dtype=dtype)
+        if math.isfinite(v) and not bool(torch.isfinite(t).all()):
+            raise ValueError(f"pad_value {value!r} overflows {dtype}")
+    else:
+        if isinstance(value, float) and not value.is_integer():
+            raise ValueError(f"pad_value {value!r} is not an integer ({dtype})")
+        iv, info = int(value), torch.iinfo(dtype)
+        if not info.min <= iv <= info.max:
+            raise ValueError(f"pad_value {value!r} is outside the range of {dtype}")
+        t = torch.tensor([iv], dtype=dtype)
+    n = t.element_size()
+    return int(t.view(getattr(torch, _INT_VIEW[n])).item()) & ((1 << (8 * n)) - 1)
+
+
 def _lut_bits(t):
     """a 256-entry torch table as a host int16 / int32 array of its bits"""
     import torch
@@ -223,7 +256,7 @@ class PyDDStore:
 
     # ---------------------------------------------------------------- the batched hot path
     def get_batch(self, name, starts, counts=None, out=None, count=None, offsets=None, stream=None, wait=True,
-                  overlap=False, src_dtype=None, lut=None, normalize=False):
+                  overlap=False, src_dtype=None, lut=None, normalize=False, pad_rows=None, pad_value=0, lengths=None):
         """Fetch len(starts) requests in ONE kernel launch, packed back to back in request order.
 
         starts/counts: int64 index arrays (host ndarray/list, or CUDA int64 tensors). counts=None means
@@ -249,9 +282,21 @@ class PyDDStore:
         normalize=True (with src_dtype): deliver (x - mean[ch]) / std[ch], computed in float32 with the tables registered
         by set_normalization, as out.dtype: float32 -> float32 / bfloat16 / float16, float64 -> float32, uint8 -> float32 /
         bfloat16 / float16 (decoded through `lut`, 256 float32 entries, default torch.arange(256).float()).
+        pad_rows=M (with counts and a CUDA `out`): a padded batch. Request i fills slot i of `out`, viewed as
+        [len(starts), M, row]: its first min(counts[i], M) rows (raw, or converted / normalised as above), then
+        `pad_value` encoded in out.dtype (or a one-element out.dtype tensor, used bit for bit) up to the slot's end.
+        out.dtype must have the delivered element size. An invalid request leaves a slot of padding and length 0, and
+        every valid slot is still delivered; then the reference's ValueError is raised for the first invalid one.
+        lengths (optional int64 CUDA tensor of len(starts)) receives the delivered row counts. Returns out's padded
+        size in bytes, len(starts) * M * row elements * out.element_size().
         """
         if out is None:
             raise ValueError("get_batch needs an `out` buffer (like get(), it never allocates)")
+        if pad_rows is not None:
+            if counts is None:
+                raise ValueError("pad_rows needs counts (there is no fixed-count padded batch)")
+            if count is not None or offsets is not None:
+                raise ValueError("a padded batch takes neither `count` nor `offsets`")
         cv = lut_keep = None
         if normalize and src_dtype is None:
             raise ValueError("normalize=True needs src_dtype")
@@ -261,7 +306,7 @@ class PyDDStore:
             itemsize = self._itemsize.get(name)
             if itemsize is None:
                 itemsize = self._itemsize[name] = self.query(name)["itemsize"]
-        ob = _Buf(out, writable=True, half_ok=cv is not None)
+        ob = _Buf(out, writable=True, half_ok=cv is not None or pad_rows is not None)
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
         if s_dev:
             nreq = starts.numel()
@@ -278,6 +323,9 @@ class PyDDStore:
         flags = (_capi.IDX_ON_DEVICE if s_dev else 0) | (_capi.DST_ON_DEVICE if ob.on_device else 0)
         if not wait:
             flags |= _capi.NO_SYNC | (_capi.OVERLAP if overlap else 0)
+        if pad_rows is not None:
+            return self._padded(name, False, sp, cp, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream,
+                                (keep, lut_keep))
         op = None
         if offsets is not None:
             fb = _Buf(offsets, writable=True)
@@ -346,9 +394,12 @@ class PyDDStore:
         del m, s
 
     def get_samples(self, name, sample_ids, out, offsets=None, stream=None, wait=True, overlap=False, src_dtype=None,
-                    lut=None, normalize=False):
+                    lut=None, normalize=False, pad_rows=None, pad_value=0, lengths=None):
         """get_batch by SAMPLE ID: the id -> (start, count) lookup runs inside the launch, against the index
-        registered with set_sample_index. Same packing / offsets / error behaviour, and conversions, as get_batch."""
+        registered with set_sample_index. Same packing / offsets / error behaviour, conversions and padding (pad_rows,
+        pad_value, lengths) as get_batch."""
+        if pad_rows is not None and offsets is not None:
+            raise ValueError("a padded batch takes no `offsets`")
         cv = lut_keep = None
         if normalize and src_dtype is None:
             raise ValueError("normalize=True needs src_dtype")
@@ -358,7 +409,7 @@ class PyDDStore:
             itemsize = self._itemsize.get(name)
             if itemsize is None:
                 itemsize = self._itemsize[name] = self.query(name)["itemsize"]
-        ob = _Buf(out, writable=True, half_ok=cv is not None)
+        ob = _Buf(out, writable=True, half_ok=cv is not None or pad_rows is not None)
         s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
         if s_dev:
             nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
@@ -368,6 +419,9 @@ class PyDDStore:
         flags = (_capi.IDX_ON_DEVICE if s_dev else 0) | (_capi.DST_ON_DEVICE if ob.on_device else 0)
         if not wait:
             flags |= _capi.NO_SYNC | (_capi.OVERLAP if overlap else 0)
+        if pad_rows is not None:
+            return self._padded(name, True, sp, None, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream,
+                                (keep, lut_keep))
         op = None
         if offsets is not None:
             fb = _Buf(offsets, writable=True)
@@ -382,6 +436,37 @@ class PyDDStore:
             rc = self._L.dds_get_samples_convert(self._h, name.encode(), sp, nreq, ob.ptr, ob.nbytes, op, flags,
                                                  self._stream_arg(stream), C.byref(cv), C.byref(total), C.byref(bad))
         del keep, lut_keep
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    def _padded(self, name, by_sample, sp, cp, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream, keep):
+        """the padded form of get_batch / get_samples (arguments already converted by them)"""
+        pad_rows = int(pad_rows)
+        if pad_rows < 0:
+            raise ValueError("pad_rows must be >= 0")
+        if not (ob.on_device and hasattr(out, "dtype") and str(out.dtype).startswith("torch.")):
+            raise ValueError("a padded batch delivers into a CUDA tensor")
+        itemsize = self._itemsize.get(name)
+        if itemsize is None:
+            itemsize = self._itemsize[name] = self.query(name)["itemsize"]
+        if cv is None and ob.itemsize != itemsize:
+            raise ValueError(f"out.dtype {out.dtype} does not have the variable's itemsize ({itemsize})")
+        pad = _capi.Pad(pad_rows, _pad_bits(pad_value, out.dtype), None)
+        if lengths is not None:
+            lb = _Buf(lengths, writable=True)
+            if not lb.on_device or lb.itemsize != 8 or lb.size < nreq:
+                raise ValueError("lengths must be an int64 CUDA tensor of len(starts)")
+            pad.lengths = lb.ptr
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        cvp = C.byref(cv) if cv is not None else None
+        if by_sample:
+            rc = self._L.dds_get_samples_padded(self._h, name.encode(), sp, nreq, itemsize, cvp, C.byref(pad), ob.ptr,
+                                                ob.nbytes, flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
+        else:
+            rc = self._L.dds_get_batch_padded(self._h, name.encode(), sp, cp, nreq, itemsize, cvp, C.byref(pad), ob.ptr,
+                                              ob.nbytes, flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
+        del keep
         self.last_bad_index = bad.value
         _capi.raise_for(rc)
         return total.value

@@ -22,7 +22,9 @@
 extern "C" {
 #endif
 
-#define DDS_VERSION 111 /* 110: converting batches (dds_get_batch_convert & co.); 111: normalising conversions */
+#define DDS_VERSION 111 /* 110: converting batches (dds_get_batch_convert & co.); 111: normalising conversions.
+                           The padded batches (dds_get_batch_padded, dds_get_samples_padded) add entries only: callers
+                           that built against 111 are unaffected, and a caller finds them by symbol. */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -243,6 +245,34 @@ int dds_get_samples_multi_convert(dds_store_t *s, int nvars, const char *const *
                                   int64_t nreq, void *const *dsts, const int64_t *dst_capacities,
                                   int64_t *const *dst_offsets, unsigned flags, void *cuda_stream,
                                   const dds_convert_t *cvts, int64_t *total_bytes, int64_t *bad_index);
+
+/* ---- padded batches: variable-length requests delivered as [nreq, max_rows, disp] slots plus lengths --------------
+ * Let S = max_rows * disp * out_itemsize (out_itemsize: the variable's itemsize for a raw batch, the code's output
+ * itemsize with a conversion). Request i owns bytes [i * S, (i + 1) * S) of dst: its first min(count_i, max_rows) rows,
+ * raw or converted / normalised exactly as by the *_convert entries (cvt NULL: raw), then pad_bits, one output element
+ * at a time, written verbatim (padding is never converted). lengths[i] (nullable, device) receives the delivered row
+ * count; *total_bytes = nreq * S.
+ * Requests are validated on their FULL (start, count), by the rules of dds_get_batch: a valid request longer than
+ * max_rows is truncated (not an error); an invalid one gets a slot of padding only and length 0, and the first invalid
+ * request's code and index are returned as dds_get_batch returns them. Unlike the packed entries, every valid request's
+ * slot is delivered even when some are invalid.
+ * DDS_ERR_ARG, with nothing enqueued or written: counts == NULL (padding needs counts; dds_get_samples_padded takes them
+ * from the sample index), a host destination (DDS_DST_ON_DEVICE is required), dst not aligned to out_itemsize or lengths
+ * not aligned to 8, max_rows < 0, nreq * S overflowing, a raw variable whose itemsize is not 1, 2, 4 or 8, and
+ * dst_capacity < nreq * S (checked on the host: the padded size does not depend on the requests). DDS_ERR_DTYPE as for
+ * the raw and the converting entries. DDS_NO_SYNC and DDS_OVERLAP work as for fixed-count batches (overlap is honoured
+ * at every size); a queued padded batch's total is nreq * S. */
+typedef struct {
+    int64_t max_rows;  /* rows per slot, >= 0 */
+    uint64_t pad_bits; /* one OUTPUT element's bits, in the low out_itemsize bytes (e.g. a bf16 -inf, an int32 pad id) */
+    int64_t *lengths;  /* device, nullable: nreq delivered row counts */
+} dds_pad_t;
+int dds_get_batch_padded(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts, int64_t nreq,
+                         int itemsize, const dds_convert_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity,
+                         unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
+                           const dds_convert_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity, unsigned flags,
+                           void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
 
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite

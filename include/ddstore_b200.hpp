@@ -13,6 +13,7 @@
 #define DDSTORE_B200_HPP
 
 #include <cstdint>
+#include <cstring>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -97,6 +98,36 @@ class DDStore {
         check(dds_get_batch(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts, fixed_count, nreq,
                             (int)sizeof(T), dst, dst_capacity_bytes, (int64_t *)dst_offsets, flags, cuda_stream, &total,
                             &bad));
+        return (long)total;
+    }
+    // The same requests delivered padded (dds_get_batch_padded): request i fills the max_rows * disp * sizeof(T) bytes of
+    // slot i of dst with its first min(counts[i], max_rows) rows, then pad elements. dst (and lengths, nullable: the
+    // delivered row counts) are device memory. Returns the padded bytes, nreq * slot.
+    template <typename T>
+    long get_batch_padded(std::string name, const long *starts, const long *counts, long nreq, long max_rows, T pad, T *dst,
+                          long dst_capacity_bytes, long *lengths = nullptr, bool idx_on_device = true,
+                          void *cuda_stream = nullptr) {
+        static_assert(sizeof(T) == 1 || sizeof(T) == 2 || sizeof(T) == 4 || sizeof(T) == 8, "element of 1, 2, 4 or 8 bytes");
+        uint64_t bits = 0;
+        memcpy(&bits, &pad, sizeof(T));
+        return get_batch_padded_convert(name, starts, counts, nreq, (int)sizeof(T), DDS_CVT_NONE, nullptr, max_rows, bits,
+                                        dst, dst_capacity_bytes, lengths, idx_on_device, cuda_stream);
+    }
+    // The general form: `itemsize` is the variable's, `code` a DDS_CVT_* code (DDS_CVT_NONE: raw rows; `lut` as for
+    // get_batch_convert), pad_bits one OUTPUT element's bits in its low bytes.
+    long get_batch_padded_convert(std::string name, const long *starts, const long *counts, long nreq, int itemsize, int code,
+                                  const void *lut, long max_rows, uint64_t pad_bits, void *dst, long dst_capacity_bytes,
+                                  long *lengths = nullptr, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        dds_pad_t p;
+        p.max_rows = max_rows;
+        p.pad_bits = pad_bits;
+        p.lengths = (int64_t *)lengths;
+        const dds_convert_t cvt = {code, lut};
+        const unsigned flags = DDS_DST_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_get_batch_padded(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts, nreq, itemsize,
+                                   code == DDS_CVT_NONE ? nullptr : &cvt, &p, dst, dst_capacity_bytes, flags, cuda_stream,
+                                   &total, &bad));
         return (long)total;
     }
     // The per-channel normalisation of variable `name` for the DDS_CVT_NORM_* codes (dds_set_normalization): nchan
