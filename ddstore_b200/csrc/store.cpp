@@ -764,6 +764,18 @@ int drain_pending(dds_store *s) {
     return DDS_OK;
 }
 
+// An empty DDS_NO_SYNC batch launches nothing, yet it is the last batch queued: the next dds_batch_wait reports its
+// total, 0. Chained onto a pending queue, that queue's drain keeps the 0; otherwise nothing is pending any more.
+void note_empty_async(dds_store *s, bool no_sync) {
+    if (!no_sync) return;
+    if (s->pending) {
+        s->pending_fixed_total = 0;
+        s->pending_cvt = DDSK_CVT_NONE;
+    } else {
+        s->kept_total = 0;
+    }
+}
+
 // The kernels tag every status report with the launch's position in its queue of DDS_NO_SYNC batches (0 for a
 // synchronous call or the first of a queue), so the sticky word ends up holding the first failing batch in queue order.
 // The tag has 16 bits: a launch that would be the kQueueMax-th of its queue first drains the queue and starts a new one
@@ -1287,6 +1299,7 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
             else dst_offsets[0] = 0;
             if (dst_dev) CU(cudaStreamSynchronize(st));
         }
+        note_empty_async(s, no_sync);
         return DDS_OK;
     }
 
@@ -1644,7 +1657,10 @@ static int padded_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *st
     if (s->pending && !chain) {
         if (int rc = drain_pending(s)) return rc;
     }
-    if (nreq == 0) return DDS_OK;
+    if (nreq == 0) {
+        note_empty_async(s, no_sync);
+        return DDS_OK;
+    }
     const int64_t *d_starts = starts, *d_counts = counts;
     if (int rc = stage_indices(s, starts, by_sample ? nullptr : counts, nreq, idx_dev, st, &d_starts, &d_counts)) return rc;
     ddsk_index_t ix;
@@ -1757,7 +1773,10 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
     }
     if (total_bytes)
         for (int v = 0; v < nvars; v++) total_bytes[v] = 0;
-    if (nreq == 0) return DDS_OK;
+    if (nreq == 0) {
+        note_empty_async(s, no_sync);
+        return DDS_OK;
+    }
     if (key != s->multi_key) { // (re)build the device array of windows for this combination of variables
         if (!s->d_multi_vars) CU(cudaMalloc((void **)&s->d_multi_vars, sizeof(ddsk_var_t) * DDSK_MAX_MULTI));
         CU(cudaStreamSynchronize(st)); // nothing in flight may still read the previous combination

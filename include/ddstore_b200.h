@@ -297,8 +297,9 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
  * next dds_batch_wait reports the kept failure, with its index and text, after completing any queue still pending; a
  * failure kept from earlier wins over any failure queued after it, since it is earlier in queue order. After it has
  * been reported, the next call returns DDS_OK. *total_bytes is the packed size of the last batch queued since the
- * previous dds_batch_wait, 0 if there was none. A queue reaching 65535 launches is completed the same way before its
- * next launch (the status word's queue ordinal has 16 bits), so its failures are still reported in queue order.
+ * previous dds_batch_wait (an empty one, nreq = 0, counts with size 0), 0 if there was none. A queue reaching 65535
+ * launches is completed the same way before its next launch (the status word's queue ordinal has 16 bits), so its
+ * failures are still reported in queue order.
  * dds_destroy drops a kept outcome that no dds_batch_wait has reported. */
 int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index);
 

@@ -9,7 +9,8 @@ output itemsize allows; explicit counts and sample ids, host and device indices;
 code with pad bits that must come out verbatim; every kind of invalid request at window lanes 0, 31, 32 and at the end;
 every argument error; overlapped queues mixing padded, packed and converting batches, also under SM contention; one
 batch whose padded output passes 4 GiB; RaggedDataset(pad=...) and RaggedPrefetchLoader over two epochs; the Cython
-binding. A subprocess repeats the batch and loader tests with DDS_PDL=0 and DDS_GATHER_CTAS_PER_SM=2.
+binding; the wait() total after an empty batch queued behind a padded one, through every entry. A subprocess
+repeats the batch and loader tests with DDS_PDL=0 and DDS_GATHER_CTAS_PER_SM=2.
 
 On an H100 80GB HBM3 (700 W power limit) the module takes about 30 s, the subprocess included.
 """
@@ -433,6 +434,35 @@ def test_queue(env):
     with pytest.raises(ValueError):
         store.wait()
     assert store.last_bad_index == 40
+
+
+def test_empty_batch_wait_total(env):
+    """an empty (nreq = 0) DDS_NO_SYNC batch queued behind a padded batch on the same stream is the last batch queued:
+    wait() reports its total, 0 -- through the padded, packed, converting and multi-array entries alike"""
+    store, rng = env["store"], env["rng"]
+    st = torch.cuda.Stream()
+    s, c = _requests(rng, 300, 6)
+    ds, dc = torch.as_tensor(s, device=DEV), torch.as_tensor(c, device=DEV)
+    out = torch.empty(300 * 4 * 80, dtype=torch.float32, device=DEV)
+    e = torch.empty(0, dtype=torch.int64, device=DEV)
+    small = torch.empty(16, dtype=torch.uint8, device=DEV)
+    sb = torch.empty(16, dtype=torch.bfloat16, device=DEV)
+    tab = (env["sstart"][:-1], env["L"])
+    empties = {"padded": lambda: store.get_batch("f80", e, e, out=out, pad_rows=4, wait=False, stream=st.cuda_stream),
+               "padded by sample": lambda: store.get_samples("f80", e, out, pad_rows=4, wait=False, stream=st.cuda_stream),
+               "packed": lambda: store.get_batch("f80", e, e, out=small, wait=False, stream=st.cuda_stream),
+               "converting": lambda: store.get_batch("f80", e, e, out=sb, src_dtype=torch.float32, wait=False,
+                                                     stream=st.cuda_stream),
+               "multi-array": lambda: store.get_samples_multi(["f80", "d5"], e, [small, small], wait=False,
+                                                              stream=st.cuda_stream)}
+    assert tab[0].size == NSAMP
+    for kind, empty in empties.items():
+        full = store.get_batch("f80", ds, dc, out=out, pad_rows=4, wait=False, stream=st.cuda_stream)
+        assert full == 300 * 4 * 80 * 4
+        empty()
+        assert store.wait() == 0, kind
+        store.get_batch("f80", ds, dc, out=out, pad_rows=4, wait=False, stream=st.cuda_stream)
+        assert store.wait() == 300 * 4 * 80 * 4, kind  # (and a non-empty last batch still reports its own)
 
 
 def test_over_4gib(env):
