@@ -15,6 +15,7 @@ ERR_DTYPE, ERR_START, ERR_COUNT, ERR_DISP, ERR_FENCE_ACTIVE, ERR_FENCE_INACTIVE 
 ERR_UNKNOWN_VAR, ERR_EXISTS, ERR_CUDA, ERR_COMM, ERR_ARG, ERR_CAPACITY, ERR_NO_DEVICE, ERR_WATCHDOG = \
     7, 8, 9, 10, 11, 12, 13, 14
 IDX_ON_DEVICE, DST_ON_DEVICE, NO_SYNC, OVERLAP = 1, 2, 4, 8
+SRC_ON_DEVICE = 2  # dds_put_*: the packed source rows are device memory (same bit as DST_ON_DEVICE)
 
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 BARRIER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
@@ -85,6 +86,10 @@ SIGNATURES = {
                                        I64P, I64P]),
     "dds_get_samples_padded": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.POINTER(Convert),
                                          C.POINTER(Pad), C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_put_batch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int,
+                                C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_put_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
+                                  C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

@@ -252,7 +252,9 @@ __device__ __forceinline__ longlong2 ldg_pair(const longlong2 *p) { return __ldg
 // (ids, then table rows, then arithmetic) so that the K independent -- and for the sample index, dependent
 // two-level -- global loads of a thread are all in flight together instead of one DRAM latency after another.
 // `limit`: requests idx >= limit are not this thread's business (dead lanes).
-template <int K>
+// PUT (a batched put): an invalid request keeps its bytes in the caller's layout -- count * row_bytes when 0 < count <=
+// the variable's rows, 0 otherwise and for a sample id outside the index -- with source address 0 (nothing is written).
+template <int K, bool PUT = false>
 __device__ __forceinline__ void plan_many(const ddsk_var_t &var, const PlanSrc &p, const int64_t (&idx)[K], int64_t limit,
                                           unsigned long long *status, unsigned long long tag, uint64_t (&src)[K],
                                           int64_t (&nbytes)[K]) {
@@ -316,6 +318,10 @@ __device__ __forceinline__ void plan_many(const ddsk_var_t &var, const PlanSrc &
         const int code = dev_locate(*vp[k], start[k], count[k], &s);
         if (code) {
             report(status, tag, idx[k], code);
+            if constexpr (PUT) {
+                const int64_t rows = vp[k]->lenlist[vp[k]->nranks - 1];
+                nbytes[k] = count[k] > 0 && count[k] <= rows ? count[k] * vp[k]->row_bytes : 0;
+            }
             continue;
         }
         src[k] = s;
@@ -349,8 +355,8 @@ struct GatherArgs {
     PlanSrc plan;
     int64_t *total_out; // VAR + shared plan: CTA 0 publishes the packed total here (one device word)
     int64_t nreq;
-    char *dst;
-    int64_t dst_cap;
+    char *dst;            // the packed buffer (a put: the caller's packed SOURCE rows, only read)
+    int64_t dst_cap;      // its size in bytes
     int64_t *offsets_out; // optional [nreq+1]
     unsigned long long *status;
     unsigned long long status_tag; // this launch's ordinal in its queue, as OR-ed into every status report
@@ -484,7 +490,10 @@ __device__ __forceinline__ void pad_fill(char *d, int64_t n, uint64_t bits, int 
 // of a variable that starts at an odd offset
 // PAD (padded batches, with FIXED): slot i of the walk holds request i's payload followed by padding; the walk copies the
 // payload and each warp fills the padding of the segments it claims
-template <bool FIXED, int CH, int PCAP, bool VALIGN = false, bool PAD = false>
+// PUT (batched puts): the same walk with the roles of the two addresses swapped: a piece's src is its packed position in
+// a.dst (the caller's rows, where the TMA load reads, so the stage offsets follow that address's 16-byte phase) and its
+// dpos the shard address its drain writes
+template <bool FIXED, int CH, int PCAP, bool VALIGN = false, bool PAD = false, bool PUT = false>
 struct ChunkWalker {
     // warp-uniform state
     int64_t seg_pos = 0, seg_end = 0, T = 0, seg_bytes = 0, nseg = 0, nb = 0;
@@ -507,6 +516,7 @@ struct ChunkWalker {
     // per-lane window of 32 request descriptors
     uint64_t w_src = 0;
     int64_t w_dst = 0, w_n = 0;
+    uint64_t w_shard; // PUT: the request's shard address (w_src is then its packed position in the caller's buffer)
 
     __device__ __forceinline__ void load_window(const GatherArgs &a, int lane) {
         win_base = r;
@@ -550,6 +560,10 @@ struct ChunkWalker {
                 w_src = pv.s(idx);
                 w_dst = pv.d(idx);
                 w_n = pv.d(idx + 1) - w_dst;
+            }
+            if constexpr (PUT) { // the pieces load from the caller's rows and are written to the shard
+                w_shard = w_src;
+                w_src = w_src ? (uint64_t)a.dst + (uint64_t)w_dst : 0;
             }
         }
     }
@@ -686,6 +700,7 @@ struct ChunkWalker {
                     pc.dpos = p0;
                     pc.n = lane == 0 ? (uint32_t)len : 0u;
                     pc.off = 0;
+                    if constexpr (PUT) pc.dpos = (int64_t)(__shfl_sync(0xffffffffu, w_shard, wl) + (uint64_t)(p0 - d0));
                     return ((uint32_t)(src & 15u) + (uint32_t)len + 15u) & ~15u;
                 }
             }
@@ -723,6 +738,7 @@ struct ChunkWalker {
             if (total == 0) continue; // only empty / rejected requests in this run
             pc.src = (active && copy) ? src : 0;
             pc.dpos = p0;
+            if constexpr (PUT) pc.dpos = (int64_t)(__shfl_sync(0xffffffffu, w_shard, srcl & 31) + (uint64_t)(p0 - q_d0));
             pc.n = (active && copy) ? (uint32_t)len : 0u;
             pc.off = end - sz;
             return total;
@@ -1150,7 +1166,8 @@ using CvtParam = typename std::conditional<CVT, ddsk_cvt_t, NoCvt>::type;
 // when the destination capacity is below 4 GiB, so T > 2^32 is a capacity error and nothing is copied).
 // ------------------------------------------------------------------------------------------------
 // (CVT: the offsets the caller sees are in output bytes of conversion `code`; the plan itself stays in source bytes)
-template <int NW, int PCAP, bool CVT = false, bool NORM = false>
+// (PUT: the put form of the lookup, plan_many<4, true>)
+template <int NW, int PCAP, bool CVT = false, bool NORM = false, bool PUT = false>
 __device__ __forceinline__ int64_t plan_in_smem(const GatherArgs &a, const PlanView<PCAP> &pv, int64_t *wtot, int warp,
                                                 int lane, bool writer, int code = 0) {
     auto out = [&](int64_t x) -> int64_t {
@@ -1166,7 +1183,7 @@ __device__ __forceinline__ int64_t plan_in_smem(const GatherArgs &a, const PlanV
         uint64_t sv[4];
 #pragma unroll
         for (int k = 0; k < 4; k++) idx[k] = b + k * 32 + lane;
-        plan_many<4>(a.var, a.plan, idx, w1, a.status, a.status_tag, sv, nb);
+        plan_many<4, PUT>(a.var, a.plan, idx, w1, a.status, a.status_tag, sv, nb);
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             if (idx[k] < w1) {
@@ -1230,13 +1247,22 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // since a multi-array launch may mix normalised, plainly converted and raw variables.
 // PAD (with FIXED): a padded batch -- a fixed-stride walk over slots of a.pad_slot source bytes (see ChunkWalker), the
 // padding filled by the warps that claim it, the lengths written after the walk. No plan, no offsets, no push fetch.
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false>
+// PUT: a batched put (DDSK_F_PUT) -- the raw walk with every copy reversed. Lookup, checks, plan, segment claims and
+// status reports are the gather's; a piece's TMA load reads its packed position in a.dst (the caller's rows, a.dst_cap
+// bytes) and the drain writes its shard address, through the same drain paths, which store exactly the piece's bytes
+// (plain byte / 16-byte stores and bulk stores, never a read-modify-write of a neighbouring byte: other warps and other
+// ranks may be writing the adjacent rows). Nothing is written outside the requests' rows, so a shard's zero slack stays
+// zero. The load reads the 16-byte-aligned superset of the piece's range in the caller's buffer: up to 15 bytes on
+// either side that belong to no request, in the same 16-byte block (which never crosses a page), whose values are
+// discarded. Never overlapped, no offsets, no conversion, no push.
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
                                                                 const __grid_constant__ CvtParam<CVT> c) {
     static_assert(CVT || !NORM, "a normalising launch is a converting one");
     static_assert(FIXED || !PAD, "a padded batch is a fixed-stride walk");
+    static_assert(!PUT || (!CVT && !PAD), "a put writes raw rows");
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
-    constexpr bool PUSH = FIXED && !CVT && !PAD;
+    constexpr bool PUSH = FIXED && !CVT && !PAD && !PUT;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
     __shared__ __align__(8) uint64_t full_bar[NW][S];
     __shared__ __align__(16) PieceDesc desc[NW][S][32];
@@ -1287,14 +1313,14 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     };
 
     // ---- the plan (variable counts) ------------------------------------------------------------
-    ChunkWalker<FIXED, CH, PCAP, CVT, PAD> w;
+    ChunkWalker<FIXED, CH, PCAP, CVT, PAD, PUT> w;
     if (!FIXED) {
         if constexpr (PCAP > 0) {
             w.pv.src_s = smem_u32(smem_dyn) + (uint32_t)(NW * S * STAGE);
             w.pv.dst_s = w.pv.src_s + (uint32_t)PCAP * 8u;
             const bool writer = blockIdx.x == 0;
             if (writer) pass_gate(); // CTA 0 writes the offsets / the total for the caller
-            w.T = plan_in_smem<NW, PCAP, CVT, NORM>(a, w.pv, wtot, warp, lane, writer, code0);
+            w.T = plan_in_smem<NW, PCAP, CVT, NORM, PUT>(a, w.pv, wtot, warp, lane, writer, code0);
         } else {
             w.pv.src = a.req_src;
             w.pv.dst = a.req_dst;
@@ -1564,7 +1590,22 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         const int64_t my_dpos = desc[warp][st][lane].dpos;
         const uint32_t my_n = desc[warp][st][lane].n;
         const uint32_t my_pack = desc[warp][st][lane].pack;
-        if constexpr (CVT) {
+        if constexpr (PUT) {
+            // put: the raw drain (the last branch) into the shard address the descriptor carries -- a branch of its own,
+            // so that the raw instantiations compile exactly as they did
+            char *const my_dst = (char *)my_dpos;
+            const bool direct = my_n != 0 && (((uint32_t)(uint64_t)my_dst | my_n | (my_pack >> 16)) & 15u) == 0;
+            if (direct) tma_store_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n);
+            unsigned todo = __ballot_sync(0xffffffffu, my_n != 0 && !direct);
+            while (todo) {
+                const int j = __ffs(todo) - 1;
+                todo &= todo - 1;
+                const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
+                const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
+                const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
+                drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane);
+            }
+        } else if constexpr (CVT) {
             // converting launch: a converted piece is always drained cooperatively; the raw variables of a multi-array
             // batch (code 0) keep the raw paths below
             int my_code;
@@ -1619,8 +1660,10 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         __syncwarp();  // all lanes are done reading the stage before it is refilled
         consumed++;
     }
-    if (a.overlap || (FIXED && push)) {
-        bulk_wait_all<0>(); // every lane: its bulk stores have been performed (the done / arrive word below promises that)
+    if (PUT || a.overlap || (FIXED && push)) {
+        // every lane: its bulk stores have been performed (the done / arrive word below promises that; a put's rows are
+        // complete when its last warp finishes)
+        bulk_wait_all<0>();
         fence_proxy_async_global();
     } else {
         bulk_wait_read<0>(); // every lane: its stages have been read out; the global writes complete with the grid
@@ -1790,6 +1833,8 @@ __device__ __forceinline__ unsigned long long tile_pack(unsigned int tag, unsign
            ((unsigned long long)v & 0xFFFFFFFFFFull);
 }
 
+// PUT: the plan of a batched put (plan_many's put form: an invalid request keeps its layout bytes, source address 0)
+template <bool PUT = false>
 __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_constant__ ddsk_var_t var,
                                                                 const __grid_constant__ PlanSrc p, int64_t nreq,
                                                                 uint64_t *__restrict__ req_src, int64_t *__restrict__ req_dst,
@@ -1811,7 +1856,7 @@ __global__ void __launch_bounds__(PLAN_THREADS) dds_plan_kernel(const __grid_con
     uint64_t sv[PLAN_ITEMS];
 #pragma unroll
     for (int k = 0; k < PLAN_ITEMS; k++) idx[k] = base + k;
-    plan_many<PLAN_ITEMS>(var, p, idx, nreq, status, status_tag, sv, nb); // (only reads: may run before the slot is known to be free)
+    plan_many<PLAN_ITEMS, PUT>(var, p, idx, nreq, status, status_tag, sv, nb); // (only reads: may run before the slot is known to be free)
     int64_t mine = 0;
 #pragma unroll
     for (int k = 0; k < PLAN_ITEMS; k++) mine += nb[k];
@@ -2006,13 +2051,16 @@ __global__ void __launch_bounds__(256) dds_doorbell_kernel(const ddsk_var_t *__r
         if (code) st = (unsigned long long)code;
         else if (n > cap) st = DDSK_CODE_CAPACITY;
         if (st == 0 && n > 0) {
+            // The row loads bypass L1 (ld.global.cg): this CTA stays resident across calls, and its SM's L1 is not
+            // coherent with writes from other SMs or GPUs -- a batched put by any rank -- so a cached line could
+            // return a row as it was before a put the caller has fenced since.
             const char *sp = (const char *)src;
             if ((((uint64_t)sp | (uint64_t)dp | (uint64_t)n) & 15u) == 0) {
-                for (int64_t i = threadIdx.x; i < (n >> 4); i += blockDim.x) ((uint4 *)dp)[i] = ((const uint4 *)sp)[i];
+                for (int64_t i = threadIdx.x; i < (n >> 4); i += blockDim.x) ((uint4 *)dp)[i] = __ldcg((const uint4 *)sp + i);
             } else if ((((uint64_t)sp | (uint64_t)dp | (uint64_t)n) & 3u) == 0) {
-                for (int64_t i = threadIdx.x; i < (n >> 2); i += blockDim.x) ((uint32_t *)dp)[i] = ((const uint32_t *)sp)[i];
+                for (int64_t i = threadIdx.x; i < (n >> 2); i += blockDim.x) ((uint32_t *)dp)[i] = __ldcg((const unsigned int *)sp + i);
             } else {
-                for (int64_t i = threadIdx.x; i < n; i += blockDim.x) dp[i] = sp[i];
+                for (int64_t i = threadIdx.x; i < n; i += blockDim.x) dp[i] = __ldcg(sp + i);
             }
             __threadfence_system(); // the payload is visible (host memory or HBM) before the answer is
         }
@@ -2142,12 +2190,12 @@ bool cvt_has_norm(const ddsk_cvt_t *cvt) {
     return false;
 }
 
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false>
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
     // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan)
     const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD>;
+    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD, PUT>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -2235,8 +2283,10 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
 }
 
 template <bool FIXED>
-int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
-    // converting launches: the default variant of each entry (kGeomLarge = kGeomVar), whatever DDS_GATHER_GEOM* say
+int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false) {
+    // converting launches and puts: the default variant of each entry (kGeomLarge = kGeomVar), whatever
+    // DDS_GATHER_GEOM* say
+    if (put) return launch_gather_t<FIXED, 12, 4, 4096, 0, false, false, false, true>(args, stream);
     if (cvt) return cvt_has_norm(cvt) ? launch_gather_t<FIXED, 12, 4, 4096, 0, true, true>(args, stream, cvt)
                                       : launch_gather_t<FIXED, 12, 4, 4096, 0, true>(args, stream, cvt);
     // (the request size only picks a variant: a count too large to multiply safely counts as large)
@@ -2252,7 +2302,10 @@ int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t 
     default: return launch_gather_t<FIXED, 8, 4, 4096, 0>(args, stream);
     }
 }
-int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
+int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put) {
+    if (put)
+        return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, false, false, false, true>(args, stream)
+                      : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true>(args, stream);
     if (cvt && cvt_has_norm(cvt))
         return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, true, true>(args, stream, cvt)
                       : launch_gather_t<false, 12, 3, 4096, 4096, true, true>(args, stream, cvt);
@@ -2268,11 +2321,13 @@ int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const dd
 }
 
 // The shared-memory-plan variant for a batch of nreq requests into cap bytes (-1: the plan kernels). Converting launches
-// use the default variants only (DDS_GATHER_GEOM_S applies to raw batches), and need room for their tables.
-int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt) {
+// use the default variants only (DDS_GATHER_GEOM_S applies to raw gets), and need room for their tables. Puts take the
+// raw gets' placement rule with the default variants.
+int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool put = false) {
     if (!g_smem_plan || cap >= ((int64_t)1 << 32)) return -1;
-    if (!cvt) return geometry_s_for(nreq);
+    if (!cvt && !put) return geometry_s_for(nreq);
     if (nreq > kPlanSmemMax || nreq > g_plan_smem_default) return -1;
+    if (put) return nreq <= 4096 ? 0 : 1;
     if (nreq <= 4096) return cvt_s_fits_t<12, 3, 4096, 4096>(cvt->lut_bytes) ? 0 : -1;
     return cvt_s_fits_t<12, 3, 3072, 8192>(cvt->lut_bytes) ? 1 : -1;
 }
@@ -2343,7 +2398,7 @@ int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t 
     a.min_seg_chunks = 1;
     fill_overlap(a, scr, flags);
     a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
-    return launch_gather<true>(a, st, cvt);
+    return launch_gather<true>(a, st, cvt, (flags & DDSK_F_PUT) != 0);
 }
 
 int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const ddsk_push_t *push_dev,
@@ -2420,13 +2475,14 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
-    const int gs = select_s(nreq, cap_total, cvt);
+    const bool put = (flags & DDSK_F_PUT) != 0;
+    const int gs = select_s(nreq, cap_total, cvt, put);
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
         fill_overlap(a, scr, flags); // no scratch is shared between launches: independent batches may overlap
         if (a.overlap) a.tickets = scr->ovl + 8 + (a.seq & 3u);
-        return launch_gather_s(gs, a, st, cvt);
+        return launch_gather_s(gs, a, st, cvt, put);
     }
     if (nreq > scr->cap_req || cap_total / SEG_GRAIN + 2 > scr->seg_cap) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_gather_var: scratch too small (%lld requests > %lld, or %lld segments > %lld)",
@@ -2454,7 +2510,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
         g_l2_base = p.tab ? (const void *)p.tab : (const void *)p.mtab[0];
         g_l2_bytes = (size_t)(p.tab ? p.nsamples : p.mnsamples[0]) * 16;
     }
-    if (int rc = launch_pdl(dds_plan_kernel, dim3(tiles), dim3(PLAN_THREADS), st, *var, p, nreq, scr->req_src, scr->req_dst,
+    if (int rc = launch_pdl(put ? dds_plan_kernel<true> : dds_plan_kernel<false>, dim3(tiles), dim3(PLAN_THREADS), st, *var, p, nreq, scr->req_src, scr->req_dst,
                             (unsigned long long *)scr->tile_sums, scr->plan_tag, offsets_dev_or_null, scr->seg_tab, scr->seg_cap,
                             scr->status, scr->status_tag, pr, cvt && p.nvars <= 1 ? (int)cvt->code[0] : 0))
         return rc;
@@ -2471,7 +2527,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
         a.plan_word = scr->plan_word;
         a.plan_tiles = tiles;
     }
-    return launch_gather<false>(a, st, cvt);
+    return launch_gather<false>(a, st, cvt, put);
 }
 
 int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt) {

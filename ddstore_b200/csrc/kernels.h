@@ -71,6 +71,12 @@ typedef struct ddsk_scratch {
 #define DDSK_F_PREV1 32     /* overlap launch ovl_seq-1 belongs to the same run (retire after it) */
 #define DDSK_F_PREV2 64     /* overlap launch ovl_seq-2 belongs to the same run (do not write before it retired) */
 #define DDSK_F_PREV4 128    /* overlap launch ovl_seq-4 belongs to the same run (it used the same plan scratch slot) */
+#define DDSK_F_PUT 256      /* a batched put (ddsk_gather_fixed / ddsk_gather_var, raw, never with DDSK_F_OVERLAP): the same
+                               walk with every copy reversed. dst_dev is the caller's packed SOURCE rows and dst_capacity
+                               its size; request i's bytes are taken from its packed position and written to its rows in
+                               the owner's shard. The layout keeps an invalid request's bytes (count * row_bytes when
+                               0 < count <= the variable's rows, else 0; 0 for a sample id outside the index); it writes
+                               nothing, like a layout above dst_capacity. No offsets. */
 
 /* Element conversion inside the gather (same values as DDS_CVT_* in include/ddstore_b200.h). Source byte p of a
  * variable's packed rows goes to output byte (p >> in_log2) << out_log2. */

@@ -229,6 +229,7 @@ struct dds_store {
     int64_t pending_nreq = 0;
     const int64_t *pending_total_ptr = nullptr; // device word holding the packed total of the last queued launch
     int pending_cvt = 0;                        // that word is in source bytes of this conversion (DDSK_CVT_*)
+    bool pending_put = false;                   // the pending queue holds a batched put (dds_epoch_begin completes it)
     ddsk_var_t *d_multi_vars = nullptr; // device copy of the windows of the last multi-array combination
     std::string multi_key;
     // overlap protocol (DDS_OVERLAP): sequence number of the next overlap launch, and how many overlap launches in a
@@ -748,6 +749,7 @@ void rearm_status(dds_store *s, cudaStream_t stream) {
 int drain_pending(dds_store *s) {
     if (!s->pending) return DDS_OK;
     s->pending = false;
+    s->pending_put = false;
     s->run_len = 0;
     cudaStream_t st = s->pending_stream;
     // queued launches skip the host mirror (it costs time at the end of every kernel): read the words back here
@@ -1727,6 +1729,123 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
                        cuda_stream, total_bytes, bad_index);
 }
 
+// The batched put behind dds_put_batch / dds_put_samples (by_sample: starts = sample ids): the gather's launch with every
+// copy reversed (DDSK_F_PUT). Request i's rows come from src bytes [o_i, o_i + n_i), n_i = req_bytes(count_i) even for
+// an invalid request, o_i the exclusive scan. Like batch_impl, the host knows the layout of a fixed count or of host
+// indices and leaves capacity and validation to the kernel. A put is never overlapped and never takes the
+// single-request kernels.
+static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
+                    int64_t fixed_count, int64_t nreq, const void *src, int64_t src_bytes, unsigned flags,
+                    void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    if (!(flags & DDS_SRC_ON_DEVICE)) return fail(DDS_ERR_ARG, "puts take their rows from device memory (DDS_SRC_ON_DEVICE)");
+    if (nreq < 0 || src_bytes < 0) return fail(DDS_ERR_ARG, "negative nreq or src_bytes");
+    if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
+    if (by_sample && !v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
+    const bool idx_dev = flags & DDS_IDX_ON_DEVICE, no_sync = flags & DDS_NO_SYNC;
+    if (no_sync && !idx_dev) return fail(DDS_ERR_ARG, "async puts need device indices");
+    const int64_t R = v->kv.row_bytes;
+    const bool fixed = !by_sample && counts == nullptr;
+    const int64_t rows = v->lenlist.empty() ? 0 : v->lenlist.back();
+    auto req_bytes = [&](int64_t c) { return c > 0 && c <= rows ? c * R : (int64_t)0; };
+    // ---- the layout total as far as the host can know it (-1: only the kernel knows it)
+    int64_t layout = -1;
+    if (fixed)
+        layout = sat_mul(nreq, req_bytes(fixed_count));
+    else if (!idx_dev && !by_sample) {
+        layout = 0;
+        for (int64_t i = 0; i < nreq; i++) layout = sat_add(layout, req_bytes(counts[i]));
+    } else if (!idx_dev && by_sample && !v->h_tab_count.empty()) {
+        layout = 0;
+        for (int64_t i = 0; i < nreq; i++) {
+            const int64_t id = starts[i];
+            if (id >= 0 && id < v->nsamples) layout = sat_add(layout, req_bytes(v->h_tab_count[(size_t)id]));
+        }
+    }
+    if (!src && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null src");
+
+    CU(cudaSetDevice(s->device));
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
+    const bool chain = s->pending && no_sync && st == s->pending_stream;
+    if (s->pending && !chain) {
+        if (int rc = drain_pending(s)) return rc;
+    }
+    if (nreq == 0) {
+        note_empty_async(s, no_sync);
+        return DDS_OK;
+    }
+    const int64_t *d_starts = starts, *d_counts = counts;
+    if (int rc = stage_indices(s, starts, !fixed && !by_sample ? counts : nullptr, nreq, idx_dev, st, &d_starts, &d_counts))
+        return rc;
+    const bool uses_scratch = !fixed && ddsk_var_uses_scratch(nreq, src_bytes, nullptr);
+    if (uses_scratch) {
+        if (int rc = renew_plan_tags(s)) return rc;
+        if (int rc = ensure_scratch(s, nreq, src_bytes)) return rc;
+    }
+    if (int rc = tag_launch(s, chain)) return rc;
+    // (overlap_flags(.., false, ..) ends any overlap run: the next overlapped batch starts a new one and waits for the grid)
+    const int kflags = DDSK_F_PUT | (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, false, chain);
+    ddsk_scratch_t scr = scratch_view(s, false);
+    int krc;
+    if (fixed) {
+        krc = ddsk_gather_fixed(&v->kv, d_starts, fixed_count, nreq, const_cast<void *>(src), src_bytes, nullptr, &scr, kflags,
+                                nullptr, st);
+    } else {
+        ddsk_index_t ix;
+        memset(&ix, 0, sizeof(ix));
+        if (by_sample) {
+            ix.sample_ids = d_starts;
+            ix.table = v->d_tab;
+            ix.nsamples = v->nsamples;
+        } else {
+            ix.starts = d_starts;
+            ix.counts = d_counts;
+        }
+        krc = ddsk_gather_var(&v->kv, &ix, nreq, const_cast<void *>(src), src_bytes, nullptr, &scr, kflags, nullptr, st);
+        s->scr.plan_tag = scr.plan_tag;
+        s->pending_total_ptr = uses_scratch ? &scr.req_dst[nreq] : scr.total;
+    }
+    if (krc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
+    s->pending_fixed_total = fixed ? layout : -1;
+    s->pending_cvt = DDSK_CVT_NONE;
+    s->pending_nreq = nreq;
+    if (no_sync) {
+        s->pending = true;
+        s->pending_put = true;
+        s->pending_stream = st;
+        return DDS_OK;
+    }
+    CU(cudaStreamSynchronize(st)); // status + total arrive in the pinned mirror words with the end of the kernel
+    if (total_bytes) *total_bytes = fixed ? layout : (int64_t)s->h_status[1];
+    return decode_status(s, st, s->h_status[0], bad_index);
+}
+
+int dds_put_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts, int64_t fixed_count,
+                  int64_t nreq, int itemsize, const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream,
+                  int64_t *total_bytes, int64_t *bad_index) {
+    clear_error();
+    if (bad_index) *bad_index = -1;
+    if (total_bytes) *total_bytes = 0;
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    Var *v = find_var(s, name);
+    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE); // ddstore.hpp:189-190, as update() reports it
+    return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
+                    bad_index);
+}
+
+int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
+                    const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                    int64_t *bad_index) {
+    clear_error();
+    if (bad_index) *bad_index = -1;
+    if (total_bytes) *total_bytes = 0;
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    Var *v = find_var(s, name);
+    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
+    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index);
+}
+
 // The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,
 // or NULL for raw bytes)
 static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const int64_t *sample_ids, int64_t nreq,
@@ -2002,6 +2121,9 @@ int dds_epoch_begin(dds_store_t *s) {
     for (auto &x : s->vars)
         if (x.second.fence_active) return fail(DDS_ERR_FENCE_ACTIVE);
     CU(cudaSetDevice(s->device));
+    // queued puts are part of the epoch that ends here (a queue of gets is left to dds_batch_wait)
+    if (s->pending_put)
+        if (int rc = drain_pending(s)) return rc;
     CU(cudaStreamSynchronize(s->stream));
     if (int rc = drain_update_streams(s)) return rc; // dds_update_async copies on caller streams are part of the epoch
     if (int rc = dds_comm_barrier(s->comm)) return rc;

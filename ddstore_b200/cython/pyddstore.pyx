@@ -54,6 +54,8 @@ cdef extern from "ddstore_b200.hpp" nogil:
                                       long* lengths, cbool idx_on_device, void* stream) except +dds_translate_exception
         void set_normalization(string name, const float* mean, const float* std, long nchan, long inner,
                                cbool tables_on_device) except +dds_translate_exception
+        long put_batch[T](string name, const long* starts, const long* counts, long fixed_count, long nreq, const T* src,
+                          long src_bytes, cbool idx_on_device, void* stream) except +dds_translate_exception
         void epoch_begin() except +dds_translate_exception
         void epoch_end() except +dds_translate_exception
         void free() except +dds_translate_exception
@@ -249,6 +251,44 @@ cdef class PyDDStore:
                                                             <const void*> lp, max_rows, bits, <void*> dp, cap,
                                                             <long*> lnp, idx_dev, <void*> st)
         del keep, lut_keep
+        return total
+
+    def put_batch(self, str name, starts, counts=None, src=None, count=None, stream=None):
+        """one kernel launch writing len(starts) requests from the CUDA tensor `src` into the owners' shards; see
+        ddstore_b200.store.PyDDStore.put_batch (this binding's put is synchronous). Returns the layout's bytes."""
+        if src is None:
+            raise ValueError("a put needs `src` rows")
+        if not (hasattr(src, "data_ptr") and getattr(src, "is_cuda", False)):
+            raise ValueError(f"put into {name!r}: src must be a CUDA tensor (copy host rows to the device first)")
+        if not src.is_contiguous():
+            raise ValueError("src must be C-contiguous")
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        cdef size_t sp, cp = 0, dp = src.data_ptr()
+        cdef long nreq
+        if s_dev:
+            nreq = starts.numel(); sp = starts.data_ptr()
+            if counts is not None: cp = counts.data_ptr()
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
+            ca = _i64(counts) if counts is not None else None
+            if ca is not None: cp = ca.ctypes.data
+            keep = (sa, ca)
+        cdef long fixed = 1 if count is None else int(count)
+        cdef int w = src.element_size()
+        cdef long nbytes = src.numel() * w
+        cdef size_t st = 0
+        if stream is not None:
+            st = int(stream) if int(stream) != 0 else 1
+        cdef string nm = name.encode()
+        cdef cbool idx_dev = bool(s_dev)
+        cdef long total
+        with nogil:
+            if w == 1: total = self.c_ddstore.put_batch[char](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const char*> dp, nbytes, idx_dev, <void*> st)
+            elif w == 2: total = self.c_ddstore.put_batch[short](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const short*> dp, nbytes, idx_dev, <void*> st)
+            elif w == 4: total = self.c_ddstore.put_batch[int](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const int*> dp, nbytes, idx_dev, <void*> st)
+            else: total = self.c_ddstore.put_batch[long](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const long*> dp, nbytes, idx_dev, <void*> st)
+        del keep
         return total
 
     def set_normalization(self, str name, mean, std, long inner=1):

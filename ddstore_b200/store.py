@@ -346,6 +346,78 @@ class PyDDStore:
         _capi.raise_for(rc)
         return total.value
 
+    # ---------------------------------------------------------------- batched puts (update<T> from any rank)
+    def put_batch(self, name, starts, counts=None, src=None, count=None, stream=None, wait=True):
+        """Write len(starts) requests into the owners' shards in ONE kernel launch -- update() from any rank, the dual
+        of get_batch (MPI_Put between fences). Request i writes global rows [starts[i], starts[i] + counts[i]) (or
+        `count` rows, default 1, when counts is None) from `src`, a C-contiguous CUDA tensor of any shape whose element
+        size is the variable's itemsize. src holds the requests' rows back to back in request order; an invalid
+        request keeps its counts[i] rows' worth of bytes in that layout (0 when counts[i] <= 0 or above the variable's
+        rows), so the requests after it are read where the caller put them. Returns the layout's size in bytes.
+        Raises the reference's ValueError for the first invalid request (last_bad_index: its index); every VALID
+        request is still written, an invalid one writes nothing. A layout larger than src writes nothing at all.
+        A host `src` raises ValueError (copy it to the device first). wait=False (device indices only): enqueue on
+        `stream` and return; wait() reports the outcome. Other ranks see the rows after the next epoch fence both
+        sides have passed (epoch_begin / epoch_end complete queued puts); later work on the same stream sees them at
+        once. Two writes to the same bytes in one epoch leave one writer's byte; reading rows being put in the same
+        epoch is undefined."""
+        sb, keep_src = self._put_src(name, src)
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        if s_dev:
+            nreq, sp = starts.numel(), starts.data_ptr()
+            cp = counts.data_ptr() if counts is not None else None
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts)
+            ca = _i64(counts) if counts is not None else None
+            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
+            keep = (sa, ca)
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_put_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq, sb.itemsize,
+                                   sb.ptr, sb.nbytes, flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    def put_samples(self, name, sample_ids, src, stream=None, wait=True):
+        """put_batch by SAMPLE ID: request i writes the rows of sample sample_ids[i] in the index registered with
+        set_sample_index. Same layout, error behaviour (every valid request is still written), ordering and
+        visibility as put_batch; a sample id outside the index keeps 0 bytes of the layout."""
+        sb, keep_src = self._put_src(name, src)
+        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
+        if s_dev:
+            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
+        else:
+            sa = _i64(sample_ids)
+            nreq, sp, keep = sa.size, sa.ctypes.data, sa
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_put_samples(self._h, name.encode(), sp, nreq, sb.itemsize, sb.ptr, sb.nbytes, flags,
+                                     self._stream_arg(stream), C.byref(total), C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    @staticmethod
+    def _put_src(name, src):
+        """the _Buf of a put's source rows (a CUDA tensor or CAI object; ValueError for host memory)"""
+        if src is None:
+            raise ValueError("a put needs `src` rows")
+        if hasattr(src, "data_ptr") and hasattr(src, "element_size"):  # any torch dtype: only its element size matters
+            if not src.is_contiguous():
+                raise ValueError("src must be C-contiguous")
+            sb = _Buf.__new__(_Buf)
+            sb.ptr, sb.on_device, sb.itemsize = src.data_ptr(), 1 if src.is_cuda else 0, src.element_size()
+            sb.nbytes = src.numel() * sb.itemsize
+        else:
+            sb = _Buf(src)
+        if not sb.on_device:
+            raise ValueError(f"put into {name!r}: src must be device memory (copy host rows to the device first)")
+        return sb, src
+
     # ---------------------------------------------------------------- collective owner-push fetch
     def push_setup(self, max_requests, max_bytes):
         """COLLECTIVE: allocate and peer-map the windows of the push fetch (see dds_push_setup)."""
@@ -545,8 +617,8 @@ class PyDDStore:
         order (last_bad_index: its first invalid request); returns the packed bytes of the last batch queued since the
         previous wait() (0 if none).
         wait() alone reports the outcome of queued batches, exactly once. Any other call that meets a pending queue
-        (a synchronous get_batch / get / get_samples / get_samples_multi, a batch on another stream, set_sample_index,
-        set_normalization, epoch_end, free) completes it, keeps its first failure for the next wait(), and raises only
+        (a synchronous get_batch / get / get_samples / get_samples_multi / put_batch / put_samples, a batch on another
+        stream, set_sample_index, set_normalization, epoch_end, epoch_begin when the queue holds a put, free) completes it, keeps its first failure for the next wait(), and raises only
         for its own requests. A failure kept from earlier wins over later ones; after wait() has raised it, the next
         wait() is clean. close() drops an outcome no wait() has reported."""
         total, bad = C.c_int64(0), C.c_int64(-1)

@@ -24,7 +24,8 @@ extern "C" {
 
 #define DDS_VERSION 111 /* 110: converting batches (dds_get_batch_convert & co.); 111: normalising conversions.
                            The padded batches (dds_get_batch_padded, dds_get_samples_padded) add entries only: callers
-                           that built against 111 are unaffected, and a caller finds them by symbol. */
+                           that built against 111 are unaffected, and a caller finds them by symbol. So do the batched
+                           puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -274,6 +275,45 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
                            const dds_convert_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity, unsigned flags,
                            void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
 
+/* ---- batched puts: rows written into ANY rank's shard from this GPU (update<T> from any rank / MPI_Put between fences)
+ * The dual of dds_get_batch / dds_get_samples. Request i writes global rows [start_i, start_i + count_i) of `name` (count_i
+ * = counts[i], or fixed_count when counts == NULL); for dds_put_samples it is sample sample_ids[i]'s (row_start,
+ * row_count) from the sample index. The rows are raw, in the variable's dtype.
+ * Layout of src: request i's rows are src bytes [o_i, o_i + n_i), where n_i = count_i * disp * itemsize when
+ * 0 < count_i <= the variable's total rows and 0 otherwise (0 for a sample id outside the index), and o_i is the
+ * exclusive scan of the n_i. Unlike the packed get, an INVALID request keeps its bytes in the layout: the caller built
+ * src from its own counts, so the requests after it find their rows where the caller put them. *total_bytes = the layout
+ * total sum n_i. src may have any byte alignment.
+ * Validation: requests are checked by dds_get_batch's rules, with its codes, texts and documented divergences (a negative
+ * count, or one for which start + count overflows, is "Invalid count on target"); a sample id outside the index is
+ * DDS_ERR_ARG, "sample id outside the variable's sample index", as in dds_get_samples. An invalid request writes nothing;
+ * EVERY valid request is written, as in the padded entries; the first (lowest-index) invalid request's code and index are
+ * returned. If the layout total exceeds src_bytes, nothing at all is written: DDS_ERR_CAPACITY (*bad_index = -1), unless
+ * a request is invalid -- then that request's error is reported, as in dds_get_batch.
+ * Argument errors, DDS_ERR_ARG with nothing enqueued: flags without DDS_SRC_ON_DEVICE (a host src: copy it to the device
+ * first), nreq < 0, src_bytes < 0, src == NULL with src_bytes > 0 or with a layout the host knows to be non-empty (fixed
+ * count, or host indices; with device indices an empty src is the kernel's DDS_ERR_CAPACITY), DDS_NO_SYNC with host
+ * indices, and dds_put_samples on a variable without a sample index. An itemsize other than the variable's is
+ * DDS_ERR_DTYPE ("Invalid data type", ddstore.hpp:189-190, as update reports it). nreq = 0 writes nothing and returns
+ * DDS_OK with *total_bytes = 0.
+ * Flags: DDS_IDX_ON_DEVICE as in the get entries (host indices are staged the same way). DDS_NO_SYNC queues the put on
+ * cuda_stream; dds_batch_wait reports it like a queued get, *total_bytes being its layout total. DDS_OVERLAP is ignored:
+ * a put is never overlapped with the launch before it or after it. It ends an overlap run, so the next DDS_OVERLAP batch
+ * starts a new run, whose first launch waits for the grid before it.
+ * Ordering and visibility: later work on the same stream sees the rows; a synchronous put returns after its rows are
+ * written; other ranks see them after the next fence (dds_epoch_begin or dds_epoch_end) that both sides have passed.
+ * Both fences complete a pending queue that holds a put (dds_epoch_begin leaves a queue of gets alone).
+ * Conflicts are undefined, as for conflicting MPI_Puts: two writes to the same bytes in one epoch -- from one batch or
+ * from several ranks -- leave each byte equal to that byte of one of the writers; a read of rows that are being put in
+ * the same epoch returns undefined bytes; a src that overlaps a shard gives undefined rows. */
+#define DDS_SRC_ON_DEVICE 2u /* dds_put_*: the packed source rows are device memory (same bit as DDS_DST_ON_DEVICE); required */
+int dds_put_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts, int64_t fixed_count,
+                  int64_t nreq, int itemsize, const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream,
+                  int64_t *total_bytes, int64_t *bad_index);
+int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
+                    const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                    int64_t *bad_index);
+
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite
  * flow. When all ranks fetch in the same
@@ -292,7 +332,7 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
  * failing batch in queue order is reported, with that batch's first invalid request in *bad_index.
  * The outcome of queued batches is reported here and only here, exactly once. Any other call that meets a pending
  * queue (a synchronous batch or get(), a batch on another stream, dds_set_sample_index, dds_set_normalization,
- * dds_epoch_end, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
+ * dds_epoch_end, dds_epoch_begin when the queue holds a put, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
  * then does its own work and reports only its own outcome (its error and *bad_index describe its own requests). The
  * next dds_batch_wait reports the kept failure, with its index and text, after completing any queue still pending; a
  * failure kept from earlier wins over any failure queued after it, since it is earlier in queue order. After it has

@@ -150,6 +150,30 @@ class DDStore {
                                     &total, &bad));
         return (long)total;
     }
+    // Batched put (dds_put_batch): request i writes global rows [starts[i], starts[i] + counts[i]) (counts == nullptr:
+    // fixed_count rows) into the owner's shard, from src (device memory), which holds the requests' rows back to back in
+    // request order -- an invalid request keeps its rows' bytes in that layout. Every valid request is written; the
+    // first invalid one throws like get_batch. Other ranks see the rows after the next epoch fence. Returns the layout's
+    // bytes. idx_on_device: starts / counts are device pointers.
+    template <typename T>
+    long put_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq, const T *src,
+                   long src_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_put_batch(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts, fixed_count, nreq,
+                            (int)sizeof(T), src, src_bytes, flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    // The same by sample id (dds_put_samples): request i = the rows of sample sample_ids[i] in the sample index.
+    template <typename T>
+    long put_samples(std::string name, const long *sample_ids, long nreq, const T *src, long src_bytes,
+                     bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_put_samples(store_, name.c_str(), (const int64_t *)sample_ids, nreq, (int)sizeof(T), src, src_bytes, flags,
+                              cuda_stream, &total, &bad));
+        return (long)total;
+    }
     // device-pointer variants of add/get for callers that already hold the data in HBM
     template <typename T>
     void add_device(std::string name, const T *dev_buffer, long nrows, int disp) {
