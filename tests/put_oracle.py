@@ -80,6 +80,17 @@ def put(shards, src, src_bytes=None, **req):
     return new, codes, bad, total
 
 
+def put_many(shards, calls):
+    """Apply `calls` = [(src, src_bytes or None, request keywords)] one after the other (any ranks' calls of one epoch:
+    each is a put() of its own) -> (new shards, [(status code, bad index, layout total)] as each call reports them)"""
+    out = []
+    for src, src_bytes, req in calls:
+        sb = np.asarray(src).size if src_bytes is None else src_bytes
+        shards, codes, bad, total = put(shards, src, src_bytes=sb, **req)
+        out.append(expected_error(codes, bad, total, sb) + (total,))
+    return shards, out
+
+
 def expected_error(codes, bad, total, src_bytes):
     """(status code, bad index) the entry reports: the first invalid request's, else CODE_CAPACITY (-1) when the layout
     does not fit, else (0, -1)"""

@@ -15,6 +15,7 @@ import pytest
 
 from tests import put_oracle as po
 from tests.gpu_helpers import padded_requests, run_world, sweep_requests
+from tests.put_world import dense_cover
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -28,44 +29,55 @@ CONFIGS = {"default": {},
 
 
 # ------------------------------------------------------------------------------------------------ helpers
-def dev_bytes(torch, ptr, n):
+def dev_bytes(torch, ptr, n, device="cuda:0"):
     """n bytes of device memory at ptr, copied to the host"""
     from ddstore_b200.store import _DevMem
-    torch.cuda.synchronize()
-    return torch.as_tensor(_DevMem(ptr, n), device="cuda:0").cpu().numpy().copy() if n else np.zeros(0, np.uint8)
+    torch.cuda.synchronize(device)
+    return torch.as_tensor(_DevMem(ptr, n), device=device).cpu().numpy().copy() if n else np.zeros(0, np.uint8)
 
 
-def shard_state(torch, store, name, payload):
+def shard_state(torch, store, name, payload, device="cuda:0"):
     """the local shard's rows and its slack (the 16 bytes every shard keeps past its rows, up to the 256-byte
     allocation granule)"""
     slack = ((payload + 16 + 255) // 256) * 256 - payload
-    return dev_bytes(torch, store.query(name)["local_base"], payload + slack), slack
+    return dev_bytes(torch, store.query(name)["local_base"], payload + slack, device), slack
 
 
-def to_device(torch, data, off):
+def to_device(torch, data, off, device="cuda:0"):
     """a device copy of the bytes `data` starting `off` bytes past a 16-byte boundary; returns (keepalive, pointer)"""
-    buf = torch.empty(off + data.size + 16, dtype=torch.uint8, device="cuda:0")
+    buf = torch.empty(off + data.size + 16, dtype=torch.uint8, device=device)
     if data.size:
         buf[off:off + data.size].copy_(torch.from_numpy(data))
-    torch.cuda.synchronize()
+    torch.cuda.synchronize(device)
     return buf, buf.data_ptr() + off
+
+
+def _index(x):
+    """(keepalive, pointer, length, IDX_ON_DEVICE or 0) of an index array: a CUDA int64 tensor as it is, anything else as
+    a host int64 array"""
+    from ddstore_b200 import _capi
+    if hasattr(x, "data_ptr"):
+        return x, x.data_ptr(), x.numel(), _capi.IDX_ON_DEVICE
+    a = np.ascontiguousarray(x, np.int64)
+    return a, a.ctypes.data, a.size, 0
 
 
 def raw_put(store, name, itemsize, src_ptr, src_bytes, starts=None, counts=None, fixed=1, ids=None, flags=0,
             stream=None):
-    """the C-ABI entry itself (any itemsize; src at any byte address) -> (rc, total, bad)"""
+    """the C-ABI entry itself (any itemsize; src at any byte address; host index arrays, or CUDA int64 tensors)
+    -> (rc, total, bad)"""
     from ddstore_b200 import _capi
     L, total, bad = store._L, C.c_int64(0), C.c_int64(-1)
     fl = _capi.SRC_ON_DEVICE | flags
     if ids is not None:
-        ia = np.ascontiguousarray(ids, np.int64)
-        rc = L.dds_put_samples(store._h, name.encode(), ia.ctypes.data, ia.size, itemsize, src_ptr, src_bytes, fl, stream,
+        keep, ip, n, dev = _index(ids)
+        rc = L.dds_put_samples(store._h, name.encode(), ip, n, itemsize, src_ptr, src_bytes, fl | dev, stream,
                                C.byref(total), C.byref(bad))
     else:
-        sa = np.ascontiguousarray(starts, np.int64)
-        ca = np.ascontiguousarray(counts, np.int64) if counts is not None else None
-        rc = L.dds_put_batch(store._h, name.encode(), sa.ctypes.data, ca.ctypes.data if ca is not None else None, fixed,
-                             sa.size, itemsize, src_ptr, src_bytes, fl, stream, C.byref(total), C.byref(bad))
+        keep, sp, n, dev = _index(starts)
+        keep2, cp = (None, None) if counts is None else _index(counts)[:2]
+        rc = L.dds_put_batch(store._h, name.encode(), sp, cp, fixed, n, itemsize, src_ptr, src_bytes, fl | dev, stream,
+                             C.byref(total), C.byref(bad))
     return rc, total.value, bad.value
 
 
@@ -150,6 +162,7 @@ def inject_invalid(rng, starts, counts, rows, where):
 
 # ------------------------------------------------------------------------------------------------ the sweep
 SHAPES = {1: (1, 13 << 20), 2: (3, (13 << 20) // 6), 4: (5, (13 << 20) // 20), 8: (3, (13 << 20) // 24)}
+DENSE_ROWS = 16400  # rows of the small second variable that the dense batches write completely
 
 
 def put_sweep_main():
@@ -187,6 +200,18 @@ def put_sweep_main():
             w.check(torch, store, f"[{cfg}] itemsize {itemsize} invalid ids", sample_ids=np.where(np.isin(np.arange(ids.size), where), -5, ids), table=table)
         w.check(torch, store, f"[{cfg}] itemsize {itemsize} capacity", src_bytes=int(counts.sum()) * R - 1, starts=starts, counts=counts)
         w.check(torch, store, f"[{cfg}] itemsize {itemsize} fixed capacity", src_bytes=300 * 3 * R - 1, starts=fs, fixed_count=3)
+        # the dense form: each batch writes EVERY row of a small second variable exactly once, so every piece's
+        # neighbours are written by other warps and CTAs of the same launch and a write wider than its piece is seen.
+        # Batch sizes on both sides of the plan thresholds again: the placement decides who computes the shard addresses
+        ds, dc = dense_cover(rng, DENSE_ROWS, 4097)
+        d = World(torch, store, f"d{itemsize}", itemsize, disp, DENSE_ROWS, 100 + itemsize, (ds.copy(), dc.copy()))
+        d.check(torch, store, f"[{cfg}] itemsize {itemsize} dense sample ids", src_off=9, sample_ids=rng.permutation(4097), table=d.table)
+        for n in (1024, 1025, 4096, 4097, 8192, 8193):
+            ds, dc = dense_cover(rng, DENSE_ROWS, n)
+            d.check(torch, store, f"[{cfg}] itemsize {itemsize} dense n={n}", src_off=n % 16, starts=ds, counts=dc)
+        for cnt in (1, 4):
+            d.check(torch, store, f"[{cfg}] itemsize {itemsize} dense fixed {cnt}", src_off=5 * cnt,
+                    starts=rng.permutation(DENSE_ROWS // cnt) * cnt, fixed_count=cnt)
     store.free()
     store.close()
 
@@ -203,7 +228,8 @@ print("put-sweep-ok")
 @pytest.mark.parametrize("config", list(CONFIGS))
 def test_put_sweep(tmp_path, config):
     """raw itemsizes 1/2/4/8 over the variant sweep's request sizes, src at base offsets 0/1/4/8/13, every entry,
-    batch sizes around the plan thresholds, invalid requests and capacity errors, in the environment of `config`"""
+    batch sizes around the plan thresholds, invalid requests and capacity errors, and batches that write every row of
+    a small variable exactly once, in the environment of `config`"""
     script = tmp_path / "put_sweep.py"
     script.write_text(SWEEP_SCRIPT.format(root=ROOT))
     env = {k: v for k, v in os.environ.items() if not k.startswith("DDS_") or k == "DDS_COMM_TIMEOUT_S"}
