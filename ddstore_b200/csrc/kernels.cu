@@ -2332,7 +2332,17 @@ int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool put = false)
     return cvt_s_fits_t<12, 3, 3072, 8192>(cvt->lut_bytes) ? 1 : -1;
 }
 
-void fill_overlap(GatherArgs &a, const ddsk_scratch_t *scr, int flags) {
+// The fields every gather launch shares: the variable's window, status reporting, the host mirror (DDSK_F_MIRROR), the
+// overlap protocol and segment tickets, and the default smallest segment. Picks the geometry on first use.
+int gather_args(GatherArgs &a, const ddsk_var_t *var, const ddsk_scratch_t *scr, int flags) {
+    if (int rc = pick_geometry()) return rc;
+    memset(&a, 0, sizeof(a));
+    a.var = *var;
+    a.status = scr->status;
+    a.status_tag = scr->status_tag;
+    a.counters = scr->counters;
+    a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
+    a.min_seg_chunks = 1;
     a.overlap = (flags & DDSK_F_OVERLAP) ? 1 : 0;
     a.skip_wait = (flags & DDSK_F_SKIP_WAIT) ? 1 : 0;
     a.wait1_valid = (flags & DDSK_F_PREV1) ? 1 : 0;
@@ -2344,6 +2354,7 @@ void fill_overlap(GatherArgs &a, const ddsk_scratch_t *scr, int flags) {
     // GPU either); the variable-count entries set the slot's own word below (their CTAs
     // may start late, behind the plan kernel, and must not keep a fixed share of the work).
     a.tickets = a.overlap ? nullptr : scr->counters;
+    return 0;
 }
 
 } // namespace
@@ -2379,45 +2390,27 @@ void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk
 int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t count, int64_t nreq, void *dst_dev,
                       int64_t dst_capacity, int64_t *offsets_dev_or_null, const ddsk_scratch_t *scr, int flags,
                       const ddsk_cvt_t *cvt, void *stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
     if (nreq <= 0) return 0;
-    if (int rc = pick_geometry()) return rc;
     GatherArgs a;
-    memset(&a, 0, sizeof(a));
-    a.var = *var;
+    if (int rc = gather_args(a, var, scr, flags)) return rc;
     a.starts = starts_dev;
     a.count = count;
     a.nreq = nreq;
     a.dst = (char *)dst_dev;
     a.dst_cap = dst_capacity;
     a.offsets_out = offsets_dev_or_null;
-    a.status = scr->status;
-    a.status_tag = scr->status_tag;
-    a.counters = scr->counters;
-    a.min_seg_chunks = 1;
-    fill_overlap(a, scr, flags);
-    a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
-    return launch_gather<true>(a, st, cvt, (flags & DDSK_F_PUT) != 0);
+    return launch_gather<true>(a, (cudaStream_t)stream, cvt, (flags & DDSK_F_PUT) != 0);
 }
 
 int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const ddsk_push_t *push_dev,
                      const int64_t *starts_dev, int64_t count, int64_t nreq, unsigned long long step,
                      const ddsk_scratch_t *scr, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (int rc = pick_geometry()) return rc;
     GatherArgs a;
-    memset(&a, 0, sizeof(a));
-    a.var = *var;
+    if (int rc = gather_args(a, var, scr, 0)) return rc;
     a.count = count;
     a.nreq = nreq; // (this rank's own requests; the walk covers every rank's)
-    a.dst = nullptr;
     a.dst_cap = INT64_MAX;
-    a.status = scr->status;
-    a.status_tag = scr->status_tag;
-    a.counters = scr->counters;
-    a.tickets = scr->counters;
-    a.min_seg_chunks = 1;
     a.push = push_dev;
     if (nreq > 0) // this rank's list into its window, stream-ordered before the kernel that publishes it
         CUDA_TRY(cudaMemcpyAsync(push_host->win[push_host->me] + push_host->idx_off[step & 1ull], starts_dev, (size_t)nreq * 8,
@@ -2431,12 +2424,9 @@ int ddsk_gather_padded(const ddsk_var_t *var, const ddsk_index_t *index, int64_t
                        int pad_log2, int64_t *lengths, void *dst_dev, const ddsk_scratch_t *scr, int flags,
                        const ddsk_cvt_t *cvt, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
     if (nreq <= 0) return 0;
-    if (int rc = pick_geometry()) return rc;
     GatherArgs a;
-    memset(&a, 0, sizeof(a));
-    a.var = *var;
+    if (int rc = gather_args(a, var, scr, flags)) return rc;
     a.plan.starts = index->starts;
     a.plan.counts = index->counts;
     a.plan.ids = index->sample_ids;
@@ -2452,27 +2442,18 @@ int ddsk_gather_padded(const ddsk_var_t *var, const ddsk_index_t *index, int64_t
     a.pad_in_log2 = cvt ? cvt_in_log2<true>(cvt->code[0]) : 0;
     a.pad_out_log2 = cvt ? cvt_out_log2<true>(cvt->code[0]) : 0;
     a.pad_lengths = lengths;
-    a.status = scr->status;
-    a.status_tag = scr->status_tag;
-    a.counters = scr->counters;
-    a.min_seg_chunks = 1;
-    fill_overlap(a, scr, flags);
-    a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
     // the default fixed-count geometry, whatever DDS_GATHER_GEOM says
     if (!cvt) return launch_gather_t<true, 12, 4, 4096, 0, false, false, true>(a, st);
     return cvt_has_norm(cvt) ? launch_gather_t<true, 12, 4, 4096, 0, true, true, true>(a, st, cvt)
                              : launch_gather_t<true, 12, 4, 4096, 0, true, false, true>(a, st, cvt);
 }
 
-// shared by ddsk_gather_var / ddsk_gather_multi: plan (in the launch, or by the two plan kernels) + gather
+// shared by ddsk_gather_var / ddsk_gather_multi: plan (in the launch, or by the two plan kernels) + gather. `a` comes
+// from gather_args.
 static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq, int64_t cap_total, GatherArgs &a,
                            int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt,
                            cudaStream_t st) {
     a.nreq = nreq;
-    a.status = scr->status;
-    a.status_tag = scr->status_tag;
-    a.counters = scr->counters;
-    a.host_mirror = (flags & DDSK_F_MIRROR) ? scr->host_mirror : nullptr;
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
     const bool put = (flags & DDSK_F_PUT) != 0;
@@ -2480,7 +2461,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
-        fill_overlap(a, scr, flags); // no scratch is shared between launches: independent batches may overlap
+        // (no scratch is shared between launches: independent batches may overlap)
         if (a.overlap) a.tickets = scr->ovl + 8 + (a.seq & 3u);
         return launch_gather_s(gs, a, st, cvt, put);
     }
@@ -2520,7 +2501,6 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     // (a converting multi-array batch has no single source total: its gather writes the output total here)
     a.total_out = (cvt && p.nvars > 1) ? scr->total : nullptr;
     a.min_seg_chunks = g_min_seg_var;
-    fill_overlap(a, scr, flags);
     if (a.overlap) {
         a.tickets = scr->ovl + 8 + (a.seq & 3u);
         a.wait_plan = 1; // (a.skip_wait: inside a run the gather skips the grid wait and spins on the plan-ready word)
@@ -2537,10 +2517,9 @@ int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *
 
 int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, void *dst_dev, int64_t dst_capacity,
                     int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt, void *stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
     if (nreq <= 0) return 0;
-    if (int rc = pick_geometry()) return rc;
+    GatherArgs a;
+    if (int rc = gather_args(a, var, scr, flags)) return rc;
     PlanSrc p;
     memset(&p, 0, sizeof(p));
     p.starts = index->starts;
@@ -2548,24 +2527,22 @@ int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nr
     p.ids = index->sample_ids;
     p.tab = (const longlong2 *)index->table;
     p.nsamples = index->nsamples;
-    GatherArgs a;
-    memset(&a, 0, sizeof(a));
-    a.var = *var;
     a.dst = (char *)dst_dev;
     a.dst_cap = dst_capacity;
-    return plan_and_gather(var, p, nreq, dst_capacity, a, offsets_dev_or_null, scr, flags, cvt, st);
+    return plan_and_gather(var, p, nreq, dst_capacity, a, offsets_dev_or_null, scr, flags, cvt, (cudaStream_t)stream);
 }
 
 int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int64_t nreq, ddsk_scratch_t *scr, int flags,
                       const ddsk_cvt_t *cvt, void *stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (flags & DDSK_F_RESET) CUDA_TRY(cudaMemsetAsync(scr->status, 0xFF, sizeof(unsigned long long), st));
     if (nreq <= 0 || m->nvars <= 0) return 0;
     if (m->nvars > DDSK_MAX_MULTI) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_gather_multi: more than %d variables", DDSK_MAX_MULTI);
         return -2;
     }
-    if (int rc = pick_geometry()) return rc;
+    ddsk_var_t dummy; // (each variable's window is read from m->vars_dev)
+    memset(&dummy, 0, sizeof(dummy));
+    GatherArgs a;
+    if (int rc = gather_args(a, &dummy, scr, flags)) return rc;
     PlanSrc p;
     memset(&p, 0, sizeof(p));
     p.ids = sample_ids_dev;
@@ -2579,18 +2556,13 @@ int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int6
         cap_total += m->cap[v]; // (saturation is irrelevant: anything >= 4 GiB selects the plan kernels)
         if (cap_total < 0 || m->cap[v] < 0) cap_total = INT64_MAX / 2;
     }
-    ddsk_var_t dummy;
-    memset(&dummy, 0, sizeof(dummy));
-    GatherArgs a;
-    memset(&a, 0, sizeof(a));
-    a.dst = nullptr;
     a.dst_cap = INT64_MAX;
     for (int v = 0; v < m->nvars; v++) {
         a.mdst[v] = (char *)m->dst[v];
         a.mcap[v] = m->cap[v];
         a.moffsets[v] = m->offsets[v];
     }
-    return plan_and_gather(&dummy, p, nreq * m->nvars, cap_total, a, nullptr, scr, flags, cvt, st);
+    return plan_and_gather(&dummy, p, nreq * m->nvars, cap_total, a, nullptr, scr, flags, cvt, (cudaStream_t)stream);
 }
 
 int ddsk_small_get(const ddsk_var_t *var, int64_t start, int64_t count, void *dst, int64_t dst_capacity,

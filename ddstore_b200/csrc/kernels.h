@@ -63,7 +63,6 @@ typedef struct ddsk_scratch {
 } ddsk_scratch_t;
 
 /* `flags` of the launchers */
-#define DDSK_F_RESET 1      /* reset the status word first */
 #define DDSK_F_MIRROR 2     /* the kernel's last warp mirrors status + total into scr->host_mirror (synchronous calls;
                                costs time at the kernel's end, so async queues skip it) */
 #define DDSK_F_OVERLAP 4    /* independent batch: static segment striding, overlap protocol (see kernels.cu) */

@@ -222,25 +222,27 @@ struct dds_store {
     // small-call fast path (the legacy one-get-per-sample loader): zero-copy pinned bounce buffers the kernel reads
     // indices from / writes the payload to directly, so a small host-to-host call is one launch + one sync
     char *h_small = nullptr, *d_small = nullptr; // kSmallIdx*16 bytes of indices + kSmallOut bytes of payload
-    // pending async batch
-    bool pending = false;
-    cudaStream_t pending_stream = nullptr;
-    int64_t pending_fixed_total = -1;
-    int64_t pending_nreq = 0;
-    const int64_t *pending_total_ptr = nullptr; // device word holding the packed total of the last queued launch
-    int pending_cvt = 0;                        // that word is in source bytes of this conversion (DDSK_CVT_*)
-    bool pending_put = false;                   // the pending queue holds a batched put (dds_epoch_begin completes it)
+    // The queue of DDS_NO_SYNC batches and the overlap run it may hold. Only the queue functions touch it (begin_call,
+    // launch_flags, end_launch, note_empty_async, break_run, drain_pending, dds_batch_wait).
+    struct Queue {
+        bool pending = false; // launches are queued and not drained yet
+        cudaStream_t pending_stream = nullptr;
+        int64_t pending_fixed_total = -1;           // total of the last queued batch as the host knows it (-1: below)
+        const int64_t *pending_total_ptr = nullptr; // device word holding the packed total of the last queued launch
+        int pending_cvt = 0;                        // that word is in source bytes of this conversion (DDSK_CVT_*)
+        bool pending_put = false;                   // the pending queue holds a batched put (dds_epoch_begin completes it)
+        unsigned int queue_len = 0; // launches in the current queue (< kQueueMax, see launch_flags)
+        // overlap protocol (DDS_OVERLAP): sequence number of the next overlap launch, and how many overlap launches in
+        // a row were chained on the pending stream right before it (0: the next one starts a new run)
+        unsigned int ovl_seq = 1;
+        int run_len = 0;
+        // outcome of queues completed by calls other than dds_batch_wait (drain_pending), reported by the next
+        // dds_batch_wait: the first failing status word in queue order, and the total of the last batch queued
+        unsigned long long kept_status = DDSK_STATUS_OK;
+        int64_t kept_total = 0;
+    } q;
     ddsk_var_t *d_multi_vars = nullptr; // device copy of the windows of the last multi-array combination
     std::string multi_key;
-    // overlap protocol (DDS_OVERLAP): sequence number of the next overlap launch, and how many overlap launches in a
-    // row were chained on the pending stream right before it (0: the next one starts a new run)
-    unsigned int ovl_seq = 1;
-    int run_len = 0;
-    unsigned int queue_len = 0; // launches in the current queue of DDS_NO_SYNC batches (< kQueueMax, see tag_launch)
-    // outcome of queues completed by calls other than dds_batch_wait (drain_pending), reported by the next
-    // dds_batch_wait: the first failing status word in queue order, and the total of the last batch queued
-    unsigned long long kept_status = DDSK_STATUS_OK;
-    int64_t kept_total = 0;
     // plan scratch slots of overlapped variable-count batches: launch q plans into slot q & 3, so its plan kernels can
     // run while the gather of launch q-1 is still reading slot (q-1) & 3
     struct Slot {
@@ -312,6 +314,9 @@ cudaError_t device_sync(dds_store *s) {
     return cudaDeviceSynchronize();
 }
 
+// The next overlap launch starts a new run: it waits for the grid before it rather than overlapping with its tail.
+void break_run(dds_store *s) { s->q.run_len = 0; }
+
 // scratch of the plan kernels (variable-count batches the shared-memory plan does not take)
 int ensure_scratch(dds_store *s, int64_t nreq, int64_t cap_bytes) {
     if (nreq > s->scr.cap_req) {
@@ -352,7 +357,7 @@ int ensure_slots(dds_store *s, int64_t nreq, int64_t cap_bytes) {
     while (cap < nreq) cap *= 2;
     while (scap < need_seg) scap *= 2;
     CU(device_sync(s)); // nothing queued may still be using the old slots
-    s->run_len = 0;              // ... so the next overlap launch starts a new run
+    break_run(s);
     for (auto &sl : s->slots) {
         if (sl.req_src) cudaFree(sl.req_src);
         if (sl.req_dst) cudaFree(sl.req_dst);
@@ -370,14 +375,12 @@ int ensure_slots(dds_store *s, int64_t nreq, int64_t cap_bytes) {
     return DDS_OK;
 }
 
-// the scratch a launch works in: the store's own arrays, or -- for an overlap launch planned by the plan kernels --
-// slot (sequence number & 3)
 // The plan kernel tags its look-back words with a 22-bit launch counter instead of clearing them; shortly before the
 // counter wraps, clear every scratch area once and start over.
 int renew_plan_tags(dds_store *s) {
     if (s->scr.plan_tag < 0x3FFFF0u) return DDS_OK;
     CU(device_sync(s));
-    s->run_len = 0;
+    break_run(s);
     if (s->scr.tile_sums) CU(cudaMemset(s->scr.tile_sums, 0, (size_t)(s->scr.cap_req / 1024 + 2) * 8));
     for (auto &sl : s->slots)
         if (sl.tile_sums) CU(cudaMemset(sl.tile_sums, 0, (size_t)(sl.cap_req / 1024 + 2) * 8));
@@ -385,10 +388,27 @@ int renew_plan_tags(dds_store *s) {
     return DDS_OK;
 }
 
-ddsk_scratch_t scratch_view(dds_store *s, bool slot) {
+// Whether a variable-count launch of nreq requests into cap (source) bytes is planned by the plan kernels rather than
+// in shared memory, and if so their scratch made ready: an overlapped launch plans into a slot of its own.
+int plan_scratch(dds_store *s, int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool ovl, bool *uses_scratch) {
+    *uses_scratch = ddsk_var_uses_scratch(nreq, cap, cvt);
+    if (!*uses_scratch) return DDS_OK;
+    if (int rc = renew_plan_tags(s)) return rc;
+    return ovl ? ensure_slots(s, nreq, cap) : ensure_scratch(s, nreq, cap);
+}
+
+// The scratch a launch works in: the store's own arrays, or -- for an overlap launch planned by the plan kernels
+// (`slot`) -- slot (sequence number & 3).
+// An overlap launch (`ovl`) reports its packed total in a device word of its slot, behind the plan words. The store's
+// single total word cannot serve an overlapped run: a launch planned in shared memory writes it at its start, a
+// converting multi-array launch at the end of its walk, and launch q may start before launch q-1 has retired, so q-1
+// could overwrite q's total. Slot q & 3 is next written by launch q+4, which writes nothing before launch q+2 -- and
+// so q -- has retired.
+ddsk_scratch_t scratch_view(dds_store *s, bool ovl, bool slot) {
     ddsk_scratch_t v = s->scr;
+    const unsigned int q = s->scr.ovl_seq & 3u;
     if (slot) {
-        const dds_store::Slot &sl = s->slots[s->scr.ovl_seq & 3u];
+        const dds_store::Slot &sl = s->slots[q];
         v.req_src = sl.req_src;
         v.req_dst = sl.req_dst;
         v.tile_sums = sl.tile_sums;
@@ -396,15 +416,9 @@ ddsk_scratch_t scratch_view(dds_store *s, bool slot) {
         v.cap_req = sl.cap_req;
         v.seg_cap = sl.seg_cap;
     }
+    if (ovl) v.total = (int64_t *)(s->scr.counters + 48) + q;
     return v;
 }
-
-// The device word an overlap launch reports its packed total in, one per slot (sequence number & 3), behind the plan
-// words. The store's single total word cannot serve an overlapped run: a launch planned in shared memory writes it
-// at its start, a converting multi-array launch at the end of its walk, and launch q may start before launch q-1 has
-// retired, so q-1 could overwrite q's total. Slot q & 3 is next written by launch q+4, which writes nothing before
-// launch q+2 -- and so q -- has retired.
-int64_t *ovl_total_word(dds_store *s) { return (int64_t *)(s->scr.counters + 48) + (s->scr.ovl_seq & 3u); }
 
 int ensure_offs(dds_store *s, int64_t n) {
     if (n <= s->offs_cap) return DDS_OK;
@@ -449,6 +463,19 @@ Var *find_var(dds_store *s, const char *name) {
     if (!name) return nullptr;
     auto it = s->vars.find(name);
     return it == s->vars.end() ? nullptr : &it->second;
+}
+
+// What the entries do first: clear the error, reset the outputs, resolve the store and the variable, and check
+// the variable's itemsize when the entry takes one (ddstore.hpp:189-190, 202-203; NULL: none, or checked per conversion).
+int entry_var(dds_store *s, const char *name, const int *itemsize, int64_t *total_bytes, int64_t *bad_index, Var **v) {
+    clear_error();
+    if (bad_index) *bad_index = -1;
+    if (total_bytes) *total_bytes = 0;
+    if (!s) return fail(DDS_ERR_ARG, "null store");
+    *v = find_var(s, name);
+    if (!*v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    if (itemsize && (*v)->itemsize != *itemsize) return fail(DDS_ERR_DTYPE);
+    return DDS_OK;
 }
 
 void release_var(Var &v, int rank) {
@@ -742,59 +769,6 @@ void rearm_status(dds_store *s, cudaStream_t stream) {
     cudaStreamSynchronize(stream);
 }
 
-// Complete the pending queue of DDS_NO_SYNC batches without reporting its outcome: dds_batch_wait alone reports it,
-// once. The queue's first failure is kept unless an earlier one already is (that one is earlier in queue order), and
-// so is the total of its last batch. Every call that must complete a queue before its own work comes through here,
-// and then reports only its own outcome. Returns nothing but a CUDA error of the drain itself.
-int drain_pending(dds_store *s) {
-    if (!s->pending) return DDS_OK;
-    s->pending = false;
-    s->pending_put = false;
-    s->run_len = 0;
-    cudaStream_t st = s->pending_stream;
-    // queued launches skip the host mirror (it costs time at the end of every kernel): read the words back here
-    CU(cudaMemcpyAsync(&s->h_status[0], s->scr.status, 8, cudaMemcpyDeviceToHost, st));
-    if (s->pending_fixed_total < 0 && s->pending_total_ptr)
-        CU(cudaMemcpyAsync(&s->h_status[1], s->pending_total_ptr, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    s->kept_total = s->pending_fixed_total >= 0 ? s->pending_fixed_total : cvt_to_out((int64_t)s->h_status[1], s->pending_cvt);
-    const unsigned long long stw = s->h_status[0];
-    if (stw != DDSK_STATUS_OK) {
-        if (s->kept_status == DDSK_STATUS_OK) s->kept_status = stw;
-        rearm_status(s, st);
-    }
-    return DDS_OK;
-}
-
-// An empty DDS_NO_SYNC batch launches nothing, yet it is the last batch queued: the next dds_batch_wait reports its
-// total, 0. Chained onto a pending queue, that queue's drain keeps the 0; otherwise nothing is pending any more.
-void note_empty_async(dds_store *s, bool no_sync) {
-    if (!no_sync) return;
-    if (s->pending) {
-        s->pending_fixed_total = 0;
-        s->pending_cvt = DDSK_CVT_NONE;
-    } else {
-        s->kept_total = 0;
-    }
-}
-
-// The kernels tag every status report with the launch's position in its queue of DDS_NO_SYNC batches (0 for a
-// synchronous call or the first of a queue), so the sticky word ends up holding the first failing batch in queue order.
-// The tag has 16 bits: a launch that would be the kQueueMax-th of its queue first drains the queue and starts a new one
-// (one stream synchronise per kQueueMax launches), so no two launches of a queue share a tag.
-// `chain`: the launch goes behind batches still pending on the same stream.
-constexpr unsigned int kQueueMax = 0xFFFF;
-int tag_launch(dds_store *s, bool chain) {
-    if (chain && s->queue_len >= kQueueMax) {
-        if (int rc = drain_pending(s)) return rc;
-        chain = false;
-    }
-    const unsigned int ord = chain ? s->queue_len : 0u;
-    s->queue_len = ord + 1u;
-    s->scr.status_tag = (unsigned long long)ord << DDSK_STATUS_ORD_SHIFT;
-    return DDS_OK;
-}
-
 int decode_status_word(unsigned long long st, int64_t *bad_index) {
     if (st == DDSK_STATUS_OK) {
         if (bad_index) *bad_index = -1;
@@ -816,6 +790,119 @@ int decode_status_word(unsigned long long st, int64_t *bad_index) {
 int decode_status(dds_store *s, cudaStream_t stream, unsigned long long st, int64_t *bad_index) {
     if (st != DDSK_STATUS_OK) rearm_status(s, stream);
     return decode_status_word(st, bad_index);
+}
+
+// ---- the queue of DDS_NO_SYNC batches: every batched call goes begin_call -> launch_flags -> launch -> end_launch
+// Async batches may queue up behind each other on ONE stream (the status word is then sticky, and every launch tags its
+// reports with its position in the queue: dds_batch_wait reports the first failing batch of the queue, with that
+// batch's first invalid request). Anything else drains the queue first.
+
+// Complete the pending queue without reporting its outcome: dds_batch_wait alone reports it, once. The queue's first
+// failure is kept unless an earlier one already is (that one is earlier in queue order), and so is the total of its
+// last batch. Every call that must complete a queue before its own work comes through here, and then reports only its
+// own outcome. `puts_only`: only a queue that holds a put. Returns nothing but a CUDA error of the drain itself.
+int drain_pending(dds_store *s, bool puts_only = false) {
+    dds_store::Queue &q = s->q;
+    if (!q.pending || (puts_only && !q.pending_put)) return DDS_OK;
+    q.pending = false;
+    q.pending_put = false;
+    break_run(s);
+    cudaStream_t st = q.pending_stream;
+    // queued launches skip the host mirror (it costs time at the end of every kernel): read the words back here
+    CU(cudaMemcpyAsync(&s->h_status[0], s->scr.status, 8, cudaMemcpyDeviceToHost, st));
+    if (q.pending_fixed_total < 0 && q.pending_total_ptr)
+        CU(cudaMemcpyAsync(&s->h_status[1], q.pending_total_ptr, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    q.kept_total = q.pending_fixed_total >= 0 ? q.pending_fixed_total : cvt_to_out((int64_t)s->h_status[1], q.pending_cvt);
+    const unsigned long long stw = s->h_status[0];
+    if (stw != DDSK_STATUS_OK) {
+        if (q.kept_status == DDSK_STATUS_OK) q.kept_status = stw;
+        rearm_status(s, st);
+    }
+    return DDS_OK;
+}
+
+// A batched call's stream, and whether it goes behind batches still pending on that stream (`chain`)
+struct Call {
+    cudaStream_t st;
+    bool no_sync, chain;
+};
+
+// Begin a batched call on the caller's stream (NULL: the store's). A DDS_NO_SYNC call chains onto a queue pending on
+// the same stream; anything else drains the queue first. (The push fetch passes no_sync: it is always queued.)
+int begin_call(dds_store *s, void *cuda_stream, bool no_sync, Call *c) {
+    CU(cudaSetDevice(s->device));
+    c->st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
+    c->no_sync = no_sync;
+    c->chain = s->q.pending && no_sync && c->st == s->q.pending_stream;
+    if (s->q.pending && !c->chain) return drain_pending(s);
+    return DDS_OK;
+}
+
+// An empty DDS_NO_SYNC batch launches nothing, yet it is the last batch queued: the next dds_batch_wait reports its
+// total, 0. Chained onto a pending queue, that queue's drain keeps the 0; otherwise nothing is pending any more.
+void note_empty_async(dds_store *s, const Call &c) {
+    if (!c.no_sync) return;
+    if (s->q.pending) {
+        s->q.pending_fixed_total = 0;
+        s->q.pending_cvt = DDSK_CVT_NONE;
+    } else {
+        s->q.kept_total = 0;
+    }
+}
+
+// The kernel flags of a launch and the scratch it works in (scratch_view; `plan_slot`: the plan kernels plan it).
+// The kernels tag every status report with the launch's position in its queue (0 for a synchronous call or the first
+// of a queue), so the sticky word ends up holding the first failing batch in queue order. The tag has 16 bits: a launch
+// that would be the kQueueMax-th of its queue first drains the queue and starts a new one (one stream synchronise per
+// kQueueMax launches), so no two launches of a queue share a tag.
+// A synchronous launch mirrors status + total into pinned host words (DDSK_F_MIRROR). An overlap launch (`ovl`:
+// DDS_OVERLAP, declared independent of the batch queued right before it) joins the run of overlap launches chained
+// right before it or starts one; any other launch -- a put and a push included -- ends the run.
+constexpr unsigned int kQueueMax = 0xFFFF;
+int launch_flags(dds_store *s, const Call &c, bool ovl, bool plan_slot, int *kflags, ddsk_scratch_t *scr) {
+    dds_store::Queue &q = s->q;
+    bool chain = c.chain;
+    if (chain && q.queue_len >= kQueueMax) {
+        if (int rc = drain_pending(s)) return rc;
+        chain = false;
+    }
+    const unsigned int ord = chain ? q.queue_len : 0u;
+    q.queue_len = ord + 1u;
+    s->scr.status_tag = (unsigned long long)ord << DDSK_STATUS_ORD_SHIFT;
+    int f = c.no_sync ? 0 : DDSK_F_MIRROR;
+    if (!ovl || !chain) break_run(s);
+    if (ovl) {
+        f |= DDSK_F_OVERLAP;
+        if (q.run_len >= 1) f |= DDSK_F_SKIP_WAIT | DDSK_F_PREV1;
+        if (q.run_len >= 2) f |= DDSK_F_PREV2;
+        if (q.run_len >= 4) f |= DDSK_F_PREV4;
+        s->scr.ovl_seq = q.ovl_seq++;
+        q.run_len++;
+    }
+    *kflags = f;
+    *scr = scratch_view(s, ovl, plan_slot && ovl);
+    return DDS_OK;
+}
+
+// The outcome of a launch (its total: `fixed_total` when the host knows it, else the device word `total_ptr` in source
+// bytes of conversion `cvt`). Queued: it is the pending queue's last batch now (`put`: a batched put). Synchronous:
+// wait for it -- status and total arrive in the pinned mirror words with the end of the kernel -- and report both.
+int end_launch(dds_store *s, const Call &c, int64_t fixed_total, const int64_t *total_ptr, int cvt, bool put,
+               int64_t *total_bytes, int64_t *bad_index) {
+    if (c.no_sync) { // nothing but the kernel(s) goes on the stream; the status word is read back by drain_pending
+        dds_store::Queue &q = s->q;
+        q.pending = true;
+        q.pending_put |= put;
+        q.pending_stream = c.st;
+        q.pending_fixed_total = fixed_total;
+        q.pending_total_ptr = total_ptr;
+        q.pending_cvt = cvt;
+        return DDS_OK;
+    }
+    CU(cudaStreamSynchronize(c.st));
+    if (total_bytes) *total_bytes = fixed_total >= 0 ? fixed_total : cvt_to_out((int64_t)s->h_status[1], cvt);
+    return decode_status(s, c.st, s->h_status[0], bad_index);
 }
 
 } // namespace
@@ -902,7 +989,7 @@ dds_store_t *dds_create(dds_comm_t *comm, int device, int method) {
               cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) == cudaSuccess &&
               cudaMalloc((void **)&s->scr.status, 16) == cudaSuccess && // [0] sticky status, [1] packed total
               cudaMalloc((void **)&s->scr.counters, 256) == cudaSuccess && // 2 ticket words (+pad), 24 protocol words, 8 plan
-                                                                           // words, 4 total words (ovl_total_word)
+                                                                           // words, 4 total words (scratch_view)
               cudaMemset(s->scr.counters, 0, 256) == cudaSuccess &&
               cudaMemset(s->scr.status, 0xFF, 8) == cudaSuccess &&
               cudaHostAlloc((void **)&s->h_status, 32, cudaHostAllocMapped) == cudaSuccess &&
@@ -963,11 +1050,8 @@ int dds_init(dds_store_t *s, const char *name, int64_t nrows, int disp, int item
 
 static int update_impl(dds_store_t *s, const char *name, const void *buffer, int64_t nrows, int64_t offset, int itemsize,
                        int buffer_on_device, cudaStream_t st, bool sync) {
-    clear_error();
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE); // ddstore.hpp:189-190
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, nullptr, nullptr, &v)) return rc;
     if (nrows < 0 || offset < 0 || offset + nrows > v->nrows)
         return fail(DDS_ERR_ARG, "update outside the local shard (unchecked memcpy in the reference)");
     CU(cudaSetDevice(s->device));
@@ -1023,11 +1107,8 @@ int dds_ingest(dds_store_t *s, const char *name, const void *host_rows, int64_t 
     // update<T> (ddstore.hpp:181-195) for a chunk of PAGEABLE host rows, pipelined: parallel CPU copy into pinned staging
     // buffers + async H2D. Returns once the source has been consumed (the caller may reuse it); the last copies complete
     // at the next fence, dds_ingest_wait, or free.
-    clear_error();
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE); // ddstore.hpp:189-190
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, nullptr, nullptr, &v)) return rc;
     if (nrows < 0 || offset < 0 || offset + nrows > v->nrows)
         return fail(DDS_ERR_ARG, "update outside the local shard (unchecked memcpy in the reference)");
     const size_t row = (size_t)v->disp * (size_t)v->itemsize;
@@ -1119,25 +1200,6 @@ static int drain_update_streams(dds_store_t *s) {
     }
     s->update_streams.clear();
     return DDS_OK;
-}
-
-int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index);
-
-// flags of an overlap launch (DDS_OVERLAP), and the bookkeeping of the run it belongs to. `chain`: the launch goes on
-// the stream the previous async launch went on, with nothing synchronised in between.
-static int overlap_flags(dds_store_t *s, bool ovl, bool chain) {
-    if (!ovl) {
-        s->run_len = 0;
-        return 0;
-    }
-    if (!chain) s->run_len = 0;
-    int f = DDSK_F_OVERLAP;
-    if (s->run_len >= 1) f |= DDSK_F_SKIP_WAIT | DDSK_F_PREV1;
-    if (s->run_len >= 2) f |= DDSK_F_PREV2;
-    if (s->run_len >= 4) f |= DDSK_F_PREV4;
-    s->scr.ovl_seq = s->ovl_seq++;
-    s->run_len++;
-    return f;
 }
 
 // One request through the 1-CTA kernel: the legacy one-get()-per-sample call. One launch, no stream synchronize: the
@@ -1237,30 +1299,59 @@ static int small_get(dds_store_t *s, Var *v, int64_t start, int64_t count, void 
     return decode_status_word(stw, bad_index);
 }
 
-// The indices of a batch as the kernels read them (counts: NULL when the batch has none of its own). Host indices:
-// few requests are read by the kernel straight from pinned host memory (no H2D copy to wait for), more are copied on
-// `st` into the store's index arrays.
-static int stage_indices(dds_store_t *s, const int64_t *starts, const int64_t *counts, int64_t nreq, bool idx_dev,
-                         cudaStream_t st, const int64_t **d_starts, const int64_t **d_counts) {
-    if (idx_dev) return DDS_OK;
-    if (nreq <= kSmallIdx) {
+// The requests of a batch as the kernels read them: explicit starts (and counts; NULL for a fixed count), or -- by_sample
+// -- sample ids looked up in v's per-sample table. Host indices: few requests are read by the kernel straight from
+// pinned host memory (no H2D copy to wait for), more are copied on `st` into the store's index arrays.
+static int stage_indices(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts, int64_t nreq,
+                         bool idx_dev, cudaStream_t st, ddsk_index_t *ix) {
+    if (by_sample) counts = nullptr;
+    if (!idx_dev && nreq <= kSmallIdx) {
         int64_t *hs = (int64_t *)s->h_small, *hc = hs + kSmallIdx;
         memcpy(hs, starts, (size_t)nreq * 8);
-        *d_starts = (const int64_t *)s->d_small;
-        if (counts) {
-            memcpy(hc, counts, (size_t)nreq * 8);
-            *d_counts = (const int64_t *)s->d_small + kSmallIdx;
-        }
-        return DDS_OK;
+        if (counts) memcpy(hc, counts, (size_t)nreq * 8);
+        starts = (const int64_t *)s->d_small;
+        if (counts) counts = (const int64_t *)s->d_small + kSmallIdx;
+    } else if (!idx_dev) {
+        if (int rc = ensure_idx(s, nreq)) return rc;
+        CU(cudaMemcpyAsync(s->d_starts, starts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
+        if (counts) CU(cudaMemcpyAsync(s->d_counts, counts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
+        starts = s->d_starts;
+        if (counts) counts = s->d_counts;
     }
-    if (int rc = ensure_idx(s, nreq)) return rc;
-    CU(cudaMemcpyAsync(s->d_starts, starts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
-    *d_starts = s->d_starts;
-    if (counts) {
-        CU(cudaMemcpyAsync(s->d_counts, counts, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
-        *d_counts = s->d_counts;
+    memset(ix, 0, sizeof(*ix));
+    if (by_sample) {
+        ix->sample_ids = starts;
+        ix->table = v->d_tab;
+        ix->nsamples = v->nsamples;
+    } else {
+        ix->starts = starts;
+        ix->counts = counts;
     }
     return DDS_OK;
+}
+
+// The bytes a request of c rows packs. A count above the variable's row total cannot be valid for any start (and
+// c * row_bytes may not fit in 64 bits): such requests pack nothing, so every product is bounded by the variable's size.
+static int64_t req_bytes(const Var *v, int64_t c) {
+    const int64_t rows = v->lenlist.empty() ? 0 : v->lenlist.back();
+    return c > 0 && c <= rows ? c * v->kv.row_bytes : 0;
+}
+
+// The packed bytes of a batch as far as the host can know them (-1: only the kernel knows): exact for a fixed count,
+// else an upper bound -- the total when every request is valid -- from host counts, or from host sample ids and the
+// host copy of the variable's sample table. Sums saturate.
+static int64_t host_layout(const Var *v, bool by_sample, const int64_t *starts, const int64_t *counts, int64_t fixed_count,
+                           int64_t nreq, bool idx_dev) {
+    if (!by_sample && !counts) return sat_mul(nreq, req_bytes(v, fixed_count));
+    if (idx_dev || (by_sample && v->h_tab_count.empty())) return -1;
+    int64_t n = 0;
+    for (int64_t i = 0; i < nreq; i++) {
+        if (!by_sample)
+            n = sat_add(n, req_bytes(v, counts[i]));
+        else if (starts[i] >= 0 && starts[i] < v->nsamples)
+            n = sat_add(n, req_bytes(v, v->h_tab_count[(size_t)starts[i]]));
+    }
+    return n;
 }
 
 // The one batched path behind dds_get_batch / dds_get_samples / dds_get.
@@ -1277,31 +1368,19 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     const bool idx_dev = flags & DDS_IDX_ON_DEVICE, dst_dev = flags & DDS_DST_ON_DEVICE;
     const bool no_sync = flags & DDS_NO_SYNC;
     if (no_sync && !(idx_dev && dst_dev)) return fail(DDS_ERR_ARG, "async batches need device indices and a device destination");
-    CU(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    // Async batches may queue up behind each other on ONE stream (the status word is then sticky, and every launch tags
-    // its reports with its position in the queue: dds_batch_wait reports the first failing batch of the queue, with that
-    // batch's first invalid request). Anything else drains the queue first.
-    const bool chain = s->pending && no_sync && st == s->pending_stream;
-    if (s->pending && !chain) {
-        if (int rc = drain_pending(s)) return rc;
-    }
-    const int64_t R = v->kv.row_bytes;
+    Call c;
+    if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
     const bool fixed = !by_sample && counts == nullptr;
-    // A count above the variable's row total cannot be valid for any start (and count * R may not fit in 64 bits):
-    // such requests pack nothing. Every product below is then bounded by the variable's size, every sum saturates.
-    const int64_t rows = v->lenlist.empty() ? 0 : v->lenlist.back();
-    auto req_bytes = [&](int64_t c) { return c > 0 && c <= rows ? c * R : (int64_t)0; };
-    const int64_t nb_fixed = fixed ? req_bytes(fixed_count) : 0;
+    const int64_t nb_fixed = fixed ? req_bytes(v, fixed_count) : 0;
 
     if (nreq == 0) {
         if (dst_offsets) {
             int64_t z = 0;
-            if (dst_dev) CU(cudaMemcpyAsync(dst_offsets, &z, 8, cudaMemcpyHostToDevice, st));
+            if (dst_dev) CU(cudaMemcpyAsync(dst_offsets, &z, 8, cudaMemcpyHostToDevice, c.st));
             else dst_offsets[0] = 0;
-            if (dst_dev) CU(cudaStreamSynchronize(st));
+            if (dst_dev) CU(cudaStreamSynchronize(c.st));
         }
-        note_empty_async(s, no_sync);
+        note_empty_async(s, c);
         return DDS_OK;
     }
 
@@ -1314,24 +1393,9 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     }
 
     // ---- indices to the device (8-16 B per request)
-    const int64_t *d_starts = starts, *d_counts = counts;
-    if (int rc = stage_indices(s, starts, !fixed && !by_sample ? counts : nullptr, nreq, idx_dev, st, &d_starts, &d_counts))
-        return rc;
-
-    // ---- packed size as far as the host can know it
-    int64_t upper = -1; // upper bound of the packed bytes (== total when every request is valid)
-    if (fixed)
-        upper = sat_mul(nreq, nb_fixed);
-    else if (!idx_dev && !by_sample) {
-        upper = 0;
-        for (int64_t i = 0; i < nreq; i++) upper = sat_add(upper, req_bytes(counts[i]));
-    } else if (!idx_dev && by_sample && !v->h_tab_count.empty()) {
-        upper = 0;
-        for (int64_t i = 0; i < nreq; i++) {
-            const int64_t id = starts[i];
-            if (id >= 0 && id < v->nsamples) upper = sat_add(upper, req_bytes(v->h_tab_count[(size_t)id]));
-        }
-    }
+    ddsk_index_t ix;
+    if (int rc = stage_indices(s, v, by_sample, starts, counts, nreq, idx_dev, c.st, &ix)) return rc;
+    const int64_t upper = host_layout(v, by_sample, starts, counts, fixed_count, nreq, idx_dev);
 
     // ---- destination: the caller's device buffer, or the store's staging buffer for a host destination
     void *d_dst = dst;
@@ -1353,13 +1417,10 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     const int code = cvt ? cvt->code[0] : DDSK_CVT_NONE;
     if (cvt) cap = cvt_cap_to_src(dst_capacity, code);
     if (!d_dst && cap > 0) return fail(DDS_ERR_ARG, "null destination");
-    // DDS_OVERLAP: declared independent of the batch queued right before it (see the protocol in kernels.cu)
     const bool ovl = no_sync && (flags & DDS_OVERLAP);
-    const bool uses_scratch = !fixed && ddsk_var_uses_scratch(nreq, cap, cvt);
-    if (uses_scratch) {
-        if (int rc = renew_plan_tags(s)) return rc;
-        if (int rc = ovl ? ensure_slots(s, nreq, cap) : ensure_scratch(s, nreq, cap)) return rc;
-    }
+    bool uses_scratch = false;
+    if (!fixed)
+        if (int rc = plan_scratch(s, nreq, cap, cvt, ovl, &uses_scratch)) return rc;
 
     // ---- launch
     int64_t *d_offsets = dst_dev ? dst_offsets : nullptr;
@@ -1368,45 +1429,19 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
         if (int rc = ensure_offs(s, nreq + 1)) return rc;
         d_offsets = s->d_offs;
     }
-    if (int rc = tag_launch(s, chain)) return rc;
-    const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
-    ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
-    if (ovl) scr.total = ovl_total_word(s);
-    int krc;
-    if (fixed) {
-        krc = ddsk_gather_fixed(&v->kv, d_starts, fixed_count, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, st);
-    } else {
-        ddsk_index_t ix;
-        memset(&ix, 0, sizeof(ix));
-        if (by_sample) {
-            ix.sample_ids = d_starts;
-            ix.table = v->d_tab;
-            ix.nsamples = v->nsamples;
-        } else {
-            ix.starts = d_starts;
-            ix.counts = d_counts;
-        }
-        krc = ddsk_gather_var(&v->kv, &ix, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, st);
-        s->scr.plan_tag = scr.plan_tag;
-        s->pending_total_ptr = uses_scratch ? &scr.req_dst[nreq] : scr.total;
-    }
+    int kflags;
+    ddsk_scratch_t scr;
+    if (int rc = launch_flags(s, c, ovl, uses_scratch, &kflags, &scr)) return rc;
+    const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, c.st)
+                          : ddsk_gather_var(&v->kv, &ix, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, c.st);
+    s->scr.plan_tag = scr.plan_tag;
     if (krc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
-
-    s->pending_fixed_total = fixed ? cvt_to_out(upper, code) : -1;
-    s->pending_cvt = code; // (the device word of a variable-count total is in source bytes)
-    s->pending_nreq = nreq;
-    if (no_sync) { // nothing but the kernel(s) goes on the stream; the status word is read back in dds_batch_wait
-        s->pending = true;
-        s->pending_stream = st;
-        return DDS_OK;
-    }
-    // status + total arrive in the pinned mirror words with the end of the kernel (no D2H copy)
 
     // ---- results back to a host destination: exactly what the serial get() loop would have left there. The status
     // comes first: after an invalid request only the requests before it are copied, after a capacity error nothing --
     // the rest of the staging buffer holds whatever an earlier batch left in it.
     if (!dst_dev) {
-        CU(cudaStreamSynchronize(st));
+        CU(cudaStreamSynchronize(c.st));
         const unsigned long long stw = s->h_status[0];
         const int64_t total = fixed ? upper : (int64_t)s->h_status[1];
         int64_t n = total; // bytes the caller receives
@@ -1419,27 +1454,27 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
             else if (fixed)
                 n = bad * nb_fixed;
             else { // the packed offset of the first invalid request
-                CU(cudaMemcpyAsync(&n, d_offsets + bad, 8, cudaMemcpyDeviceToHost, st));
-                CU(cudaStreamSynchronize(st));
+                CU(cudaMemcpyAsync(&n, d_offsets + bad, 8, cudaMemcpyDeviceToHost, c.st));
+                CU(cudaStreamSynchronize(c.st));
             }
         }
         if (n > 0) {
             if (small_out) {
                 memcpy(dst, s->h_small + kSmallIdx * 16, (size_t)n); // pinned bounce -> the caller's buffer
             } else if (n >= (int64_t)(4u << 20) && is_pageable(dst)) {
-                if (int rc = d2h_pageable(s, dst, d_dst, (size_t)n, st)) return rc;
+                if (int rc = d2h_pageable(s, dst, d_dst, (size_t)n, c.st)) return rc;
             } else {
-                CU(cudaMemcpyAsync(dst, d_dst, (size_t)n, cudaMemcpyDeviceToHost, st));
+                CU(cudaMemcpyAsync(dst, d_dst, (size_t)n, cudaMemcpyDeviceToHost, c.st));
             }
         }
         if (dst_offsets && !fixed)
-            CU(cudaMemcpyAsync(dst_offsets, d_offsets, (size_t)(nreq + 1) * 8, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(dst_offsets, d_offsets, (size_t)(nreq + 1) * 8, cudaMemcpyDeviceToHost, c.st));
         if (dst_offsets && fixed)
             for (int64_t i = 0; i <= nreq; i++) dst_offsets[i] = i * nb_fixed;
     }
-    CU(cudaStreamSynchronize(st));
-    if (total_bytes) *total_bytes = cvt_to_out(fixed ? upper : (int64_t)s->h_status[1], code);
-    return decode_status(s, st, s->h_status[0], bad_index);
+    // (the device word of a variable-count total is in source bytes)
+    return end_launch(s, c, fixed ? cvt_to_out(upper, code) : -1, uses_scratch ? &scr.req_dst[nreq] : scr.total, code, false,
+                      total_bytes, bad_index);
 }
 
 // Validate the conversions of a converting call (one per variable) and pack them, tables included, into the launch's
@@ -1477,10 +1512,8 @@ static int make_cvt(Var *const *vars, const dds_convert_t *cv, int nvars, bool n
 
 int dds_set_normalization(dds_store_t *s, const char *name, const float *mean, const float *std, int64_t nchan,
                           int64_t inner, int tables_on_device) {
-    clear_error();
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, nullptr, nullptr, &v)) return rc;
     if (nchan < 0 || inner < 1) return fail(DDS_ERR_ARG, "bad normalization layout (nchan >= 0, inner >= 1)");
     if (nchan > 0 && (!mean || !std)) return fail(DDS_ERR_ARG, "null normalization table");
     // (both factors are bounded by disp before they are multiplied: no overflow, and the pattern stays below 2^31)
@@ -1519,12 +1552,8 @@ int dds_get_batch_convert(dds_store_t *s, const char *name, const int64_t *start
                           int64_t fixed_count, int64_t nreq, void *dst, int64_t dst_capacity, int64_t *dst_offsets,
                           unsigned flags, void *cuda_stream, const dds_convert_t *cvt, int64_t *total_bytes,
                           int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, &v)) return rc;
     ddsk_cvt_t kc;
     if (int rc = convert_args(v, cvt, dst, dst_offsets, flags, &kc)) return rc;
     return batch_impl(s, v, false, starts, counts, fixed_count, nreq, dst, dst_capacity, dst_offsets, flags, cuda_stream,
@@ -1535,23 +1564,16 @@ int dds_get_batch(dds_store_t *s, const char *name, const int64_t *starts, const
                   int64_t fixed_count, int64_t nreq, int itemsize, void *dst, int64_t dst_capacity,
                   int64_t *dst_offsets, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                   int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE); // ddstore.hpp:202-203
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
     return batch_impl(s, v, false, starts, counts, fixed_count, nreq, dst, dst_capacity, dst_offsets, flags, cuda_stream,
                       total_bytes, bad_index);
 }
 
 int dds_set_sample_index(dds_store_t *s, const char *name, const int64_t *row_start, const int64_t *row_count,
                          int64_t nsamples, int tables_on_device) {
-    clear_error();
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, nullptr, nullptr, &v)) return rc;
     if (nsamples < 0 || (nsamples > 0 && (!row_start || !row_count))) return fail(DDS_ERR_ARG, "bad sample index");
     CU(cudaSetDevice(s->device));
     if (int rc = drain_pending(s)) return rc;
@@ -1592,13 +1614,8 @@ int dds_set_sample_index(dds_store_t *s, const char *name, const int64_t *row_st
 int dds_get_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize, void *dst,
                     int64_t dst_capacity, int64_t *dst_offsets, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                     int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
     if (!v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
     return batch_impl(s, v, true, sample_ids, nullptr, 0, nreq, dst, dst_capacity, dst_offsets, flags, cuda_stream,
                       total_bytes, bad_index);
@@ -1607,12 +1624,8 @@ int dds_get_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
 int dds_get_samples_convert(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, void *dst,
                             int64_t dst_capacity, int64_t *dst_offsets, unsigned flags, void *cuda_stream,
                             const dds_convert_t *cvt, int64_t *total_bytes, int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, &v)) return rc;
     ddsk_cvt_t kc;
     if (int rc = convert_args(v, cvt, dst, dst_offsets, flags, &kc)) return rc;
     if (!v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
@@ -1653,63 +1666,31 @@ static int padded_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *st
     if (total > 0 && !dst) return fail(DDS_ERR_ARG, "null destination");
     if (by_sample && !v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
 
-    CU(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    const bool chain = s->pending && no_sync && st == s->pending_stream;
-    if (s->pending && !chain) {
-        if (int rc = drain_pending(s)) return rc;
-    }
+    Call c;
+    if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
     if (nreq == 0) {
-        note_empty_async(s, no_sync);
+        note_empty_async(s, c);
         return DDS_OK;
     }
-    const int64_t *d_starts = starts, *d_counts = counts;
-    if (int rc = stage_indices(s, starts, by_sample ? nullptr : counts, nreq, idx_dev, st, &d_starts, &d_counts)) return rc;
     ddsk_index_t ix;
-    memset(&ix, 0, sizeof(ix));
-    if (by_sample) {
-        ix.sample_ids = d_starts;
-        ix.table = v->d_tab;
-        ix.nsamples = v->nsamples;
-    } else {
-        ix.starts = d_starts;
-        ix.counts = d_counts;
-    }
-    if (int rc = tag_launch(s, chain)) return rc;
-    const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, no_sync && (flags & DDS_OVERLAP), chain);
-    ddsk_scratch_t scr = scratch_view(s, false);
-    if (ddsk_gather_padded(&v->kv, &ix, nreq, pad->max_rows, pad->pad_bits, out_log2, pad->lengths, dst, &scr, kflags, cvt, st))
+    if (int rc = stage_indices(s, v, by_sample, starts, counts, nreq, idx_dev, c.st, &ix)) return rc;
+    int kflags;
+    ddsk_scratch_t scr;
+    if (int rc = launch_flags(s, c, no_sync && (flags & DDS_OVERLAP), false, &kflags, &scr)) return rc;
+    if (ddsk_gather_padded(&v->kv, &ix, nreq, pad->max_rows, pad->pad_bits, out_log2, pad->lengths, dst, &scr, kflags, cvt, c.st))
         return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
-    s->pending_fixed_total = total;
-    s->pending_cvt = DDSK_CVT_NONE;
-    s->pending_nreq = nreq;
-    if (total_bytes) *total_bytes = total;
-    if (no_sync) {
-        s->pending = true;
-        s->pending_stream = st;
-        return DDS_OK;
-    }
-    CU(cudaStreamSynchronize(st)); // status arrives in the pinned mirror word with the end of the kernel
-    return decode_status(s, st, s->h_status[0], bad_index);
-}
-
-// the checks the padded entries share with the raw and the converting ones: the itemsize, and the conversion if any
-static int padded_args(Var *v, int itemsize, const dds_convert_t *cvt, ddsk_cvt_t *kc) {
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
-    return cvt ? make_cvt(&v, cvt, 1, false, kc) : DDS_OK;
+    if (total_bytes) *total_bytes = total; // (the padded size, whatever the status says)
+    return end_launch(s, c, total, nullptr, DDSK_CVT_NONE, false, nullptr, bad_index);
 }
 
 int dds_get_batch_padded(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts, int64_t nreq,
                          int itemsize, const dds_convert_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity,
                          unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
     ddsk_cvt_t kc;
-    if (int rc = padded_args(v, itemsize, cvt, &kc)) return rc;
+    if (cvt)
+        if (int rc = make_cvt(&v, cvt, 1, false, &kc)) return rc;
     return padded_impl(s, v, false, starts, counts, nreq, cvt ? &kc : nullptr, pad, dst, dst_capacity, flags, cuda_stream,
                        total_bytes, bad_index);
 }
@@ -1717,14 +1698,11 @@ int dds_get_batch_padded(dds_store_t *s, const char *name, const int64_t *starts
 int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
                            const dds_convert_t *cvt, const dds_pad_t *pad, void *dst, int64_t dst_capacity, unsigned flags,
                            void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
     ddsk_cvt_t kc;
-    if (int rc = padded_args(v, itemsize, cvt, &kc)) return rc;
+    if (cvt)
+        if (int rc = make_cvt(&v, cvt, 1, false, &kc)) return rc;
     return padded_impl(s, v, true, sample_ids, nullptr, nreq, cvt ? &kc : nullptr, pad, dst, dst_capacity, flags,
                        cuda_stream, total_bytes, bad_index);
 }
@@ -1743,92 +1721,40 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     if (by_sample && !v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
     const bool idx_dev = flags & DDS_IDX_ON_DEVICE, no_sync = flags & DDS_NO_SYNC;
     if (no_sync && !idx_dev) return fail(DDS_ERR_ARG, "async puts need device indices");
-    const int64_t R = v->kv.row_bytes;
     const bool fixed = !by_sample && counts == nullptr;
-    const int64_t rows = v->lenlist.empty() ? 0 : v->lenlist.back();
-    auto req_bytes = [&](int64_t c) { return c > 0 && c <= rows ? c * R : (int64_t)0; };
-    // ---- the layout total as far as the host can know it (-1: only the kernel knows it)
-    int64_t layout = -1;
-    if (fixed)
-        layout = sat_mul(nreq, req_bytes(fixed_count));
-    else if (!idx_dev && !by_sample) {
-        layout = 0;
-        for (int64_t i = 0; i < nreq; i++) layout = sat_add(layout, req_bytes(counts[i]));
-    } else if (!idx_dev && by_sample && !v->h_tab_count.empty()) {
-        layout = 0;
-        for (int64_t i = 0; i < nreq; i++) {
-            const int64_t id = starts[i];
-            if (id >= 0 && id < v->nsamples) layout = sat_add(layout, req_bytes(v->h_tab_count[(size_t)id]));
-        }
-    }
+    const int64_t layout = host_layout(v, by_sample, starts, counts, fixed_count, nreq, idx_dev);
     if (!src && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null src");
 
-    CU(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    const bool chain = s->pending && no_sync && st == s->pending_stream;
-    if (s->pending && !chain) {
-        if (int rc = drain_pending(s)) return rc;
-    }
+    Call c;
+    if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
     if (nreq == 0) {
-        note_empty_async(s, no_sync);
+        note_empty_async(s, c);
         return DDS_OK;
     }
-    const int64_t *d_starts = starts, *d_counts = counts;
-    if (int rc = stage_indices(s, starts, !fixed && !by_sample ? counts : nullptr, nreq, idx_dev, st, &d_starts, &d_counts))
-        return rc;
-    const bool uses_scratch = !fixed && ddsk_var_uses_scratch(nreq, src_bytes, nullptr);
-    if (uses_scratch) {
-        if (int rc = renew_plan_tags(s)) return rc;
-        if (int rc = ensure_scratch(s, nreq, src_bytes)) return rc;
-    }
-    if (int rc = tag_launch(s, chain)) return rc;
-    // (overlap_flags(.., false, ..) ends any overlap run: the next overlapped batch starts a new one and waits for the grid)
-    const int kflags = DDSK_F_PUT | (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, false, chain);
-    ddsk_scratch_t scr = scratch_view(s, false);
-    int krc;
-    if (fixed) {
-        krc = ddsk_gather_fixed(&v->kv, d_starts, fixed_count, nreq, const_cast<void *>(src), src_bytes, nullptr, &scr, kflags,
-                                nullptr, st);
-    } else {
-        ddsk_index_t ix;
-        memset(&ix, 0, sizeof(ix));
-        if (by_sample) {
-            ix.sample_ids = d_starts;
-            ix.table = v->d_tab;
-            ix.nsamples = v->nsamples;
-        } else {
-            ix.starts = d_starts;
-            ix.counts = d_counts;
-        }
-        krc = ddsk_gather_var(&v->kv, &ix, nreq, const_cast<void *>(src), src_bytes, nullptr, &scr, kflags, nullptr, st);
-        s->scr.plan_tag = scr.plan_tag;
-        s->pending_total_ptr = uses_scratch ? &scr.req_dst[nreq] : scr.total;
-    }
+    ddsk_index_t ix;
+    if (int rc = stage_indices(s, v, by_sample, starts, counts, nreq, idx_dev, c.st, &ix)) return rc;
+    bool uses_scratch = false;
+    if (!fixed)
+        if (int rc = plan_scratch(s, nreq, src_bytes, nullptr, false, &uses_scratch)) return rc;
+    // (never overlapped: a put ends any overlap run, and the next overlapped batch starts a new one and waits for the grid)
+    int kflags;
+    ddsk_scratch_t scr;
+    if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
+    void *d_src = const_cast<void *>(src);
+    kflags |= DDSK_F_PUT;
+    const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st)
+                          : ddsk_gather_var(&v->kv, &ix, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st);
+    s->scr.plan_tag = scr.plan_tag;
     if (krc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
-    s->pending_fixed_total = fixed ? layout : -1;
-    s->pending_cvt = DDSK_CVT_NONE;
-    s->pending_nreq = nreq;
-    if (no_sync) {
-        s->pending = true;
-        s->pending_put = true;
-        s->pending_stream = st;
-        return DDS_OK;
-    }
-    CU(cudaStreamSynchronize(st)); // status + total arrive in the pinned mirror words with the end of the kernel
-    if (total_bytes) *total_bytes = fixed ? layout : (int64_t)s->h_status[1];
-    return decode_status(s, st, s->h_status[0], bad_index);
+    return end_launch(s, c, fixed ? layout : -1, uses_scratch ? &scr.req_dst[nreq] : scr.total, DDSK_CVT_NONE, true,
+                      total_bytes, bad_index);
 }
 
 int dds_put_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts, int64_t fixed_count,
                   int64_t nreq, int itemsize, const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream,
                   int64_t *total_bytes, int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE); // ddstore.hpp:189-190, as update() reports it
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
                     bad_index);
 }
@@ -1836,13 +1762,8 @@ int dds_put_batch(dds_store_t *s, const char *name, const int64_t *starts, const
 int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
                     const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                     int64_t *bad_index) {
-    clear_error();
-    if (bad_index) *bad_index = -1;
-    if (total_bytes) *total_bytes = 0;
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index);
 }
 
@@ -1884,21 +1805,17 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
     }
     const bool idx_dev = flags & DDS_IDX_ON_DEVICE, no_sync = flags & DDS_NO_SYNC;
     if (no_sync && !idx_dev) return fail(DDS_ERR_ARG, "async batches need device indices and a device destination");
-    CU(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    const bool chain = s->pending && no_sync && st == s->pending_stream;
-    if (s->pending && !chain) {
-        if (int rc = drain_pending(s)) return rc;
-    }
+    Call c;
+    if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
     if (total_bytes)
         for (int v = 0; v < nvars; v++) total_bytes[v] = 0;
     if (nreq == 0) {
-        note_empty_async(s, no_sync);
+        note_empty_async(s, c);
         return DDS_OK;
     }
     if (key != s->multi_key) { // (re)build the device array of windows for this combination of variables
         if (!s->d_multi_vars) CU(cudaMalloc((void **)&s->d_multi_vars, sizeof(ddsk_var_t) * DDSK_MAX_MULTI));
-        CU(cudaStreamSynchronize(st)); // nothing in flight may still read the previous combination
+        CU(cudaStreamSynchronize(c.st)); // nothing in flight may still read the previous combination
         for (int v = 0; v < nvars; v++)
             CU(cudaMemcpy(&s->d_multi_vars[v], &vv[v]->kv, sizeof(ddsk_var_t), cudaMemcpyHostToDevice));
         s->multi_key = key;
@@ -1906,15 +1823,12 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
     const int64_t *d_ids = sample_ids;
     if (!idx_dev) {
         if (int rc = ensure_idx(s, nreq)) return rc;
-        CU(cudaMemcpyAsync(s->d_starts, sample_ids, (size_t)nreq * 8, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(s->d_starts, sample_ids, (size_t)nreq * 8, cudaMemcpyHostToDevice, c.st));
         d_ids = s->d_starts;
     }
     const bool ovl = no_sync && (flags & DDS_OVERLAP);
-    const bool uses_scratch = ddsk_var_uses_scratch(nreq * nvars, cap_total, kcp);
-    if (uses_scratch) {
-        if (int rc = renew_plan_tags(s)) return rc;
-        if (int rc = ovl ? ensure_slots(s, nreq * nvars, cap_total) : ensure_scratch(s, nreq * nvars, cap_total)) return rc;
-    }
+    bool uses_scratch;
+    if (int rc = plan_scratch(s, nreq * nvars, cap_total, kcp, ovl, &uses_scratch)) return rc;
     // a synchronous caller wants the per-variable totals: they are the last entries of the per-variable offsets, which
     // go to the caller's arrays or to a staging array of the store
     const bool stage_offs = !no_sync && total_bytes != nullptr;
@@ -1932,28 +1846,21 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
         m.cap[v] = cap_src[v];
         m.offsets[v] = dst_offsets && dst_offsets[v] ? dst_offsets[v] : (stage_offs ? s->d_offs + (int64_t)v * (nreq + 1) : nullptr);
     }
-    if (int rc = tag_launch(s, chain)) return rc;
-    const int kflags = (no_sync ? 0 : DDSK_F_MIRROR) | overlap_flags(s, ovl, chain);
-    ddsk_scratch_t scr = scratch_view(s, uses_scratch && ovl);
-    if (ovl) scr.total = ovl_total_word(s);
-    const int mrc = ddsk_gather_multi(&m, d_ids, nreq, &scr, kflags, kcp, st);
+    int kflags;
+    ddsk_scratch_t scr;
+    if (int rc = launch_flags(s, c, ovl, uses_scratch, &kflags, &scr)) return rc;
+    const int mrc = ddsk_gather_multi(&m, d_ids, nreq, &scr, kflags, kcp, c.st);
     s->scr.plan_tag = scr.plan_tag;
     if (mrc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
-    s->pending_fixed_total = -1;
-    s->pending_nreq = nreq * nvars;
     // (a converting launch writes its total in output bytes to the total word, whichever plan it used)
-    s->pending_total_ptr = (uses_scratch && !kcp) ? &scr.req_dst[nreq * nvars] : scr.total;
-    s->pending_cvt = DDSK_CVT_NONE;
-    if (no_sync) {
-        s->pending = true;
-        s->pending_stream = st;
-        return DDS_OK;
-    }
+    if (no_sync)
+        return end_launch(s, c, -1, (uses_scratch && !kcp) ? &scr.req_dst[nreq * nvars] : scr.total, DDSK_CVT_NONE, false,
+                          nullptr, nullptr);
     int64_t *hb = (int64_t *)s->h_small;
     if (total_bytes)
-        for (int v = 0; v < nvars; v++) CU(cudaMemcpyAsync(&hb[v], m.offsets[v] + nreq, 8, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    int rc = decode_status(s, st, s->h_status[0], bad_index);
+        for (int v = 0; v < nvars; v++) CU(cudaMemcpyAsync(&hb[v], m.offsets[v] + nreq, 8, cudaMemcpyDeviceToHost, c.st));
+    CU(cudaStreamSynchronize(c.st));
+    int rc = decode_status(s, c.st, s->h_status[0], bad_index);
     if (total_bytes)
         for (int v = 0; v < nvars; v++) total_bytes[v] = rc == DDS_ERR_CAPACITY ? 0 : hb[v];
     if (bad_index && *bad_index >= 0) *bad_index %= nreq; // index of the sample in the id list
@@ -1983,14 +1890,15 @@ int dds_get_samples_multi_convert(dds_store_t *s, int nvars, const char *const *
 // completes the batches issued with DDS_NO_SYNC, and reports what every queue completed since the last call left
 int dds_batch_wait(dds_store_t *s, int64_t *total_bytes, int64_t *bad_index) {
     if (!s) return fail(DDS_ERR_ARG, "null store");
-    if (s->pending) {
+    dds_store::Queue &q = s->q;
+    if (q.pending) {
         CU(cudaSetDevice(s->device));
         if (int rc = drain_pending(s)) return rc;
     }
-    const unsigned long long st = s->kept_status;
-    if (total_bytes) *total_bytes = s->kept_total;
-    s->kept_status = DDSK_STATUS_OK;
-    s->kept_total = 0;
+    const unsigned long long st = q.kept_status;
+    if (total_bytes) *total_bytes = q.kept_total;
+    q.kept_status = DDSK_STATUS_OK;
+    q.kept_total = 0;
     return decode_status_word(st, bad_index);
 }
 
@@ -2004,8 +1912,7 @@ int dds_get(dds_store_t *s, const char *name, int64_t start, int64_t count, int 
         return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
     }
     // (a count above the variable's row total is invalid whatever the start: no room is needed for it)
-    const int64_t rows = v->lenlist.empty() ? 0 : v->lenlist.back();
-    const int64_t cap = count > 0 && count <= rows ? count * v->kv.row_bytes : 0;
+    const int64_t cap = req_bytes(v, count);
     return dds_get_batch(s, name, &start, nullptr, count, 1, itemsize, buffer, cap, nullptr,
                          buffer_on_device ? DDS_DST_ON_DEVICE : 0u, nullptr, nullptr, nullptr);
 }
@@ -2069,39 +1976,32 @@ int dds_push_setup(dds_store_t *s, int64_t max_requests, int64_t max_bytes) {
 
 int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_dev, int64_t fixed_count, int64_t nreq,
                        int itemsize, void **dst_out, void *cuda_stream) {
-    clear_error();
     if (!s || !dst_out) return fail(DDS_ERR_ARG, "null store or dst_out");
     if (!s->push.ready) return fail(DDS_ERR_ARG, "no push windows (call dds_push_setup on every rank first)");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
-    if (v->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
+    Var *v;
+    if (int rc = entry_var(s, name, &itemsize, nullptr, nullptr, &v)) return rc;
     const int64_t nb = fixed_count * v->kv.row_bytes;
     if (fixed_count <= 0 || nreq < 0 || (nreq > 0 && !starts_dev)) return fail(DDS_ERR_ARG, "push batches fetch count >= 1 rows per request");
     if (nreq > s->push.table.max_requests || nreq * nb > s->push.table.max_bytes)
         return fail(DDS_ERR_CAPACITY, "batch larger than the push window");
-    CU(cudaSetDevice(s->device));
-    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-    if (s->pending && st != s->pending_stream) {
-        if (int rc = drain_pending(s)) return rc;
-    }
-    s->run_len = 0;
-    if (int rc = tag_launch(s, s->pending)) return rc;
+    // always queued: dds_batch_wait reports what the owners found wrong with this rank's requests. Never overlapped: a
+    // push ends any overlap run.
+    Call c;
+    if (int rc = begin_call(s, cuda_stream, true, &c)) return rc;
+    int kflags;
+    ddsk_scratch_t scr;
+    if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
     const unsigned long long step = ++s->push.step;
-    if (ddsk_gather_push(&v->kv, &s->push.table, s->push.d_table, starts_dev, fixed_count, nreq, step, &s->scr, st))
+    if (ddsk_gather_push(&v->kv, &s->push.table, s->push.d_table, starts_dev, fixed_count, nreq, step, &scr, c.st))
         return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
     *dst_out = s->push.table.win[s->push.table.me] + s->push.table.dst_off[step & 1ull];
-    s->pending = true; // dds_batch_wait reports what the owners found wrong with this rank's requests
-    s->pending_stream = st;
-    s->pending_fixed_total = nreq * nb;
-    s->pending_nreq = nreq;
-    return DDS_OK;
+    return end_launch(s, c, nreq * nb, nullptr, DDSK_CVT_NONE, false, nullptr, nullptr);
 }
 
 int dds_query(dds_store_t *s, const char *name, dds_varinfo_t *out) {
-    clear_error();
     if (!s || !out) return fail(DDS_ERR_ARG, "null store or out");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, nullptr, nullptr, &v)) return rc;
     memset(out, 0, sizeof(*out));
     out->itemsize = v->itemsize;
     out->disp = v->disp;
@@ -2122,8 +2022,7 @@ int dds_epoch_begin(dds_store_t *s) {
         if (x.second.fence_active) return fail(DDS_ERR_FENCE_ACTIVE);
     CU(cudaSetDevice(s->device));
     // queued puts are part of the epoch that ends here (a queue of gets is left to dds_batch_wait)
-    if (s->pending_put)
-        if (int rc = drain_pending(s)) return rc;
+    if (int rc = drain_pending(s, true)) return rc;
     CU(cudaStreamSynchronize(s->stream));
     if (int rc = drain_update_streams(s)) return rc; // dds_update_async copies on caller streams are part of the epoch
     if (int rc = dds_comm_barrier(s->comm)) return rc;
@@ -2231,10 +2130,8 @@ void dds_destroy(dds_store_t *s) {
 }
 
 int dds_synth_fill(dds_store_t *s, const char *name, uint64_t seed) {
-    clear_error();
-    if (!s) return fail(DDS_ERR_ARG, "null store");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, nullptr, nullptr, &v)) return rc;
     CU(cudaSetDevice(s->device));
     int64_t first = s->rank > 0 ? v->lenlist[(size_t)s->rank - 1] : 0;
     if (ddsk_synth_fill(v->base, first, v->nrows, v->disp, v->itemsize, seed, s->stream))
@@ -2246,10 +2143,9 @@ int dds_synth_fill(dds_store_t *s, const char *name, uint64_t seed) {
 int dds_synth_verify(dds_store_t *s, const char *name, const void *packed_dev, const int64_t *starts_dev,
                      const int64_t *counts_dev, int64_t fixed_count, const int64_t *offsets_dev, int64_t nreq, uint64_t seed,
                      void *cuda_stream, uint64_t *result) {
-    clear_error();
     if (!s || !result) return fail(DDS_ERR_ARG, "null store or result");
-    Var *v = find_var(s, name);
-    if (!v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, nullptr, nullptr, &v)) return rc;
     CU(cudaSetDevice(s->device));
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
     const size_t words = 2 + DDSK_MAX_RANKS;
