@@ -16,6 +16,10 @@ ERR_UNKNOWN_VAR, ERR_EXISTS, ERR_CUDA, ERR_COMM, ERR_ARG, ERR_CAPACITY, ERR_NO_D
     7, 8, 9, 10, 11, 12, 13, 14
 IDX_ON_DEVICE, DST_ON_DEVICE, NO_SYNC, OVERLAP = 1, 2, 4, 8
 SRC_ON_DEVICE = 2  # dds_put_*: the packed source rows are device memory (same bit as DST_ON_DEVICE)
+# element types of the batched accumulates (DDS_ACC_*), by dtype name
+ACC_F32, ACC_F64, ACC_I32, ACC_I64, ACC_F16, ACC_BF16 = 1, 2, 3, 4, 5, 6
+ACC_TYPES = {"float32": ACC_F32, "float64": ACC_F64, "int32": ACC_I32, "int64": ACC_I64, "float16": ACC_F16,
+             "bfloat16": ACC_BF16}
 
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 BARRIER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
@@ -90,6 +94,10 @@ SIGNATURES = {
                                 C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_put_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
                                   C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_accumulate_batch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int,
+                                       C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_accumulate_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
+                                         C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

@@ -197,6 +197,87 @@ __device__ __forceinline__ uint64_t lds64(uint32_t addr) {
 }
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 __device__ __forceinline__ void sts64(uint32_t addr, uint64_t v) { asm volatile("st.shared.u64 [%0], %1;" ::"r"(addr), "l"(v) : "memory"); }
+__device__ __forceinline__ unsigned short lds16h(uint32_t addr) { // (into a 16-bit register, for f16 / bf16 operands)
+    unsigned short v;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
+    return v;
+}
+
+// Reductions of the accumulate (ACC), element type t = DDSK_ACC_* (warp-uniform). Every one is atomic per element: the
+// element reductions at .sys scope (a peer's reductions into the same shard must combine with the owner's), the bulk
+// ones at the scope the ISA gives them. The f32 element and vector reductions flush subnormal inputs and results to
+// zero (atomicAdd's rule; the f32 bulk reduction kept them on H100, see DESIGN.md 3.8); f16 / bf16 are .noftz; f64 is
+// exact IEEE, the integer types wrap.
+// shared -> global bulk reduction, dst[e] += staged[e]: tma_store_1d's rules (16-byte aligned addresses and size) and
+// bulk async-group (SASS: UBLKRED)
+__device__ __forceinline__ void tma_red_add_1d(void *dst_gmem, uint32_t src_smem, uint32_t bytes, int t) {
+    switch (t) {
+    case DDSK_ACC_F32:
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
+        break;
+    case DDSK_ACC_F64:
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f64 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
+        break;
+    case DDSK_ACC_I32:
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u32 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
+        break;
+    case DDSK_ACC_I64:
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
+        break;
+    case DDSK_ACC_F16:
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.noftz.f16 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
+        break;
+    default:
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.noftz.bf16 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
+        break;
+    }
+}
+// one element: *d += the element staged at shared address s (both aligned to the element size)
+__device__ __forceinline__ void red_add1(char *d, uint32_t s, int t) {
+    switch (t) {
+    case DDSK_ACC_F32:
+        asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(d), "f"(__uint_as_float(lds32(s))) : "memory");
+        break;
+    case DDSK_ACC_F64:
+        asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__longlong_as_double((long long)lds64(s))) : "memory");
+        break;
+    case DDSK_ACC_I32: asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(lds32(s)) : "memory"); break;
+    case DDSK_ACC_I64: asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"(lds64(s)) : "memory"); break;
+    case DDSK_ACC_F16: asm volatile("red.relaxed.sys.global.add.noftz.f16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
+    default: asm volatile("red.relaxed.sys.global.add.noftz.bf16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
+    }
+}
+// 16 bytes at a 16-byte aligned d: *d += v, element-wise
+__device__ __forceinline__ void red_add16(char *d, uint4 v, int t) {
+    switch (t) {
+    case DDSK_ACC_F32:
+        asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(d), "f"(__uint_as_float(v.x)),
+                     "f"(__uint_as_float(v.y)), "f"(__uint_as_float(v.z)), "f"(__uint_as_float(v.w)) : "memory");
+        break;
+    case DDSK_ACC_F64:
+        asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__hiloint2double((int)v.y, (int)v.x)) : "memory");
+        asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d + 8), "d"(__hiloint2double((int)v.w, (int)v.z)) : "memory");
+        break;
+    case DDSK_ACC_I32:
+        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(v.x) : "memory");
+        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 4), "r"(v.y) : "memory");
+        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 8), "r"(v.z) : "memory");
+        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 12), "r"(v.w) : "memory");
+        break;
+    case DDSK_ACC_I64:
+        asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"((uint64_t)v.y << 32 | v.x) : "memory");
+        asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d + 8), "l"((uint64_t)v.w << 32 | v.z) : "memory");
+        break;
+    case DDSK_ACC_F16:
+        asm volatile("red.relaxed.sys.global.add.noftz.v4.f16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z),
+                     "r"(v.w) : "memory");
+        break;
+    default:
+        asm volatile("red.relaxed.sys.global.add.noftz.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z),
+                     "r"(v.w) : "memory");
+        break;
+    }
+}
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
     unsigned int v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -373,6 +454,9 @@ struct GatherArgs {
             uint64_t pad_bits;
             int pad_log2, pad_in_log2, pad_out_log2; // output element size; source -> output position shifts
             int64_t *pad_lengths;                    // optional [nreq] delivered row counts
+        };
+        struct { // accumulates (ACC, a put: neither padded nor multi-array)
+            int acc_type; // DDSK_ACC_*: the element type of the sum
         };
     };
     int min_seg_chunks;                // smallest segment, in chunks (claims cost more when the plan is in global memory)
@@ -749,8 +833,9 @@ struct ChunkWalker {
 // Re-phase loop: output vector j = staged bytes [q16 + 16j + 4*WS + bs, +16). Specialised on the word shift WS
 // (and on whether a sub-word byte shift is needed at all) so the loop body is branch-free: two aligned 128-bit
 // shared loads, at most four funnel shifts, one aligned 128-bit global store.
-template <int WS, bool BYTES>
-__device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t nv, uint32_t bs8, int lane) {
+// ACC: the vector is added to the destination's (red_add16 of element type acc_t) instead of stored.
+template <int WS, bool BYTES, bool ACC = false>
+__device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t nv, uint32_t bs8, int lane, int acc_t = 0) {
 #pragma unroll 4
     for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
         const uint4 lo = lds128(sbase + (j << 4));
@@ -768,7 +853,8 @@ __device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t 
             out.z = w[WS + 2];
             out.w = w[WS + 3];
         }
-        stg128(dv + ((size_t)j << 4), out);
+        if constexpr (ACC) red_add16(dv + ((size_t)j << 4), out, acc_t);
+        else stg128(dv + ((size_t)j << 4), out);
     }
 }
 
@@ -808,6 +894,46 @@ __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, ui
     if ((uint32_t)lane < tail) {
         uint32_t k = head + (nv << 4) + (uint32_t)lane;
         d[k] = (char)lds8(sb + a + k);
+    }
+}
+
+// The accumulate's drain_chunk: the same three cases with every store an atomic add of element type t (DDSK_ACC_*).
+// Same phase: lane 0 bulk-reduces the body. Different phase: re-phased vectors, each reduced (red_add16). The head and
+// tail, below 16 bytes, are reduced element by element by the first lanes. A piece never cuts an element and the
+// caller's rows are element-aligned (see cvt_in_log2), so head, body and tail are whole, aligned elements.
+__device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t) {
+    const uint32_t el = (uint32_t)DDSK_ACC_LOG2(t);
+    uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
+    if (head > n) head = n;
+    uint32_t nv = (n - head) >> 4;
+    uint32_t tail = n - head - (nv << 4);
+    uint32_t s = a + head;
+    uint32_t sh = s & 15u;
+    if (nv) {
+        if (sh == 0) {
+            if (lane == 0) {
+                fence_proxy_async();
+                tma_red_add_1d(d + head, sb + s, nv << 4, t);
+            }
+        } else {
+            const uint32_t sbase = sb + (s & ~15u);
+            const uint32_t bs8 = (sh & 3u) * 8u;
+            char *dv = d + head;
+            switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform (2-byte elements: bs8 is 0 or 16)
+            case 1: rephase_loop<0, true, true>(sbase, dv, nv, bs8, lane, t); break;
+            case 2: rephase_loop<1, false, true>(sbase, dv, nv, bs8, lane, t); break;
+            case 3: rephase_loop<1, true, true>(sbase, dv, nv, bs8, lane, t); break;
+            case 4: rephase_loop<2, false, true>(sbase, dv, nv, bs8, lane, t); break;
+            case 5: rephase_loop<2, true, true>(sbase, dv, nv, bs8, lane, t); break;
+            case 6: rephase_loop<3, false, true>(sbase, dv, nv, bs8, lane, t); break;
+            default: rephase_loop<3, true, true>(sbase, dv, nv, bs8, lane, t); break;
+            }
+        }
+    }
+    if ((uint32_t)lane < (head >> el)) red_add1(d + ((uint32_t)lane << el), sb + a + ((uint32_t)lane << el), t);
+    if ((uint32_t)lane < (tail >> el)) {
+        const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
+        red_add1(d + k, sb + a + k, t);
     }
 }
 
@@ -1255,12 +1381,17 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // zero. The load reads the 16-byte-aligned superset of the piece's range in the caller's buffer: up to 15 bytes on
 // either side that belong to no request, in the same 16-byte block (which never crosses a page), whose values are
 // discarded. Never overlapped, no offsets, no conversion, no push.
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false>
+// ACC (with PUT): a batched accumulate (DDSK_F_ACC) -- the put whose drain adds instead of storing, in the element type
+// a.acc_type: bulk reductions where the put bulk-stores, element reductions for the ragged ends, vector reductions of
+// the re-phased body. Each is atomic per element, so requests of any batch or rank that hit the same element combine.
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
+          bool ACC = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
                                                                 const __grid_constant__ CvtParam<CVT> c) {
     static_assert(CVT || !NORM, "a normalising launch is a converting one");
     static_assert(FIXED || !PAD, "a padded batch is a fixed-stride walk");
     static_assert(!PUT || (!CVT && !PAD), "a put writes raw rows");
+    static_assert(PUT || !ACC, "an accumulate is a put that adds");
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
     constexpr bool PUSH = FIXED && !CVT && !PAD && !PUT;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
@@ -1595,7 +1726,11 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             // so that the raw instantiations compile exactly as they did
             char *const my_dst = (char *)my_dpos;
             const bool direct = my_n != 0 && (((uint32_t)(uint64_t)my_dst | my_n | (my_pack >> 16)) & 15u) == 0;
-            if (direct) tma_store_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n);
+            if constexpr (ACC) {
+                if (direct) tma_red_add_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n, a.acc_type);
+            } else {
+                if (direct) tma_store_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n);
+            }
             unsigned todo = __ballot_sync(0xffffffffu, my_n != 0 && !direct);
             while (todo) {
                 const int j = __ffs(todo) - 1;
@@ -1603,7 +1738,8 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
                 const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
                 const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
-                drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane);
+                if constexpr (ACC) acc_drain_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type);
+                else drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane);
             }
         } else if constexpr (CVT) {
             // converting launch: a converted piece is always drained cooperatively; the raw variables of a multi-array
@@ -2190,12 +2326,13 @@ bool cvt_has_norm(const ddsk_cvt_t *cvt) {
     return false;
 }
 
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false>
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
+          bool ACC = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
     // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan)
     const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD, PUT>;
+    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD, PUT, ACC>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -2283,9 +2420,10 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
 }
 
 template <bool FIXED>
-int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false) {
-    // converting launches and puts: the default variant of each entry (kGeomLarge = kGeomVar), whatever
+int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false, bool acc = false) {
+    // converting launches, puts and accumulates: the default variant of each entry (kGeomLarge = kGeomVar), whatever
     // DDS_GATHER_GEOM* say
+    if (acc) return launch_gather_t<FIXED, 12, 4, 4096, 0, false, false, false, true, true>(args, stream);
     if (put) return launch_gather_t<FIXED, 12, 4, 4096, 0, false, false, false, true>(args, stream);
     if (cvt) return cvt_has_norm(cvt) ? launch_gather_t<FIXED, 12, 4, 4096, 0, true, true>(args, stream, cvt)
                                       : launch_gather_t<FIXED, 12, 4, 4096, 0, true>(args, stream, cvt);
@@ -2302,7 +2440,10 @@ int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t 
     default: return launch_gather_t<FIXED, 8, 4, 4096, 0>(args, stream);
     }
 }
-int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put) {
+int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put, bool acc) {
+    if (acc)
+        return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, false, false, false, true, true>(args, stream)
+                      : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true, true>(args, stream);
     if (put)
         return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, false, false, false, true>(args, stream)
                       : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true>(args, stream);
@@ -2322,7 +2463,7 @@ int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const dd
 
 // The shared-memory-plan variant for a batch of nreq requests into cap bytes (-1: the plan kernels). Converting launches
 // use the default variants only (DDS_GATHER_GEOM_S applies to raw gets), and need room for their tables. Puts take the
-// raw gets' placement rule with the default variants.
+// raw gets' placement rule with the default variants (and so do accumulates, which are puts).
 int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool put = false) {
     if (!g_smem_plan || cap >= ((int64_t)1 << 32)) return -1;
     if (!cvt && !put) return geometry_s_for(nreq);
@@ -2354,6 +2495,7 @@ int gather_args(GatherArgs &a, const ddsk_var_t *var, const ddsk_scratch_t *scr,
     // GPU either); the variable-count entries set the slot's own word below (their CTAs
     // may start late, behind the plan kernel, and must not keep a fixed share of the work).
     a.tickets = a.overlap ? nullptr : scr->counters;
+    if (flags & DDSK_F_ACC) a.acc_type = DDSK_F_ACC_TYPE(flags);
     return 0;
 }
 
@@ -2399,7 +2541,7 @@ int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t 
     a.dst = (char *)dst_dev;
     a.dst_cap = dst_capacity;
     a.offsets_out = offsets_dev_or_null;
-    return launch_gather<true>(a, (cudaStream_t)stream, cvt, (flags & DDSK_F_PUT) != 0);
+    return launch_gather<true>(a, (cudaStream_t)stream, cvt, (flags & DDSK_F_PUT) != 0, (flags & DDSK_F_ACC) != 0);
 }
 
 int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const ddsk_push_t *push_dev,
@@ -2456,14 +2598,14 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     a.nreq = nreq;
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
-    const bool put = (flags & DDSK_F_PUT) != 0;
+    const bool put = (flags & DDSK_F_PUT) != 0, acc = (flags & DDSK_F_ACC) != 0;
     const int gs = select_s(nreq, cap_total, cvt, put);
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
         // (no scratch is shared between launches: independent batches may overlap)
         if (a.overlap) a.tickets = scr->ovl + 8 + (a.seq & 3u);
-        return launch_gather_s(gs, a, st, cvt, put);
+        return launch_gather_s(gs, a, st, cvt, put, acc);
     }
     if (nreq > scr->cap_req || cap_total / SEG_GRAIN + 2 > scr->seg_cap) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_gather_var: scratch too small (%lld requests > %lld, or %lld segments > %lld)",
@@ -2507,7 +2649,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
         a.plan_word = scr->plan_word;
         a.plan_tiles = tiles;
     }
-    return launch_gather<false>(a, st, cvt, put);
+    return launch_gather<false>(a, st, cvt, put, acc);
 }
 
 int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt) {

@@ -76,6 +76,20 @@ typedef struct ddsk_scratch {
                                the owner's shard. The layout keeps an invalid request's bytes (count * row_bytes when
                                0 < count <= the variable's rows, else 0; 0 for a sample id outside the index); it writes
                                nothing, like a layout above dst_capacity. No offsets. */
+#define DDSK_F_ACC 512      /* with DDSK_F_PUT: a batched accumulate -- the put's walk, layout and checks, whose drain adds
+                               every staged element to the shard's (atomically) instead of storing it. The element type
+                               is DDSK_F_ACC_TYPE(flags); the caller's rows are aligned to its size. */
+#define DDSK_F_ACC_SHIFT 10 /* bits 10..12 of the flags: the accumulate's element type (DDSK_ACC_*) */
+#define DDSK_F_ACC_TYPE(f) (((f) >> DDSK_F_ACC_SHIFT) & 7)
+
+/* element types of an accumulate (same values as DDS_ACC_* in include/ddstore_b200.h) */
+#define DDSK_ACC_F32 1
+#define DDSK_ACC_F64 2
+#define DDSK_ACC_I32 3
+#define DDSK_ACC_I64 4
+#define DDSK_ACC_F16 5
+#define DDSK_ACC_BF16 6
+#define DDSK_ACC_LOG2(t) ((t) == DDSK_ACC_F64 || (t) == DDSK_ACC_I64 ? 3 : (t) >= DDSK_ACC_F16 ? 1 : 2)
 
 /* Element conversion inside the gather (same values as DDS_CVT_* in include/ddstore_b200.h). Source byte p of a
  * variable's packed rows goes to output byte (p >> in_log2) << out_log2. */

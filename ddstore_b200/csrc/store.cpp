@@ -1712,9 +1712,11 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
 // an invalid request, o_i the exclusive scan. Like batch_impl, the host knows the layout of a fixed count or of host
 // indices and leaves capacity and validation to the kernel. A put is never overlapped and never takes the
 // single-request kernels.
+// acc: 0 for a put; a DDS_ACC_* element type for the accumulate behind dds_accumulate_batch / dds_accumulate_samples,
+// the same launch whose drain adds (DDSK_F_ACC). Its src must be aligned to the element size.
 static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
                     int64_t fixed_count, int64_t nreq, const void *src, int64_t src_bytes, unsigned flags,
-                    void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+                    void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, int acc = 0) {
     if (!(flags & DDS_SRC_ON_DEVICE)) return fail(DDS_ERR_ARG, "puts take their rows from device memory (DDS_SRC_ON_DEVICE)");
     if (nreq < 0 || src_bytes < 0) return fail(DDS_ERR_ARG, "negative nreq or src_bytes");
     if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
@@ -1724,6 +1726,8 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     const bool fixed = !by_sample && counts == nullptr;
     const int64_t layout = host_layout(v, by_sample, starts, counts, fixed_count, nreq, idx_dev);
     if (!src && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null src");
+    if (acc && (uintptr_t)src % (uintptr_t)v->itemsize)
+        return fail(DDS_ERR_ARG, "accumulates take src aligned to the element size");
 
     Call c;
     if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
@@ -1741,7 +1745,7 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     ddsk_scratch_t scr;
     if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
     void *d_src = const_cast<void *>(src);
-    kflags |= DDSK_F_PUT;
+    kflags |= DDSK_F_PUT | (acc ? DDSK_F_ACC | acc << DDSK_F_ACC_SHIFT : 0);
     const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st)
                           : ddsk_gather_var(&v->kv, &ix, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st);
     s->scr.plan_tag = scr.plan_tag;
@@ -1765,6 +1769,37 @@ int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
     Var *v;
     if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index);
+}
+
+static_assert(DDS_ACC_F32 == DDSK_ACC_F32 && DDS_ACC_F64 == DDSK_ACC_F64 && DDS_ACC_I32 == DDSK_ACC_I32 &&
+                  DDS_ACC_I64 == DDSK_ACC_I64 && DDS_ACC_F16 == DDSK_ACC_F16 && DDS_ACC_BF16 == DDSK_ACC_BF16,
+              "the kernels' accumulate types are the public ones");
+
+// The accumulates' prologue: entry_var with the dtype in place of the itemsize (an unknown type is an argument error, a
+// size other than the variable's itemsize the reference's "Invalid data type")
+static int acc_entry(dds_store_t *s, const char *name, int dtype, int64_t *total_bytes, int64_t *bad_index, Var **v) {
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, v)) return rc;
+    if (dtype < DDS_ACC_F32 || dtype > DDS_ACC_BF16) return fail(DDS_ERR_ARG, "unknown accumulate dtype");
+    if ((*v)->itemsize != 1 << DDSK_ACC_LOG2(dtype)) return fail(DDS_ERR_DTYPE);
+    return DDS_OK;
+}
+
+int dds_accumulate_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                         int64_t fixed_count, int64_t nreq, int dtype, const void *src, int64_t src_bytes, unsigned flags,
+                         void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    Var *v;
+    if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, &v)) return rc;
+    return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
+                    bad_index, dtype);
+}
+
+int dds_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int dtype,
+                           const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                           int64_t *bad_index) {
+    Var *v;
+    if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, &v)) return rc;
+    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
+                    dtype);
 }
 
 // The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,

@@ -56,6 +56,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
                                cbool tables_on_device) except +dds_translate_exception
         long put_batch[T](string name, const long* starts, const long* counts, long fixed_count, long nreq, const T* src,
                           long src_bytes, cbool idx_on_device, void* stream) except +dds_translate_exception
+        long accumulate_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
+                              int dtype, const void* src, long src_bytes, cbool idx_on_device,
+                              void* stream) except +dds_translate_exception
         void epoch_begin() except +dds_translate_exception
         void epoch_end() except +dds_translate_exception
         void free() except +dds_translate_exception
@@ -64,6 +67,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
         int rank()
         int size()
 
+
+# element types of accumulate_batch (DDS_ACC_*), by dtype name
+_ACC_TYPES = {"float32": 1, "float64": 2, "int32": 3, "int64": 4, "float16": 5, "bfloat16": 6}
 
 cdef class PyDDStore:
     cdef DDStore* c_ddstore
@@ -288,6 +294,46 @@ cdef class PyDDStore:
             elif w == 2: total = self.c_ddstore.put_batch[short](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const short*> dp, nbytes, idx_dev, <void*> st)
             elif w == 4: total = self.c_ddstore.put_batch[int](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const int*> dp, nbytes, idx_dev, <void*> st)
             else: total = self.c_ddstore.put_batch[long](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const long*> dp, nbytes, idx_dev, <void*> st)
+        del keep
+        return total
+
+    def accumulate_batch(self, str name, starts, counts=None, src=None, count=None, stream=None):
+        """one kernel launch ADDING len(starts) requests of the CUDA tensor `src` into the owners' shards, in src's dtype
+        (float32, float64, int32, int64, float16 or bfloat16); see ddstore_b200.store.PyDDStore.accumulate_batch (this
+        binding's accumulate is synchronous). Returns the layout's bytes."""
+        if src is None:
+            raise ValueError("an accumulate needs `src` rows")
+        if not (hasattr(src, "data_ptr") and getattr(src, "is_cuda", False)):
+            raise ValueError(f"accumulate into {name!r}: src must be a CUDA tensor (copy host rows to the device first)")
+        if not src.is_contiguous():
+            raise ValueError("src must be C-contiguous")
+        dt = str(src.dtype).replace("torch.", "")
+        if dt not in _ACC_TYPES:
+            raise ValueError(f"accumulate into {name!r}: src dtype {dt} is not one of {', '.join(_ACC_TYPES)}")
+        cdef int code = _ACC_TYPES[dt]
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        cdef size_t sp, cp = 0, dp = src.data_ptr()
+        cdef long nreq
+        if s_dev:
+            nreq = starts.numel(); sp = starts.data_ptr()
+            if counts is not None: cp = counts.data_ptr()
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
+            ca = _i64(counts) if counts is not None else None
+            if ca is not None: cp = ca.ctypes.data
+            keep = (sa, ca)
+        cdef long fixed = 1 if count is None else int(count)
+        cdef long nbytes = src.numel() * src.element_size()
+        cdef size_t st = 0
+        if stream is not None:
+            st = int(stream) if int(stream) != 0 else 1
+        cdef string nm = name.encode()
+        cdef cbool idx_dev = bool(s_dev)
+        cdef long total
+        with nogil:
+            total = self.c_ddstore.accumulate_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, code,
+                                                    <const void*> dp, nbytes, idx_dev, <void*> st)
         del keep
         return total
 

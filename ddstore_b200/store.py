@@ -401,6 +401,67 @@ class PyDDStore:
         _capi.raise_for(rc)
         return total.value
 
+    # ---------------------------------------------------------------- batched accumulates (MPI_Accumulate, MPI_SUM)
+    def accumulate_batch(self, name, starts, counts=None, src=None, count=None, stream=None, wait=True):
+        """ADD len(starts) requests into the owners' shards in ONE kernel launch: every element e of request i's rows
+        becomes shard[e] + src[e]. Requests, the layout of `src`, errors (every valid request is still applied, an
+        invalid one changes nothing), wait=False, ordering and visibility are put_batch's. The sum is taken in
+        src.dtype -- float32, float64, int32, int64, float16 or bfloat16, whose size must be the variable's itemsize
+        (another dtype raises ValueError before the call). Accumulates into the same element in one epoch combine
+        atomically, from any batch, rank or duplicate request: integers exactly (wrapping), floats with one rounding per
+        addition in an unspecified order (float32 may flush subnormals to zero). Mixing puts and accumulates on the same
+        rows in one epoch, or reading rows being accumulated, is undefined. Returns the layout's size in bytes."""
+        sb, keep_src = self._put_src(name, src)
+        code = self._acc_type(name, src)
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        if s_dev:
+            nreq, sp = starts.numel(), starts.data_ptr()
+            cp = counts.data_ptr() if counts is not None else None
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts)
+            ca = _i64(counts) if counts is not None else None
+            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
+            keep = (sa, ca)
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_accumulate_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
+                                          code, sb.ptr, sb.nbytes, flags, self._stream_arg(stream), C.byref(total),
+                                          C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    def accumulate_samples(self, name, sample_ids, src, stream=None, wait=True):
+        """accumulate_batch by SAMPLE ID: request i adds into the rows of sample sample_ids[i] in the index registered
+        with set_sample_index. Layout and errors as put_samples, sums as accumulate_batch."""
+        sb, keep_src = self._put_src(name, src)
+        code = self._acc_type(name, src)
+        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
+        if s_dev:
+            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
+        else:
+            sa = _i64(sample_ids)
+            nreq, sp, keep = sa.size, sa.ctypes.data, sa
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_accumulate_samples(self._h, name.encode(), sp, nreq, code, sb.ptr, sb.nbytes, flags,
+                                            self._stream_arg(stream), C.byref(total), C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    @staticmethod
+    def _acc_type(name, src):
+        """the DDS_ACC_* element type of an accumulate's src, from its dtype (ValueError for any other)"""
+        dt = str(getattr(src, "dtype", "")).replace("torch.", "")
+        if dt not in _capi.ACC_TYPES:
+            raise ValueError(f"accumulate into {name!r}: src dtype {dt or type(src).__name__} is not one of "
+                             f"{', '.join(_capi.ACC_TYPES)}")
+        return _capi.ACC_TYPES[dt]
+
     @staticmethod
     def _put_src(name, src):
         """the _Buf of a put's source rows (a CUDA tensor or CAI object; ValueError for host memory)"""
@@ -617,8 +678,9 @@ class PyDDStore:
         order (last_bad_index: its first invalid request); returns the packed bytes of the last batch queued since the
         previous wait() (0 if none).
         wait() alone reports the outcome of queued batches, exactly once. Any other call that meets a pending queue
-        (a synchronous get_batch / get / get_samples / get_samples_multi / put_batch / put_samples, a batch on another
-        stream, set_sample_index, set_normalization, epoch_end, epoch_begin when the queue holds a put, free) completes it, keeps its first failure for the next wait(), and raises only
+        (a synchronous get_batch / get / get_samples / get_samples_multi / put_batch / put_samples / accumulate_batch /
+        accumulate_samples, a batch on another stream, set_sample_index, set_normalization, epoch_end, epoch_begin
+        when the queue holds a put or an accumulate, free) completes it, keeps its first failure for the next wait(), and raises only
         for its own requests. A failure kept from earlier wins over later ones; after wait() has raised it, the next
         wait() is clean. close() drops an outcome no wait() has reported."""
         total, bad = C.c_int64(0), C.c_int64(-1)

@@ -25,7 +25,8 @@ extern "C" {
 #define DDS_VERSION 111 /* 110: converting batches (dds_get_batch_convert & co.); 111: normalising conversions.
                            The padded batches (dds_get_batch_padded, dds_get_samples_padded) add entries only: callers
                            that built against 111 are unaffected, and a caller finds them by symbol. So do the batched
-                           puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE). */
+                           puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE) and the batched accumulates
+                           (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -314,6 +315,32 @@ int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
                     const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                     int64_t *bad_index);
 
+/* ---- batched accumulates: rows ADDED into any rank's shard from this GPU (MPI_Accumulate with MPI_SUM between fences)
+ * Every element e of request i's rows becomes shard[e] + src[e], the sum taken in `dtype` (DDS_ACC_*). Requests, the
+ * layout of src, validation, error reporting (every valid request is applied, an invalid one changes nothing, the
+ * first invalid one is reported; a layout total above src_bytes applies nothing, DDS_ERR_CAPACITY), flags, queueing and
+ * fences are dds_put_batch's / dds_put_samples's, word for word. In addition, with DDS_ERR_ARG and nothing enqueued:
+ * an unknown dtype, and a src not aligned to the element size. A dtype whose size is not the variable's itemsize is
+ * DDS_ERR_DTYPE ("Invalid data type").
+ * Concurrency -- this replaces the put's conflict rule: accumulates into the same element in one epoch, from any batch,
+ * any rank, or duplicate requests of one batch, combine atomically. The element ends at its starting value plus every
+ * contribution: exactly for the integer types (two's complement, wrapping), with one rounding per addition in an
+ * unspecified order for the floating types. f32 may flush subnormal inputs and results to (sign-preserving) zero, as
+ * atomicAdd(float *) does; f16 and bf16 do not flush; f64 is IEEE. Mixing puts and accumulates on the same bytes in one
+ * epoch, or reading rows while they are being accumulated, is undefined (as in MPI). */
+#define DDS_ACC_F32 1 /* element types of an accumulate: the sum is taken in this type */
+#define DDS_ACC_F64 2
+#define DDS_ACC_I32 3 /* two's-complement, wraps */
+#define DDS_ACC_I64 4
+#define DDS_ACC_F16 5
+#define DDS_ACC_BF16 6
+int dds_accumulate_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                         int64_t fixed_count, int64_t nreq, int dtype, const void *src, int64_t src_bytes, unsigned flags,
+                         void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+int dds_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int dtype,
+                           const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                           int64_t *bad_index);
+
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite
  * flow. When all ranks fetch in the same
@@ -332,7 +359,7 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
  * failing batch in queue order is reported, with that batch's first invalid request in *bad_index.
  * The outcome of queued batches is reported here and only here, exactly once. Any other call that meets a pending
  * queue (a synchronous batch or get(), a batch on another stream, dds_set_sample_index, dds_set_normalization,
- * dds_epoch_end, dds_epoch_begin when the queue holds a put, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
+ * dds_epoch_end, dds_epoch_begin when the queue holds a put or an accumulate, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
  * then does its own work and reports only its own outcome (its error and *bad_index describe its own requests). The
  * next dds_batch_wait reports the kept failure, with its index and text, after completing any queue still pending; a
  * failure kept from earlier wins over any failure queued after it, since it is earlier in queue order. After it has

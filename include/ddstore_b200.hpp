@@ -16,6 +16,7 @@
 #include <cstring>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "ddstore_b200.h"
@@ -173,6 +174,48 @@ class DDStore {
         check(dds_put_samples(store_, name.c_str(), (const int64_t *)sample_ids, nreq, (int)sizeof(T), src, src_bytes, flags,
                               cuda_stream, &total, &bad));
         return (long)total;
+    }
+    // Batched accumulate (dds_accumulate_batch): put_batch's requests and layout, each element of the rows becoming
+    // shard + src, atomically across requests, batches and ranks. T = float, double, int32_t or int64_t; the overload
+    // with an explicit DDS_ACC_* code takes any element type (DDS_ACC_F16 / DDS_ACC_BF16 for 2-byte floats).
+    long accumulate_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq,
+                          int dtype, const void *src, long src_bytes, bool idx_on_device = true,
+                          void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_accumulate_batch(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts, fixed_count,
+                                   nreq, dtype, src, src_bytes, flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    template <typename T>
+    long accumulate_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq,
+                          const T *src, long src_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        return accumulate_batch(name, starts, counts, fixed_count, nreq, acc_type<T>(), src, src_bytes, idx_on_device,
+                                cuda_stream);
+    }
+    // The same by sample id (dds_accumulate_samples).
+    long accumulate_samples(std::string name, const long *sample_ids, long nreq, int dtype, const void *src,
+                            long src_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_accumulate_samples(store_, name.c_str(), (const int64_t *)sample_ids, nreq, dtype, src, src_bytes,
+                                     flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    template <typename T>
+    long accumulate_samples(std::string name, const long *sample_ids, long nreq, const T *src, long src_bytes,
+                            bool idx_on_device = true, void *cuda_stream = nullptr) {
+        return accumulate_samples(name, sample_ids, nreq, acc_type<T>(), src, src_bytes, idx_on_device, cuda_stream);
+    }
+    // the DDS_ACC_* code of an element type
+    template <typename T>
+    static constexpr int acc_type() {
+        static_assert(std::is_same<T, float>::value || std::is_same<T, double>::value ||
+                          std::is_same<T, int32_t>::value || std::is_same<T, int64_t>::value,
+                      "accumulate_batch<T>: T is float, double, int32_t or int64_t (2-byte floats: pass DDS_ACC_F16 / "
+                      "DDS_ACC_BF16)");
+        return std::is_same<T, float>::value ? DDS_ACC_F32 : std::is_same<T, double>::value ? DDS_ACC_F64
+               : std::is_same<T, int32_t>::value ? DDS_ACC_I32 : DDS_ACC_I64;
     }
     // device-pointer variants of add/get for callers that already hold the data in HBM
     template <typename T>
