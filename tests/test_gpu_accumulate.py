@@ -351,64 +351,6 @@ def test_stream_ordering_with_overlapped_gets(torch, store):
         assert outs[k].eq(0.0 if k < 3 else 3.0 if k < 6 else 4.0).all(), k
 
 
-@pytest.mark.parametrize("dtype", ["float32", "float64", "float16", "bfloat16"])
-def test_special_values(torch, store, dtype):
-    """NaN and +-inf propagate (compared by class: NaN, +inf, -inf, finite value) through an aligned and a re-phased
-    piece, and through the element head / tail"""
-    dt = getattr(torch, dtype)
-    disp, nrows = 61, 8  # (odd rows: pieces with element heads and tails)
-    es = torch.tensor([], dtype=dt).element_size()
-    store._L.dds_init(store._h, b"s", nrows, disp, es)
-    sh = _shard(torch, store, "s", nrows, disp, dt)
-    vals = torch.tensor([float("nan"), float("inf"), float("-inf"), 1.0, -2.0, 0.0], dtype=torch.float64)
-    g = torch.Generator().manual_seed(3)
-    start = vals[torch.randint(0, 6, (nrows, disp), generator=g)]
-    add = vals[torch.randint(0, 6, (nrows, disp), generator=g)]
-    sh.copy_(start.to(dt).cuda())
-    for off in (0, 1, 3):  # (element offset of src past a 16-byte boundary)
-        buf = torch.zeros(nrows * disp + 16, dtype=dt, device="cuda:0")
-        buf[off:off + nrows * disp] = add.reshape(-1).to(dt)
-        sh.copy_(start.to(dt).cuda())
-        torch.cuda.synchronize()
-        store.accumulate_batch("s", [0, 3, 7], np.array([3, 4, 1]), src=buf[off:off + nrows * disp])
-        exp = (start.to(dt).double() + add.to(dt).double())
-        got = sh.double().cpu()
-
-        def cls(x):
-            return torch.where(x.isnan(), 0, torch.where(x == float("inf"), 1, torch.where(x == float("-inf"), 2, 3)))
-        assert torch.equal(cls(got), cls(exp)), off
-        fin = cls(exp) == 3
-        assert torch.equal(got[fin], exp[fin].to(dt).double()), off
-
-
-def test_f32_subnormals(torch, store):
-    """f32 subnormal contributions through a bulk reduction (16-byte aligned piece) and through element / vector
-    reductions (a misaligned piece): each result is the exact IEEE sum or its flush to sign-preserving zero -- what
-    the header promises ("f32 may flush subnormals"). Prints which each path does."""
-    disp, nrows = 64, 4
-    store.add("u", np.zeros((nrows, disp), np.float32))
-    sh = _shard(torch, store, "u", nrows, disp, torch.float32)
-    tiny = torch.tensor([1e-40, -3e-41, 2e-39, 1.0], dtype=torch.float32)  # three subnormals and a normal
-    start = tiny[torch.arange(disp) % 4].repeat(nrows, 1)
-    add = tiny[(torch.arange(disp) + 1) % 4].repeat(nrows, 1)
-    outcome = {}
-    for path, off in (("bulk", 0), ("element/vector", 1)):
-        buf = torch.zeros(nrows * disp + 4, device="cuda:0")
-        buf[off:off + nrows * disp] = add.reshape(-1).cuda()
-        sh.copy_(start.cuda())
-        torch.cuda.synchronize()
-        store.accumulate_batch("u", [0], src=buf[off:off + nrows * disp], count=nrows)
-        got = sh.cpu()
-        exact = (start.double() + add.double()).float()
-        ftz = (torch.where(start.abs() < 1.1754944e-38, torch.zeros_like(start) * start.sign(), start).double()
-               + torch.where(add.abs() < 1.1754944e-38, torch.zeros_like(add), add).double()).float()
-        ftz = torch.where(ftz.abs() < 1.1754944e-38, torch.zeros_like(ftz), ftz)
-        ok_exact, ok_ftz = got.eq(exact), got.eq(ftz)
-        assert (ok_exact | ok_ftz).all(), (path, got[~(ok_exact | ok_ftz)][:8])
-        outcome[path] = "exact" if ok_exact.all() else "flushed" if ok_ftz.all() else "mixed"
-    print("f32 subnormal accumulates:", outcome)
-
-
 def test_round_trips(torch, store):
     """after accumulates, get_batch, get_samples and get() (doorbell on and off) read the sums"""
     rng = np.random.default_rng(3)
