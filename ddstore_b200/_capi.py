@@ -20,6 +20,9 @@ SRC_ON_DEVICE = 2  # dds_put_*: the packed source rows are device memory (same b
 ACC_F32, ACC_F64, ACC_I32, ACC_I64, ACC_F16, ACC_BF16 = 1, 2, 3, 4, 5, 6
 ACC_TYPES = {"float32": ACC_F32, "float64": ACC_F64, "int32": ACC_I32, "int64": ACC_I64, "float16": ACC_F16,
              "bfloat16": ACC_BF16}
+# ops of the batched fetch-ops (DDS_OP_*), by name
+OP_SUM, OP_REPLACE = 1, 2
+FOP_OPS = {"sum": OP_SUM, "replace": OP_REPLACE}
 
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 BARRIER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
@@ -98,6 +101,11 @@ SIGNATURES = {
                                        C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_accumulate_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
                                          C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_get_accumulate_batch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                           C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p,
+                                           I64P, I64P]),
+    "dds_get_accumulate_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_int,
+                                             C.c_void_p, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

@@ -278,6 +278,134 @@ __device__ __forceinline__ void red_add16(char *d, uint4 v, int t) {
         break;
     }
 }
+
+// Fetch-ops (FETCH), element type t = DDSK_ACC_*, swap or add (both warp-uniform): atomics that return the element's
+// previous value, at .sys scope for the accumulate's reason. Adds round and flush exactly as the accumulate's element and
+// vector reductions do (f32 flushes, f16 / bf16 are .noftz, f64 is IEEE, integers wrap).
+__device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
+    asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ void sts16(uint32_t addr, uint32_t v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"((unsigned short)v) : "memory"); }
+__device__ __forceinline__ uint32_t atom_add_u32(char *d, uint32_t v) {
+    uint32_t o;
+    asm volatile("atom.relaxed.sys.global.add.u32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory");
+    return o;
+}
+__device__ __forceinline__ uint64_t atom_add_u64(char *d, uint64_t v) {
+    uint64_t o;
+    asm volatile("atom.relaxed.sys.global.add.u64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory");
+    return o;
+}
+__device__ __forceinline__ uint64_t atom_add_f64(char *d, uint64_t v) {
+    double o;
+    asm volatile("atom.relaxed.sys.global.add.f64 %0, [%1], %2;" : "=d"(o) : "l"(d), "d"(__longlong_as_double((long long)v)) : "memory");
+    return (uint64_t)__double_as_longlong(o);
+}
+__device__ __forceinline__ uint32_t atom_exch_b32(char *d, uint32_t v) {
+    uint32_t o;
+    asm volatile("atom.relaxed.sys.global.exch.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory");
+    return o;
+}
+__device__ __forceinline__ uint64_t atom_exch_b64(char *d, uint64_t v) {
+    uint64_t o;
+    asm volatile("atom.relaxed.sys.global.exch.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory");
+    return o;
+}
+// 16-bit swap (there is no 16-bit exchange): a compare-and-swap loop on the aligned 32-bit word that holds the element,
+// which replaces the element's 16 bits and leaves the other 16 exactly as it finds them
+__device__ __forceinline__ uint32_t atom_exch_b16(char *d, uint32_t v) {
+    unsigned int *w = (unsigned int *)((uint64_t)d & ~(uint64_t)3);
+    const uint32_t sh = ((uint32_t)(uint64_t)d & 2u) * 8u, mask = 0xFFFFu << sh;
+    uint32_t cur;
+    asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(cur) : "l"(w) : "memory");
+    while (true) {
+        const uint32_t want = (cur & ~mask) | ((v & 0xFFFFu) << sh);
+        uint32_t seen;
+        asm volatile("atom.relaxed.sys.global.cas.b32 %0, [%1], %2, %3;" : "=r"(seen) : "l"(w), "r"(cur), "r"(want) : "memory");
+        if (seen == cur) break;
+        cur = seen;
+    }
+    return (cur >> sh) & 0xFFFFu;
+}
+// one element at d: the operand staged at shared address s is replaced by the element's previous value (both aligned to
+// the element size)
+__device__ __forceinline__ void fop1(char *d, uint32_t s, int t, bool swap) {
+    if (swap) {
+        switch (DDSK_ACC_LOG2(t)) {
+        case 3: sts64(s, atom_exch_b64(d, lds64(s))); break;
+        case 2: sts32(s, atom_exch_b32(d, lds32(s))); break;
+        default: sts16(s, atom_exch_b16(d, lds16h(s))); break;
+        }
+        return;
+    }
+    switch (t) {
+    case DDSK_ACC_F32: {
+        float o;
+        asm volatile("atom.relaxed.sys.global.add.f32 %0, [%1], %2;" : "=f"(o) : "l"(d), "f"(__uint_as_float(lds32(s))) : "memory");
+        sts32(s, __float_as_uint(o));
+        break;
+    }
+    case DDSK_ACC_F64: sts64(s, atom_add_f64(d, lds64(s))); break;
+    case DDSK_ACC_I32: sts32(s, atom_add_u32(d, lds32(s))); break;
+    case DDSK_ACC_I64: sts64(s, atom_add_u64(d, lds64(s))); break;
+    case DDSK_ACC_F16: {
+        unsigned short o;
+        asm volatile("atom.relaxed.sys.global.add.noftz.f16 %0, [%1], %2;" : "=h"(o) : "l"(d), "h"(lds16h(s)) : "memory");
+        sts16(s, o);
+        break;
+    }
+    default: {
+        unsigned short o;
+        asm volatile("atom.relaxed.sys.global.add.noftz.bf16 %0, [%1], %2;" : "=h"(o) : "l"(d), "h"(lds16h(s)) : "memory");
+        sts16(s, o);
+        break;
+    }
+    }
+}
+// 16 bytes at a 16-byte aligned d: the operands v, element-wise; returns the previous 16 bytes
+__device__ __forceinline__ uint4 fop16(char *d, uint4 v, int t, bool swap) {
+    uint4 o;
+    if (swap) {
+        if (DDSK_ACC_LOG2(t) == 3) {
+            const uint64_t a = atom_exch_b64(d, (uint64_t)v.y << 32 | v.x), b = atom_exch_b64(d + 8, (uint64_t)v.w << 32 | v.z);
+            o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+        } else { // (a 32-bit exchange is atomic for each 16-bit element it holds)
+            o = make_uint4(atom_exch_b32(d, v.x), atom_exch_b32(d + 4, v.y), atom_exch_b32(d + 8, v.z), atom_exch_b32(d + 12, v.w));
+        }
+        return o;
+    }
+    switch (t) {
+    case DDSK_ACC_F32:
+        asm volatile("atom.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                     : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                     : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        break;
+    case DDSK_ACC_F64: {
+        const uint64_t a = atom_add_f64(d, (uint64_t)v.y << 32 | v.x), b = atom_add_f64(d + 8, (uint64_t)v.w << 32 | v.z);
+        o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+        break;
+    }
+    case DDSK_ACC_I32:
+        o = make_uint4(atom_add_u32(d, v.x), atom_add_u32(d + 4, v.y), atom_add_u32(d + 8, v.z), atom_add_u32(d + 12, v.w));
+        break;
+    case DDSK_ACC_I64: {
+        const uint64_t a = atom_add_u64(d, (uint64_t)v.y << 32 | v.x), b = atom_add_u64(d + 8, (uint64_t)v.w << 32 | v.z);
+        o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+        break;
+    }
+    case DDSK_ACC_F16:
+        asm volatile("atom.relaxed.sys.global.add.noftz.v4.f16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                     : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                     : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        break;
+    default:
+        asm volatile("atom.relaxed.sys.global.add.noftz.v4.bf16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                     : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                     : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        break;
+    }
+    return o;
+}
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
     unsigned int v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -455,8 +583,10 @@ struct GatherArgs {
             int pad_log2, pad_in_log2, pad_out_log2; // output element size; source -> output position shifts
             int64_t *pad_lengths;                    // optional [nreq] delivered row counts
         };
-        struct { // accumulates (ACC, a put: neither padded nor multi-array)
-            int acc_type; // DDSK_ACC_*: the element type of the sum
+        struct { // accumulates (ACC) and fetch-ops (FETCH), puts: neither padded nor multi-array
+            int acc_type;     // DDSK_ACC_*: the element type of the sum (or swap)
+            int fop_swap;     // FETCH: the op is a swap (else an add)
+            char *fop_result; // FETCH: the previous values, at the operands' positions (the layout of dst)
         };
     };
     int min_seg_chunks;                // smallest segment, in chunks (claims cost more when the plan is in global memory)
@@ -858,6 +988,46 @@ __device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t 
     }
 }
 
+// The fetch-op's re-phase loop: operand vector j (rephase_loop's shift), applied to the shard's 16 bytes at dv + 16j
+// (fop16), and the previous 16 bytes written back over the operand's staged bytes at s + 16j. Those are element-aligned
+// (2-byte elements: s may be 2 mod 4), and the stores touch exactly them: the neighbouring vectors are other lanes'.
+// (rephase_loop is not shared: the existing instantiations' register allocation changed when it was.)
+template <int WS, bool BYTES>
+__device__ __forceinline__ void fop_rephase_loop(uint32_t sbase, uint32_t s, char *dv, uint32_t nv, uint32_t bs8, int lane, int t,
+                                                 bool swap) {
+#pragma unroll 4
+    for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
+        const uint4 lo = lds128(sbase + (j << 4));
+        const uint4 hi = lds128(sbase + (j << 4) + 16);
+        const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+        uint4 v;
+        if (BYTES) {
+            v.x = __funnelshift_r(w[WS + 0], w[WS + 1], bs8);
+            v.y = __funnelshift_r(w[WS + 1], w[WS + 2], bs8);
+            v.z = __funnelshift_r(w[WS + 2], w[WS + 3], bs8);
+            v.w = __funnelshift_r(w[WS + 3], w[WS + 4], bs8);
+        } else {
+            v = make_uint4(w[WS + 0], w[WS + 1], w[WS + 2], w[WS + 3]);
+        }
+        const uint4 o = fop16(dv + ((size_t)j << 4), v, t, swap);
+        const uint32_t p = s + (j << 4);
+        if (!BYTES && WS == 0) {
+            sts128(p, o);
+        } else if (!BYTES) {
+            sts32(p, o.x);
+            sts32(p + 4, o.y);
+            sts32(p + 8, o.z);
+            sts32(p + 12, o.w);
+        } else {
+            sts16(p, o.x);
+            sts32(p + 2, __funnelshift_r(o.x, o.y, 16));
+            sts32(p + 6, __funnelshift_r(o.y, o.z, 16));
+            sts32(p + 10, __funnelshift_r(o.z, o.w, 16));
+            sts16(p + 14, o.w >> 16);
+        }
+    }
+}
+
 // Drain one staged piece: payload byte k lives at shared address sb + a + k and goes to d[k].
 template <int CH>
 __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane) {
@@ -934,6 +1104,41 @@ __device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d
     if ((uint32_t)lane < (tail >> el)) {
         const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
         red_add1(d + k, sb + a + k, t);
+    }
+}
+
+// The fetch-op's first pass over one staged piece (payload byte k at shared address sb + a + k, shard byte d[k]): every
+// element is combined with the shard's by a returning atomic (fop1 / fop16) in the shard's 16-byte phase -- the head and
+// tail element by element, the body as 16-byte vectors re-phased like acc_drain_chunk's -- and its previous value replaces
+// the operand in the stage. (No bulk form returns the old values.) The caller then drains the stage to the result with
+// the raw drain. Head, body and tail are whole, aligned elements, as in acc_drain_chunk.
+__device__ __forceinline__ void fop_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t, bool swap) {
+    const uint32_t el = (uint32_t)DDSK_ACC_LOG2(t);
+    uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
+    if (head > n) head = n;
+    const uint32_t nv = (n - head) >> 4;
+    const uint32_t tail = n - head - (nv << 4);
+    const uint32_t s = a + head;
+    const uint32_t sh = s & 15u;
+    if (nv) {
+        const uint32_t sbase = sb + (s & ~15u);
+        const uint32_t bs8 = (sh & 3u) * 8u;
+        char *dv = d + head;
+        switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform (2-byte elements: bs8 is 0 or 16)
+        case 0: fop_rephase_loop<0, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        case 1: fop_rephase_loop<0, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        case 2: fop_rephase_loop<1, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        case 3: fop_rephase_loop<1, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        case 4: fop_rephase_loop<2, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        case 5: fop_rephase_loop<2, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        case 6: fop_rephase_loop<3, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        default: fop_rephase_loop<3, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        }
+    }
+    if ((uint32_t)lane < (head >> el)) fop1(d + ((uint32_t)lane << el), sb + a + ((uint32_t)lane << el), t, swap);
+    if ((uint32_t)lane < (tail >> el)) {
+        const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
+        fop1(d + k, sb + a + k, t, swap);
     }
 }
 
@@ -1352,6 +1557,13 @@ struct PieceDesc {
     int64_t dpos;
     uint32_t n, pack; // pack = stage offset | (source misalignment << 16)
 };
+// FETCH: the shared address of a piece's result address, [NW][S][32] in dynamic shared memory behind the rings and the
+// plan. (A function: a constant of the kernel itself changed the other instantiations' register allocation.)
+template <int NW, int S, int STAGE, int PCAP>
+__device__ __forceinline__ uint32_t fop_rdst(const unsigned char *smem_dyn, int warp, uint32_t st, int lane) {
+    return smem_u32(smem_dyn) + (uint32_t)(NW * S * STAGE + (PCAP ? PCAP * 12 + 16 : 0)) +
+           (uint32_t)((warp * S + (int)st) * 32 + lane) * 8u;
+}
 
 // wait until overlap launch q has retired (its done word carries a sequence number >= q)
 __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigned int q, unsigned long long *status,
@@ -1384,14 +1596,20 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // ACC (with PUT): a batched accumulate (DDSK_F_ACC) -- the put whose drain adds instead of storing, in the element type
 // a.acc_type: bulk reductions where the put bulk-stores, element reductions for the ragged ends, vector reductions of
 // the re-phased body. Each is atomic per element, so requests of any batch or rank that hit the same element combine.
+// FETCH (with PUT): a batched fetch-op (DDSK_F_FOP) -- the put whose drain applies a returning atomic (add or swap,
+// a.fop_swap, in the element type a.acc_type) to every element and sends the previous values to a.fop_result, at the
+// operands' positions. Every piece is drained cooperatively in two passes: fop_chunk replaces the staged operands by the
+// previous values, then the raw drain (bulk stores where the phases allow) writes the stage to the result. The result
+// address of each piece is kept beside its descriptor, in dynamic shared memory behind the rings and the plan.
 template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
-          bool ACC = false>
+          bool ACC = false, bool FETCH = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
                                                                 const __grid_constant__ CvtParam<CVT> c) {
     static_assert(CVT || !NORM, "a normalising launch is a converting one");
     static_assert(FIXED || !PAD, "a padded batch is a fixed-stride walk");
     static_assert(!PUT || (!CVT && !PAD), "a put writes raw rows");
     static_assert(PUT || !ACC, "an accumulate is a put that adds");
+    static_assert((PUT && !ACC) || !FETCH, "a fetch-op is a put that returns the previous rows");
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
     constexpr bool PUSH = FIXED && !CVT && !PAD && !PUT;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
@@ -1690,6 +1908,9 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             desc[warp][st][lane].dpos = pc.dpos;
             desc[warp][st][lane].n = pc.n;
             desc[warp][st][lane].pack = pc.off | (al << 16);
+            if constexpr (FETCH) // the piece's result address: its source position, in the result buffer
+                sts64(fop_rdst<NW, S, STAGE, PCAP>(smem_dyn, warp, st, lane),
+                      pc.n ? (uint64_t)a.fop_result + (pc.src - (uint64_t)a.dst) : 0);
             if (pc.n) // every lane issues its own piece's TMA load; all complete on the stage's mbarrier
                 tma_load_1d(ring + st * STAGE + pc.off, (const void *)(pc.src - al), (al + pc.n + 15u) & ~15u, bar);
             issued++;
@@ -1721,7 +1942,31 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         const int64_t my_dpos = desc[warp][st][lane].dpos;
         const uint32_t my_n = desc[warp][st][lane].n;
         const uint32_t my_pack = desc[warp][st][lane].pack;
-        if constexpr (PUT) {
+        if constexpr (FETCH) {
+            // fetch-op: pass 1, the atomics, every piece cooperatively; pass 2, the previous values to the result
+            unsigned todo = __ballot_sync(0xffffffffu, my_n != 0);
+            for (unsigned rest = todo; rest; rest &= rest - 1) {
+                const int j = __ffs(rest) - 1;
+                const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
+                const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
+                const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
+                fop_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type, a.fop_swap != 0);
+            }
+            fence_proxy_async(); // (every lane: its stage writes, before any lane's bulk store reads them)
+            __syncwarp();
+            char *const my_res = (char *)lds64(fop_rdst<NW, S, STAGE, PCAP>(smem_dyn, warp, st, lane));
+            const bool direct = my_n != 0 && (((uint32_t)(uint64_t)my_res | my_n | (my_pack >> 16)) & 15u) == 0;
+            if (direct) tma_store_1d(my_res, ring + st * STAGE + (my_pack & 0xffffu), my_n);
+            todo = __ballot_sync(0xffffffffu, my_n != 0 && !direct);
+            while (todo) {
+                const int j = __ffs(todo) - 1;
+                todo &= todo - 1;
+                char *const d = (char *)__shfl_sync(0xffffffffu, (uint64_t)my_res, j);
+                const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
+                const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
+                drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, d, n, lane);
+            }
+        } else if constexpr (PUT) {
             // put: the raw drain (the last branch) into the shard address the descriptor carries -- a branch of its own,
             // so that the raw instantiations compile exactly as they did
             char *const my_dst = (char *)my_dpos;
@@ -2327,12 +2572,13 @@ bool cvt_has_norm(const ddsk_cvt_t *cvt) {
 }
 
 template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
-          bool ACC = false>
+          bool ACC = false, bool FETCH = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
-    // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan)
-    const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0);
+    // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan; a fetch-op its
+    //  pieces' result addresses)
+    const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0) + (FETCH ? NW * S * 32 * 8 : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD, PUT, ACC>;
+    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD, PUT, ACC, FETCH>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -2420,9 +2666,11 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
 }
 
 template <bool FIXED>
-int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false, bool acc = false) {
+int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false, bool acc = false,
+                  bool fop = false) {
     // converting launches, puts and accumulates: the default variant of each entry (kGeomLarge = kGeomVar), whatever
-    // DDS_GATHER_GEOM* say
+    // DDS_GATHER_GEOM* say. Fetch-ops: one stage fewer (variant 7), which leaves room for their result addresses.
+    if (fop) return launch_gather_t<FIXED, 12, 3, 4096, 0, false, false, false, true, false, true>(args, stream);
     if (acc) return launch_gather_t<FIXED, 12, 4, 4096, 0, false, false, false, true, true>(args, stream);
     if (put) return launch_gather_t<FIXED, 12, 4, 4096, 0, false, false, false, true>(args, stream);
     if (cvt) return cvt_has_norm(cvt) ? launch_gather_t<FIXED, 12, 4, 4096, 0, true, true>(args, stream, cvt)
@@ -2440,7 +2688,11 @@ int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t 
     default: return launch_gather_t<FIXED, 8, 4, 4096, 0>(args, stream);
     }
 }
-int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put, bool acc) {
+int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put, bool acc, bool fop) {
+    // (fetch-ops: the 8192-request plan leaves room for the result addresses with 2 KiB chunks only)
+    if (fop)
+        return g == 1 ? launch_gather_t<false, 12, 3, 2048, 8192, false, false, false, true, false, true>(args, stream)
+                      : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true, false, true>(args, stream);
     if (acc)
         return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, false, false, false, true, true>(args, stream)
                       : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true, true>(args, stream);
@@ -2495,7 +2747,11 @@ int gather_args(GatherArgs &a, const ddsk_var_t *var, const ddsk_scratch_t *scr,
     // GPU either); the variable-count entries set the slot's own word below (their CTAs
     // may start late, behind the plan kernel, and must not keep a fixed share of the work).
     a.tickets = a.overlap ? nullptr : scr->counters;
-    if (flags & DDSK_F_ACC) a.acc_type = DDSK_F_ACC_TYPE(flags);
+    if (flags & (DDSK_F_ACC | DDSK_F_FOP)) a.acc_type = DDSK_F_ACC_TYPE(flags);
+    if (flags & DDSK_F_FOP) {
+        a.fop_swap = (flags & DDSK_F_FOP_SWAP) ? 1 : 0;
+        a.fop_result = (char *)scr->fop_result;
+    }
     return 0;
 }
 
@@ -2541,7 +2797,8 @@ int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t 
     a.dst = (char *)dst_dev;
     a.dst_cap = dst_capacity;
     a.offsets_out = offsets_dev_or_null;
-    return launch_gather<true>(a, (cudaStream_t)stream, cvt, (flags & DDSK_F_PUT) != 0, (flags & DDSK_F_ACC) != 0);
+    return launch_gather<true>(a, (cudaStream_t)stream, cvt, (flags & DDSK_F_PUT) != 0, (flags & DDSK_F_ACC) != 0,
+                               (flags & DDSK_F_FOP) != 0);
 }
 
 int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const ddsk_push_t *push_dev,
@@ -2598,14 +2855,14 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     a.nreq = nreq;
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
-    const bool put = (flags & DDSK_F_PUT) != 0, acc = (flags & DDSK_F_ACC) != 0;
+    const bool put = (flags & DDSK_F_PUT) != 0, acc = (flags & DDSK_F_ACC) != 0, fop = (flags & DDSK_F_FOP) != 0;
     const int gs = select_s(nreq, cap_total, cvt, put);
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
         // (no scratch is shared between launches: independent batches may overlap)
         if (a.overlap) a.tickets = scr->ovl + 8 + (a.seq & 3u);
-        return launch_gather_s(gs, a, st, cvt, put, acc);
+        return launch_gather_s(gs, a, st, cvt, put, acc, fop);
     }
     if (nreq > scr->cap_req || cap_total / SEG_GRAIN + 2 > scr->seg_cap) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_gather_var: scratch too small (%lld requests > %lld, or %lld segments > %lld)",
@@ -2649,7 +2906,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
         a.plan_word = scr->plan_word;
         a.plan_tiles = tiles;
     }
-    return launch_gather<false>(a, st, cvt, put, acc);
+    return launch_gather<false>(a, st, cvt, put, acc, fop);
 }
 
 int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt) {

@@ -60,6 +60,8 @@ typedef struct ddsk_scratch {
     int64_t seg_cap;
     unsigned long long *host_mirror; /* device alias of pinned host words: [0] status, [1] packed total (written by the
                                         last warp of a gather launch that asks for it), [2] ticket of dds_small_get */
+    void *fop_result;           /* host side, set by the caller of a DDSK_F_FOP launch: the caller's result buffer (device
+                                   memory, the layout of the source rows) */
 } ddsk_scratch_t;
 
 /* `flags` of the launchers */
@@ -81,6 +83,11 @@ typedef struct ddsk_scratch {
                                is DDSK_F_ACC_TYPE(flags); the caller's rows are aligned to its size. */
 #define DDSK_F_ACC_SHIFT 10 /* bits 10..12 of the flags: the accumulate's element type (DDSK_ACC_*) */
 #define DDSK_F_ACC_TYPE(f) (((f) >> DDSK_F_ACC_SHIFT) & 7)
+#define DDSK_F_FOP 8192     /* with DDSK_F_PUT: a batched fetch-op -- the put's walk, layout and checks, whose drain applies
+                               an atomic that returns each element's previous value and writes that value to the same
+                               position of scr->fop_result as the operand's in the caller's rows. The element type is
+                               DDSK_F_ACC_TYPE(flags); the caller's rows and fop_result are aligned to its size. */
+#define DDSK_F_FOP_SWAP 16384 /* with DDSK_F_FOP: the op is a swap (shard = src); else an add (shard = shard + src) */
 
 /* element types of an accumulate (same values as DDS_ACC_* in include/ddstore_b200.h) */
 #define DDSK_ACC_F32 1

@@ -1714,9 +1714,13 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
 // single-request kernels.
 // acc: 0 for a put; a DDS_ACC_* element type for the accumulate behind dds_accumulate_batch / dds_accumulate_samples,
 // the same launch whose drain adds (DDSK_F_ACC). Its src must be aligned to the element size.
+// op: 0, or a DDS_OP_* for the fetch-op behind dds_get_accumulate_batch / dds_get_accumulate_samples (with acc its element
+// type): the same launch whose drain applies a returning atomic and writes the previous rows to `result`, in the layout
+// of src (DDSK_F_FOP). result must be aligned to the element size too.
 static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
                     int64_t fixed_count, int64_t nreq, const void *src, int64_t src_bytes, unsigned flags,
-                    void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, int acc = 0) {
+                    void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, int acc = 0, int op = 0,
+                    void *result = nullptr) {
     if (!(flags & DDS_SRC_ON_DEVICE)) return fail(DDS_ERR_ARG, "puts take their rows from device memory (DDS_SRC_ON_DEVICE)");
     if (nreq < 0 || src_bytes < 0) return fail(DDS_ERR_ARG, "negative nreq or src_bytes");
     if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
@@ -1728,6 +1732,9 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     if (!src && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null src");
     if (acc && (uintptr_t)src % (uintptr_t)v->itemsize)
         return fail(DDS_ERR_ARG, "accumulates take src aligned to the element size");
+    if (op && !result && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null result");
+    if (op && (uintptr_t)result % (uintptr_t)v->itemsize)
+        return fail(DDS_ERR_ARG, "fetch-ops take result aligned to the element size");
 
     Call c;
     if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
@@ -1745,7 +1752,12 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     ddsk_scratch_t scr;
     if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
     void *d_src = const_cast<void *>(src);
-    kflags |= DDSK_F_PUT | (acc ? DDSK_F_ACC | acc << DDSK_F_ACC_SHIFT : 0);
+    if (op) {
+        kflags |= DDSK_F_PUT | DDSK_F_FOP | acc << DDSK_F_ACC_SHIFT | (op == DDS_OP_REPLACE ? DDSK_F_FOP_SWAP : 0);
+        scr.fop_result = result;
+    } else {
+        kflags |= DDSK_F_PUT | (acc ? DDSK_F_ACC | acc << DDSK_F_ACC_SHIFT : 0);
+    }
     const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st)
                           : ddsk_gather_var(&v->kv, &ix, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st);
     s->scr.plan_tag = scr.plan_tag;
@@ -1800,6 +1812,33 @@ int dds_accumulate_samples(dds_store_t *s, const char *name, const int64_t *samp
     if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
                     dtype);
+}
+
+// The fetch-ops' prologue: the accumulates' and an unknown op
+static int fop_entry(dds_store_t *s, const char *name, int op, int dtype, int64_t *total_bytes, int64_t *bad_index,
+                     Var **v) {
+    if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, v)) return rc;
+    if (op != DDS_OP_SUM && op != DDS_OP_REPLACE) return fail(DDS_ERR_ARG, "unknown fetch-op");
+    return DDS_OK;
+}
+
+int dds_get_accumulate_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                             int64_t fixed_count, int64_t nreq, int op, int dtype, const void *src, void *result,
+                             int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                             int64_t *bad_index) {
+    Var *v;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v)) return rc;
+    return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
+                    bad_index, dtype, op, result);
+}
+
+int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
+                               int dtype, const void *src, void *result, int64_t src_bytes, unsigned flags,
+                               void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    Var *v;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v)) return rc;
+    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
+                    dtype, op, result);
 }
 
 // The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,

@@ -59,6 +59,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
         long accumulate_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                               int dtype, const void* src, long src_bytes, cbool idx_on_device,
                               void* stream) except +dds_translate_exception
+        long get_accumulate_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
+                                  int op, int dtype, const void* src, void* result, long src_bytes, cbool idx_on_device,
+                                  void* stream) except +dds_translate_exception
         void epoch_begin() except +dds_translate_exception
         void epoch_end() except +dds_translate_exception
         void free() except +dds_translate_exception
@@ -70,6 +73,8 @@ cdef extern from "ddstore_b200.hpp" nogil:
 
 # element types of accumulate_batch (DDS_ACC_*), by dtype name
 _ACC_TYPES = {"float32": 1, "float64": 2, "int32": 3, "int64": 4, "float16": 5, "bfloat16": 6}
+# ops of get_accumulate_batch (DDS_OP_*), by name
+_FOP_OPS = {"sum": 1, "replace": 2}
 
 cdef class PyDDStore:
     cdef DDStore* c_ddstore
@@ -334,6 +339,54 @@ cdef class PyDDStore:
         with nogil:
             total = self.c_ddstore.accumulate_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, code,
                                                     <const void*> dp, nbytes, idx_dev, <void*> st)
+        del keep
+        return total
+
+    def get_accumulate_batch(self, str name, starts, counts=None, src=None, out=None, op="sum", count=None,
+                             stream=None):
+        """one kernel launch ADDING (op="sum") or SWAPPING (op="replace") len(starts) requests of the CUDA tensor `src`
+        into the owners' shards and writing the previous rows to the CUDA tensor `out` (src's layout, at least its
+        bytes; it may be src); see ddstore_b200.store.PyDDStore.get_accumulate_batch (this binding's fetch-op is
+        synchronous). Returns the layout's bytes."""
+        if src is None:
+            raise ValueError("a fetch-op needs `src` rows")
+        if not (hasattr(src, "data_ptr") and getattr(src, "is_cuda", False)):
+            raise ValueError(f"fetch-op on {name!r}: src must be a CUDA tensor (copy host rows to the device first)")
+        if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)):
+            raise ValueError(f"fetch-op on {name!r}: out must be a CUDA tensor")
+        if not src.is_contiguous() or not out.is_contiguous():
+            raise ValueError("src and out must be C-contiguous")
+        dt = str(src.dtype).replace("torch.", "")
+        if dt not in _ACC_TYPES:
+            raise ValueError(f"fetch-op on {name!r}: src dtype {dt} is not one of {', '.join(_ACC_TYPES)}")
+        if op not in _FOP_OPS:
+            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(_FOP_OPS)}")
+        cdef long nbytes = src.numel() * src.element_size()
+        if out.numel() * out.element_size() < nbytes:
+            raise ValueError(f"fetch-op on {name!r}: out holds {out.numel() * out.element_size()} bytes, src {nbytes}")
+        cdef int code = _ACC_TYPES[dt], opc = _FOP_OPS[op]
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        cdef size_t sp, cp = 0, dp = src.data_ptr(), rp = out.data_ptr()
+        cdef long nreq
+        if s_dev:
+            nreq = starts.numel(); sp = starts.data_ptr()
+            if counts is not None: cp = counts.data_ptr()
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
+            ca = _i64(counts) if counts is not None else None
+            if ca is not None: cp = ca.ctypes.data
+            keep = (sa, ca)
+        cdef long fixed = 1 if count is None else int(count)
+        cdef size_t st = 0
+        if stream is not None:
+            st = int(stream) if int(stream) != 0 else 1
+        cdef string nm = name.encode()
+        cdef cbool idx_dev = bool(s_dev)
+        cdef long total
+        with nogil:
+            total = self.c_ddstore.get_accumulate_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, opc, code,
+                                                        <const void*> dp, <void*> rp, nbytes, idx_dev, <void*> st)
         del keep
         return total
 

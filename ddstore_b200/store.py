@@ -453,6 +453,78 @@ class PyDDStore:
         _capi.raise_for(rc)
         return total.value
 
+    # ---------------------------------------------------------------- batched fetch-ops (MPI_Get_accumulate)
+    def get_accumulate_batch(self, name, starts, counts=None, src=None, out=None, op="sum", count=None, stream=None,
+                             wait=True):
+        """ADD (op="sum") or SWAP (op="replace") len(starts) requests into the owners' shards in ONE kernel launch and
+        get the previous rows back: for every element e of request i's rows, in one atomic step, out[e] = shard[e]
+        and shard[e] becomes shard[e] + src[e] (sum) or src[e] (replace). Requests, the layout of `src`, dtypes,
+        errors (every valid request is still applied, an invalid one changes nothing), wait=False, ordering and
+        visibility are accumulate_batch's. `out` is a C-contiguous CUDA tensor of at least src's bytes -- it may be src
+        itself -- that receives the previous rows in src's layout; the bytes of invalid requests and every byte beyond
+        the layout are left as they were. Fetch-ops on one element in one epoch are linearisable, from any batch, rank
+        or duplicate request: each gets the value right before its own contribution (duplicate +1 requests of one batch
+        get distinct tickets). Sums also combine atomically with accumulate_batch; mixing "replace" with sums, puts or
+        accumulates on one element in one epoch is undefined. Returns the layout's size in bytes."""
+        sb, keep_src = self._put_src(name, src)
+        code = self._acc_type(name, src)
+        opc, res = self._fop_args(name, op, out, sb)
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        if s_dev:
+            nreq, sp = starts.numel(), starts.data_ptr()
+            cp = counts.data_ptr() if counts is not None else None
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts)
+            ca = _i64(counts) if counts is not None else None
+            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
+            keep = (sa, ca)
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_get_accumulate_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
+                                              opc, code, sb.ptr, res, sb.nbytes, flags, self._stream_arg(stream),
+                                              C.byref(total), C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    def get_accumulate_samples(self, name, sample_ids, src, out, op="sum", stream=None, wait=True):
+        """get_accumulate_batch by SAMPLE ID: request i adds into (or swaps) the rows of sample sample_ids[i] in the
+        index registered with set_sample_index. Layout and errors as put_samples, ops as get_accumulate_batch."""
+        sb, keep_src = self._put_src(name, src)
+        code = self._acc_type(name, src)
+        opc, res = self._fop_args(name, op, out, sb)
+        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
+        if s_dev:
+            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
+        else:
+            sa = _i64(sample_ids)
+            nreq, sp, keep = sa.size, sa.ctypes.data, sa
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_get_accumulate_samples(self._h, name.encode(), sp, nreq, opc, code, sb.ptr, res, sb.nbytes,
+                                                flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    @staticmethod
+    def _fop_args(name, op, out, sb):
+        """the DDS_OP_* code of a fetch-op and the address of its `out` tensor (ValueError for an unknown op, or an out
+        that is not a contiguous CUDA tensor of at least src's bytes)"""
+        if op not in _capi.FOP_OPS:
+            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(_capi.FOP_OPS)}")
+        if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)):
+            raise ValueError(f"fetch-op on {name!r}: out must be a CUDA tensor")
+        if not out.is_contiguous():
+            raise ValueError("out must be C-contiguous")
+        if out.numel() * out.element_size() < sb.nbytes:
+            raise ValueError(f"fetch-op on {name!r}: out holds {out.numel() * out.element_size()} bytes, src "
+                             f"{sb.nbytes}")
+        return _capi.FOP_OPS[op], out.data_ptr()
+
     @staticmethod
     def _acc_type(name, src):
         """the DDS_ACC_* element type of an accumulate's src, from its dtype (ValueError for any other)"""
@@ -679,8 +751,9 @@ class PyDDStore:
         previous wait() (0 if none).
         wait() alone reports the outcome of queued batches, exactly once. Any other call that meets a pending queue
         (a synchronous get_batch / get / get_samples / get_samples_multi / put_batch / put_samples / accumulate_batch /
-        accumulate_samples, a batch on another stream, set_sample_index, set_normalization, epoch_end, epoch_begin
-        when the queue holds a put or an accumulate, free) completes it, keeps its first failure for the next wait(), and raises only
+        accumulate_samples / get_accumulate_batch / get_accumulate_samples, a batch on another stream,
+        set_sample_index, set_normalization, epoch_end, epoch_begin when the queue holds a put, an accumulate or a
+        fetch-op, free) completes it, keeps its first failure for the next wait(), and raises only
         for its own requests. A failure kept from earlier wins over later ones; after wait() has raised it, the next
         wait() is clean. close() drops an outcome no wait() has reported."""
         total, bad = C.c_int64(0), C.c_int64(-1)

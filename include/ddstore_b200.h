@@ -25,8 +25,9 @@ extern "C" {
 #define DDS_VERSION 111 /* 110: converting batches (dds_get_batch_convert & co.); 111: normalising conversions.
                            The padded batches (dds_get_batch_padded, dds_get_samples_padded) add entries only: callers
                            that built against 111 are unaffected, and a caller finds them by symbol. So do the batched
-                           puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE) and the batched accumulates
-                           (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*). */
+                           puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE), the batched accumulates
+                           (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*) and the batched fetch-ops
+                           (dds_get_accumulate_batch, dds_get_accumulate_samples, DDS_OP_*). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -341,6 +342,37 @@ int dds_accumulate_samples(dds_store_t *s, const char *name, const int64_t *samp
                            const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                            int64_t *bad_index);
 
+/* ---- batched fetch-ops: rows added into or swapped with any rank's shard, the previous rows returned (MPI_Get_accumulate
+ * with MPI_SUM or MPI_REPLACE between fences). For every element e of request i's rows, in one atomic step:
+ *   DDS_OP_SUM:     result[e] = shard[e]; shard[e] = shard[e] + src[e]   (the sum taken in dtype)
+ *   DDS_OP_REPLACE: result[e] = shard[e]; shard[e] = src[e]              (a swap)
+ * Requests, the layout of src, validation, error reporting (every valid request is applied, an invalid one changes
+ * nothing, the first invalid one is reported; a layout total above src_bytes applies nothing, DDS_ERR_CAPACITY), dtype
+ * (a DDS_ACC_* code; a size other than the variable's itemsize is DDS_ERR_DTYPE), flags, DDS_NO_SYNC queueing, fences
+ * and the ignored DDS_OVERLAP (a fetch-op ends an overlap run) are dds_accumulate_batch's / dds_accumulate_samples's,
+ * word for word.
+ * result has the layout of src: request i's previous rows go to result bytes [o_i, o_i + n_i), the offsets its src rows
+ * occupy. It is device memory of at least src_bytes bytes. An invalid request's result bytes, and every byte outside
+ * the valid requests' ranges, are left untouched; a capacity error writes nothing to the shards or to result. result ==
+ * src is allowed (an in-place exchange); any other overlap of result with src, or of either with a shard, is undefined.
+ * Atomicity is per element, as in MPI: fetch-ops on one element in one epoch -- from any batch, any rank, or duplicate
+ * requests of one batch -- are linearisable, and each one's result is the element's value immediately before its own
+ * contribution. DDS_OP_SUM fetch-ops also combine atomically with dds_accumulate_* of the same dtype on the same element.
+ * Mixing DDS_OP_REPLACE with sums, accumulates or puts on one element in one epoch is undefined (MPI allows only the
+ * same op or MPI_NO_OP). Rows are not atomic as a whole. Float sums round once per addition, f32 may flush subnormal
+ * inputs and results to zero as the accumulate's may; f16 and bf16 do not flush; f64 is IEEE; integers wrap.
+ * In addition to the accumulate's argument errors, with DDS_ERR_ARG and nothing enqueued: an unknown op, result == NULL
+ * while the layout is non-empty, and a result not aligned to the element size. */
+#define DDS_OP_SUM 1     /* result[e] = shard[e]; shard[e] = shard[e] + src[e]   (MPI_SUM, in dtype) */
+#define DDS_OP_REPLACE 2 /* result[e] = shard[e]; shard[e] = src[e]              (MPI_REPLACE: swap) */
+int dds_get_accumulate_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                             int64_t fixed_count, int64_t nreq, int op, int dtype, const void *src, void *result,
+                             int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                             int64_t *bad_index);
+int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
+                               int dtype, const void *src, void *result, int64_t src_bytes, unsigned flags,
+                               void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite
  * flow. When all ranks fetch in the same
@@ -359,7 +391,7 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
  * failing batch in queue order is reported, with that batch's first invalid request in *bad_index.
  * The outcome of queued batches is reported here and only here, exactly once. Any other call that meets a pending
  * queue (a synchronous batch or get(), a batch on another stream, dds_set_sample_index, dds_set_normalization,
- * dds_epoch_end, dds_epoch_begin when the queue holds a put or an accumulate, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
+ * dds_epoch_end, dds_epoch_begin when the queue holds a put, an accumulate or a fetch-op, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
  * then does its own work and reports only its own outcome (its error and *bad_index describe its own requests). The
  * next dds_batch_wait reports the kept failure, with its index and text, after completing any queue still pending; a
  * failure kept from earlier wins over any failure queued after it, since it is earlier in queue order. After it has
