@@ -2476,35 +2476,31 @@ __global__ void dds_occupy_kernel(unsigned long long ns, int smem_bytes) {
 // ------------------------------------------------------------------------------------------------
 // launch geometry
 // ------------------------------------------------------------------------------------------------
+// Every geometry dds_gather_kernel is launched with: warps per CTA, ring stages per warp, chunk bytes, and the capacity of
+// a plan held in shared memory (0: the plan, if any, is in global memory). Each is named here once; every launch, fit
+// check and plan threshold below reads it from these constants. Every geometry runs one CTA per SM.
 struct Geometry {
     int nw, stages, ch, pcap;
 };
-// plan-in-global variants (fixed-count entry, and variable-count batches above 8192 requests)
-constexpr Geometry kGeoms[] = {{8, 4, 4096, 0}, {8, 6, 4096, 0}, {16, 3, 4096, 0}, {4, 4, 8192, 0}, {12, 4, 4096, 0}, {4, 6, 4096, 0},
-                               {6, 4, 4096, 0},   // (5-6: half-size CTAs, two per SM with DDS_GATHER_CTAS_PER_SM=2)
-                               {12, 3, 4096, 0}}; // (7: less in flight per SM -> shorter memory queues)
-constexpr int kNumGeoms = (int)(sizeof(kGeoms) / sizeof(kGeoms[0]));
-// plan-in-shared-memory variants (variable-count entry): the plan's 12 B per request come out of the stage budget
-constexpr Geometry kGeomsS[] = {{12, 3, 4096, 4096}, {12, 3, 3072, 8192}, {16, 3, 2048, 8192}, {16, 3, 3072, 4096}, {8, 4, 4096, 4096}};
-constexpr int kNumGeomsS = (int)(sizeof(kGeomsS) / sizeof(kGeomsS[0]));
-constexpr int64_t kPlanSmemMax = 8192;
+// On an H100 SXM (400 W limit) config 2 (4 KiB rows) is HBM-bound with every fixed-count geometry tried: they measured
+// within 0.3 % of each other, so large rows keep 12 warps x 4 stages (also used for the instruction-heavier variable /
+// re-phase path); rows under 2 KiB take more warps to keep more small copies in flight.
+constexpr Geometry kLargeRows = {12, 4, 4096, 0}; // every plan-in-global launch but the two below
+constexpr Geometry kSmallRows = {16, 3, 4096, 0}; // fixed-count raw gets of requests under 2 KiB
+constexpr Geometry kFetch = {12, 3, 4096, 0};     // fetch-ops: one stage fewer leaves room for their result addresses
+// plan in shared memory (variable-count entries): the plan's 12 B per request come out of the stage budget
+constexpr Geometry kPlan4K = {12, 3, 4096, 4096};
+constexpr Geometry kPlan8K = {12, 3, 3072, 8192};
+constexpr Geometry kPlan8KFetch = {12, 3, 2048, 8192}; // (with their result addresses too, fetch-ops fit 2 KiB chunks only)
+constexpr int64_t kPlanSmemMax = kPlan8K.pcap;
 // The redundant plan grows with the batch (every SM reads the same index lines), while the plan kernels cost ~0 when
 // they run under the previous batch's gather -- so by default only small batches, where one launch beats three, plan
 // in shared memory.
 int64_t g_plan_smem_default = 1024; // DDS_SMEM_PLAN_MAX
 
-// On an H100 SXM (400 W limit) config 2 (4 KiB rows) is HBM-bound with every fixed-count variant: 0-4 and 7 are within
-// 0.3 % of each other, so 12 warps x 4 stages (also used for the instruction-heavier variable / re-phase path) stays
-// the default; rows under 2 KiB take more warps (16 x 3) to keep more small copies in flight.
-constexpr int kGeomLarge = 4, kGeomSmall = 2, kGeomVar = 4;
-
-int g_geom_fixed_env = -1; // DDS_GATHER_GEOM      (tuning: force one variant for the fixed-count entry)
-int g_geom_var_env = -1;   // DDS_GATHER_GEOM_VAR  (... for the variable-count entry, plan in global; defaults to the former)
-int g_geom_s_env = -1;     // DDS_GATHER_GEOM_S    (... for the variable-count entry, plan in shared memory)
 int g_min_seg_var = 4, g_min_seg_s = 2; // DDS_VAR_MINSEG / DDS_S_MINSEG: smallest segment in chunks
 bool g_geom_init = false;
 int g_sms = 0;
-int g_ctas_per_sm = 1;
 int g_pdl = 1;
 // DDS_DEBUG_TIMING=1: device buffer of globaltimer stamps, two regions (overlap launches alternate by sequence parity):
 // [cta * 4 + {entry, plan known, first data, last warp done}] for cta < 1024, then [4096 + {lookup last CTA start, lookup
@@ -2519,16 +2515,8 @@ int pick_geometry() {
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     CUDA_TRY(cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev));
-    if (const char *e = getenv("DDS_GATHER_GEOM")) g_geom_fixed_env = atoi(e);
-    if (g_geom_fixed_env >= kNumGeoms) g_geom_fixed_env = -1;
-    g_geom_var_env = g_geom_fixed_env;
-    if (const char *e = getenv("DDS_GATHER_GEOM_VAR")) g_geom_var_env = atoi(e);
-    if (g_geom_var_env >= kNumGeoms) g_geom_var_env = -1;
-    if (const char *e = getenv("DDS_GATHER_GEOM_S")) g_geom_s_env = atoi(e);
-    if (g_geom_s_env >= kNumGeomsS) g_geom_s_env = -1;
     if (const char *e = getenv("DDS_VAR_MINSEG")) g_min_seg_var = atoi(e) > 0 ? atoi(e) : 4;
     if (const char *e = getenv("DDS_S_MINSEG")) g_min_seg_s = atoi(e) > 0 ? atoi(e) : 2;
-    if (const char *e = getenv("DDS_GATHER_CTAS_PER_SM")) g_ctas_per_sm = atoi(e) > 0 ? atoi(e) : 1;
     if (const char *e = getenv("DDS_PDL")) g_pdl = atoi(e) != 0;
     if (const char *e = getenv("DDS_SMEM_PLAN")) g_smem_plan = atoi(e);
     if (const char *e = getenv("DDS_SMEM_PLAN_MAX")) g_plan_smem_default = atoll(e);
@@ -2542,27 +2530,7 @@ int pick_geometry() {
     return 0;
 }
 
-int geometry_for(bool fixed, int64_t request_bytes) {
-    if (fixed) {
-        if (g_geom_fixed_env >= 0) return g_geom_fixed_env;
-        return request_bytes < 2048 ? kGeomSmall : kGeomLarge;
-    }
-    return g_geom_var_env >= 0 ? g_geom_var_env : kGeomVar;
-}
-// shared-memory-plan variant for a batch of nreq requests (-1: does not fit)
-int geometry_s_for(int64_t nreq) {
-    if (nreq > kPlanSmemMax || nreq > g_plan_smem_default) return -1;
-    if (g_geom_s_env >= 0 && kGeomsS[g_geom_s_env].pcap >= nreq) return g_geom_s_env;
-    return nreq <= 4096 ? 0 : 1;
-}
-
-constexpr int smem_bytes_of(int nw, int s, int ch, int pcap) { return nw * s * (ch + 32) + (pcap ? pcap * 12 + 16 : 0); }
-int static_smem_of(int nw, int s) { return nw * s * (8 + 32 * 16) + 16 * 8 + 64; }
-int ctas_per_sm_for(int nw, int s, int ch, int pcap) {
-    int per_sm = g_ctas_per_sm;
-    while (per_sm > 1 && per_sm * (smem_bytes_of(nw, s, ch, pcap) + static_smem_of(nw, s) + 1024) > 227 * 1024) per_sm--;
-    return per_sm;
-}
+constexpr int smem_bytes_of(const Geometry &g) { return g.nw * g.stages * (g.ch + 32) + (g.pcap ? g.pcap * 12 + 16 : 0); }
 
 // does a converting launch carry a normalising code? (then it takes the NORM form of the kernel; unused slots are 0)
 bool cvt_has_norm(const ddsk_cvt_t *cvt) {
@@ -2571,14 +2539,14 @@ bool cvt_has_norm(const ddsk_cvt_t *cvt) {
     return false;
 }
 
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
+template <bool FIXED, const Geometry &G, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
           bool ACC = false, bool FETCH = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
     // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan; a fetch-op its
     //  pieces' result addresses)
-    const int smem = smem_bytes_of(NW, S, CH, PCAP) + (CVT ? cvt->lut_bytes : 0) + (FETCH ? NW * S * 32 * 8 : 0);
+    const int smem = smem_bytes_of(G) + (CVT ? cvt->lut_bytes : 0) + (FETCH ? G.nw * G.stages * 32 * 8 : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, NW, S, CH, PCAP, CVT, NORM, PAD, PUT, ACC, FETCH>;
+    auto kern = dds_gather_kernel<FIXED, G.nw, G.stages, G.ch, G.pcap, CVT, NORM, PAD, PUT, ACC, FETCH>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -2587,7 +2555,7 @@ int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_c
             int optin = 0;
             CUDA_TRY(cudaFuncGetAttributes(&fa, kern));
             CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-            const int most = std::min(smem_bytes_of(NW, S, CH, PCAP) + DDSK_MAX_MULTI * 1024, optin - (int)fa.sharedSizeBytes);
+            const int most = std::min(smem_bytes_of(G) + DDSK_MAX_MULTI * 1024, optin - (int)fa.sharedSizeBytes);
             CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
             if (dev < 64) configured.fetch_or(1ull << dev);
         }
@@ -2595,12 +2563,11 @@ int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_c
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         if (dev < 64) configured.fetch_or(1ull << dev);
     }
-    const int per_sm = ctas_per_sm_for(NW, S, CH, PCAP);
     GatherArgs args = args_in;
     args.dbg = g_dbg ? g_dbg + (size_t)(args.overlap ? (args.seq & 1u) : 0u) * kDbgRegion : nullptr;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(g_sms * per_sm));
-    cfg.blockDim = dim3(NW * 32);
+    cfg.gridDim = dim3((unsigned)g_sms);
+    cfg.blockDim = dim3(G.nw * 32);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
@@ -2617,18 +2584,19 @@ int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_c
     return 0;
 }
 
-// Does a converting launch of shared-memory-plan variant g with `lut_bytes` of tables fit in shared memory? (With four
-// 1 KiB tables the 8192-request variant does not: such batches plan in global memory instead.)
-template <int NW, int S, int CH, int PCAP>
+// Does a converting launch of shared-memory-plan geometry G with `lut_bytes` of tables fit in shared memory? (With four
+// 1 KiB tables the 8192-request plan does not: such batches plan in global memory instead.)
+template <const Geometry &G>
 bool cvt_s_fits_t(int lut_bytes) {
     cudaFuncAttributes fa;
     int dev = 0, optin = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaFuncGetAttributes(&fa, dds_gather_kernel<false, NW, S, CH, PCAP, true>) != cudaSuccess ||
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaFuncGetAttributes(&fa, dds_gather_kernel<false, G.nw, G.stages, G.ch, G.pcap, true>) != cudaSuccess ||
         cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) {
         (void)cudaGetLastError();
         return false;
     }
-    return smem_bytes_of(NW, S, CH, PCAP) + lut_bytes + (int)fa.sharedSizeBytes <= optin;
+    return smem_bytes_of(G) + lut_bytes + (int)fa.sharedSizeBytes <= optin;
 }
 
 // launch with the programmatic-dependent-launch attribute (the kernels call griddepcontrol.wait themselves)
@@ -2665,64 +2633,36 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
     return 0;
 }
 
+// One launch of the kind the flags ask for: a fetch-op at geometry GF, every other kind (accumulate, put, normalising,
+// converting, raw) at G.
+template <bool FIXED, const Geometry &G, const Geometry &GF>
+int launch_kind(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put, bool acc, bool fop) {
+    if (fop) return launch_gather_t<FIXED, GF, false, false, false, true, false, true>(args, stream);
+    if (acc) return launch_gather_t<FIXED, G, false, false, false, true, true>(args, stream);
+    if (put) return launch_gather_t<FIXED, G, false, false, false, true>(args, stream);
+    if (cvt) return cvt_has_norm(cvt) ? launch_gather_t<FIXED, G, true, true>(args, stream, cvt)
+                                      : launch_gather_t<FIXED, G, true>(args, stream, cvt);
+    return launch_gather_t<FIXED, G>(args, stream);
+}
+
+// plan in global memory (or none): small rows for fixed-count raw gets of requests under 2 KiB, large rows otherwise
 template <bool FIXED>
 int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false, bool acc = false,
                   bool fop = false) {
-    // converting launches, puts and accumulates: the default variant of each entry (kGeomLarge = kGeomVar), whatever
-    // DDS_GATHER_GEOM* say. Fetch-ops: one stage fewer (variant 7), which leaves room for their result addresses.
-    if (fop) return launch_gather_t<FIXED, 12, 3, 4096, 0, false, false, false, true, false, true>(args, stream);
-    if (acc) return launch_gather_t<FIXED, 12, 4, 4096, 0, false, false, false, true, true>(args, stream);
-    if (put) return launch_gather_t<FIXED, 12, 4, 4096, 0, false, false, false, true>(args, stream);
-    if (cvt) return cvt_has_norm(cvt) ? launch_gather_t<FIXED, 12, 4, 4096, 0, true, true>(args, stream, cvt)
-                                      : launch_gather_t<FIXED, 12, 4, 4096, 0, true>(args, stream, cvt);
-    // (the request size only picks a variant: a count too large to multiply safely counts as large)
-    const int64_t request_bytes = args.count < ((int64_t)1 << 20) ? args.count * args.var.row_bytes : INT64_MAX;
-    switch (geometry_for(FIXED, FIXED ? request_bytes : 0)) {
-    case 1: return launch_gather_t<FIXED, 8, 6, 4096, 0>(args, stream);
-    case 2: return launch_gather_t<FIXED, 16, 3, 4096, 0>(args, stream);
-    case 3: return launch_gather_t<FIXED, 4, 4, 8192, 0>(args, stream);
-    case 4: return launch_gather_t<FIXED, 12, 4, 4096, 0>(args, stream);
-    case 5: return launch_gather_t<FIXED, 4, 6, 4096, 0>(args, stream);
-    case 6: return launch_gather_t<FIXED, 6, 4, 4096, 0>(args, stream);
-    case 7: return launch_gather_t<FIXED, 12, 3, 4096, 0>(args, stream);
-    default: return launch_gather_t<FIXED, 8, 4, 4096, 0>(args, stream);
+    if constexpr (FIXED) {
+        // (a count too large to multiply safely counts as large)
+        const int64_t request_bytes = args.count < ((int64_t)1 << 20) ? args.count * args.var.row_bytes : INT64_MAX;
+        if (!put && !acc && !fop && !cvt && request_bytes < 2048) return launch_gather_t<true, kSmallRows>(args, stream);
     }
-}
-int launch_gather_s(int g, const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put, bool acc, bool fop) {
-    // (fetch-ops: the 8192-request plan leaves room for the result addresses with 2 KiB chunks only)
-    if (fop)
-        return g == 1 ? launch_gather_t<false, 12, 3, 2048, 8192, false, false, false, true, false, true>(args, stream)
-                      : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true, false, true>(args, stream);
-    if (acc)
-        return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, false, false, false, true, true>(args, stream)
-                      : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true, true>(args, stream);
-    if (put)
-        return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, false, false, false, true>(args, stream)
-                      : launch_gather_t<false, 12, 3, 4096, 4096, false, false, false, true>(args, stream);
-    if (cvt && cvt_has_norm(cvt))
-        return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, true, true>(args, stream, cvt)
-                      : launch_gather_t<false, 12, 3, 4096, 4096, true, true>(args, stream, cvt);
-    if (cvt) return g == 1 ? launch_gather_t<false, 12, 3, 3072, 8192, true>(args, stream, cvt)
-                           : launch_gather_t<false, 12, 3, 4096, 4096, true>(args, stream, cvt);
-    switch (g) {
-    case 1: return launch_gather_t<false, 12, 3, 3072, 8192>(args, stream);
-    case 2: return launch_gather_t<false, 16, 3, 2048, 8192>(args, stream);
-    case 3: return launch_gather_t<false, 16, 3, 3072, 4096>(args, stream);
-    case 4: return launch_gather_t<false, 8, 4, 4096, 4096>(args, stream);
-    default: return launch_gather_t<false, 12, 3, 4096, 4096>(args, stream);
-    }
+    return launch_kind<FIXED, kLargeRows, kFetch>(args, stream, cvt, put, acc, fop);
 }
 
-// The shared-memory-plan variant for a batch of nreq requests into cap bytes (-1: the plan kernels). Converting launches
-// use the default variants only (DDS_GATHER_GEOM_S applies to raw gets), and need room for their tables. Puts take the
-// raw gets' placement rule with the default variants (and so do accumulates, which are puts).
-int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool put = false) {
-    if (!g_smem_plan || cap >= ((int64_t)1 << 32)) return -1;
-    if (!cvt && !put) return geometry_s_for(nreq);
-    if (nreq > kPlanSmemMax || nreq > g_plan_smem_default) return -1;
-    if (put) return nreq <= 4096 ? 0 : 1;
-    if (nreq <= 4096) return cvt_s_fits_t<12, 3, 4096, 4096>(cvt->lut_bytes) ? 0 : -1;
-    return cvt_s_fits_t<12, 3, 3072, 8192>(cvt->lut_bytes) ? 1 : -1;
+// The shared-memory plan for a batch of nreq requests into cap bytes: 0 = kPlan4K, 1 = kPlan8K (-1: the plan kernels).
+// A converting launch also needs room for its tables.
+int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt) {
+    if (!g_smem_plan || cap >= ((int64_t)1 << 32) || nreq > kPlanSmemMax || nreq > g_plan_smem_default) return -1;
+    if (nreq <= kPlan4K.pcap) return !cvt || cvt_s_fits_t<kPlan4K>(cvt->lut_bytes) ? 0 : -1;
+    return !cvt || cvt_s_fits_t<kPlan8K>(cvt->lut_bytes) ? 1 : -1;
 }
 
 // The fields every gather launch shares: the variable's window, status reporting, the host mirror (DDSK_F_MIRROR), the
@@ -2777,12 +2717,11 @@ void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk
         *ctas = *warps_per_cta = *stages = *chunk_bytes = *smem_bytes = 0;
         return;
     }
-    const Geometry &g = kGeoms[geometry_for(true, 4096)];
-    *ctas = g_sms * ctas_per_sm_for(g.nw, g.stages, g.ch, 0);
-    *warps_per_cta = g.nw;
-    *stages = g.stages;
-    *chunk_bytes = g.ch;
-    *smem_bytes = smem_bytes_of(g.nw, g.stages, g.ch, 0);
+    *ctas = g_sms;
+    *warps_per_cta = kLargeRows.nw;
+    *stages = kLargeRows.stages;
+    *chunk_bytes = kLargeRows.ch;
+    *smem_bytes = smem_bytes_of(kLargeRows);
 }
 
 int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t count, int64_t nreq, void *dst_dev,
@@ -2841,10 +2780,9 @@ int ddsk_gather_padded(const ddsk_var_t *var, const ddsk_index_t *index, int64_t
     a.pad_in_log2 = cvt ? cvt_in_log2<true>(cvt->code[0]) : 0;
     a.pad_out_log2 = cvt ? cvt_out_log2<true>(cvt->code[0]) : 0;
     a.pad_lengths = lengths;
-    // the default fixed-count geometry, whatever DDS_GATHER_GEOM says
-    if (!cvt) return launch_gather_t<true, 12, 4, 4096, 0, false, false, true>(a, st);
-    return cvt_has_norm(cvt) ? launch_gather_t<true, 12, 4, 4096, 0, true, true, true>(a, st, cvt)
-                             : launch_gather_t<true, 12, 4, 4096, 0, true, false, true>(a, st, cvt);
+    if (!cvt) return launch_gather_t<true, kLargeRows, false, false, true>(a, st);
+    return cvt_has_norm(cvt) ? launch_gather_t<true, kLargeRows, true, true, true>(a, st, cvt)
+                             : launch_gather_t<true, kLargeRows, true, false, true>(a, st, cvt);
 }
 
 // shared by ddsk_gather_var / ddsk_gather_multi: plan (in the launch, or by the two plan kernels) + gather. `a` comes
@@ -2856,13 +2794,14 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
     const bool put = (flags & DDSK_F_PUT) != 0, acc = (flags & DDSK_F_ACC) != 0, fop = (flags & DDSK_F_FOP) != 0;
-    const int gs = select_s(nreq, cap_total, cvt, put);
+    const int gs = select_s(nreq, cap_total, cvt);
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
         // (no scratch is shared between launches: independent batches may overlap)
         if (a.overlap) a.tickets = scr->ovl + 8 + (a.seq & 3u);
-        return launch_gather_s(gs, a, st, cvt, put, acc, fop);
+        return gs ? launch_kind<false, kPlan8K, kPlan8KFetch>(a, st, cvt, put, acc, fop)
+                  : launch_kind<false, kPlan4K, kPlan4K>(a, st, cvt, put, acc, fop);
     }
     if (nreq > scr->cap_req || cap_total / SEG_GRAIN + 2 > scr->seg_cap) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_gather_var: scratch too small (%lld requests > %lld, or %lld segments > %lld)",

@@ -10,7 +10,7 @@ code with pad bits that must come out verbatim; every kind of invalid request at
 every argument error; overlapped queues mixing padded, packed and converting batches, also under SM contention; one
 batch whose padded output passes 4 GiB; RaggedDataset(pad=...) and RaggedPrefetchLoader over two epochs; the Cython
 binding; the wait() total after an empty batch queued behind a padded one, through every entry. A subprocess
-repeats the batch and loader tests with DDS_PDL=0 and DDS_GATHER_CTAS_PER_SM=2.
+repeats the batch and loader tests with DDS_PDL=0.
 
 On an H100 80GB HBM3 (700 W power limit) the module takes about 30 s, the subprocess included.
 """
@@ -522,8 +522,8 @@ def test_world():
 
 
 @pytest.mark.skipif(os.environ.get("DDS_PAD_SUBPROCESS") == "1", reason="already in the subprocess")
-def test_subprocess_pdl_off_two_ctas_per_sm():
-    env = dict(os.environ, DDS_PDL="0", DDS_GATHER_CTAS_PER_SM="2", DDS_PAD_SUBPROCESS="1")
+def test_subprocess_pdl_off():
+    env = dict(os.environ, DDS_PDL="0", DDS_PAD_SUBPROCESS="1")
     r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-x", "-p", "no:cacheprovider", __file__, "-k",
                         "shapes_raw or offsets or sample_ids or invalid or conversions or queue or loaders"],
                        cwd=ROOT, env=env, capture_output=True, text=True, timeout=1800)

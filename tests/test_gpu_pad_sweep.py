@@ -11,8 +11,8 @@ checked on every slot, `lengths`, the returned total, the first invalid request'
 64-byte sentinel bands on both sides of the destination and of `lengths`; a mismatch names the slot, its request, the
 row and element, and whether the element is payload or padding.
 
-The workload is tests/pad_sweep.workload() for the warp count of this GPU (12 warps per SM; the padded launch always runs
-one CTA per SM, whatever DDS_GATHER_GEOM or DDS_GATHER_CTAS_PER_SM say). The module asserts that it hits every category
+The workload is tests/pad_sweep.workload() for the warp count of this GPU (12 warps per SM; the padded launch runs one
+CTA per SM). The module asserts that it hits every category
 of pad_sweep.REQUIRED: whole-slot and whole-chunk segments, segments of more than 32 and 64 slots, segment and chunk
 cuts mid-row, at a row boundary, at the payload end and (segments) in padding, padding runs shorter than, equal to and
 one element either side of a multiple of 16 bytes at every 16-byte phase, and invalid requests at window lanes 0, 31,

@@ -1,8 +1,8 @@
-"""Every compiled gather variant, and the limits the code handles explicitly, against the oracle (-m gpu).
+"""Every raw gather geometry, and the limits the code handles explicitly, against the oracle (-m gpu).
 
-A. every plan-in-global (kGeoms) and shared-memory-plan (kGeomsS) geometry of dds_gather_kernel, selected through the
-   environment in a subprocess each, on one adversarial workload through every entry, into destinations at every base
-   phase, with sentinel guard bands around them;
+A. one adversarial workload through every entry, into destinations at every base phase, with sentinel guard bands
+   around them: it reaches every raw geometry of dds_gather_kernel the launcher selects (small and large rows, both
+   shared-memory plans, the plan kernels); in a subprocess each by default, with 1-chunk segments and with PDL off;
 B. packed results beyond 4 GiB (fixed count, variable count, by sample id, multi-array, capacity error, pageable host);
 C. the on-device verifier the benchmark trusts (dds_synth_verify) reports the corruptions it must;
 D. a world of DDSK_MAX_RANKS = 64 owners, a third of them empty, and the refusal of a 65th rank."""
@@ -31,18 +31,18 @@ def _torch():
 
 
 # ------------------------------------------------------------------------------- A. variant sweep
-# (warps, stages, chunk) of kGeoms and (warps, stages, chunk, plan capacity) of kGeomsS in kernels.cu
-GEOMS = [(8, 4, 4096), (8, 6, 4096), (16, 3, 4096), (4, 4, 8192), (12, 4, 4096), (4, 6, 4096), (6, 4, 4096),
-         (12, 3, 4096)]
-GEOMS_S = [(12, 3, 4096, 4096), (12, 3, 3072, 8192), (16, 3, 2048, 8192), (16, 3, 3072, 4096), (8, 4, 4096, 4096)]
-DEFAULT_GEOM = 4  # kGeomLarge / kGeomVar
+# (warps, stages, chunk, plan capacity) of the raw gets' geometries in kernels.cu. The sweep reaches each of them:
+#   large rows  fixed-count requests of 2 KiB and more (one row of f4096 / f4100, every variable's requests just over
+#               a chunk), and every variable-count batch that plans in global memory (9000 requests: "var-big",
+#               get_samples and get_samples_multi);
+#   small rows  fixed-count requests under 2 KiB (one row of b1 ... i20);
+#   plan 4K     variable-count batches of up to 4096 requests (the "var" base workload, get_samples with 500 ids);
+#   plan 8K     4097 to 8192 requests ("var-mid", 6000 requests, under DDS_SMEM_PLAN_MAX=8192).
+LARGE_ROWS, SMALL_ROWS = (12, 4, 4096, 0), (16, 3, 4096, 0)
+PLAN_4K, PLAN_8K = (12, 3, 4096, 4096), (12, 3, 3072, 8192)
+CHUNKS = sorted({g[2] for g in (LARGE_ROWS, SMALL_ROWS, PLAN_4K, PLAN_8K)})  # (3072, 4096: the walk's cuts)
 
-CONFIGS = {f"geom{g}": {"DDS_GATHER_GEOM": str(g), **({"DDS_GATHER_GEOM_S": str(g)} if g < len(GEOMS_S) else {})}
-           for g in range(len(GEOMS))}
-CONFIGS["geom5-2cta"] = {"DDS_GATHER_GEOM": "5", "DDS_GATHER_CTAS_PER_SM": "2"}
-CONFIGS["geom6-2cta"] = {"DDS_GATHER_GEOM": "6", "DDS_GATHER_CTAS_PER_SM": "2"}
-CONFIGS["minseg1"] = {"DDS_VAR_MINSEG": "1", "DDS_S_MINSEG": "1"}
-CONFIGS["nopdl"] = {"DDS_PDL": "0"}
+CONFIGS = {"default": {}, "minseg1": {"DDS_VAR_MINSEG": "1", "DDS_S_MINSEG": "1"}, "nopdl": {"DDS_PDL": "0"}}
 
 # name -> (dtype, disp, rows): 1-byte rows for the phase sweep, then 3, 4, 12, 20, 4096 and 4100-byte rows
 SWEEP_VARS = {"b1": (np.uint8, 1, 8 << 20), "b3": (np.uint8, 3, 3 << 20), "f4": (np.float32, 1, 5 << 19),
@@ -62,22 +62,19 @@ def sweep_main():
     rng = np.random.default_rng(20260)
     store = PyDDStore(device=0)
 
-    # the fixed-count geometry in use is the one asked for (a typo must not silently run the default)
-    g = int(env.get("DDS_GATHER_GEOM", DEFAULT_GEOM))
+    # the geometry the store reports is the large-rows one, one CTA per SM
     vals = [C.c_int() for _ in range(5)]
     _capi.lib().dds_gather_geometry(*[C.byref(v) for v in vals])
     ctas, nw, stages, ch, _ = [v.value for v in vals]
-    assert (nw, stages, ch) == GEOMS[g], (cfg, (nw, stages, ch), GEOMS[g])
+    assert (nw, stages, ch) == LARGE_ROWS[:3], (cfg, (nw, stages, ch), LARGE_ROWS)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
-    assert ctas == sms * int(env.get("DDS_GATHER_CTAS_PER_SM", "1")), (cfg, ctas, sms)
-    gs = env.get("DDS_GATHER_GEOM_S")
-    chunks = sorted({ch} | ({GEOMS_S[int(gs)][2]} if gs is not None else {GEOMS_S[0][2], GEOMS_S[1][2]}))
+    assert ctas == sms, (cfg, ctas, sms)
 
     shards, base = {}, {}
     for name, (dt, disp, n) in SWEEP_VARS.items():
         shards[name] = rng.integers(0, 256, size=n * disp * np.dtype(dt).itemsize, dtype=np.uint8).view(dt).reshape(n, disp)
         store.add(name, shards[name])
-        base[name] = sweep_requests(rng, n, disp * np.dtype(dt).itemsize, chunks)
+        base[name] = sweep_requests(rng, n, disp * np.dtype(dt).itemsize, CHUNKS)
         store.set_sample_index(name, *base[name])
 
     ncall = [0]
@@ -200,8 +197,8 @@ print("sweep-ok")
 
 @pytest.mark.parametrize("config", list(CONFIGS))
 def test_gather_variant_sweep(tmp_path, config):
-    """every kernel instantiation (8 plan-in-global geometries x fixed/variable count, 5 shared-plan geometries) on the
-    same adversarial workload: bytes, offsets, totals and guard bands against the oracle"""
+    """every raw kernel instantiation (small and large rows, both shared-memory plans, the plan kernels) on the same
+    adversarial workload: bytes, offsets, totals and guard bands against the oracle"""
     script = tmp_path / "variant_sweep.py"
     script.write_text(SWEEP_SCRIPT.format(root=ROOT))
     env = {k: v for k, v in os.environ.items() if not k.startswith("DDS_") or k == "DDS_COMM_TIMEOUT_S"}
