@@ -8,14 +8,26 @@ result has src's layout; an invalid request's result bytes, every byte past the 
 the whole buffer are left as they were.
 
 `fetch_op` applies the calls' requests in order, one element after the other: that is one of the orders the device may
-take, so its shards and results are exact for every element one epoch touches once. For elements touched by several
-fetch-ops, `check` compares each with a chain instead: the previous values the fetch-ops got and the final value must
-be explained by ONE order of the contributions --
-  * OP_SUM (integer-valued, positive contributions): sorted by the value each got back, contribution k got v0 plus the
-    k before it, and the final value is v0 plus all of them;
-  * OP_REPLACE (distinct src values): v0 -> s_a -> s_b -> ... -> final, each value got back exactly once.
+take. `check` compares a device outcome with the calls:
+  * an element touched once: its previous value is the shard's bits exactly (NaN payloads, -0 and f32 subnormals
+    included); its new value is the operand's bits (OP_REPLACE) or one correctly rounded addition, compared by
+    `acc_oracle.keys` (every NaN alike), for f32 IEEE or flushed (`acc_oracle.add_flushed`);
+  * an element touched several times: the previous values the fetch-ops got and the final value must be explained by
+    ONE order of the contributions --
+      - OP_SUM: each step one addition of the type (`acc_oracle.add`, for f32 or `add_flushed`) onto the value the
+        step got; the first step got v0 bit for bit, a later one the previous step's sum (a NaN by class), and the
+        final value is the last sum (by keys). Repeated previous values are allowed (a NaN, a contribution absorbed
+        by rounding) as long as one order explains them;
+      - OP_REPLACE (distinct src values): v0 -> s_a -> s_b -> ... -> final, each value got back exactly once, by bits.
 `check` reports the first inconsistency with its element and inputs, or None.
+
+The second half checks the arithmetic at single elements: `admissible_fetch` (every admissible tuple of previous values
+and final value of an element with a few fetch-adds, and optionally one plain accumulate), `fetch_verdict` (names the
+first element outside it), `fop_path` (which atomic and which result write an element of a one-piece call takes), and
+the value generators of the GPU module.
 """
+import itertools
+
 import numpy as np
 
 from tests import acc_oracle as ao
@@ -107,21 +119,104 @@ def _elem(what, r, e, disp, lenlist):
     return f"{what}: rank {r} global row {row} column {e % disp}"
 
 
-def sum_chain(v0, contribs, got, final):
-    """None when the previous values `got` of an integer-valued SUM chain and the final value are explained by one
-    order of the (positive) contributions; else what is wrong"""
-    order = sorted(range(len(got)), key=lambda i: got[i])
-    acc = v0
-    for k, i in enumerate(order):
-        if k and got[i] == got[order[k - 1]]:
-            return f"two fetch-ops got the same value {got[i]} (a duplicated ticket)"
-        if got[i] != acc:
-            return f"fetch-op {i} got {got[i]}, the chain expects {acc} (contributions {contribs}, got {got}, v0 {v0})"
-        acc += contribs[i]
-    if final != acc:
-        return f"final value {final}, the chain expects {acc} (a lost or extra contribution; v0 {v0}, contributions " \
-               f"{contribs}, got {got})"
-    return None
+SEARCH = 8  # chains of at most this many fetch-adds are searched over every order when the first walk fails
+
+
+def bits64(a, t):
+    """the bit patterns of storage array `a` as int64"""
+    return ao.bits(np.asarray(a, ao.STORAGE[t]), t).astype(np.uint64).view(np.int64)
+
+
+def fmt(v, t):
+    """one storage element as its bits and value"""
+    a = np.asarray(v, ao.STORAGE[t]).reshape(1)
+    w = 2 * np.dtype(ao.BITS[t]).itemsize
+    return f"{int(ao.bits(a, t)[0]):#0{w + 2}x} ({ao.values(a, t)[0]!r})"
+
+
+def _fmt_keys(ks, t):
+    w = 2 * np.dtype(ao.BITS[t]).itemsize
+    return "{" + ", ".join(sorted({"NaN" if k == ao.NAN else f"{int(k) & ((1 << 4 * w) - 1):#0{w + 2}x}"
+                                   for k in np.asarray(ks).tolist()})) + "}"
+
+
+def new_values(v0, x, t, op):
+    """the admissible new values of elements touched once, [options, N]: sums by keys (IEEE, and for f32 flushed),
+    swaps the operand's bits"""
+    if op == OP_REPLACE:
+        return bits64(x, t)[None]
+    opts = [ao.keys(ao.add(v0, x, t), t)]
+    if t == ao.ACC_F32:
+        opts.append(ao.keys(ao.add_flushed(v0, x), t))
+    return np.stack(opts)
+
+
+def _sum_order(v0, x, got, final, t):
+    """one order (member indices) that explains a SUM chain -- step 0 got v0 bit for bit, each later step the previous
+    sum (bits; a NaN by class), each sum one addition of type t (f32: IEEE or flushed), the final value the last sum
+    by keys -- or None. Searched depth first over every order; members with the same operand and value got are
+    interchangeable, and (members used, current value) states are visited once."""
+    n = x.size
+    gb, gn = bits64(got, t), ao.is_nan(got, t)
+    xb = bits64(x, t)
+    fk = int(ao.keys(final, t)[0])
+    seen = set()
+
+    def walk(cur, used, step):
+        if step == n:
+            return [] if int(ao.keys(cur, t)[0]) == fk else None
+        cb = int(bits64(cur, t)[0])
+        if (used, cb) in seen:
+            return None
+        seen.add((used, cb))
+        cnan = bool(ao.is_nan(cur, t)[0])
+        tried = set()
+        for i in range(n):
+            if used >> i & 1 or (int(gb[i]), int(xb[i])) in tried:
+                continue
+            if not (gb[i] == cb or (step and cnan and gn[i])):
+                continue
+            tried.add((int(gb[i]), int(xb[i])))
+            nxt = {int(bits64(s, t)[0]): s for s in
+                   [ao.add(got[i:i + 1], x[i:i + 1], t)] + ([ao.add_flushed(got[i:i + 1], x[i:i + 1])]
+                                                           if t == ao.ACC_F32 else [])}
+            for s in nxt.values():
+                rest = walk(s, used | 1 << i, step + 1)
+                if rest is not None:
+                    return [i] + rest
+        return None
+    return walk(np.asarray(v0, ao.STORAGE[t]).reshape(1), 0, 0)
+
+
+def sum_chain(v0, contribs, got, final, t=ao.ACC_I64):
+    """None when the previous values `got` of a SUM chain and the final value are explained by one order of the
+    contributions (see the module's docstring; chains of at most SEARCH are searched over every order, longer ones
+    walked: each step the first fetch-op that got the current value); else what is wrong. Values: storage arrays or
+    numbers of type t (the default: int64)"""
+    dt = ao.STORAGE[t]
+    v0, final = np.asarray(v0, dt).reshape(1), np.asarray(final, dt).reshape(1)
+    x, g = np.asarray(contribs, dt).reshape(-1), np.asarray(got, dt).reshape(-1)
+    n = x.size
+    if n <= SEARCH and _sum_order(v0, x, g, final, t) is not None:
+        return None
+    gb, gk = bits64(g, t), ao.keys(g, t)
+    ctx = (f"(v0 {fmt(v0, t)}, contributions [{', '.join(fmt(a, t) for a in x)}], got "
+           f"[{', '.join(fmt(a, t) for a in g)}])") if n <= 16 else f"(v0 {fmt(v0, t)}, {n} fetch-ops)"
+    uvals, cnt = np.unique(gb, return_counts=True)
+    dup = "" if cnt.max() == 1 else (f"; two fetch-ops got the same value "
+                                     f"{fmt(g[np.flatnonzero(gb == uvals[cnt > 1][0])[0]], t)} (a duplicated ticket)")
+    cur, used = v0, np.zeros(n, bool)
+    for step in range(n):
+        ck = int(ao.keys(cur, t)[0])
+        hit = np.flatnonzero(~used & ((gb == bits64(cur, t)[0]) if step == 0 else (gk == ck)))
+        if not hit.size:
+            return f"no fetch-op got {fmt(cur, t)}: the chain expects it after {step} step(s){dup} {ctx}"
+        i = hit[0]
+        used[i] = True
+        cur = ao.add(g[i:i + 1], x[i:i + 1], t)
+    if ao.keys(final, t)[0] != ao.keys(cur, t)[0]:
+        return f"final value {fmt(final, t)}, the chain expects {fmt(cur, t)} (a lost or extra contribution){dup} {ctx}"
+    return f"no order of the contributions explains the values got and the final value, with one rounding per step{dup} {ctx}"
 
 
 def replace_chain(v0, srcs, got, final):
@@ -201,63 +296,65 @@ def check(shards0, calls, t, op, got_shards, got_results):
             for c in np.unique(call[sel]).tolist():
                 m = call[sel] == c
                 x[m], got[m] = src_el[c][si[sel][m]], res_el[c][si[sel][m]]
-            exp_new = ao.add(v0, x, t) if op == OP_SUM else x
             b = ao.BITS[t]
             bad = np.nonzero(got.view(b) != v0.view(b))[0]
             if bad.size:
                 j = bad[0]
                 return (_elem("previous value", r, int(el[sel][j]), disp, lenlist) +
-                        f" (call {int(call[sel][j])}): got {got[j]!r}, the shard held {v0[j]!r}")
-            bad = np.nonzero(flatg[r][el[sel]].view(b) != exp_new.view(b))[0]
+                        f" (call {int(call[sel][j])}): got {fmt(got[j], t)}, the shard held {fmt(v0[j], t)}")
+            new = flatg[r][el[sel]]
+            opts = new_values(v0, x, t, op)
+            ok = (opts == (ao.keys(new, t) if op == OP_SUM else bits64(new, t))[None]).any(0)
+            bad = np.nonzero(~ok)[0]
             if bad.size:
                 j = bad[0]
                 return (_elem("new value", r, int(el[sel][j]), disp, lenlist) +
-                        f": {flatg[r][el[sel][j]]!r}, expected {exp_new[j]!r} (v0 {v0[j]!r}, src {x[j]!r})")
+                        f": {fmt(new[j], t)}, admissible {_fmt_keys(opts[:, j], t)} (v0 {fmt(v0[j], t)}, src "
+                        f"{fmt(x[j], t)})")
     # touched several times: one chain per element (values converted once, the chains walked in plain Python)
     multi = np.flatnonzero((ends - starts) > 1)
     if not multi.size:
         return None
-    if op == OP_SUM:
-        def conv(a):
-            return ao.values(np.asarray(a, dt), t)
-    else:
-        def conv(a):
-            return np.asarray(a, dt).view(ao.BITS[t]).astype(np.int64)
     members = np.flatnonzero(np.repeat((ends - starts) > 1, ends - starts))
     heads = starts[multi]
     v0, final = np.empty(multi.size, dt), np.empty(multi.size, dt)
     for r in range(len(shards0)):
         m = rk[heads] == r
         v0[m], final[m] = flat0[r][el[heads][m]], flatg[r][el[heads][m]]
-    v0, final = conv(v0), conv(final)
     xs, gs = np.empty(members.size, dt), np.empty(members.size, dt)
     for c in np.unique(call[members]).tolist():
         m = call[members] == c
         xs[m], gs[m] = src_el[c][si[members][m]], res_el[c][si[members][m]]
-    bad = _first_bad_chain(np.repeat(np.arange(multi.size), (ends - starts)[multi]), conv(xs), conv(gs), v0, final, op)
+    gid = np.repeat(np.arange(multi.size), (ends - starts)[multi])
+    bad = _first_bad_chain(gid, xs, gs, v0, final, op, t)
     if bad is None:
         return None
     g = int(multi[bad])
-    b, e = starts[g], ends[g]
-    xs_g = conv(np.array([src_el[c][i] for c, i in zip(call[b:e].tolist(), si[b:e].tolist())], dt))
-    gs_g = conv(np.array([res_el[c][i] for c, i in zip(call[b:e].tolist(), si[b:e].tolist())], dt))
-    msg = (sum_chain if op == OP_SUM else replace_chain)(v0[bad].item(), xs_g.tolist(), gs_g.tolist(), final[bad].item())
+    b = starts[g]
+    m = gid == bad
+    msg = (sum_chain(v0[bad], xs[m], gs[m], final[bad], t) if op == OP_SUM else
+           replace_chain(int(bits64(v0[bad], t)[0]), bits64(xs[m], t).tolist(), bits64(gs[m], t).tolist(),
+                         int(bits64(final[bad], t)[0])))
     return _elem("chain", int(rk[b]), int(el[b]), disp, lenlist) + f": {msg}"
 
 
-def _first_bad_chain(gid, x, got, v0, final, op):
-    """the first group whose chain fails (sum_chain / replace_chain, all groups at once), or None. gid: each member's
-    group (sorted), x / got: its operand and previous value, v0 / final: per group (lists of numbers)"""
-    x, got = np.asarray(x), np.asarray(got)
-    v0, final = np.asarray(v0), np.asarray(final)
+def _first_bad_chain(gid, x, got, v0, final, op, t):
+    """the first group whose chain fails, or None: all groups walked at once, each step taking the first unused member
+    that got the chain's current value (sums: one IEEE addition per step); a group that fails that walk and has at
+    most SEARCH members is then searched over every order and f32 mode (sum_chain). gid: each member's group (sorted),
+    x / got: its operand and previous value, v0 / final: per group (storage arrays)"""
     G = v0.size
     n_g = np.bincount(gid, minlength=G)
     failed = np.zeros(G, bool)
-    o = np.lexsort((got, gid))  # two members of a group with the same previous value
-    same = (gid[o][1:] == gid[o][:-1]) & (got[o][1:] == got[o][:-1])
-    failed[gid[o][1:][same]] = True
-    uv = np.unique(got)
-    key = gid.astype(np.int64) * uv.size + np.searchsorted(uv, got)
+    if op == OP_SUM:
+        gk = ao.keys(got, t)  # (a NaN got matches a NaN sum by class; the first step is checked bit for bit below)
+    else:
+        gk = bits64(got, t)
+        o = np.lexsort((gk, gid))  # distinct operands: each value is got once
+        same = (gid[o][1:] == gid[o][:-1]) & (gk[o][1:] == gk[o][:-1])
+        failed[gid[o][1:][same]] = True
+    uv = np.unique(gk)
+    key = gid.astype(np.int64) * uv.size + np.searchsorted(uv, gk)
     ko = np.argsort(key, kind="stable")
     ks = key[ko]
     used = np.zeros(got.size, bool)
@@ -266,16 +363,215 @@ def _first_bad_chain(gid, x, got, v0, final, op):
         act = np.flatnonzero((step < n_g) & ~failed)
         if not act.size:
             break
-        pos = np.minimum(np.searchsorted(uv, cur[act]), uv.size - 1)
+        ck = ao.keys(cur[act], t) if op == OP_SUM else bits64(cur[act], t)
+        pos = np.minimum(np.searchsorted(uv, ck), uv.size - 1)
         k = act.astype(np.int64) * uv.size + pos
         j = np.minimum(np.searchsorted(ks, k), ks.size - 1)
-        hit = (uv[pos] == cur[act]) & (ks[j] == k)
+        hit = (uv[pos] == ck) & (ks[j] == k)
         m = ko[j]
         hit &= ~used[m]
+        if op == OP_SUM and step == 0:
+            hit &= bits64(got[m], t) == bits64(cur[act], t)
         failed[act[~hit]] = True
         act, m = act[hit], m[hit]
         used[m] = True
-        cur[act] = cur[act] + x[m] if op == OP_SUM else x[m]
-    failed |= cur != final
+        cur[act] = ao.add(got[m], x[m], t) if op == OP_SUM else x[m]
+    failed |= (ao.keys(cur, t) != ao.keys(final, t)) if op == OP_SUM else (bits64(cur, t) != bits64(final, t))
+    for g in np.flatnonzero(failed & (n_g <= SEARCH)) if op == OP_SUM else ():
+        m = gid == g
+        failed[g] = _sum_order(v0[g:g + 1], x[m], got[m], final[g:g + 1], t) is None
     bad = np.flatnonzero(failed)
     return int(bad[0]) if bad.size else None
+
+
+# ------------------------------------------------------------------------------------------------ the arithmetic
+def admissible_fetch(start, contribs, t, acc=None):
+    """every (previous value of each fetch-add, final value) tuple the header allows for elements with start value
+    `start` ([N] storage array) and k <= 3 fetch-adds `contribs` (k arrays of start's shape), plus, when given, one
+    plain accumulate `acc` (no previous value): all orders, each f32 step IEEE or flushed. Returns (prev [options, k,
+    N], final [options, N]): final values as acc_oracle.keys; previous values as bits (int64), except NAN where the
+    value is a NaN some addition made (its payload is not specified), so that a previous value matches when its bits
+    are equal or both are NaN there (`fetch_match`)."""
+    contribs = list(contribs)
+    assert len(contribs) <= 3
+    items = list(range(len(contribs))) + ([-1] if acc is not None else [])
+    prevs, finals = [], []
+    for order in itertools.permutations(items):
+        for mask in range(1 << len(items)) if t == ao.ACC_F32 else (0,):
+            cur = np.asarray(start, ao.STORAGE[t])
+            made = np.zeros(cur.shape, bool)  # cur is a NaN an addition made
+            prev = [None] * len(contribs)
+            for step, i in enumerate(order):
+                if i >= 0:
+                    prev[i] = np.where(made, ao.NAN, bits64(cur, t))
+                x = acc if i < 0 else contribs[i]
+                cur = ao.add_flushed(cur, x) if mask >> step & 1 else ao.add(cur, x, t)
+                made = ao.is_nan(cur, t)
+            prevs.append(np.stack(prev) if prev else np.zeros((0,) + cur.shape, np.int64))
+            finals.append(ao.keys(cur, t))
+    return np.stack(prevs), np.stack(finals)
+
+
+def fetch_match(opts, got_prev, got_final, t):
+    """[N] bool: the observed tuple -- got_prev [k, N], got_final [N] (storage arrays) -- is one of admissible_fetch's
+    options `opts`"""
+    prev, final = opts
+    gb = bits64(got_prev, t)[None]
+    gn = ao.is_nan(got_prev, t)[None]
+    okp = ((prev == gb) | ((prev == ao.NAN) & gn)).all(1)
+    return (okp & (final == ao.keys(got_final, t)[None])).any(0)
+
+
+def discrimination(opts):
+    """the fraction of elements with more than one distinct admissible tuple"""
+    prev, final = opts
+    differ = (prev != prev[:1]).any(1) | (final != final[:1])
+    return float(differ.any(0).mean()) if final.shape[1] else 0.0
+
+
+def fetch_verdict(got_prev, got_final, start, contribs, t, acc=None, opts=None, where=None, paths=None, what=""):
+    """None when every element's observed tuple (got_prev [k, N], got_final [N]) is admissible; else a message naming
+    the first bad element -- `where(i)` -> (rank, global row, column) -- with its inputs, the bits it got, the
+    admissible tuples and, when given, its predicted path"""
+    opts = admissible_fetch(start, contribs, t, acc) if opts is None else opts
+    ok = fetch_match(opts, got_prev, got_final, t)
+    if ok.all():
+        return None
+    i = int(np.argmin(ok))
+    rank, row, col = where(i) if where else (0, i, 0)
+    w = 2 * np.dtype(ao.BITS[t]).itemsize
+    f = lambda k: "NaN" if k == ao.NAN else f"{int(k) & ((1 << 4 * w) - 1):#0{w + 2}x}"  # noqa: E731
+    tuples = sorted({"(" + ", ".join(f(k) for k in list(opts[0][o, :, i]) + [opts[1][o, i]]) + ")"
+                     for o in range(opts[1].shape[0])})
+    ins = ", ".join(fmt(np.asarray(c)[i], t) for c in contribs)
+    got = ", ".join(fmt(np.asarray(got_prev)[j, i], t) for j in range(len(contribs)))
+    return (f"{what}: {int((~ok).sum())} of {ok.size} elements outside the admissible set; first: rank {rank}, global row "
+            f"{row}, column {col}{'' if paths is None else f' (path {paths[i]})'}: start {fmt(np.asarray(start)[i], t)}, "
+            f"fetch-adds [{ins}]{'' if acc is None else f', accumulate {fmt(np.asarray(acc)[i], t)}'}: got previous "
+            f"values [{got}], final {fmt(np.asarray(got_final)[i], t)}; admissible (previous values..., final): "
+            f"{', '.join(tuples[:12])}{' ...' if len(tuples) > 12 else ''}")
+
+
+def once_verdict(got_prev, got_new, start, x, t, op, where=None, paths=None, what=""):
+    """None when every once-touched element (all [N] storage arrays) got the shard's bits back and holds an admissible
+    new value; else a message naming the first bad element with its inputs, the bits got, the admissible bits and,
+    when given, its predicted path"""
+    okp = bits64(got_prev, t) == bits64(start, t)
+    opts = new_values(start, x, t, op)
+    okn = (opts == (ao.keys(got_new, t) if op == OP_SUM else bits64(got_new, t))[None]).any(0)
+    ok = okp & okn
+    if ok.all():
+        return None
+    i = int(np.argmin(ok))
+    rank, row, col = where(i) if where else (0, i, 0)
+    return (f"{what}: {int((~okp).sum())} previous and {int((~okn).sum())} new values of {ok.size} wrong; first: rank "
+            f"{rank}, global row {row}, column {col}{'' if paths is None else f' (path {paths[i]})'}: shard "
+            f"{fmt(start[i], t)}, src {fmt(x[i], t)}: got previous value {fmt(got_prev[i], t)} (admissible: the shard's "
+            f"bits), new value {fmt(got_new[i], t)} (admissible {_fmt_keys(opts[:, i], t)})")
+
+
+# ------------------------------------------------------------------------------------------------ paths
+def fop_path(dst_phase, src_phase, nbytes, k, res_phase=0):
+    """which atomic the fetch drain (fop_chunk) applies to byte k of ONE staged piece of nbytes bytes whose shard
+    bytes start dst_phase and whose staged operands start src_phase bytes past a 16-byte boundary: "element" (fop1)
+    for the head before the shard's first 16-byte boundary and the tail after its last; for the body between,
+    "vector WS/B", fop_rephase_loop<WS, BYTES> with the word shift WS and BYTES (0 / 1) of the staged phase
+    (src_phase + head) % 16. k may be an array. Also returns how the previous values reach the result whose bytes start
+    res_phase past a boundary: "bulk" (one bulk store) when result, size and staged phase are all 16-byte aligned,
+    else "drain_chunk" (the raw drain's head / body / tail)."""
+    k = np.asarray(k)
+    head = min((16 - dst_phase) % 16, nbytes)
+    body = ((nbytes - head) >> 4) << 4
+    sh = (src_phase + head) % 16
+    path = np.where((k < head) | (k >= head + body), "element", f"vector {sh >> 2}/{int(sh % 4 != 0)}")
+    return path, "bulk" if (res_phase | nbytes | src_phase) % 16 == 0 else "drain_chunk"
+
+
+def vector_paths(t):
+    """the fop_rephase_loop variants elements of type t can take: 8 for 2-byte types, 4 for 4-byte, 2 for 8-byte"""
+    E = np.dtype(ao.STORAGE[t]).itemsize
+    return [f"vector {sh >> 2}/{int(sh % 4 != 0)}" for sh in range(0, 16, E)]
+
+
+# ------------------------------------------------------------------------------------------------ test data
+def swap_patterns(rng, t, n):
+    """n bit patterns from the whole range of type t: signalling NaNs with payload 1, negative and low-payload NaNs,
+    +-0, subnormals, +-inf, +-max and random bits (integers: random bits and the range's ends)"""
+    nb = np.dtype(ao.BITS[t]).itemsize * 8
+    rnd = rng.integers(0, 2**63, size=n, dtype=np.uint64) * np.uint64(2) + rng.integers(0, 2, size=n, dtype=np.uint64)
+    rnd = rnd.astype(ao.BITS[t])
+    if t not in ao.FLOATS:
+        ends = np.array([0, 1, (1 << (nb - 1)) - 1, 1 << (nb - 1), (1 << nb) - 1], np.uint64).astype(ao.BITS[t])
+        return ao.from_bits(np.where(rng.random(n) < 0.3, ends[rng.integers(0, ends.size, size=n)], rnd), t)
+    p = ao.PREC[t]
+    sign = np.uint64(1) << np.uint64(nb - 1)
+    special = [ao._nan_bits(t, q) for q in range(4)] + [0, 1, (1 << (p - 1)) - 1, 1 << (p - 1), ao._max_bits(t),
+                                                        ((1 << (nb - 1)) - 1) & ~((1 << (p - 1)) - 1)]
+    special = np.array(special, np.uint64)
+    sp = special[rng.integers(0, special.size, size=n)] | np.where(rng.random(n) < 0.5, sign, np.uint64(0))
+    sub = rng.integers(1, 1 << (p - 1), size=n).astype(np.uint64) | np.where(rng.random(n) < 0.5, sign, np.uint64(0))
+    k = rng.integers(0, 4, size=n)
+    return ao.from_bits(np.where(k == 0, rnd, np.where(k == 1, sub, sp)).astype(ao.BITS[t]), t)
+
+
+def distinct_patterns(rng, t, n, avoid=()):
+    """n distinct bit patterns of type t, every NaN kind, +-0, subnormals, +-inf and max among them when n allows,
+    none of them in `avoid` (bits)"""
+    nb = np.dtype(ao.BITS[t]).itemsize * 8
+    first = ao.bits(swap_patterns(rng, t, 4 * n + 64), t)
+    if t in ao.FLOATS:
+        p = ao.PREC[t]
+        sign = 1 << (nb - 1)
+        e = ((1 << (nb - 1)) - 1) & ~((1 << (p - 1)) - 1)
+        first = np.concatenate([np.array([ao._nan_bits(t, q) | s for q in range(4) for s in (0, sign)] +
+                                         [0, sign, 1, 1 | sign, e, e | sign, ao._max_bits(t)], np.uint64
+                                         ).astype(ao.BITS[t]), first])
+    _, idx = np.unique(first, return_index=True)
+    out = first[np.sort(idx)]
+    out = out[~np.isin(out, np.asarray(avoid, ao.BITS[t]))]
+    assert out.size >= n, (t, n, out.size)
+    sel = np.concatenate([np.arange(min(15, n)), 15 + rng.permutation(out.size - 15)[:max(n - 15, 0)]])
+    return ao.from_bits(out[rng.permutation(sel)], t)
+
+
+# hot elements: fetch-adds per element of positive operands in (1, 2) onto a start value in [1, 2). Below these counts
+# every addition raises the running sum (the sum stays below 2^(p+1): an ulp of at most 2), so sorting the previous
+# values gives the only order
+HOT_FETCH = {ao.ACC_F32: 4096, ao.ACC_F64: 65536, ao.ACC_F16: 512, ao.ACC_BF16: 128, ao.ACC_I32: 4096, ao.ACC_I64: 4096}
+
+
+def hot_values(rng, t, shape):
+    """positive operands of type t: floats in (1, 2) with random full-precision significands, integers in [1, 2^18)"""
+    if t not in ao.FLOATS:
+        return rng.integers(1, 1 << 18, size=shape).astype(ao.STORAGE[t])
+    p = ao.PREC[t]
+    m = (1 << (p - 1)) + rng.integers(1, 1 << (p - 1), size=shape, dtype=np.int64)
+    return ao.encode(np.ldexp(m.astype(np.float64), -(p - 1)), t)
+
+
+def increasing_chain(v0, x, got, final, t):
+    """the hot-element check of elements whose contributions all raise the running sum: per column of x / got
+    ([n, D] storage arrays; v0, final [D]), the previous values sorted give the only order, so sorted[0] is v0 bit for
+    bit, sorted[j + 1] = add(sorted[j], its contribution) bit for bit and final = add(last, its contribution). Returns
+    None or (column, what is wrong)."""
+    gv = ao.values(got, t)
+    order = np.argsort(gv, axis=0, kind="stable")
+    gs = np.take_along_axis(got, order, 0)
+    xs = np.take_along_axis(x, order, 0)
+    nxt = ao.add(gs, xs, t)
+    b = lambda a: bits64(a, t)  # noqa: E731
+    bad0 = b(gs[0]) != b(v0)
+    if bad0.any():
+        c = int(np.argmax(bad0))
+        return c, f"the smallest previous value {fmt(gs[0, c], t)} is not the start {fmt(v0[c], t)}"
+    badm = b(gs[1:]) != b(nxt[:-1])
+    if badm.any():
+        j, c = (int(v) for v in np.argwhere(badm)[0])
+        eq = " (two fetch-ops got the same value: a duplicated ticket)" if b(gs[j + 1, c]) == b(gs[j, c]) else ""
+        return c, (f"step {j + 1} of {got.shape[0]}: got {fmt(gs[j + 1, c], t)}, one rounded addition of "
+                   f"{fmt(xs[j, c], t)} onto {fmt(gs[j, c], t)} gives {fmt(nxt[j, c], t)}{eq}")
+    badf = b(final) != b(nxt[-1])
+    if badf.any():
+        c = int(np.argmax(badf))
+        return c, f"final value {fmt(final[c], t)}, the chain ends at {fmt(nxt[-1, c], t)}"
+    return None

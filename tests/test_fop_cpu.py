@@ -1,6 +1,11 @@
 """The batched fetch-op's NumPy oracle (tests/fop_oracle.py) against the compiled reference and on seeded worlds, its
 chain checkers against results made wrong on purpose, and the Python-side checks of get_accumulate_batch that need no
-device."""
+device. The second half checks the arithmetic checkers the GPU numerics module relies on: that they accept every order
+of fetch-adds simulated with one rounding per step (f32: IEEE or flushed) on every value family, that they name the
+element of each kind of wrong result (an ulp off, rounded toward zero, a flushed subnormal, a changed NaN payload, a
+quieted signalling NaN, a duplicated ticket), that the hot-element generators raise every sum, and fop_path."""
+from fractions import Fraction
+
 import numpy as np
 import pytest
 
@@ -272,3 +277,235 @@ def test_fetch_op_rejects_bad_arguments_before_the_call():
     with pytest.raises(ValueError, match="CUDA tensor"):
         PyDDStore._fop_args("x", "sum", torch.zeros(16), _Src())
     assert (_capi.OP_SUM, _capi.OP_REPLACE) == (1, 2) and _capi.FOP_OPS == {"sum": 1, "replace": 2}
+
+
+# ------------------------------------------------------------------------------------------------ the arithmetic
+FLOATS = (ao.ACC_F32, ao.ACC_F64, ao.ACC_F16, ao.ACC_BF16)
+
+
+def _simulate(rng, t, start, contribs):
+    """each element's fetch-adds in a random order, each f32 step IEEE or flushed at random -> (previous values [k,
+    N], final [N])"""
+    k, n = len(contribs), start.size
+    orders = np.argsort(rng.random((n, k)), axis=1)
+    modes = rng.random((n, k)) < 0.5 if t == ao.ACC_F32 else np.zeros((n, k), bool)
+    cur, prev = start.copy(), np.empty((k, n), start.dtype)
+    X = np.stack(contribs)
+    for step in range(k):
+        i = orders[:, step]
+        x = X[i, np.arange(n)]
+        prev[i, np.arange(n)] = cur
+        cur = np.where(modes[:, step], ao.add_flushed(cur, x) if t == ao.ACC_F32 else cur, ao.add(cur, x, t))
+    return prev, cur
+
+
+def _family_world(t, k, seed=0, n=64):
+    """n elements per value family, k fetch-adds each (one call per fetch-add, one request of row 0): (names, family
+    of each element, start, contribs, shards, calls) with the calls' results still to fill in"""
+    rng = np.random.default_rng([seed, t, k])
+    fams = ao.families(rng, t, n)
+    names = list(fams)
+    start = np.concatenate([fams[nm][0] for nm in names])
+    contribs = [np.concatenate([ao.families(rng, t, n)[nm][1] for nm in names]) for _ in range(k)]
+    fam = np.repeat(np.array(names), n)
+    return rng, names, fam, start, contribs
+
+
+def _check_world(t, start, contribs, prev, final, op=fo.OP_SUM):
+    """check() of one row holding every element, one call per fetch-op"""
+    shards = [start[None].copy()]
+    calls = [(c.view(np.uint8), None, np.zeros(c.nbytes, np.uint8), {"starts": [0], "counts": [1]}) for c in contribs]
+    return fo.check(shards, calls, t, op, [final[None]], [p.copy().view(np.uint8) for p in prev])
+
+
+@pytest.mark.parametrize("k", [2, 3])
+@pytest.mark.parametrize("t", ALL)
+def test_fetch_checkers_accept_every_simulated_order(t, k):
+    """on every value family, fetch-adds applied in random orders with ao.add / add_flushed: admissible_fetch holds
+    every outcome, and so does check() (the chain walk, and the search where the walk is not enough)"""
+    rng, names, fam, start, contribs = _family_world(t, k)
+    for seed in range(3):
+        prev, final = _simulate(rng, t, start, contribs)
+        opts = fo.admissible_fetch(start, contribs, t)
+        assert fo.fetch_match(opts, prev, final, t).all()
+        assert fo.fetch_verdict(prev, final, start, contribs, t, opts=opts) is None
+        assert _check_world(t, start, contribs, prev, final) is None
+    # one plain accumulate beside one fetch-add, in either order
+    acc = contribs[1]
+    for first in (True, False):
+        cur = ao.add(start, acc, t) if first else start
+        prev = cur[None].copy()
+        cur = ao.add(cur, contribs[0], t)
+        final = cur if first else ao.add(cur, acc, t)
+        assert fo.fetch_match(fo.admissible_fetch(start, contribs[:1], t, acc), prev, final, t).all()
+
+
+def _W(i):
+    return 0, 0, i
+
+
+def _where_in(msg, e):
+    return msg is not None and f"global row 0, column {e}:" in msg
+
+
+def _first(mask):
+    assert mask.any()
+    return int(np.argmax(mask))
+
+
+@pytest.mark.parametrize("t", FLOATS)
+def test_fetch_checkers_report_wrong_arithmetic(t):
+    """a previous value one ulp off, a final value rounded toward zero, two equal tickets on strictly increasing data:
+    each reported at the right element, by fetch_verdict and by check()"""
+    rng, names, fam, start, contribs = _family_world(t, 2, seed=1)
+    prev, final = _simulate(rng, t, start, contribs)
+    opts = fo.admissible_fetch(start, contribs, t)
+    fin = ~ao.is_nan(prev, t).any(0) & np.isfinite(ao.values(final, t))
+    # a previous value one ulp off
+    e = _first(fin & (fam == "random"))
+    bad = prev.copy()
+    bad[1].view(ao.BITS[t])[e] += 1
+    assert _where_in(fo.fetch_verdict(bad, final, start, contribs, t, opts=opts, where=_W), e)
+    assert f"chain: rank 0 global row 0 column {e}" in _check_world(t, start, contribs, bad, final)
+    # a final value rounded toward zero (one fetch-add: a once-touched element)
+    x = contribs[0]
+    rn = ao.add(start, x, t)
+    ties = np.flatnonzero(fam == "ties")
+    sv, xv, rv = (ao.values(a[ties], t) for a in (start, x, rn))
+    up = np.array([abs(Fraction(float(r))) > abs(Fraction(float(a)) + Fraction(float(b))) for a, b, r in zip(sv, xv, rv)])
+    e = int(ties[_first(up & (rv != 0))])
+    rz = rn.copy()
+    rz.view(ao.BITS[t])[e] -= 1
+    msg = fo.once_verdict(start, rz, start, x, t, fo.OP_SUM, where=_W)
+    assert _where_in(msg, e) and "new value" in msg, msg
+    msg = _check_world(t, start, [x], [start], rz)
+    assert msg and f"new value: rank 0 global row 0 column {e}" in msg, msg
+    # two tickets equal on strictly increasing data
+    rng = np.random.default_rng(5)
+    v0 = fo.hot_values(rng, t, (3,))
+    xs = fo.hot_values(rng, t, (40, 3))
+    got, cur = np.empty_like(xs), v0.copy()
+    for j in range(40):
+        got[j], cur = cur, ao.add(cur, xs[j], t)
+    assert fo.increasing_chain(v0, xs, got, cur, t) is None
+    dup = got.copy()
+    dup[17, 2] = dup[16, 2]
+    bad = fo.increasing_chain(v0, xs, dup, cur, t)
+    assert bad is not None and bad[0] == 2 and "duplicated ticket" in bad[1], bad
+    calls = [(xs[j:j + 1].view(np.uint8).reshape(-1), None, np.zeros(xs[j:j + 1].nbytes, np.uint8),
+              {"starts": [0], "counts": [1]}) for j in range(40)]
+    assert fo.check([v0[None]], calls, t, fo.OP_SUM, [cur[None]], [g.view(np.uint8) for g in got]) is None
+    msg = fo.check([v0[None]], calls, t, fo.OP_SUM, [cur[None]], [g.view(np.uint8) for g in dup])
+    assert msg and "chain: rank 0 global row 0 column 2" in msg and "duplicated ticket" in msg, msg
+
+
+@pytest.mark.parametrize("t", FLOATS)
+def test_fetch_checkers_report_flushed_and_changed_bits(t):
+    """a subnormal flushed (f16 / bf16 new values; any type's previous values, f32 included), a NaN payload changed in
+    a previous value or a swap, a signalling NaN quieted by a swap: each reported at the right element"""
+    rng = np.random.default_rng([2, t])
+    n = 64
+    p = ao.PREC[t]
+    sub = ao.encode(rng.integers(1, 1 << (p - 1), size=n) * 2.0 ** (ao.EMIN[t] - p + 1), t)
+    zero = ao.encode(np.zeros(n), t)
+    # the shard holds subnormals; a sum of +0 keeps them: previous and new value are the subnormal
+    assert fo.once_verdict(sub, sub, sub, zero, t, fo.OP_SUM, where=_W) is None
+    e = 17
+    flushed = sub.copy()
+    flushed[e] = zero[e]
+    msg = fo.once_verdict(flushed, sub, sub, zero, t, fo.OP_SUM, where=_W)
+    assert _where_in(msg, e) and "previous value 0x0" in msg, msg
+    msg = _check_world(t, sub, [zero], [flushed], sub)
+    assert msg and f"previous value: rank 0 global row 0 column {e}" in msg, msg
+    if t != ao.ACC_F32:  # (f32 may flush a subnormal result; f16 and bf16 may not)
+        msg = fo.once_verdict(sub, flushed, sub, zero, t, fo.OP_SUM, where=_W)
+        assert _where_in(msg, e) and "new value 0x0" in msg, msg
+    else:
+        assert fo.once_verdict(sub, flushed, sub, zero, t, fo.OP_SUM, where=_W) is None
+    # NaN payloads: a previous value must keep the shard's payload; a swap's new value must be the operand's bits
+    snan = ao.from_bits(np.full(n, ao._nan_bits(t, 1), ao.BITS[t]), t)    # signalling, payload 1
+    qnan = ao.from_bits(np.full(n, ao._nan_bits(t, 3), ao.BITS[t]), t)    # quiet, payload 3
+    quieted = ao.from_bits(ao.bits(snan, t) | ao.BITS[t](1 << (p - 2)), t)
+    x = ao.inexact(rng, n, t)
+    assert fo.once_verdict(qnan, ao.add(qnan, x, t), qnan, x, t, fo.OP_SUM, where=_W) is None
+    bad = qnan.copy()
+    bad[e] = ao.from_bits(np.array([ao._nan_bits(t, 0)], ao.BITS[t]), t)[0]
+    assert _where_in(fo.once_verdict(bad, ao.add(qnan, x, t), qnan, x, t, fo.OP_SUM, where=_W), e)
+    for op in (fo.OP_SUM, fo.OP_REPLACE):
+        msg = _check_world(t, qnan, [x], [bad], ao.add(qnan, x, t) if op == fo.OP_SUM else x, op)
+        assert msg and f"previous value: rank 0 global row 0 column {e}" in msg, msg
+    assert fo.once_verdict(x, snan, x, snan, t, fo.OP_REPLACE, where=_W) is None
+    got = snan.copy()
+    got[e] = quieted[e]
+    msg = fo.once_verdict(x, got, x, snan, t, fo.OP_REPLACE, where=_W)
+    assert _where_in(msg, e) and "new value" in msg, msg
+    msg = _check_world(t, x, [snan], [x], got, fo.OP_REPLACE)
+    assert msg and f"new value: rank 0 global row 0 column {e}" in msg, msg
+    # a swap chain v0 -> sNaN -> s1: the second swap got the sNaN quieted
+    s1 = ao.inexact(rng, n, t)
+    prev = [x.copy(), snan.copy()]
+    assert _check_world(t, x, [snan, s1], prev, s1, fo.OP_REPLACE) is None
+    prev[1][e] = quieted[e]
+    msg = _check_world(t, x, [snan, s1], prev, s1, fo.OP_REPLACE)
+    assert msg and f"chain: rank 0 global row 0 column {e}" in msg, msg
+
+
+def test_f32_subnormal_previous_value_returned_as_zero():
+    """an f32 subnormal start touched by two fetch-adds of +0: the first must get the subnormal back bit for bit,
+    although the sums may flush it"""
+    t = ao.ACC_F32
+    sub = ao.from_bits(np.array([1, 0x80000005, 0x007FFFFF], np.uint32), t)
+    zero = np.zeros(3, np.float32)
+    prev, final = [sub.copy(), ao.add_flushed(sub, zero)], ao.add_flushed(sub, zero)
+    assert _check_world(t, sub, [zero, zero], prev, final) is None
+    assert fo.fetch_match(fo.admissible_fetch(sub, [zero, zero], t), np.stack(prev), final, t).all()
+    prev[0] = np.copysign(zero, sub)
+    msg = _check_world(t, sub, [zero, zero], prev, final)
+    assert msg and "chain: rank 0 global row 0 column 0" in msg, msg
+    ok = fo.fetch_match(fo.admissible_fetch(sub, [zero, zero], t), np.stack(prev), final, t)
+    assert not ok.any()
+
+
+@pytest.mark.parametrize("t", ALL)
+def test_hot_generators_raise_every_sum(t):
+    """HOT_FETCH[t] fetch-adds of hot_values onto a hot_values start, in order: every addition raises the running sum,
+    also when every operand is the largest or the smallest the generator makes"""
+    rng = np.random.default_rng(t)
+    n = fo.HOT_FETCH[t]
+    D = 4
+    if t in FLOATS:
+        p = ao.PREC[t]
+        lo, hi = ao.encode(np.full(1, 1 + 2.0 ** -(p - 1)), t), ao.encode(np.full(1, 2 - 2.0 ** -(p - 1)), t)
+    else:
+        lo, hi = np.ones(1, ao.STORAGE[t]), np.full(1, (1 << 18) - 1, ao.STORAGE[t])
+    x = fo.hot_values(rng, t, (n, D))
+    x[:, 0], x[:, 1] = lo[0], hi[0]
+    assert (ao.values(x, t) > (1 if t in FLOATS else 0)).all() and (ao.values(x, t) < (2 if t in FLOATS else 1 << 18)).all()
+    cur = fo.hot_values(rng, t, (D,))
+    cur[1] = hi[0]
+    for j in range(n):
+        nxt = ao.add(cur, x[j], t)
+        assert (ao.values(nxt, t) > ao.values(cur, t)).all(), (ao.NAMES[t], j, cur, x[j], nxt)
+        cur = nxt
+
+
+@pytest.mark.parametrize("E", [2, 4, 8])
+def test_fop_path(E):
+    """the head and tail are element atomics, the body takes the re-phase variant of its staged phase -- every variant
+    reachable for the element size -- and the result is one bulk store only when result, size and staged bytes are
+    16-byte aligned"""
+    t = {2: ao.ACC_F16, 4: ao.ACC_F32, 8: ao.ACC_F64}[E]
+    seen = set()
+    for dp in range(0, 16, E):
+        for sp in range(0, 16, E):
+            p, rp = fo.fop_path(dp, sp, 160, np.arange(0, 160, E), res_phase=0)
+            head = (16 - dp) % 16
+            end = head + (160 - head) // 16 * 16
+            assert (p[:head // E] == "element").all() and (p[end // E:] == "element").all()
+            assert len(set(p[head // E:end // E])) == 1
+            seen.add(p[head // E])
+            assert rp == ("bulk" if sp == 0 else "drain_chunk")
+    assert seen == set(fo.vector_paths(t)) and len(seen) == 16 // E
+    assert fo.fop_path(0, 0, 150, [0], res_phase=0)[1] == "drain_chunk"
+    assert fo.fop_path(0, 0, 160, [0], res_phase=E)[1] == "drain_chunk"
+    assert (fo.fop_path(4, 0, 8, np.arange(0, 8, E))[0] == "element").all()
