@@ -106,6 +106,11 @@ SIGNATURES = {
                                            I64P, I64P]),
     "dds_get_accumulate_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_int,
                                              C.c_void_p, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_compare_and_swap_batch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                             C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint,
+                                             C.c_void_p, I64P, I64P]),
+    "dds_compare_and_swap_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

@@ -406,6 +406,143 @@ __device__ __forceinline__ uint4 fop16(char *d, uint4 v, int t, bool swap) {
     }
     return o;
 }
+
+// Compare-and-swap (FETCH, op kFopCas), element size 1 << el (warp-uniform): the element becomes the operand where it
+// equals the compare operand bit for bit, and its previous value comes back either way. 4- and 8-byte elements take one
+// atom.cas each (no atom.cas.b128: its behaviour towards a peer over NVLink is not established); 1- and 2-byte elements
+// a compare-and-swap loop on the aligned 32-bit word that holds them (cas_word). .sys scope, as the other fetch-ops.
+__device__ __forceinline__ uint32_t atom_cas_b32(char *d, uint32_t c, uint32_t v) {
+    uint32_t o;
+    asm volatile("atom.relaxed.sys.global.cas.b32 %0, [%1], %2, %3;" : "=r"(o) : "l"(d), "r"(c), "r"(v) : "memory");
+    return o;
+}
+__device__ __forceinline__ uint64_t atom_cas_b64(char *d, uint64_t c, uint64_t v) {
+    uint64_t o;
+    asm volatile("atom.relaxed.sys.global.cas.b64 %0, [%1], %2, %3;" : "=l"(o) : "l"(d), "l"(c), "l"(v) : "memory");
+    return o;
+}
+// The elements of the bytes m of the aligned word w (1 << el bytes each, el 0 or 1): each becomes v's where it equals c's;
+// every byte outside m is left exactly as it is found, whoever changes it meanwhile. Returns the word the step found.
+// When no element changes, the load was the atomic step (a failed compare is a read).
+__device__ __forceinline__ uint32_t cas_word(char *w, uint32_t c, uint32_t v, uint32_t m, uint32_t el) {
+    uint32_t cur;
+    asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(cur) : "l"(w) : "memory");
+    while (true) {
+        const uint32_t eq = (el ? __vcmpeq2(cur, c) : __vcmpeq4(cur, c)) & m;
+        const uint32_t want = (cur & ~eq) | (v & eq);
+        if (want == cur) return cur;
+        const uint32_t seen = atom_cas_b32(w, cur, want);
+        if (seen == cur) return cur;
+        cur = seen;
+    }
+}
+// Compare operands are read with plain global loads of exactly their own bytes (the compare buffer may end where the
+// layout does, and may be the result buffer)
+__device__ __forceinline__ uint32_t ldg8(const char *p) {
+    uint32_t v;
+    asm volatile("ld.global.u8 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+}
+__device__ __forceinline__ uint32_t ldg16(const char *p) {
+    uint32_t v;
+    asm volatile("ld.global.u16 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+}
+__device__ __forceinline__ uint32_t ldg32(const char *p) {
+    uint32_t v;
+    asm volatile("ld.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+}
+__device__ __forceinline__ uint64_t ldg64(const char *p) {
+    uint64_t v;
+    asm volatile("ld.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
+    return v;
+}
+// 16 bytes at p, in p's own 16-byte phase: the widest loads its alignment allows
+__device__ __forceinline__ uint4 ldg16_any(const char *p) {
+    const uint32_t ph = (uint32_t)(uint64_t)p & 15u;
+    uint4 r;
+    if (ph == 0) {
+        asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p));
+    } else if ((ph & 7u) == 0) {
+        const uint64_t a = ldg64(p), b = ldg64(p + 8);
+        r = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+    } else if ((ph & 3u) == 0) {
+        r = make_uint4(ldg32(p), ldg32(p + 4), ldg32(p + 8), ldg32(p + 12));
+    } else if ((ph & 1u) == 0) {
+        r = make_uint4(ldg16(p) | ldg16(p + 2) << 16, ldg16(p + 4) | ldg16(p + 6) << 16, ldg16(p + 8) | ldg16(p + 10) << 16,
+                       ldg16(p + 12) | ldg16(p + 14) << 16);
+    } else {
+        uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+        for (int i = 0; i < 16; i++) w[i >> 2] |= ldg8(p + i) << ((i & 3) * 8);
+        r = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    return r;
+}
+__device__ __forceinline__ void sts8(uint32_t addr, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+// 16 bytes o to shared address p of any phase, touching exactly them
+__device__ __forceinline__ void sts16_any(uint32_t p, uint4 o) {
+    switch (p & 3u) {
+    case 0:
+        sts32(p, o.x);
+        sts32(p + 4, o.y);
+        sts32(p + 8, o.z);
+        sts32(p + 12, o.w);
+        break;
+    case 1:
+        sts8(p, o.x);
+        sts16(p + 1, o.x >> 8);
+        sts32(p + 3, __funnelshift_r(o.x, o.y, 24));
+        sts32(p + 7, __funnelshift_r(o.y, o.z, 24));
+        sts32(p + 11, __funnelshift_r(o.z, o.w, 24));
+        sts8(p + 15, o.w >> 24);
+        break;
+    case 2:
+        sts16(p, o.x);
+        sts32(p + 2, __funnelshift_r(o.x, o.y, 16));
+        sts32(p + 6, __funnelshift_r(o.y, o.z, 16));
+        sts32(p + 10, __funnelshift_r(o.z, o.w, 16));
+        sts16(p + 14, o.w >> 16);
+        break;
+    default:
+        sts8(p, o.x);
+        sts32(p + 1, __funnelshift_r(o.x, o.y, 8));
+        sts32(p + 5, __funnelshift_r(o.y, o.z, 8));
+        sts32(p + 9, __funnelshift_r(o.z, o.w, 8));
+        sts16(p + 13, o.w >> 8);
+        sts8(p + 15, o.w >> 24);
+        break;
+    }
+}
+// one element at d: the operand staged at shared address s, compared with the element at c, is replaced by the
+// element's previous value (all three aligned to the element size)
+__device__ __forceinline__ void cas1(char *d, uint32_t s, const char *c, uint32_t el) {
+    switch (el) {
+    case 3: sts64(s, atom_cas_b64(d, ldg64(c), lds64(s))); break;
+    case 2: sts32(s, atom_cas_b32(d, ldg32(c), lds32(s))); break;
+    default: {
+        const uint32_t sh = ((uint32_t)(uint64_t)d & 3u) * 8u, m = (el ? 0xFFFFu : 0xFFu) << sh;
+        const uint32_t o = cas_word((char *)((uint64_t)d & ~(uint64_t)3), (el ? ldg16(c) : ldg8(c)) << sh,
+                                    (el ? (uint32_t)lds16h(s) : lds8(s)) << sh, m, el) >> sh;
+        if (el) sts16(s, o);
+        else sts8(s, o);
+        break;
+    }
+    }
+}
+// 16 bytes at a 16-byte aligned d: the operands v, compared with c, element-wise; returns the previous 16 bytes
+__device__ __forceinline__ uint4 cas16(char *d, uint4 v, uint4 c, uint32_t el) {
+    if (el == 3) {
+        const uint64_t a = atom_cas_b64(d, (uint64_t)c.y << 32 | c.x, (uint64_t)v.y << 32 | v.x);
+        const uint64_t b = atom_cas_b64(d + 8, (uint64_t)c.w << 32 | c.z, (uint64_t)v.w << 32 | v.z);
+        return make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+    }
+    if (el == 2) return make_uint4(atom_cas_b32(d, c.x, v.x), atom_cas_b32(d + 4, c.y, v.y), atom_cas_b32(d + 8, c.z, v.z),
+                                   atom_cas_b32(d + 12, c.w, v.w));
+    return make_uint4(cas_word(d, c.x, v.x, ~0u, el), cas_word(d + 4, c.y, v.y, ~0u, el), cas_word(d + 8, c.z, v.z, ~0u, el),
+                      cas_word(d + 12, c.w, v.w, ~0u, el));
+}
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
     unsigned int v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -552,6 +689,9 @@ __device__ __forceinline__ int64_t warp_sum(int64_t v) {
     return v;
 }
 
+// the ops of a fetch-op launch (GatherArgs::fop_op)
+constexpr int kFopAdd = 0, kFopSwap = 1, kFopCas = 2;
+
 struct GatherArgs {
     ddsk_var_t var;
     const int64_t *starts; // FIXED: start row per request
@@ -584,9 +724,11 @@ struct GatherArgs {
             int64_t *pad_lengths;                    // optional [nreq] delivered row counts
         };
         struct { // accumulates (ACC) and fetch-ops (FETCH), puts: neither padded nor multi-array
-            int acc_type;     // DDSK_ACC_*: the element type of the sum (or swap)
-            int fop_swap;     // FETCH: the op is a swap (else an add)
-            char *fop_result; // FETCH: the previous values, at the operands' positions (the layout of dst)
+            int acc_type;            // DDSK_ACC_*: the element type of the sum (or swap)
+            int fop_op;              // FETCH: kFopAdd, kFopSwap or kFopCas (warp-uniform)
+            char *fop_result;        // FETCH: the previous values, at the operands' positions (the layout of dst)
+            const char *fop_compare; // kFopCas: the compare operands, at the operands' positions
+            int fop_el;              // kFopCas: log2 of the element size (0..3; acc_type does not apply)
         };
     };
     int min_seg_chunks;                // smallest segment, in chunks (claims cost more when the plan is in global memory)
@@ -1142,6 +1284,67 @@ __device__ __forceinline__ void fop_chunk(uint32_t sb, uint32_t a, char *d, uint
     }
 }
 
+// The compare-and-swap's fop_rephase_loop: operand vector j re-phased from the stage, compare vector j read from global
+// memory at cv + 16j in its own phase (the compare buffer's, not the shard's), cas16 on the shard's 16 bytes at dv + 16j,
+// and the previous 16 bytes written back over the operand's staged bytes at s + 16j (any phase: 1-byte elements).
+template <int WS, bool BYTES>
+__device__ __forceinline__ void cas_rephase_loop(uint32_t sbase, uint32_t s, char *dv, const char *cv, uint32_t nv,
+                                                 uint32_t bs8, int lane, uint32_t el) {
+#pragma unroll 2
+    for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
+        const uint4 lo = lds128(sbase + (j << 4));
+        const uint4 hi = lds128(sbase + (j << 4) + 16);
+        const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+        uint4 v;
+        if (BYTES) {
+            v.x = __funnelshift_r(w[WS + 0], w[WS + 1], bs8);
+            v.y = __funnelshift_r(w[WS + 1], w[WS + 2], bs8);
+            v.z = __funnelshift_r(w[WS + 2], w[WS + 3], bs8);
+            v.w = __funnelshift_r(w[WS + 3], w[WS + 4], bs8);
+        } else {
+            v = make_uint4(w[WS + 0], w[WS + 1], w[WS + 2], w[WS + 3]);
+        }
+        const uint4 o = cas16(dv + ((size_t)j << 4), v, ldg16_any(cv + ((size_t)j << 4)), el);
+        if (!BYTES && WS == 0) sts128(s + (j << 4), o);
+        else sts16_any(s + (j << 4), o);
+    }
+}
+
+// The compare-and-swap's first pass over one staged piece: fop_chunk's cuts and phases, with the piece's compare
+// operands at c[k] (payload byte k) and elements of 1 << el bytes. Only the piece's own compare bytes are read.
+__device__ __forceinline__ void cas_chunk(uint32_t sb, uint32_t a, char *d, const char *c, uint32_t n, int lane, uint32_t el) {
+    uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
+    if (head > n) head = n;
+    const uint32_t nv = (n - head) >> 4;
+    const uint32_t tail = n - head - (nv << 4);
+    const uint32_t s = a + head;
+    const uint32_t sh = s & 15u;
+    if (nv) {
+        const uint32_t sbase = sb + (s & ~15u);
+        const uint32_t bs8 = (sh & 3u) * 8u;
+        char *dv = d + head;
+        const char *cv = c + head;
+        switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform
+        case 0: cas_rephase_loop<0, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        case 1: cas_rephase_loop<0, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        case 2: cas_rephase_loop<1, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        case 3: cas_rephase_loop<1, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        case 4: cas_rephase_loop<2, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        case 5: cas_rephase_loop<2, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        case 6: cas_rephase_loop<3, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        default: cas_rephase_loop<3, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
+        }
+    }
+    if ((uint32_t)lane < (head >> el)) {
+        const uint32_t k = (uint32_t)lane << el;
+        cas1(d + k, sb + a + k, c + k, el);
+    }
+    if ((uint32_t)lane < (tail >> el)) {
+        const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
+        cas1(d + k, sb + a + k, c + k, el);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Converting drain (DDSK_CVT_*): the load side of the walk is unchanged, the staged SOURCE elements are converted on the
 // way out of shared memory. Source byte p of a variable's packed rows goes to output byte (p >> IL) << OL; the ratio is
@@ -1596,11 +1799,11 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // ACC (with PUT): a batched accumulate (DDSK_F_ACC) -- the put whose drain adds instead of storing, in the element type
 // a.acc_type: bulk reductions where the put bulk-stores, element reductions for the ragged ends, vector reductions of
 // the re-phased body. Each is atomic per element, so requests of any batch or rank that hit the same element combine.
-// FETCH (with PUT): a batched fetch-op (DDSK_F_FOP) -- the put whose drain applies a returning atomic (add or swap,
-// a.fop_swap, in the element type a.acc_type) to every element and sends the previous values to a.fop_result, at the
-// operands' positions. Every piece is drained cooperatively in two passes: fop_chunk replaces the staged operands by the
-// previous values, then the raw drain (bulk stores where the phases allow) writes the stage to the result. The result
-// address of each piece is kept beside its descriptor, in dynamic shared memory behind the rings and the plan.
+// FETCH (with PUT): a batched fetch-op (DDSK_F_FOP) -- the put whose drain applies a returning atomic (add, swap or
+// compare-and-swap, a.fop_op; add and swap in the element type a.acc_type, compare-and-swap on 1 << a.fop_el bytes) to
+// every element and sends the previous values to a.fop_result, at the operands' positions. Every piece is drained
+// cooperatively in two passes: fop_chunk (cas_chunk) replaces the staged operands by the previous values, then the raw
+// drain (bulk stores where the phases allow) writes the stage to the result. The result address of each piece is kept beside its descriptor, in dynamic shared memory behind the rings and the plan.
 template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
           bool ACC = false, bool FETCH = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
@@ -1943,18 +2146,27 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         const uint32_t my_n = desc[warp][st][lane].n;
         const uint32_t my_pack = desc[warp][st][lane].pack;
         if constexpr (FETCH) {
-            // fetch-op: pass 1, the atomics, every piece cooperatively; pass 2, the previous values to the result
+            // fetch-op: pass 1, the atomics, every piece cooperatively; pass 2, the previous values to the result. A
+            // compare-and-swap finds a piece's compare operands at its result address's position in a.fop_compare; pass 1
+            // has read them all before pass 2 writes a result byte (result == compare is allowed).
+            char *const my_res = (char *)lds64(fop_rdst<NW, S, STAGE, PCAP>(smem_dyn, warp, st, lane));
             unsigned todo = __ballot_sync(0xffffffffu, my_n != 0);
             for (unsigned rest = todo; rest; rest &= rest - 1) {
                 const int j = __ffs(rest) - 1;
                 const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
                 const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
                 const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
-                fop_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type, a.fop_swap != 0);
+                if (a.fop_op == kFopCas) {
+                    const uint64_t r = __shfl_sync(0xffffffffu, (uint64_t)my_res, j);
+                    cas_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos,
+                              a.fop_compare + (r - (uint64_t)a.fop_result), n, lane, (uint32_t)a.fop_el);
+                } else {
+                    fop_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type,
+                              a.fop_op == kFopSwap);
+                }
             }
             fence_proxy_async(); // (every lane: its stage writes, before any lane's bulk store reads them)
             __syncwarp();
-            char *const my_res = (char *)lds64(fop_rdst<NW, S, STAGE, PCAP>(smem_dyn, warp, st, lane));
             const bool direct = my_n != 0 && (((uint32_t)(uint64_t)my_res | my_n | (my_pack >> 16)) & 15u) == 0;
             if (direct) tma_store_1d(my_res, ring + st * STAGE + (my_pack & 0xffffu), my_n);
             todo = __ballot_sync(0xffffffffu, my_n != 0 && !direct);
@@ -2689,8 +2901,10 @@ int gather_args(GatherArgs &a, const ddsk_var_t *var, const ddsk_scratch_t *scr,
     a.tickets = a.overlap ? nullptr : scr->counters;
     if (flags & (DDSK_F_ACC | DDSK_F_FOP)) a.acc_type = DDSK_F_ACC_TYPE(flags);
     if (flags & DDSK_F_FOP) {
-        a.fop_swap = (flags & DDSK_F_FOP_SWAP) ? 1 : 0;
+        a.fop_op = (flags & DDSK_F_FOP_CAS) ? kFopCas : (flags & DDSK_F_FOP_SWAP) ? kFopSwap : kFopAdd;
         a.fop_result = (char *)scr->fop_result;
+        a.fop_compare = (const char *)scr->fop_compare;
+        a.fop_el = DDSK_F_ACC_TYPE(flags); // (a compare-and-swap's log2 element size, in the element type's bits)
     }
     return 0;
 }

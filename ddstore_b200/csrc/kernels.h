@@ -62,6 +62,8 @@ typedef struct ddsk_scratch {
                                         last warp of a gather launch that asks for it), [2] ticket of dds_small_get */
     void *fop_result;           /* host side, set by the caller of a DDSK_F_FOP launch: the caller's result buffer (device
                                    memory, the layout of the source rows) */
+    const void *fop_compare;    /* host side, set by the caller of a DDSK_F_FOP_CAS launch: the caller's compare operands
+                                   (device memory, the layout of the source rows) */
 } ddsk_scratch_t;
 
 /* `flags` of the launchers */
@@ -88,6 +90,9 @@ typedef struct ddsk_scratch {
                                position of scr->fop_result as the operand's in the caller's rows. The element type is
                                DDSK_F_ACC_TYPE(flags); the caller's rows and fop_result are aligned to its size. */
 #define DDSK_F_FOP_SWAP 16384 /* with DDSK_F_FOP: the op is a swap (shard = src); else an add (shard = shard + src) */
+#define DDSK_F_FOP_CAS 32768  /* with DDSK_F_FOP: the op is a compare-and-swap (shard = src where shard == compare, bit for
+                                 bit, at the same position of scr->fop_compare). Bits 10..12 of the flags then hold log2 of
+                                 the element size (0..3), not an element type; src, compare and result are aligned to it. */
 
 /* element types of an accumulate (same values as DDS_ACC_* in include/ddstore_b200.h) */
 #define DDSK_ACC_F32 1

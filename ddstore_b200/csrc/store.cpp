@@ -1717,10 +1717,14 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
 // op: 0, or a DDS_OP_* for the fetch-op behind dds_get_accumulate_batch / dds_get_accumulate_samples (with acc its element
 // type): the same launch whose drain applies a returning atomic and writes the previous rows to `result`, in the layout
 // of src (DDSK_F_FOP). result must be aligned to the element size too.
+// op OP_CAS (acc 0): the compare-and-swap behind dds_compare_and_swap_batch / dds_compare_and_swap_samples, the fetch-op
+// launch whose drain swaps where the shard equals `compare` (the layout of src; DDSK_F_FOP_CAS) on elements of the
+// variable's itemsize. src and compare must be aligned to it too.
+static constexpr int OP_CAS = 3; // (put_impl's own op code, beside the DDS_OP_* of the fetch-ops)
 static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
                     int64_t fixed_count, int64_t nreq, const void *src, int64_t src_bytes, unsigned flags,
                     void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, int acc = 0, int op = 0,
-                    void *result = nullptr) {
+                    void *result = nullptr, const void *compare = nullptr) {
     if (!(flags & DDS_SRC_ON_DEVICE)) return fail(DDS_ERR_ARG, "puts take their rows from device memory (DDS_SRC_ON_DEVICE)");
     if (nreq < 0 || src_bytes < 0) return fail(DDS_ERR_ARG, "negative nreq or src_bytes");
     if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
@@ -1735,6 +1739,9 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     if (op && !result && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null result");
     if (op && (uintptr_t)result % (uintptr_t)v->itemsize)
         return fail(DDS_ERR_ARG, "fetch-ops take result aligned to the element size");
+    if (op == OP_CAS && !compare && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null compare");
+    if (op == OP_CAS && ((uintptr_t)src % (uintptr_t)v->itemsize || (uintptr_t)compare % (uintptr_t)v->itemsize))
+        return fail(DDS_ERR_ARG, "compare-and-swaps take src and compare aligned to the element size");
 
     Call c;
     if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
@@ -1752,7 +1759,12 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     ddsk_scratch_t scr;
     if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
     void *d_src = const_cast<void *>(src);
-    if (op) {
+    if (op == OP_CAS) {
+        const int el = v->itemsize == 8 ? 3 : v->itemsize == 4 ? 2 : v->itemsize == 2 ? 1 : 0;
+        kflags |= DDSK_F_PUT | DDSK_F_FOP | DDSK_F_FOP_CAS | el << DDSK_F_ACC_SHIFT;
+        scr.fop_result = result;
+        scr.fop_compare = compare;
+    } else if (op) {
         kflags |= DDSK_F_PUT | DDSK_F_FOP | acc << DDSK_F_ACC_SHIFT | (op == DDS_OP_REPLACE ? DDSK_F_FOP_SWAP : 0);
         scr.fop_result = result;
     } else {
@@ -1839,6 +1851,35 @@ int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *
     if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
                     dtype, op, result);
+}
+
+// The compare-and-swaps' prologue: entry_var, an itemsize outside {1, 2, 4, 8} (an argument error) and then one other
+// than the variable's (the reference's "Invalid data type")
+static int cas_entry(dds_store_t *s, const char *name, int itemsize, int64_t *total_bytes, int64_t *bad_index, Var **v) {
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, v)) return rc;
+    if (itemsize != 1 && itemsize != 2 && itemsize != 4 && itemsize != 8)
+        return fail(DDS_ERR_ARG, "compare-and-swaps take elements of 1, 2, 4 or 8 bytes");
+    if ((*v)->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
+    return DDS_OK;
+}
+
+int dds_compare_and_swap_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                               int64_t fixed_count, int64_t nreq, int itemsize, const void *src, const void *compare,
+                               void *result, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                               int64_t *bad_index) {
+    Var *v;
+    if (int rc = cas_entry(s, name, itemsize, total_bytes, bad_index, &v)) return rc;
+    return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
+                    bad_index, 0, OP_CAS, result, compare);
+}
+
+int dds_compare_and_swap_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
+                                 const void *src, const void *compare, void *result, int64_t src_bytes, unsigned flags,
+                                 void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    Var *v;
+    if (int rc = cas_entry(s, name, itemsize, total_bytes, bad_index, &v)) return rc;
+    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
+                    0, OP_CAS, result, compare);
 }
 
 // The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,

@@ -62,6 +62,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
         long get_accumulate_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                                   int op, int dtype, const void* src, void* result, long src_bytes, cbool idx_on_device,
                                   void* stream) except +dds_translate_exception
+        long compare_and_swap_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
+                                    int itemsize, const void* src, const void* compare, void* result, long src_bytes,
+                                    cbool idx_on_device, void* stream) except +dds_translate_exception
         void epoch_begin() except +dds_translate_exception
         void epoch_end() except +dds_translate_exception
         void free() except +dds_translate_exception
@@ -387,6 +390,55 @@ cdef class PyDDStore:
         with nogil:
             total = self.c_ddstore.get_accumulate_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, opc, code,
                                                         <const void*> dp, <void*> rp, nbytes, idx_dev, <void*> st)
+        del keep
+        return total
+
+    def compare_and_swap_batch(self, str name, starts, counts=None, src=None, compare=None, out=None, count=None,
+                               stream=None):
+        """one kernel launch COMPARE-AND-SWAPPING len(starts) requests: each element of the rows becomes src's where it
+        equals compare's bit for bit, and its previous value goes to `out` either way (compare and out: CUDA tensors of
+        src's element size and at least its bytes, src's layout; out may be src or compare); see
+        ddstore_b200.store.PyDDStore.compare_and_swap_batch (this binding's compare-and-swap is synchronous). Returns the
+        layout's bytes."""
+        if src is None:
+            raise ValueError("a compare-and-swap needs `src` rows")
+        for what, t in (("src", src), ("compare", compare), ("out", out)):
+            if not (hasattr(t, "data_ptr") and getattr(t, "is_cuda", False)):
+                raise ValueError(f"compare-and-swap on {name!r}: {what} must be a CUDA tensor")
+            if not t.is_contiguous():
+                raise ValueError(f"{what} must be C-contiguous")
+            if t.element_size() != src.element_size():
+                raise ValueError(f"compare-and-swap on {name!r}: {what} has {t.element_size()}-byte elements, src "
+                                 f"{src.element_size()}-byte ones")
+        cdef long nbytes = src.numel() * src.element_size()
+        for what, t in (("compare", compare), ("out", out)):
+            if t.numel() * t.element_size() < nbytes:
+                raise ValueError(f"compare-and-swap on {name!r}: {what} holds {t.numel() * t.element_size()} bytes, "
+                                 f"src {nbytes}")
+        cdef int itemsize = src.element_size()
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        cdef size_t sp, cp = 0, dp = src.data_ptr(), qp = compare.data_ptr(), rp = out.data_ptr()
+        cdef long nreq
+        if s_dev:
+            nreq = starts.numel(); sp = starts.data_ptr()
+            if counts is not None: cp = counts.data_ptr()
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
+            ca = _i64(counts) if counts is not None else None
+            if ca is not None: cp = ca.ctypes.data
+            keep = (sa, ca)
+        cdef long fixed = 1 if count is None else int(count)
+        cdef size_t st = 0
+        if stream is not None:
+            st = int(stream) if int(stream) != 0 else 1
+        cdef string nm = name.encode()
+        cdef cbool idx_dev = bool(s_dev)
+        cdef long total
+        with nogil:
+            total = self.c_ddstore.compare_and_swap_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, itemsize,
+                                                          <const void*> dp, <const void*> qp, <void*> rp, nbytes,
+                                                          idx_dev, <void*> st)
         del keep
         return total
 

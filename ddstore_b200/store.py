@@ -510,6 +510,83 @@ class PyDDStore:
         _capi.raise_for(rc)
         return total.value
 
+    # ---------------------------------------------------------------- batched compare-and-swaps (MPI_Compare_and_swap)
+    def compare_and_swap_batch(self, name, starts, counts=None, src=None, compare=None, out=None, count=None,
+                               stream=None, wait=True):
+        """COMPARE-AND-SWAP len(starts) requests against the owners' shards in ONE kernel launch: for every element e of
+        request i's rows, in one atomic step, out[e] = shard[e], and shard[e] becomes src[e] if it equalled compare[e]
+        BIT FOR BIT (on float data -0 != +0 and a NaN equals only its own bits). out always receives the previous
+        value, so element e was swapped exactly when out[e] == compare[e] bitwise. Requests, the layout of `src`, errors
+        (every valid request is still applied, an invalid one changes nothing and writes no out bytes), wait=False,
+        ordering and visibility are get_accumulate_batch's. src, compare and out may be of any dtype whose element size
+        is the variable's itemsize (1, 2, 4 or 8), the same for all three; compare and out are C-contiguous CUDA tensors
+        of at least src's bytes in src's layout, and out may be src or compare. Compare-and-swaps on one element in one
+        epoch are linearisable, from any batch, rank or duplicate request: of N that expect the same value exactly one
+        wins. Mixing them with puts, accumulates or fetch-ops on one element in one epoch is undefined. Returns the
+        layout's size in bytes."""
+        sb, keep_src = self._put_src(name, src)
+        cmp, res = self._cas_args(name, compare, out, sb)
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        if s_dev:
+            nreq, sp = starts.numel(), starts.data_ptr()
+            cp = counts.data_ptr() if counts is not None else None
+            keep = (starts, counts)
+        else:
+            sa = _i64(starts)
+            ca = _i64(counts) if counts is not None else None
+            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
+            keep = (sa, ca)
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_compare_and_swap_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count),
+                                                nreq, sb.itemsize, sb.ptr, cmp, res, sb.nbytes, flags,
+                                                self._stream_arg(stream), C.byref(total), C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    def compare_and_swap_samples(self, name, sample_ids, src, compare, out, stream=None, wait=True):
+        """compare_and_swap_batch by SAMPLE ID: request i compares and swaps the rows of sample sample_ids[i] in the
+        index registered with set_sample_index. Layout and errors as put_samples, semantics as
+        compare_and_swap_batch."""
+        sb, keep_src = self._put_src(name, src)
+        cmp, res = self._cas_args(name, compare, out, sb)
+        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
+        if s_dev:
+            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
+        else:
+            sa = _i64(sample_ids)
+            nreq, sp, keep = sa.size, sa.ctypes.data, sa
+        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        rc = self._L.dds_compare_and_swap_samples(self._h, name.encode(), sp, nreq, sb.itemsize, sb.ptr, cmp, res,
+                                                  sb.nbytes, flags, self._stream_arg(stream), C.byref(total),
+                                                  C.byref(bad))
+        del keep, keep_src
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value
+
+    @staticmethod
+    def _cas_args(name, compare, out, sb):
+        """the addresses of a compare-and-swap's `compare` and `out` tensors (ValueError unless each is a C-contiguous
+        CUDA tensor of src's element size and at least src's bytes)"""
+        ptrs = []
+        for what, t in (("compare", compare), ("out", out)):
+            if not (hasattr(t, "data_ptr") and getattr(t, "is_cuda", False)):
+                raise ValueError(f"compare-and-swap on {name!r}: {what} must be a CUDA tensor")
+            if not t.is_contiguous():
+                raise ValueError(f"{what} must be C-contiguous")
+            if t.element_size() != sb.itemsize:
+                raise ValueError(f"compare-and-swap on {name!r}: {what} has {t.element_size()}-byte elements, src "
+                                 f"{sb.itemsize}-byte ones")
+            if t.numel() * t.element_size() < sb.nbytes:
+                raise ValueError(f"compare-and-swap on {name!r}: {what} holds {t.numel() * t.element_size()} bytes, "
+                                 f"src {sb.nbytes}")
+            ptrs.append(t.data_ptr())
+        return ptrs[0], ptrs[1]
+
     @staticmethod
     def _fop_args(name, op, out, sb):
         """the DDS_OP_* code of a fetch-op and the address of its `out` tensor (ValueError for an unknown op, or an out
@@ -751,9 +828,9 @@ class PyDDStore:
         previous wait() (0 if none).
         wait() alone reports the outcome of queued batches, exactly once. Any other call that meets a pending queue
         (a synchronous get_batch / get / get_samples / get_samples_multi / put_batch / put_samples / accumulate_batch /
-        accumulate_samples / get_accumulate_batch / get_accumulate_samples, a batch on another stream,
-        set_sample_index, set_normalization, epoch_end, epoch_begin when the queue holds a put, an accumulate or a
-        fetch-op, free) completes it, keeps its first failure for the next wait(), and raises only
+        accumulate_samples / get_accumulate_batch / get_accumulate_samples / compare_and_swap_batch /
+        compare_and_swap_samples, a batch on another stream, set_sample_index, set_normalization, epoch_end,
+        epoch_begin when the queue holds a put, an accumulate, a fetch-op or a compare-and-swap, free) completes it, keeps its first failure for the next wait(), and raises only
         for its own requests. A failure kept from earlier wins over later ones; after wait() has raised it, the next
         wait() is clean. close() drops an outcome no wait() has reported."""
         total, bad = C.c_int64(0), C.c_int64(-1)

@@ -26,8 +26,9 @@ extern "C" {
                            The padded batches (dds_get_batch_padded, dds_get_samples_padded) add entries only: callers
                            that built against 111 are unaffected, and a caller finds them by symbol. So do the batched
                            puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE), the batched accumulates
-                           (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*) and the batched fetch-ops
-                           (dds_get_accumulate_batch, dds_get_accumulate_samples, DDS_OP_*). */
+                           (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*), the batched fetch-ops
+                           (dds_get_accumulate_batch, dds_get_accumulate_samples, DDS_OP_*) and the batched
+                           compare-and-swaps (dds_compare_and_swap_batch, dds_compare_and_swap_samples). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -373,6 +374,39 @@ int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *
                                int dtype, const void *src, void *result, int64_t src_bytes, unsigned flags,
                                void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
 
+/* ---- batched compare-and-swaps: elements of any rank's shard replaced where they hold an expected value, the previous
+ * rows returned (MPI_Compare_and_swap between fences, batched). For every element e of request i's rows, in one atomic
+ * step:
+ *   result[e] = shard[e]; if (shard[e] == compare[e]) shard[e] = src[e]
+ * Elements are itemsize bytes, which must be the variable's itemsize and 1, 2, 4 or 8. The comparison is BITWISE, as
+ * MPI_Compare_and_swap restricts itself to integer and byte types: on float data -0 and +0 differ, a NaN equals only the
+ * same bit pattern (payload and signalling bit included), and subnormals compare by their bits.
+ * Requests, the layout of src, validation, error reporting (every valid request is applied, an invalid one changes
+ * nothing and writes no result bytes, the first invalid one is reported; a layout total above src_bytes touches nothing,
+ * DDS_ERR_CAPACITY), flags, DDS_NO_SYNC queueing, fences and the ignored DDS_OVERLAP (a compare-and-swap ends an overlap
+ * run) are dds_get_accumulate_batch's / dds_get_accumulate_samples's, word for word.
+ * compare and result have the layout of src and are device memory of at least src_bytes bytes. result always receives
+ * the previous value, for failed compares too: element e was swapped exactly when result[e] == compare[e]. An invalid
+ * request's result bytes, and every byte outside the valid requests' ranges, are left untouched, and no compare byte
+ * outside them is read. result == src and result == compare are allowed; any other overlap of src, compare and result
+ * with each other or with a shard is undefined.
+ * Atomicity is per element: compare-and-swaps on one element in one epoch -- from any batch, any rank, or duplicate
+ * requests of one batch -- are linearisable. So of N requests that all compare against the element's value, exactly one
+ * succeeds and the others get its value back. 1- and 2-byte elements are swapped by a compare-and-swap loop on their
+ * aligned 32-bit word, which leaves every other byte of the word as it finds it, also while other requests or ranks
+ * change those bytes. Mixing compare-and-swaps with puts, accumulates or fetch-ops on one element in one epoch is
+ * undefined. Rows are not atomic as a whole.
+ * Argument errors, with DDS_ERR_ARG and nothing enqueued: the put's, an itemsize other than 1, 2, 4 or 8, compare or
+ * result == NULL while the layout is non-empty, and src, compare or result not aligned to the itemsize. An itemsize other
+ * than the variable's is DDS_ERR_DTYPE. */
+int dds_compare_and_swap_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                               int64_t fixed_count, int64_t nreq, int itemsize, const void *src, const void *compare,
+                               void *result, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
+                               int64_t *bad_index);
+int dds_compare_and_swap_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
+                                 const void *src, const void *compare, void *result, int64_t src_bytes, unsigned flags,
+                                 void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite
  * flow. When all ranks fetch in the same
@@ -391,7 +425,7 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
  * failing batch in queue order is reported, with that batch's first invalid request in *bad_index.
  * The outcome of queued batches is reported here and only here, exactly once. Any other call that meets a pending
  * queue (a synchronous batch or get(), a batch on another stream, dds_set_sample_index, dds_set_normalization,
- * dds_epoch_end, dds_epoch_begin when the queue holds a put, an accumulate or a fetch-op, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
+ * dds_epoch_end, dds_epoch_begin when the queue holds a put, an accumulate, a fetch-op or a compare-and-swap, dds_free, a push step on another stream) completes it first and keeps its first failing status; it
  * then does its own work and reports only its own outcome (its error and *bad_index describe its own requests). The
  * next dds_batch_wait reports the kept failure, with its index and text, after completing any queue still pending; a
  * failure kept from earlier wins over any failure queued after it, since it is earlier in queue order. After it has

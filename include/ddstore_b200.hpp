@@ -243,6 +243,43 @@ class DDStore {
         return get_accumulate_samples(name, sample_ids, nreq, op, acc_type<T>(), src, result, src_bytes, idx_on_device,
                                       cuda_stream);
     }
+    // Batched compare-and-swap (dds_compare_and_swap_batch): accumulate_batch's requests and layout, each element of the
+    // rows replaced by src's where it equals compare's bit for bit, atomically, its previous value written to `result`
+    // either way (compare and result: device memory of at least src_bytes, the layout of src; result may be src or
+    // compare). Elements are itemsize bytes (1, 2, 4 or 8, the variable's); T gives it as sizeof(T).
+    long compare_and_swap_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq,
+                                int itemsize, const void *src, const void *compare, void *result, long src_bytes,
+                                bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_compare_and_swap_batch(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts,
+                                         fixed_count, nreq, itemsize, src, compare, result, src_bytes, flags, cuda_stream,
+                                         &total, &bad));
+        return (long)total;
+    }
+    template <typename T>
+    long compare_and_swap_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq,
+                                const T *src, const T *compare, T *result, long src_bytes, bool idx_on_device = true,
+                                void *cuda_stream = nullptr) {
+        return compare_and_swap_batch(name, starts, counts, fixed_count, nreq, (int)sizeof(T), src, compare, result,
+                                      src_bytes, idx_on_device, cuda_stream);
+    }
+    // The same by sample id (dds_compare_and_swap_samples).
+    long compare_and_swap_samples(std::string name, const long *sample_ids, long nreq, int itemsize, const void *src,
+                                  const void *compare, void *result, long src_bytes, bool idx_on_device = true,
+                                  void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_compare_and_swap_samples(store_, name.c_str(), (const int64_t *)sample_ids, nreq, itemsize, src, compare,
+                                           result, src_bytes, flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    template <typename T>
+    long compare_and_swap_samples(std::string name, const long *sample_ids, long nreq, const T *src, const T *compare,
+                                  T *result, long src_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        return compare_and_swap_samples(name, sample_ids, nreq, (int)sizeof(T), src, compare, result, src_bytes,
+                                        idx_on_device, cuda_stream);
+    }
     // the DDS_ACC_* code of an element type
     template <typename T>
     static constexpr int acc_type() {
