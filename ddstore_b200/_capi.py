@@ -23,6 +23,9 @@ ACC_TYPES = {"float32": ACC_F32, "float64": ACC_F64, "int32": ACC_I32, "int64": 
 # ops of the batched fetch-ops (DDS_OP_*), by name
 OP_SUM, OP_REPLACE = 1, 2
 FOP_OPS = {"sum": OP_SUM, "replace": OP_REPLACE}
+# reductions beside the sum (DDS_OP_MAX..), by torch's names: the batched reductions and the fetch-ops take them
+OP_MAX, OP_MIN, OP_BAND, OP_BOR, OP_BXOR = 4, 5, 6, 7, 8
+RED_OPS = {"amax": OP_MAX, "amin": OP_MIN, "bitwise_and": OP_BAND, "bitwise_or": OP_BOR, "bitwise_xor": OP_BXOR}
 
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 BARRIER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
@@ -101,6 +104,10 @@ SIGNATURES = {
                                        C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_accumulate_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
                                          C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_accumulate_op_batch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                          C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_accumulate_op_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_int,
+                                            C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_get_accumulate_batch": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
                                            C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p,
                                            I64P, I64P]),

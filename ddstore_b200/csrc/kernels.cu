@@ -543,6 +543,247 @@ __device__ __forceinline__ uint4 cas16(char *d, uint4 v, uint4 c, uint32_t el) {
     return make_uint4(cas_word(d, c.x, v.x, ~0u, el), cas_word(d + 4, c.y, v.y, ~0u, el), cas_word(d + 8, c.z, v.z, ~0u, el),
                       cas_word(d + 12, c.w, v.w, ~0u, el));
 }
+
+// Reductions beside the sum (ACC and FETCH, op = DDSK_RED_MAX.., warp-uniform like the element type t). Integers take
+// the hardware's signed min / max and bitwise reductions and atomics. f16 / bf16 take the bulk, vector and vector-atomic
+// max / min, whose maximumNumber / minimumNumber semantics (NaN ignored, -0 < +0, nothing flushed) were measured on H100
+// (DESIGN.md 3.11); there is no scalar 16-bit max / min, so their ragged ends take a compare-and-swap loop on the aligned
+// word. f32 and f64 have no max / min atomic in any form: every element takes a compare-and-swap loop, and the bulk
+// reduction's pieces fall back to the cooperative drain (red_bulk).
+__device__ __forceinline__ bool red_bulk(int t, int op) { return op == DDSK_RED_SUM || (t != DDSK_ACC_F32 && t != DDSK_ACC_F64); }
+// maximumNumber (mx) / minimumNumber of the element bits c and operand bits o of a W-bit float (inf: its +inf bits):
+// a NaN operand leaves c, a NaN c takes o, else the larger / smaller by the total order of the bits (so -0 < +0, and
+// subnormals compare exactly whatever the ftz mode). The result is always the bits of c or of o.
+template <typename U, int W>
+__device__ __forceinline__ U fpick(U c, U o, U inf, bool mx) {
+    constexpr U S = (U)1 << (W - 1), M = S - 1;
+    if ((o & M) > inf) return c;
+    if ((c & M) > inf) return o;
+    const U kc = (c & S) ? (~c & (S | M)) : (c | S), ko = (o & S) ? (~o & (S | M)) : (o | S); // order-preserving keys
+    return (mx ? ko > kc : ko < kc) ? o : c;
+}
+// f32 / f64 max / min of one element: a compare-and-swap loop that leaves without one when the element stays (the load
+// was the atomic step). Returns the previous value.
+__device__ __forceinline__ uint32_t fmm32(char *d, uint32_t o, bool mx) {
+    uint32_t cur;
+    asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(cur) : "l"(d) : "memory");
+    while (true) {
+        const uint32_t want = fpick<uint32_t, 32>(cur, o, 0x7f800000u, mx);
+        if (want == cur) return cur;
+        const uint32_t seen = atom_cas_b32(d, cur, want);
+        if (seen == cur) return cur;
+        cur = seen;
+    }
+}
+__device__ __forceinline__ uint64_t fmm64(char *d, uint64_t o, bool mx) {
+    uint64_t cur;
+    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(cur) : "l"(d) : "memory");
+    while (true) {
+        const uint64_t want = fpick<uint64_t, 64>(cur, o, 0x7ff0000000000000ull, mx);
+        if (want == cur) return cur;
+        const uint64_t seen = atom_cas_b64(d, cur, want);
+        if (seen == cur) return cur;
+        cur = seen;
+    }
+}
+// f16 / bf16 max / min of the 16-bit elements of the aligned word w that mask m selects (low half, high half or both),
+// with the operands at the same positions of o: cas_word's loop, which leaves the other half exactly as it finds it.
+// Returns the word the step found.
+__device__ __forceinline__ uint32_t fmm_word(char *w, uint32_t o, uint32_t m, bool bf, bool mx) {
+    const uint32_t inf = bf ? 0x7f80u : 0x7c00u;
+    uint32_t cur;
+    asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(cur) : "l"(w) : "memory");
+    while (true) {
+        uint32_t want = cur;
+        if (m & 0xFFFFu) want = (want & 0xFFFF0000u) | fpick<uint32_t, 16>(cur & 0xFFFFu, o & 0xFFFFu, inf, mx);
+        if (m >> 16) want = (want & 0xFFFFu) | fpick<uint32_t, 16>(cur >> 16, o >> 16, inf, mx) << 16;
+        if (want == cur) return cur;
+        const uint32_t seen = atom_cas_b32(w, cur, want);
+        if (seen == cur) return cur;
+        cur = seen;
+    }
+}
+// integer reductions, without (red) and with (atom) the previous value
+__device__ __forceinline__ void red_i32(char *d, uint32_t v, int op) {
+    switch (op) {
+    case DDSK_RED_MAX: asm volatile("red.relaxed.sys.global.max.s32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    case DDSK_RED_MIN: asm volatile("red.relaxed.sys.global.min.s32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    case DDSK_RED_AND: asm volatile("red.relaxed.sys.global.and.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    case DDSK_RED_OR: asm volatile("red.relaxed.sys.global.or.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    default: asm volatile("red.relaxed.sys.global.xor.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    }
+}
+__device__ __forceinline__ void red_i64(char *d, uint64_t v, int op) {
+    switch (op) {
+    case DDSK_RED_MAX: asm volatile("red.relaxed.sys.global.max.s64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    case DDSK_RED_MIN: asm volatile("red.relaxed.sys.global.min.s64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    case DDSK_RED_AND: asm volatile("red.relaxed.sys.global.and.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    case DDSK_RED_OR: asm volatile("red.relaxed.sys.global.or.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    default: asm volatile("red.relaxed.sys.global.xor.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    }
+}
+__device__ __forceinline__ uint32_t atom_i32(char *d, uint32_t v, int op) {
+    uint32_t o;
+    switch (op) {
+    case DDSK_RED_MAX: asm volatile("atom.relaxed.sys.global.max.s32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    case DDSK_RED_MIN: asm volatile("atom.relaxed.sys.global.min.s32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    case DDSK_RED_AND: asm volatile("atom.relaxed.sys.global.and.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    case DDSK_RED_OR: asm volatile("atom.relaxed.sys.global.or.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    default: asm volatile("atom.relaxed.sys.global.xor.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    }
+    return o;
+}
+__device__ __forceinline__ uint64_t atom_i64(char *d, uint64_t v, int op) {
+    uint64_t o;
+    switch (op) {
+    case DDSK_RED_MAX: asm volatile("atom.relaxed.sys.global.max.s64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    case DDSK_RED_MIN: asm volatile("atom.relaxed.sys.global.min.s64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    case DDSK_RED_AND: asm volatile("atom.relaxed.sys.global.and.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    case DDSK_RED_OR: asm volatile("atom.relaxed.sys.global.or.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    default: asm volatile("atom.relaxed.sys.global.xor.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    }
+    return o;
+}
+// the bulk reduction (tma_red_add_1d's rules) of op; red_bulk(t, op) holds
+__device__ __forceinline__ void tma_red_1d(void *dst_gmem, uint32_t src_smem, uint32_t bytes, int t, int op) {
+#define DDSK_BULK_RED(OPT)                                                                                                     \
+    asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group." OPT " [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), \
+                 "r"(bytes)                                                                                                    \
+                 : "memory")
+    const bool w64 = t == DDSK_ACC_I64;
+    switch (op) {
+    case DDSK_RED_SUM: tma_red_add_1d(dst_gmem, src_smem, bytes, t); break;
+    case DDSK_RED_MAX:
+        if (t == DDSK_ACC_I32) DDSK_BULK_RED("max.s32");
+        else if (t == DDSK_ACC_I64) DDSK_BULK_RED("max.s64");
+        else if (t == DDSK_ACC_F16) DDSK_BULK_RED("max.f16");
+        else DDSK_BULK_RED("max.bf16");
+        break;
+    case DDSK_RED_MIN:
+        if (t == DDSK_ACC_I32) DDSK_BULK_RED("min.s32");
+        else if (t == DDSK_ACC_I64) DDSK_BULK_RED("min.s64");
+        else if (t == DDSK_ACC_F16) DDSK_BULK_RED("min.f16");
+        else DDSK_BULK_RED("min.bf16");
+        break;
+    case DDSK_RED_AND:
+        if (w64) DDSK_BULK_RED("and.b64");
+        else DDSK_BULK_RED("and.b32");
+        break;
+    case DDSK_RED_OR:
+        if (w64) DDSK_BULK_RED("or.b64");
+        else DDSK_BULK_RED("or.b32");
+        break;
+    default:
+        if (w64) DDSK_BULK_RED("xor.b64");
+        else DDSK_BULK_RED("xor.b32");
+        break;
+    }
+#undef DDSK_BULK_RED
+}
+// one element at d (red_add1's rules) of op
+__device__ __forceinline__ void red1(char *d, uint32_t s, int t, int op) {
+    if (op == DDSK_RED_SUM) return red_add1(d, s, t);
+    const bool mx = op == DDSK_RED_MAX;
+    switch (t) {
+    case DDSK_ACC_I32: red_i32(d, lds32(s), op); break;
+    case DDSK_ACC_I64: red_i64(d, lds64(s), op); break;
+    case DDSK_ACC_F32: fmm32(d, lds32(s), mx); break;
+    case DDSK_ACC_F64: fmm64(d, lds64(s), mx); break;
+    default: {
+        const uint32_t sh = ((uint32_t)(uint64_t)d & 2u) * 8u;
+        fmm_word((char *)((uint64_t)d & ~(uint64_t)3), (uint32_t)lds16h(s) << sh, 0xFFFFu << sh, t == DDSK_ACC_BF16, mx);
+        break;
+    }
+    }
+}
+// 16 bytes at a 16-byte aligned d (red_add16's rules) of op
+__device__ __forceinline__ void red16(char *d, uint4 v, int t, int op) {
+    if (op == DDSK_RED_SUM) return red_add16(d, v, t);
+    const bool mx = op == DDSK_RED_MAX;
+    switch (t) {
+    case DDSK_ACC_I32:
+        red_i32(d, v.x, op);
+        red_i32(d + 4, v.y, op);
+        red_i32(d + 8, v.z, op);
+        red_i32(d + 12, v.w, op);
+        break;
+    case DDSK_ACC_I64:
+        red_i64(d, (uint64_t)v.y << 32 | v.x, op);
+        red_i64(d + 8, (uint64_t)v.w << 32 | v.z, op);
+        break;
+    case DDSK_ACC_F32:
+        fmm32(d, v.x, mx);
+        fmm32(d + 4, v.y, mx);
+        fmm32(d + 8, v.z, mx);
+        fmm32(d + 12, v.w, mx);
+        break;
+    case DDSK_ACC_F64:
+        fmm64(d, (uint64_t)v.y << 32 | v.x, mx);
+        fmm64(d + 8, (uint64_t)v.w << 32 | v.z, mx);
+        break;
+    case DDSK_ACC_F16:
+        if (mx) asm volatile("red.relaxed.sys.global.max.noftz.v4.f16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        else asm volatile("red.relaxed.sys.global.min.noftz.v4.f16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        break;
+    default:
+        if (mx) asm volatile("red.relaxed.sys.global.max.noftz.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        else asm volatile("red.relaxed.sys.global.min.noftz.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        break;
+    }
+}
+// the fetch forms: fop1's and fop16's contracts, of op
+__device__ __forceinline__ void rfop1(char *d, uint32_t s, int t, int op) {
+    const bool mx = op == DDSK_RED_MAX;
+    switch (t) {
+    case DDSK_ACC_I32: sts32(s, atom_i32(d, lds32(s), op)); break;
+    case DDSK_ACC_I64: sts64(s, atom_i64(d, lds64(s), op)); break;
+    case DDSK_ACC_F32: sts32(s, fmm32(d, lds32(s), mx)); break;
+    case DDSK_ACC_F64: sts64(s, fmm64(d, lds64(s), mx)); break;
+    default: {
+        const uint32_t sh = ((uint32_t)(uint64_t)d & 2u) * 8u;
+        sts16(s, fmm_word((char *)((uint64_t)d & ~(uint64_t)3), (uint32_t)lds16h(s) << sh, 0xFFFFu << sh, t == DDSK_ACC_BF16,
+                          mx) >> sh);
+        break;
+    }
+    }
+}
+__device__ __forceinline__ uint4 rfop16(char *d, uint4 v, int t, int op) {
+    const bool mx = op == DDSK_RED_MAX;
+    uint4 o;
+    switch (t) {
+    case DDSK_ACC_I32:
+        o = make_uint4(atom_i32(d, v.x, op), atom_i32(d + 4, v.y, op), atom_i32(d + 8, v.z, op), atom_i32(d + 12, v.w, op));
+        break;
+    case DDSK_ACC_I64: {
+        const uint64_t a = atom_i64(d, (uint64_t)v.y << 32 | v.x, op), b = atom_i64(d + 8, (uint64_t)v.w << 32 | v.z, op);
+        o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+        break;
+    }
+    case DDSK_ACC_F32: o = make_uint4(fmm32(d, v.x, mx), fmm32(d + 4, v.y, mx), fmm32(d + 8, v.z, mx), fmm32(d + 12, v.w, mx)); break;
+    case DDSK_ACC_F64: {
+        const uint64_t a = fmm64(d, (uint64_t)v.y << 32 | v.x, mx), b = fmm64(d + 8, (uint64_t)v.w << 32 | v.z, mx);
+        o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+        break;
+    }
+    case DDSK_ACC_F16:
+        if (mx)
+            asm volatile("atom.relaxed.sys.global.max.noftz.v4.f16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                         : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w) : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        else
+            asm volatile("atom.relaxed.sys.global.min.noftz.v4.f16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                         : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w) : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        break;
+    default:
+        if (mx)
+            asm volatile("atom.relaxed.sys.global.max.noftz.v4.bf16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                         : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w) : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        else
+            asm volatile("atom.relaxed.sys.global.min.noftz.v4.bf16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                         : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w) : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+        break;
+    }
+    return o;
+}
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
     unsigned int v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -729,6 +970,7 @@ struct GatherArgs {
             char *fop_result;        // FETCH: the previous values, at the operands' positions (the layout of dst)
             const char *fop_compare; // kFopCas: the compare operands, at the operands' positions
             int fop_el;              // kFopCas: log2 of the element size (0..3; acc_type does not apply)
+            int acc_op;              // ACC, and FETCH's kFopAdd: DDSK_RED_SUM or another reduction (warp-uniform)
         };
     };
     int min_seg_chunks;                // smallest segment, in chunks (claims cost more when the plan is in global memory)
@@ -1105,9 +1347,10 @@ struct ChunkWalker {
 // Re-phase loop: output vector j = staged bytes [q16 + 16j + 4*WS + bs, +16). Specialised on the word shift WS
 // (and on whether a sub-word byte shift is needed at all) so the loop body is branch-free: two aligned 128-bit
 // shared loads, at most four funnel shifts, one aligned 128-bit global store.
-// ACC: the vector is added to the destination's (red_add16 of element type acc_t) instead of stored.
+// ACC: the vector is reduced into the destination's (red16 of element type acc_t and reduction acc_op) instead of stored.
 template <int WS, bool BYTES, bool ACC = false>
-__device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t nv, uint32_t bs8, int lane, int acc_t = 0) {
+__device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t nv, uint32_t bs8, int lane, int acc_t = 0,
+                                             int acc_op = 0) {
 #pragma unroll 4
     for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
         const uint4 lo = lds128(sbase + (j << 4));
@@ -1125,7 +1368,7 @@ __device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t 
             out.z = w[WS + 2];
             out.w = w[WS + 3];
         }
-        if constexpr (ACC) red_add16(dv + ((size_t)j << 4), out, acc_t);
+        if constexpr (ACC) red16(dv + ((size_t)j << 4), out, acc_t, acc_op);
         else stg128(dv + ((size_t)j << 4), out);
     }
 }
@@ -1136,7 +1379,7 @@ __device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t 
 // (rephase_loop is not shared: the existing instantiations' register allocation changed when it was.)
 template <int WS, bool BYTES>
 __device__ __forceinline__ void fop_rephase_loop(uint32_t sbase, uint32_t s, char *dv, uint32_t nv, uint32_t bs8, int lane, int t,
-                                                 bool swap) {
+                                                 bool swap, int op) {
 #pragma unroll 4
     for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
         const uint4 lo = lds128(sbase + (j << 4));
@@ -1151,7 +1394,7 @@ __device__ __forceinline__ void fop_rephase_loop(uint32_t sbase, uint32_t s, cha
         } else {
             v = make_uint4(w[WS + 0], w[WS + 1], w[WS + 2], w[WS + 3]);
         }
-        const uint4 o = fop16(dv + ((size_t)j << 4), v, t, swap);
+        const uint4 o = op == DDSK_RED_SUM ? fop16(dv + ((size_t)j << 4), v, t, swap) : rfop16(dv + ((size_t)j << 4), v, t, op);
         const uint32_t p = s + (j << 4);
         if (!BYTES && WS == 0) {
             sts128(p, o);
@@ -1209,11 +1452,12 @@ __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, ui
     }
 }
 
-// The accumulate's drain_chunk: the same three cases with every store an atomic add of element type t (DDSK_ACC_*).
-// Same phase: lane 0 bulk-reduces the body. Different phase: re-phased vectors, each reduced (red_add16). The head and
-// tail, below 16 bytes, are reduced element by element by the first lanes. A piece never cuts an element and the
-// caller's rows are element-aligned (see cvt_in_log2), so head, body and tail are whole, aligned elements.
-__device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t) {
+// The accumulate's drain_chunk: the same three cases with every store an atomic reduction op (DDSK_RED_*: the add, or
+// another) of element type t (DDSK_ACC_*). Same phase: lane 0 bulk-reduces the body, if the op has a bulk form for t
+// (red_bulk). Different phase, or no bulk form: re-phased vectors, each reduced (red16). The head and tail, below 16
+// bytes, are reduced element by element by the first lanes (red1). A piece never cuts an element and the caller's rows
+// are element-aligned (see cvt_in_log2), so head, body and tail are whole, aligned elements.
+__device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t, int op) {
     const uint32_t el = (uint32_t)DDSK_ACC_LOG2(t);
     uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
     if (head > n) head = n;
@@ -1222,30 +1466,31 @@ __device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d
     uint32_t s = a + head;
     uint32_t sh = s & 15u;
     if (nv) {
-        if (sh == 0) {
+        if (sh == 0 && red_bulk(t, op)) {
             if (lane == 0) {
                 fence_proxy_async();
-                tma_red_add_1d(d + head, sb + s, nv << 4, t);
+                tma_red_1d(d + head, sb + s, nv << 4, t, op);
             }
         } else {
             const uint32_t sbase = sb + (s & ~15u);
             const uint32_t bs8 = (sh & 3u) * 8u;
             char *dv = d + head;
             switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform (2-byte elements: bs8 is 0 or 16)
-            case 1: rephase_loop<0, true, true>(sbase, dv, nv, bs8, lane, t); break;
-            case 2: rephase_loop<1, false, true>(sbase, dv, nv, bs8, lane, t); break;
-            case 3: rephase_loop<1, true, true>(sbase, dv, nv, bs8, lane, t); break;
-            case 4: rephase_loop<2, false, true>(sbase, dv, nv, bs8, lane, t); break;
-            case 5: rephase_loop<2, true, true>(sbase, dv, nv, bs8, lane, t); break;
-            case 6: rephase_loop<3, false, true>(sbase, dv, nv, bs8, lane, t); break;
-            default: rephase_loop<3, true, true>(sbase, dv, nv, bs8, lane, t); break;
+            case 0: rephase_loop<0, false, true>(sbase, dv, nv, bs8, lane, t, op); break; // (no bulk form)
+            case 1: rephase_loop<0, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
+            case 2: rephase_loop<1, false, true>(sbase, dv, nv, bs8, lane, t, op); break;
+            case 3: rephase_loop<1, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
+            case 4: rephase_loop<2, false, true>(sbase, dv, nv, bs8, lane, t, op); break;
+            case 5: rephase_loop<2, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
+            case 6: rephase_loop<3, false, true>(sbase, dv, nv, bs8, lane, t, op); break;
+            default: rephase_loop<3, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
             }
         }
     }
-    if ((uint32_t)lane < (head >> el)) red_add1(d + ((uint32_t)lane << el), sb + a + ((uint32_t)lane << el), t);
+    if ((uint32_t)lane < (head >> el)) red1(d + ((uint32_t)lane << el), sb + a + ((uint32_t)lane << el), t, op);
     if ((uint32_t)lane < (tail >> el)) {
         const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
-        red_add1(d + k, sb + a + k, t);
+        red1(d + k, sb + a + k, t, op);
     }
 }
 
@@ -1253,8 +1498,9 @@ __device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d
 // element is combined with the shard's by a returning atomic (fop1 / fop16) in the shard's 16-byte phase -- the head and
 // tail element by element, the body as 16-byte vectors re-phased like acc_drain_chunk's -- and its previous value replaces
 // the operand in the stage. (No bulk form returns the old values.) The caller then drains the stage to the result with
-// the raw drain. Head, body and tail are whole, aligned elements, as in acc_drain_chunk.
-__device__ __forceinline__ void fop_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t, bool swap) {
+// the raw drain. Head, body and tail are whole, aligned elements, as in acc_drain_chunk. op: DDSK_RED_SUM for the add
+// and the swap, else the reduction (rfop1 / rfop16).
+__device__ __forceinline__ void fop_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t, bool swap, int op) {
     const uint32_t el = (uint32_t)DDSK_ACC_LOG2(t);
     uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
     if (head > n) head = n;
@@ -1267,20 +1513,25 @@ __device__ __forceinline__ void fop_chunk(uint32_t sb, uint32_t a, char *d, uint
         const uint32_t bs8 = (sh & 3u) * 8u;
         char *dv = d + head;
         switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform (2-byte elements: bs8 is 0 or 16)
-        case 0: fop_rephase_loop<0, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
-        case 1: fop_rephase_loop<0, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
-        case 2: fop_rephase_loop<1, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
-        case 3: fop_rephase_loop<1, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
-        case 4: fop_rephase_loop<2, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
-        case 5: fop_rephase_loop<2, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
-        case 6: fop_rephase_loop<3, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
-        default: fop_rephase_loop<3, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap); break;
+        case 0: fop_rephase_loop<0, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
+        case 1: fop_rephase_loop<0, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
+        case 2: fop_rephase_loop<1, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
+        case 3: fop_rephase_loop<1, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
+        case 4: fop_rephase_loop<2, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
+        case 5: fop_rephase_loop<2, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
+        case 6: fop_rephase_loop<3, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
+        default: fop_rephase_loop<3, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
         }
     }
-    if ((uint32_t)lane < (head >> el)) fop1(d + ((uint32_t)lane << el), sb + a + ((uint32_t)lane << el), t, swap);
+    if ((uint32_t)lane < (head >> el)) {
+        const uint32_t k = (uint32_t)lane << el;
+        if (op == DDSK_RED_SUM) fop1(d + k, sb + a + k, t, swap);
+        else rfop1(d + k, sb + a + k, t, op);
+    }
     if ((uint32_t)lane < (tail >> el)) {
         const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
-        fop1(d + k, sb + a + k, t, swap);
+        if (op == DDSK_RED_SUM) fop1(d + k, sb + a + k, t, swap);
+        else rfop1(d + k, sb + a + k, t, op);
     }
 }
 
@@ -1796,9 +2047,10 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // zero. The load reads the 16-byte-aligned superset of the piece's range in the caller's buffer: up to 15 bytes on
 // either side that belong to no request, in the same 16-byte block (which never crosses a page), whose values are
 // discarded. Never overlapped, no offsets, no conversion, no push.
-// ACC (with PUT): a batched accumulate (DDSK_F_ACC) -- the put whose drain adds instead of storing, in the element type
-// a.acc_type: bulk reductions where the put bulk-stores, element reductions for the ragged ends, vector reductions of
-// the re-phased body. Each is atomic per element, so requests of any batch or rank that hit the same element combine.
+// ACC (with PUT): a batched accumulate (DDSK_F_ACC) -- the put whose drain adds (or reduces by a.acc_op) instead of
+// storing, in the element type a.acc_type: bulk reductions where the put bulk-stores (and the op has a bulk form),
+// element reductions for the ragged ends, vector reductions of the re-phased body. Each is atomic per element, so
+// requests of any batch or rank that hit the same element combine.
 // FETCH (with PUT): a batched fetch-op (DDSK_F_FOP) -- the put whose drain applies a returning atomic (add, swap or
 // compare-and-swap, a.fop_op; add and swap in the element type a.acc_type, compare-and-swap on 1 << a.fop_el bytes) to
 // every element and sends the previous values to a.fop_result, at the operands' positions. Every piece is drained
@@ -2162,7 +2414,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                               a.fop_compare + (r - (uint64_t)a.fop_result), n, lane, (uint32_t)a.fop_el);
                 } else {
                     fop_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type,
-                              a.fop_op == kFopSwap);
+                              a.fop_op == kFopSwap, a.acc_op);
                 }
             }
             fence_proxy_async(); // (every lane: its stage writes, before any lane's bulk store reads them)
@@ -2182,9 +2434,10 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             // put: the raw drain (the last branch) into the shard address the descriptor carries -- a branch of its own,
             // so that the raw instantiations compile exactly as they did
             char *const my_dst = (char *)my_dpos;
-            const bool direct = my_n != 0 && (((uint32_t)(uint64_t)my_dst | my_n | (my_pack >> 16)) & 15u) == 0;
+            bool direct = my_n != 0 && (((uint32_t)(uint64_t)my_dst | my_n | (my_pack >> 16)) & 15u) == 0;
             if constexpr (ACC) {
-                if (direct) tma_red_add_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n, a.acc_type);
+                direct = direct && red_bulk(a.acc_type, a.acc_op);
+                if (direct) tma_red_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n, a.acc_type, a.acc_op);
             } else {
                 if (direct) tma_store_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n);
             }
@@ -2195,7 +2448,8 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
                 const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
                 const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
-                if constexpr (ACC) acc_drain_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type);
+                if constexpr (ACC)
+                    acc_drain_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type, a.acc_op);
                 else drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane);
             }
         } else if constexpr (CVT) {
@@ -2899,7 +3153,10 @@ int gather_args(GatherArgs &a, const ddsk_var_t *var, const ddsk_scratch_t *scr,
     // GPU either); the variable-count entries set the slot's own word below (their CTAs
     // may start late, behind the plan kernel, and must not keep a fixed share of the work).
     a.tickets = a.overlap ? nullptr : scr->counters;
-    if (flags & (DDSK_F_ACC | DDSK_F_FOP)) a.acc_type = DDSK_F_ACC_TYPE(flags);
+    if (flags & (DDSK_F_ACC | DDSK_F_FOP)) {
+        a.acc_type = DDSK_F_ACC_TYPE(flags);
+        a.acc_op = DDSK_F_RED_OP(flags);
+    }
     if (flags & DDSK_F_FOP) {
         a.fop_op = (flags & DDSK_F_FOP_CAS) ? kFopCas : (flags & DDSK_F_FOP_SWAP) ? kFopSwap : kFopAdd;
         a.fop_result = (char *)scr->fop_result;

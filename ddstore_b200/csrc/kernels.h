@@ -93,6 +93,19 @@ typedef struct ddsk_scratch {
 #define DDSK_F_FOP_CAS 32768  /* with DDSK_F_FOP: the op is a compare-and-swap (shard = src where shard == compare, bit for
                                  bit, at the same position of scr->fop_compare). Bits 10..12 of the flags then hold log2 of
                                  the element size (0..3), not an element type; src, compare and result are aligned to it. */
+#define DDSK_F_RED_SHIFT 16   /* bits 16..19 of the flags, with DDSK_F_ACC or DDSK_F_FOP (not swap, not compare-and-swap):
+                                 the reduction (DDSK_RED_*); 0 is the sum */
+#define DDSK_F_RED_OP(f) (((f) >> DDSK_F_RED_SHIFT) & 15)
+
+/* reductions of an accumulate or a fetch-op beside the sum (same values as DDS_OP_MAX.. in include/ddstore_b200.h). Max
+ * and min compare integers as signed and floats by IEEE 754-2019 maximumNumber / minimumNumber with -0 < +0; the bitwise
+ * ops take the integer types only. */
+#define DDSK_RED_SUM 0
+#define DDSK_RED_MAX 4
+#define DDSK_RED_MIN 5
+#define DDSK_RED_AND 6
+#define DDSK_RED_OR 7
+#define DDSK_RED_XOR 8
 
 /* element types of an accumulate (same values as DDS_ACC_* in include/ddstore_b200.h) */
 #define DDSK_ACC_F32 1

@@ -1717,6 +1717,8 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
 // op: 0, or a DDS_OP_* for the fetch-op behind dds_get_accumulate_batch / dds_get_accumulate_samples (with acc its element
 // type): the same launch whose drain applies a returning atomic and writes the previous rows to `result`, in the layout
 // of src (DDSK_F_FOP). result must be aligned to the element size too.
+// red: DDSK_RED_SUM, or the reduction (DDS_OP_MAX..) of an accumulate (result null: dds_accumulate_op_*) or of a fetch-op
+// (op == red), carried in the launch flags' DDSK_F_RED bits.
 // op OP_CAS (acc 0): the compare-and-swap behind dds_compare_and_swap_batch / dds_compare_and_swap_samples, the fetch-op
 // launch whose drain swaps where the shard equals `compare` (the layout of src; DDSK_F_FOP_CAS) on elements of the
 // variable's itemsize. src and compare must be aligned to it too.
@@ -1724,7 +1726,7 @@ static constexpr int OP_CAS = 3; // (put_impl's own op code, beside the DDS_OP_*
 static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
                     int64_t fixed_count, int64_t nreq, const void *src, int64_t src_bytes, unsigned flags,
                     void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, int acc = 0, int op = 0,
-                    void *result = nullptr, const void *compare = nullptr) {
+                    void *result = nullptr, const void *compare = nullptr, int red = DDSK_RED_SUM) {
     if (!(flags & DDS_SRC_ON_DEVICE)) return fail(DDS_ERR_ARG, "puts take their rows from device memory (DDS_SRC_ON_DEVICE)");
     if (nreq < 0 || src_bytes < 0) return fail(DDS_ERR_ARG, "negative nreq or src_bytes");
     if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
@@ -1765,10 +1767,11 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
         scr.fop_result = result;
         scr.fop_compare = compare;
     } else if (op) {
-        kflags |= DDSK_F_PUT | DDSK_F_FOP | acc << DDSK_F_ACC_SHIFT | (op == DDS_OP_REPLACE ? DDSK_F_FOP_SWAP : 0);
+        kflags |= DDSK_F_PUT | DDSK_F_FOP | acc << DDSK_F_ACC_SHIFT | (op == DDS_OP_REPLACE ? DDSK_F_FOP_SWAP : 0) |
+                  red << DDSK_F_RED_SHIFT;
         scr.fop_result = result;
     } else {
-        kflags |= DDSK_F_PUT | (acc ? DDSK_F_ACC | acc << DDSK_F_ACC_SHIFT : 0);
+        kflags |= DDSK_F_PUT | (acc ? DDSK_F_ACC | acc << DDSK_F_ACC_SHIFT | red << DDSK_F_RED_SHIFT : 0);
     }
     const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st)
                           : ddsk_gather_var(&v->kv, &ix, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st);
@@ -1808,30 +1811,56 @@ static int acc_entry(dds_store_t *s, const char *name, int dtype, int64_t *total
     return DDS_OK;
 }
 
+static_assert(DDS_OP_MAX == DDSK_RED_MAX && DDS_OP_MIN == DDSK_RED_MIN && DDS_OP_BAND == DDSK_RED_AND &&
+                  DDS_OP_BOR == DDSK_RED_OR && DDS_OP_BXOR == DDSK_RED_XOR,
+              "the kernels' reductions are the public ops");
+
+// The reductions' and fetch-ops' prologue: the accumulates', then an unknown op (fetch: DDS_OP_REPLACE is an op; not
+// fetch: it is not, a put writes rows), then a bitwise op on a float dtype. *red: the kernels' reduction (DDSK_RED_SUM for
+// the sum and the swap).
+static int fop_entry(dds_store_t *s, const char *name, int op, int dtype, int64_t *total_bytes, int64_t *bad_index,
+                     Var **v, bool fetch = true, int *red = nullptr) {
+    if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, v)) return rc;
+    if (!(op == DDS_OP_SUM || (fetch && op == DDS_OP_REPLACE) || (op >= DDS_OP_MAX && op <= DDS_OP_BXOR)))
+        return fail(DDS_ERR_ARG, fetch ? "unknown fetch-op" : "unknown accumulate op");
+    if (op >= DDS_OP_BAND && dtype != DDS_ACC_I32 && dtype != DDS_ACC_I64)
+        return fail(DDS_ERR_ARG, "bitwise ops take DDS_ACC_I32 or DDS_ACC_I64");
+    if (red) *red = op >= DDS_OP_MAX ? op : DDSK_RED_SUM;
+    return DDS_OK;
+}
+
+int dds_accumulate_op_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                            int64_t fixed_count, int64_t nreq, int op, int dtype, const void *src, int64_t src_bytes,
+                            unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    Var *v;
+    int red;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, false, &red)) return rc;
+    return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
+                    bad_index, dtype, 0, nullptr, nullptr, red);
+}
+
+int dds_accumulate_op_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
+                              int dtype, const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream,
+                              int64_t *total_bytes, int64_t *bad_index) {
+    Var *v;
+    int red;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, false, &red)) return rc;
+    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
+                    dtype, 0, nullptr, nullptr, red);
+}
+
 int dds_accumulate_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
                          int64_t fixed_count, int64_t nreq, int dtype, const void *src, int64_t src_bytes, unsigned flags,
                          void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
-    Var *v;
-    if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, &v)) return rc;
-    return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
-                    bad_index, dtype);
+    return dds_accumulate_op_batch(s, name, starts, counts, fixed_count, nreq, DDS_OP_SUM, dtype, src, src_bytes, flags,
+                                   cuda_stream, total_bytes, bad_index);
 }
 
 int dds_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int dtype,
                            const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                            int64_t *bad_index) {
-    Var *v;
-    if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, &v)) return rc;
-    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
-                    dtype);
-}
-
-// The fetch-ops' prologue: the accumulates' and an unknown op
-static int fop_entry(dds_store_t *s, const char *name, int op, int dtype, int64_t *total_bytes, int64_t *bad_index,
-                     Var **v) {
-    if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, v)) return rc;
-    if (op != DDS_OP_SUM && op != DDS_OP_REPLACE) return fail(DDS_ERR_ARG, "unknown fetch-op");
-    return DDS_OK;
+    return dds_accumulate_op_samples(s, name, sample_ids, nreq, DDS_OP_SUM, dtype, src, src_bytes, flags, cuda_stream,
+                                     total_bytes, bad_index);
 }
 
 int dds_get_accumulate_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
@@ -1839,18 +1868,20 @@ int dds_get_accumulate_batch(dds_store_t *s, const char *name, const int64_t *st
                              int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                              int64_t *bad_index) {
     Var *v;
-    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v)) return rc;
+    int red;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, true, &red)) return rc;
     return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
-                    bad_index, dtype, op, result);
+                    bad_index, dtype, op, result, nullptr, red);
 }
 
 int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
                                int dtype, const void *src, void *result, int64_t src_bytes, unsigned flags,
                                void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
     Var *v;
-    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v)) return rc;
+    int red;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, true, &red)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
-                    dtype, op, result);
+                    dtype, op, result, nullptr, red);
 }
 
 // The compare-and-swaps' prologue: entry_var, an itemsize outside {1, 2, 4, 8} (an argument error) and then one other

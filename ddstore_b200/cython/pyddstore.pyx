@@ -59,6 +59,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
         long accumulate_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                               int dtype, const void* src, long src_bytes, cbool idx_on_device,
                               void* stream) except +dds_translate_exception
+        long accumulate_op_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
+                                 int op, int dtype, const void* src, long src_bytes, cbool idx_on_device,
+                                 void* stream) except +dds_translate_exception
         long get_accumulate_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                                   int op, int dtype, const void* src, void* result, long src_bytes, cbool idx_on_device,
                                   void* stream) except +dds_translate_exception
@@ -78,6 +81,8 @@ cdef extern from "ddstore_b200.hpp" nogil:
 _ACC_TYPES = {"float32": 1, "float64": 2, "int32": 3, "int64": 4, "float16": 5, "bfloat16": 6}
 # ops of get_accumulate_batch (DDS_OP_*), by name
 _FOP_OPS = {"sum": 1, "replace": 2}
+# reductions of accumulate_batch and get_accumulate_batch beside the sum (DDS_OP_MAX..), by torch's names
+_RED_OPS = {"amax": 4, "amin": 5, "bitwise_and": 6, "bitwise_or": 7, "bitwise_xor": 8}
 
 cdef class PyDDStore:
     cdef DDStore* c_ddstore
@@ -305,10 +310,11 @@ cdef class PyDDStore:
         del keep
         return total
 
-    def accumulate_batch(self, str name, starts, counts=None, src=None, count=None, stream=None):
-        """one kernel launch ADDING len(starts) requests of the CUDA tensor `src` into the owners' shards, in src's dtype
-        (float32, float64, int32, int64, float16 or bfloat16); see ddstore_b200.store.PyDDStore.accumulate_batch (this
-        binding's accumulate is synchronous). Returns the layout's bytes."""
+    def accumulate_batch(self, str name, starts, counts=None, src=None, count=None, stream=None, op="sum"):
+        """one kernel launch ADDING (or reducing by op: "amax", "amin", "bitwise_and", "bitwise_or", "bitwise_xor")
+        len(starts) requests of the CUDA tensor `src` into the owners' shards, in src's dtype (float32, float64, int32,
+        int64, float16 or bfloat16); see ddstore_b200.store.PyDDStore.accumulate_batch (this binding's accumulate is
+        synchronous). Returns the layout's bytes."""
         if src is None:
             raise ValueError("an accumulate needs `src` rows")
         if not (hasattr(src, "data_ptr") and getattr(src, "is_cuda", False)):
@@ -318,7 +324,10 @@ cdef class PyDDStore:
         dt = str(src.dtype).replace("torch.", "")
         if dt not in _ACC_TYPES:
             raise ValueError(f"accumulate into {name!r}: src dtype {dt} is not one of {', '.join(_ACC_TYPES)}")
-        cdef int code = _ACC_TYPES[dt]
+        ops = {"sum": 1, **_RED_OPS}
+        if op not in ops:
+            raise ValueError(f"accumulate into {name!r}: op {op!r} is not one of {', '.join(ops)}")
+        cdef int code = _ACC_TYPES[dt], opc = ops[op]
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
         cdef size_t sp, cp = 0, dp = src.data_ptr()
         cdef long nreq
@@ -340,15 +349,15 @@ cdef class PyDDStore:
         cdef cbool idx_dev = bool(s_dev)
         cdef long total
         with nogil:
-            total = self.c_ddstore.accumulate_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, code,
-                                                    <const void*> dp, nbytes, idx_dev, <void*> st)
+            total = self.c_ddstore.accumulate_op_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, opc, code,
+                                                       <const void*> dp, nbytes, idx_dev, <void*> st)
         del keep
         return total
 
     def get_accumulate_batch(self, str name, starts, counts=None, src=None, out=None, op="sum", count=None,
                              stream=None):
-        """one kernel launch ADDING (op="sum") or SWAPPING (op="replace") len(starts) requests of the CUDA tensor `src`
-        into the owners' shards and writing the previous rows to the CUDA tensor `out` (src's layout, at least its
+        """one kernel launch ADDING (op="sum"), SWAPPING (op="replace") or reducing (accumulate_batch's ops) len(starts)
+        requests of the CUDA tensor `src` into the owners' shards and writing the previous rows to the CUDA tensor `out` (src's layout, at least its
         bytes; it may be src); see ddstore_b200.store.PyDDStore.get_accumulate_batch (this binding's fetch-op is
         synchronous). Returns the layout's bytes."""
         if src is None:
@@ -362,12 +371,13 @@ cdef class PyDDStore:
         dt = str(src.dtype).replace("torch.", "")
         if dt not in _ACC_TYPES:
             raise ValueError(f"fetch-op on {name!r}: src dtype {dt} is not one of {', '.join(_ACC_TYPES)}")
-        if op not in _FOP_OPS:
-            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(_FOP_OPS)}")
+        ops = {**_FOP_OPS, **_RED_OPS}
+        if op not in ops:
+            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(ops)}")
         cdef long nbytes = src.numel() * src.element_size()
         if out.numel() * out.element_size() < nbytes:
             raise ValueError(f"fetch-op on {name!r}: out holds {out.numel() * out.element_size()} bytes, src {nbytes}")
-        cdef int code = _ACC_TYPES[dt], opc = _FOP_OPS[op]
+        cdef int code = _ACC_TYPES[dt], opc = ops[op]
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
         cdef size_t sp, cp = 0, dp = src.data_ptr(), rp = out.data_ptr()
         cdef long nreq

@@ -401,8 +401,8 @@ class PyDDStore:
         _capi.raise_for(rc)
         return total.value
 
-    # ---------------------------------------------------------------- batched accumulates (MPI_Accumulate, MPI_SUM)
-    def accumulate_batch(self, name, starts, counts=None, src=None, count=None, stream=None, wait=True):
+    # ---------------------------------------------------------------- batched accumulates (MPI_Accumulate)
+    def accumulate_batch(self, name, starts, counts=None, src=None, count=None, stream=None, wait=True, op="sum"):
         """ADD len(starts) requests into the owners' shards in ONE kernel launch: every element e of request i's rows
         becomes shard[e] + src[e]. Requests, the layout of `src`, errors (every valid request is still applied, an
         invalid one changes nothing), wait=False, ordering and visibility are put_batch's. The sum is taken in
@@ -410,9 +410,15 @@ class PyDDStore:
         (another dtype raises ValueError before the call). Accumulates into the same element in one epoch combine
         atomically, from any batch, rank or duplicate request: integers exactly (wrapping), floats with one rounding per
         addition in an unspecified order (float32 may flush subnormals to zero). Mixing puts and accumulates on the same
-        rows in one epoch, or reading rows being accumulated, is undefined. Returns the layout's size in bytes."""
+        rows in one epoch, or reading rows being accumulated, is undefined. Returns the layout's size in bytes.
+        op="amax" / "amin" makes each element max(shard[e], src[e]) / min(...) instead -- signed for the integer types,
+        IEEE maximumNumber / minimumNumber for floats (a NaN operand is ignored, -0 < +0, nothing flushes) -- and
+        "bitwise_and" / "bitwise_or" / "bitwise_xor" (int32 and int64 src only) its bitwise combination with src[e].
+        Reductions with the same op and dtype on one element in one epoch combine atomically, also with
+        get_accumulate_batch's; mixing different ops on one element in one epoch is undefined."""
         sb, keep_src = self._put_src(name, src)
         code = self._acc_type(name, src)
+        opc = self._red_op(name, op)
         s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
         if s_dev:
             nreq, sp = starts.numel(), starts.data_ptr()
@@ -425,19 +431,20 @@ class PyDDStore:
             keep = (sa, ca)
         flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
         total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_accumulate_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
-                                          code, sb.ptr, sb.nbytes, flags, self._stream_arg(stream), C.byref(total),
-                                          C.byref(bad))
+        rc = self._L.dds_accumulate_op_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
+                                             opc, code, sb.ptr, sb.nbytes, flags, self._stream_arg(stream),
+                                             C.byref(total), C.byref(bad))
         del keep, keep_src
         self.last_bad_index = bad.value
         _capi.raise_for(rc)
         return total.value
 
-    def accumulate_samples(self, name, sample_ids, src, stream=None, wait=True):
-        """accumulate_batch by SAMPLE ID: request i adds into the rows of sample sample_ids[i] in the index registered
-        with set_sample_index. Layout and errors as put_samples, sums as accumulate_batch."""
+    def accumulate_samples(self, name, sample_ids, src, stream=None, wait=True, op="sum"):
+        """accumulate_batch by SAMPLE ID: request i adds into (or reduces by op into) the rows of sample sample_ids[i]
+        in the index registered with set_sample_index. Layout and errors as put_samples, ops as accumulate_batch."""
         sb, keep_src = self._put_src(name, src)
         code = self._acc_type(name, src)
+        opc = self._red_op(name, op)
         s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
         if s_dev:
             nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
@@ -446,8 +453,8 @@ class PyDDStore:
             nreq, sp, keep = sa.size, sa.ctypes.data, sa
         flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
         total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_accumulate_samples(self._h, name.encode(), sp, nreq, code, sb.ptr, sb.nbytes, flags,
-                                            self._stream_arg(stream), C.byref(total), C.byref(bad))
+        rc = self._L.dds_accumulate_op_samples(self._h, name.encode(), sp, nreq, opc, code, sb.ptr, sb.nbytes, flags,
+                                               self._stream_arg(stream), C.byref(total), C.byref(bad))
         del keep, keep_src
         self.last_bad_index = bad.value
         _capi.raise_for(rc)
@@ -465,7 +472,9 @@ class PyDDStore:
         the layout are left as they were. Fetch-ops on one element in one epoch are linearisable, from any batch, rank
         or duplicate request: each gets the value right before its own contribution (duplicate +1 requests of one batch
         get distinct tickets). Sums also combine atomically with accumulate_batch; mixing "replace" with sums, puts or
-        accumulates on one element in one epoch is undefined. Returns the layout's size in bytes."""
+        accumulates on one element in one epoch is undefined. op may also be one of accumulate_batch's reductions
+        ("amax", "amin", "bitwise_and", "bitwise_or", "bitwise_xor"), which combine atomically with accumulate_batch's
+        of the same op. Returns the layout's size in bytes."""
         sb, keep_src = self._put_src(name, src)
         code = self._acc_type(name, src)
         opc, res = self._fop_args(name, op, out, sb)
@@ -591,8 +600,9 @@ class PyDDStore:
     def _fop_args(name, op, out, sb):
         """the DDS_OP_* code of a fetch-op and the address of its `out` tensor (ValueError for an unknown op, or an out
         that is not a contiguous CUDA tensor of at least src's bytes)"""
-        if op not in _capi.FOP_OPS:
-            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(_capi.FOP_OPS)}")
+        ops = {**_capi.FOP_OPS, **_capi.RED_OPS}
+        if op not in ops:
+            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(ops)}")
         if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)):
             raise ValueError(f"fetch-op on {name!r}: out must be a CUDA tensor")
         if not out.is_contiguous():
@@ -600,7 +610,15 @@ class PyDDStore:
         if out.numel() * out.element_size() < sb.nbytes:
             raise ValueError(f"fetch-op on {name!r}: out holds {out.numel() * out.element_size()} bytes, src "
                              f"{sb.nbytes}")
-        return _capi.FOP_OPS[op], out.data_ptr()
+        return ops[op], out.data_ptr()
+
+    @staticmethod
+    def _red_op(name, op):
+        """the DDS_OP_* code of an accumulate's reduction (ValueError for an unknown one)"""
+        ops = {"sum": _capi.OP_SUM, **_capi.RED_OPS}
+        if op not in ops:
+            raise ValueError(f"accumulate into {name!r}: op {op!r} is not one of {', '.join(ops)}")
+        return ops[op]
 
     @staticmethod
     def _acc_type(name, src):

@@ -27,8 +27,9 @@ extern "C" {
                            that built against 111 are unaffected, and a caller finds them by symbol. So do the batched
                            puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE), the batched accumulates
                            (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*), the batched fetch-ops
-                           (dds_get_accumulate_batch, dds_get_accumulate_samples, DDS_OP_*) and the batched
-                           compare-and-swaps (dds_compare_and_swap_batch, dds_compare_and_swap_samples). */
+                           (dds_get_accumulate_batch, dds_get_accumulate_samples, DDS_OP_*), the batched
+                           compare-and-swaps (dds_compare_and_swap_batch, dds_compare_and_swap_samples) and the batched
+                           reductions (dds_accumulate_op_batch, dds_accumulate_op_samples, DDS_OP_MAX & co.). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -373,6 +374,39 @@ int dds_get_accumulate_batch(dds_store_t *s, const char *name, const int64_t *st
 int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
                                int dtype, const void *src, void *result, int64_t src_bytes, unsigned flags,
                                void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+
+/* ---- batched reductions: max, min and bitwise ops into any rank's shard (the rest of MPI_Accumulate's predefined ops,
+ * MPI_MAX, MPI_MIN, MPI_BAND, MPI_BOR and MPI_BXOR, between fences). dds_accumulate_op_batch / dds_accumulate_op_samples
+ * take dds_accumulate_batch's / dds_accumulate_samples's arguments plus `op`, and every element e of request i's rows
+ * becomes op(shard[e], src[e]). They accept DDS_OP_SUM (exactly dds_accumulate_batch / _samples) and ops 4-8 below.
+ * dds_get_accumulate_batch / dds_get_accumulate_samples accept ops 4-8 too: result[e] = shard[e] in the same atomic step.
+ * Requests, the layout of src, validation, error reporting, flags, DDS_NO_SYNC queueing, fences, the result rules and the
+ * ignored DDS_OVERLAP are dds_accumulate_batch's / dds_get_accumulate_batch's, word for word.
+ * Allowed (op, dtype) pairs:
+ *   DDS_OP_MAX, DDS_OP_MIN: every DDS_ACC_* type. DDS_ACC_I32 / I64 compare as signed. Floats follow IEEE 754-2019
+ *     maximumNumber / minimumNumber with -0 < +0: a NaN operand is ignored, a NaN in the shard is replaced by a non-NaN
+ *     operand, NaN with NaN gives a NaN whose bits are unspecified. Nothing flushes: every result is the bits of one of
+ *     its inputs (or that NaN).
+ *   DDS_OP_BAND, DDS_OP_BOR, DDS_OP_BXOR: DDS_ACC_I32 and DDS_ACC_I64 only (on the bits of any 4- or 8-byte variable).
+ * Argument errors, with DDS_ERR_ARG and nothing enqueued, checked after the dtype's: an unknown op, DDS_OP_REPLACE given
+ * to dds_accumulate_op_* (a put writes rows), and a bitwise op with a float dtype.
+ * Concurrency: reductions on one element in one epoch with the same op and dtype combine atomically -- from any batch,
+ * any rank, or duplicate requests of one batch, through either entry family. The element ends at the op folded over its
+ * starting value and every contribution; these ops are commutative and associative, so that does not depend on the
+ * order (but for the bits of a NaN-with-NaN result). The fetch forms are linearisable per element, each result the value
+ * immediately before its own contribution. Mixing different ops, or reductions with puts or compare-and-swaps, on one
+ * element in one epoch is undefined, as in MPI. Rows are not atomic as a whole. */
+#define DDS_OP_MAX 4  /* shard[e] = max(shard[e], src[e])   (MPI_MAX) */
+#define DDS_OP_MIN 5  /* shard[e] = min(shard[e], src[e])   (MPI_MIN) */
+#define DDS_OP_BAND 6 /* shard[e] = shard[e] & src[e]       (MPI_BAND) */
+#define DDS_OP_BOR 7  /* shard[e] = shard[e] | src[e]       (MPI_BOR) */
+#define DDS_OP_BXOR 8 /* shard[e] = shard[e] ^ src[e]       (MPI_BXOR) */
+int dds_accumulate_op_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                            int64_t fixed_count, int64_t nreq, int op, int dtype, const void *src, int64_t src_bytes,
+                            unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+int dds_accumulate_op_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
+                              int dtype, const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream,
+                              int64_t *total_bytes, int64_t *bad_index);
 
 /* ---- batched compare-and-swaps: elements of any rank's shard replaced where they hold an expected value, the previous
  * rows returned (MPI_Compare_and_swap between fences, batched). For every element e of request i's rows, in one atomic

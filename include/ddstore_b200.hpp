@@ -207,6 +207,38 @@ class DDStore {
                             bool idx_on_device = true, void *cuda_stream = nullptr) {
         return accumulate_samples(name, sample_ids, nreq, acc_type<T>(), src, src_bytes, idx_on_device, cuda_stream);
     }
+    // Batched reduction (dds_accumulate_op_batch): accumulate_batch with each element becoming op(shard, src), op one of
+    // DDS_OP_SUM, DDS_OP_MAX, DDS_OP_MIN, DDS_OP_BAND, DDS_OP_BOR, DDS_OP_BXOR (the bitwise ops on integer types only).
+    long accumulate_op_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq, int op,
+                             int dtype, const void *src, long src_bytes, bool idx_on_device = true,
+                             void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_accumulate_op_batch(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts, fixed_count,
+                                      nreq, op, dtype, src, src_bytes, flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    template <typename T>
+    long accumulate_op_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq, int op,
+                             const T *src, long src_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        return accumulate_op_batch(name, starts, counts, fixed_count, nreq, op, acc_type<T>(), src, src_bytes,
+                                   idx_on_device, cuda_stream);
+    }
+    // The same by sample id (dds_accumulate_op_samples).
+    long accumulate_op_samples(std::string name, const long *sample_ids, long nreq, int op, int dtype, const void *src,
+                               long src_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_accumulate_op_samples(store_, name.c_str(), (const int64_t *)sample_ids, nreq, op, dtype, src, src_bytes,
+                                        flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    template <typename T>
+    long accumulate_op_samples(std::string name, const long *sample_ids, long nreq, int op, const T *src, long src_bytes,
+                               bool idx_on_device = true, void *cuda_stream = nullptr) {
+        return accumulate_op_samples(name, sample_ids, nreq, op, acc_type<T>(), src, src_bytes, idx_on_device,
+                                     cuda_stream);
+    }
     // Batched fetch-op (dds_get_accumulate_batch): accumulate_batch's requests and layout, each element of the rows
     // added to (op = DDS_OP_SUM) or swapped with (DDS_OP_REPLACE) src atomically, its previous value written to `result`
     // (device memory of at least src_bytes, the layout of src; it may be src). T and the explicit-code overload as for
