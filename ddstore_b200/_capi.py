@@ -27,6 +27,10 @@ FOP_OPS = {"sum": OP_SUM, "replace": OP_REPLACE}
 OP_MAX, OP_MIN, OP_BAND, OP_BOR, OP_BXOR = 4, 5, 6, 7, 8
 RED_OPS = {"amax": OP_MAX, "amin": OP_MIN, "bitwise_and": OP_BAND, "bitwise_or": OP_BOR, "bitwise_xor": OP_BXOR}
 
+# where a variable's shards live (DDS_PLACE_*), by name
+PLACE_HBM, PLACE_HOST = 0, 1
+PLACEMENTS = {"hbm": PLACE_HBM, "host": PLACE_HOST}
+
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 BARRIER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p)
 
@@ -74,6 +78,9 @@ SIGNATURES = {
     "dds_size": (C.c_int, [C.c_void_p]),
     "dds_add": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int]),
     "dds_init": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64, C.c_int, C.c_int]),
+    "dds_add_placed": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "dds_init_placed": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64, C.c_int, C.c_int, C.c_int]),
+    "dds_query_placement": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_int)]),
     "dds_update": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int]),
     "dds_update_async": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int,
                                    C.c_void_p]),
@@ -139,6 +146,7 @@ SIGNATURES = {
     "dds_test_occupy": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p]),
     "dds_kernel_launches": (C.c_ulonglong, []),
     "dds_gather_geometry": (None, [C.POINTER(C.c_int)] * 5),
+    "dds_host_gather_ctas": (C.c_int, []),
 }
 
 _lib = None

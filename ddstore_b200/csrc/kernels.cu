@@ -111,6 +111,14 @@ __device__ __forceinline__ void tma_store_1d(void *dst_gmem, uint32_t src_smem, 
                  : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// global -> shared, 16 bytes, through L2 only (SASS: LDGSTS): the producer for sources in mapped host memory
+__device__ __forceinline__ void cp_async_16(uint32_t dst_smem, uint64_t src_gmem) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst_smem), "l"(src_gmem) : "memory");
+}
+// one arrival on `bar` once every cp.async this thread issued so far has landed (the barrier counts it: .noinc)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() {
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
@@ -2057,7 +2065,7 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // cooperatively in two passes: fop_chunk (cas_chunk) replaces the staged operands by the previous values, then the raw
 // drain (bulk stores where the phases allow) writes the stage to the result. The result address of each piece is kept beside its descriptor, in dynamic shared memory behind the rings and the plan.
 template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
-          bool ACC = false, bool FETCH = false>
+          bool ACC = false, bool FETCH = false, bool HOST = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
                                                                 const __grid_constant__ CvtParam<CVT> c) {
     static_assert(CVT || !NORM, "a normalising launch is a converting one");
@@ -2065,6 +2073,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     static_assert(!PUT || (!CVT && !PAD), "a put writes raw rows");
     static_assert(PUT || !ACC, "an accumulate is a put that adds");
     static_assert((PUT && !ACC) || !FETCH, "a fetch-op is a put that returns the previous rows");
+    static_assert(!HOST || !PUT, "HOST shards take no batched writes");
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
     constexpr bool PUSH = FIXED && !CVT && !PAD && !PUT;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
@@ -2081,7 +2090,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
 
     if (lane == 0) {
 #pragma unroll
-        for (int s = 0; s < S; s++) mbar_init(smem_u32(&full_bar[warp][s]), 1);
+        for (int s = 0; s < S; s++) mbar_init(smem_u32(&full_bar[warp][s]), HOST ? 32 : 1); // (HOST: one per lane)
         fence_mbar_init();
     }
     // the launch's tables, copied from the parameter into shared memory behind the rings and the plan
@@ -2357,7 +2366,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             // the stage's previous tenant was drained >= 2 drains ago; the bulk stores a lane issued for it (if any)
             // are at most that lane's second most recent bulk group
             bulk_wait_read<1>();
-            if (lane == 0) mbar_expect_tx(bar, total);
+            if (!HOST && lane == 0) mbar_expect_tx(bar, total);
             __syncwarp();
             const uint32_t al = (uint32_t)(pc.src & 15u);
             desc[warp][st][lane].dpos = pc.dpos;
@@ -2366,8 +2375,21 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             if constexpr (FETCH) // the piece's result address: its source position, in the result buffer
                 sts64(fop_rdst<NW, S, STAGE, PCAP>(smem_dyn, warp, st, lane),
                       pc.n ? (uint64_t)a.fop_result + (pc.src - (uint64_t)a.dst) : 0);
-            if (pc.n) // every lane issues its own piece's TMA load; all complete on the stage's mbarrier
+            if constexpr (HOST) {
+                // A source in mapped host memory never goes to the TMA unit. The lanes copy each piece's 16-byte-aligned
+                // superset window together, 16 bytes per cp.async, and every lane's arrival completes the stage.
+                const uint64_t my_src = pc.src - al;
+                const uint32_t my_dst = ring + st * STAGE + pc.off, my_len = pc.n ? (al + pc.n + 15u) & ~15u : 0u;
+                for (unsigned todo = __ballot_sync(0xffffffffu, pc.n != 0); todo; todo &= todo - 1) {
+                    const int j = __ffs(todo) - 1;
+                    const uint64_t sj = __shfl_sync(0xffffffffu, my_src, j);
+                    const uint32_t dj = __shfl_sync(0xffffffffu, my_dst, j), lj = __shfl_sync(0xffffffffu, my_len, j);
+                    for (uint32_t o = (uint32_t)lane * 16u; o < lj; o += 512u) cp_async_16(dj + o, sj + o);
+                }
+                cp_async_mbar_arrive(bar);
+            } else if (pc.n) { // every lane issues its own piece's TMA load; all complete on the stage's mbarrier
                 tma_load_1d(ring + st * STAGE + pc.off, (const void *)(pc.src - al), (al + pc.n + 15u) & ~15u, bar);
+            }
             issued++;
         }
         if (consumed == issued) break;
@@ -2384,6 +2406,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 }
             }
         }
+        if constexpr (HOST) fence_proxy_async(); // the cp.async writes, before this lane's bulk stores read the stage
         __syncwarp();
         if (dbg_first) {
             dbg_first = false;
@@ -2901,8 +2924,19 @@ __global__ void __launch_bounds__(256) dds_doorbell_kernel(const ddsk_var_t *__r
             // The row loads bypass L1 (ld.global.cg): this CTA stays resident across calls, and its SM's L1 is not
             // coherent with writes from other SMs or GPUs -- a batched put by any rank -- so a cached line could
             // return a row as it was before a put the caller has fenced since.
+            // A HOST shard is read with ld.global.cv: the owner's update rewrites host memory behind the GPU's back, and
+            // .cv drops a matching L2 line of system memory and fetches it again on every load.
             const char *sp = (const char *)src;
-            if ((((uint64_t)sp | (uint64_t)dp | (uint64_t)n) & 15u) == 0) {
+            if (var.host) {
+                if ((((uint64_t)sp | (uint64_t)dp | (uint64_t)n) & 15u) == 0) {
+                    for (int64_t i = threadIdx.x; i < (n >> 4); i += blockDim.x) ((uint4 *)dp)[i] = __ldcv((const uint4 *)sp + i);
+                } else if ((((uint64_t)sp | (uint64_t)dp | (uint64_t)n) & 3u) == 0) {
+                    for (int64_t i = threadIdx.x; i < (n >> 2); i += blockDim.x)
+                        ((uint32_t *)dp)[i] = __ldcv((const unsigned int *)sp + i);
+                } else {
+                    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) dp[i] = __ldcv(sp + i);
+                }
+            } else if ((((uint64_t)sp | (uint64_t)dp | (uint64_t)n) & 15u) == 0) {
                 for (int64_t i = threadIdx.x; i < (n >> 4); i += blockDim.x) ((uint4 *)dp)[i] = __ldcg((const uint4 *)sp + i);
             } else if ((((uint64_t)sp | (uint64_t)dp | (uint64_t)n) & 3u) == 0) {
                 for (int64_t i = threadIdx.x; i < (n >> 2); i += blockDim.x) ((uint32_t *)dp)[i] = __ldcg((const unsigned int *)sp + i);
@@ -2959,6 +2993,11 @@ constexpr Geometry kPlan4K = {12, 3, 4096, 4096};
 constexpr Geometry kPlan8K = {12, 3, 3072, 8192};
 constexpr Geometry kPlan8KFetch = {12, 3, 2048, 8192}; // (with their result addresses too, fetch-ops fit 2 KiB chunks only)
 constexpr int64_t kPlanSmemMax = kPlan8K.pcap;
+// Launches that read DDS_PLACE_HOST shards: kLargeRows with the cp.async producer on a grid of kHostCtas CTAs. Their
+// bytes cross PCIe at a small fraction of the HBM rate, so a full-machine grid would hold every SM for the whole transfer
+// (DESIGN.md 3.12 has the sweep this count comes from). They always plan in the plan kernels.
+constexpr int kHostCtas = 4;
+int g_host_ctas = kHostCtas; // DDS_HOST_CTAS (1..16): measurement switch of the sweep
 // The redundant plan grows with the batch (every SM reads the same index lines), while the plan kernels cost ~0 when
 // they run under the previous batch's gather -- so by default only small batches, where one launch beats three, plan
 // in shared memory.
@@ -2987,6 +3026,7 @@ int pick_geometry() {
     if (const char *e = getenv("DDS_SMEM_PLAN")) g_smem_plan = atoi(e);
     if (const char *e = getenv("DDS_SMEM_PLAN_MAX")) g_plan_smem_default = atoll(e);
     if (const char *e = getenv("DDS_L2_PERSIST")) g_l2_persist = atoi(e);
+    if (const char *e = getenv("DDS_HOST_CTAS")) g_host_ctas = std::max(1, std::min(16, atoi(e)));
     if (const char *e = getenv("DDS_DEBUG_TIMING"))
         if (atoi(e)) {
             CUDA_TRY(cudaMalloc((void **)&g_dbg, 2 * kDbgRegion * 8));
@@ -3006,13 +3046,13 @@ bool cvt_has_norm(const ddsk_cvt_t *cvt) {
 }
 
 template <bool FIXED, const Geometry &G, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
-          bool ACC = false, bool FETCH = false>
+          bool ACC = false, bool FETCH = false, bool HOST = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
     // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan; a fetch-op its
     //  pieces' result addresses)
     const int smem = smem_bytes_of(G) + (CVT ? cvt->lut_bytes : 0) + (FETCH ? G.nw * G.stages * 32 * 8 : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, G.nw, G.stages, G.ch, G.pcap, CVT, NORM, PAD, PUT, ACC, FETCH>;
+    auto kern = dds_gather_kernel<FIXED, G.nw, G.stages, G.ch, G.pcap, CVT, NORM, PAD, PUT, ACC, FETCH, HOST>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -3032,7 +3072,7 @@ int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_c
     GatherArgs args = args_in;
     args.dbg = g_dbg ? g_dbg + (size_t)(args.overlap ? (args.seq & 1u) : 0u) * kDbgRegion : nullptr;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)g_sms);
+    cfg.gridDim = dim3((unsigned)(HOST ? std::min(g_sms, g_host_ctas) : g_sms));
     cfg.blockDim = dim3(G.nw * 32);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
@@ -3111,10 +3151,19 @@ int launch_kind(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *c
     return launch_gather_t<FIXED, G>(args, stream);
 }
 
+// a read of HOST shards (never a write: the store refuses those), raw, converting or normalising
+template <bool FIXED, bool PAD = false>
+int launch_host(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
+    if (!cvt) return launch_gather_t<FIXED, kLargeRows, false, false, PAD, false, false, false, true>(args, stream);
+    return cvt_has_norm(cvt) ? launch_gather_t<FIXED, kLargeRows, true, true, PAD, false, false, false, true>(args, stream, cvt)
+                             : launch_gather_t<FIXED, kLargeRows, true, false, PAD, false, false, false, true>(args, stream, cvt);
+}
+
 // plan in global memory (or none): small rows for fixed-count raw gets of requests under 2 KiB, large rows otherwise
 template <bool FIXED>
 int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false, bool acc = false,
                   bool fop = false) {
+    if (args.var.host) return launch_host<FIXED>(args, stream, cvt);
     if constexpr (FIXED) {
         // (a count too large to multiply safely counts as large)
         const int64_t request_bytes = args.count < ((int64_t)1 << 20) ? args.count * args.var.row_bytes : INT64_MAX;
@@ -3125,8 +3174,8 @@ int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t 
 
 // The shared-memory plan for a batch of nreq requests into cap bytes: 0 = kPlan4K, 1 = kPlan8K (-1: the plan kernels).
 // A converting launch also needs room for its tables.
-int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt) {
-    if (!g_smem_plan || cap >= ((int64_t)1 << 32) || nreq > kPlanSmemMax || nreq > g_plan_smem_default) return -1;
+int select_s(int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool host) {
+    if (host || !g_smem_plan || cap >= ((int64_t)1 << 32) || nreq > kPlanSmemMax || nreq > g_plan_smem_default) return -1;
     if (nreq <= kPlan4K.pcap) return !cvt || cvt_s_fits_t<kPlan4K>(cvt->lut_bytes) ? 0 : -1;
     return !cvt || cvt_s_fits_t<kPlan8K>(cvt->lut_bytes) ? 1 : -1;
 }
@@ -3182,6 +3231,8 @@ int ddsk_debug_timing(unsigned long long *host_out, int max_words) { // both reg
     if (cudaMemcpy(host_out, g_dbg, n * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
     return (int)n;
 }
+
+int ddsk_host_gather_ctas(void) { return pick_geometry() ? 0 : std::min(g_sms, g_host_ctas); }
 
 void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk_bytes, int *smem_bytes) {
     if (pick_geometry()) {
@@ -3251,6 +3302,7 @@ int ddsk_gather_padded(const ddsk_var_t *var, const ddsk_index_t *index, int64_t
     a.pad_in_log2 = cvt ? cvt_in_log2<true>(cvt->code[0]) : 0;
     a.pad_out_log2 = cvt ? cvt_out_log2<true>(cvt->code[0]) : 0;
     a.pad_lengths = lengths;
+    if (var->host) return launch_host<true, true>(a, st, cvt);
     if (!cvt) return launch_gather_t<true, kLargeRows, false, false, true>(a, st);
     return cvt_has_norm(cvt) ? launch_gather_t<true, kLargeRows, true, true, true>(a, st, cvt)
                              : launch_gather_t<true, kLargeRows, true, false, true>(a, st, cvt);
@@ -3265,7 +3317,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
     const bool put = (flags & DDSK_F_PUT) != 0, acc = (flags & DDSK_F_ACC) != 0, fop = (flags & DDSK_F_FOP) != 0;
-    const int gs = select_s(nreq, cap_total, cvt);
+    const int gs = select_s(nreq, cap_total, cvt, a.var.host != 0);
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
@@ -3319,9 +3371,9 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
     return launch_gather<false>(a, st, cvt, put, acc, fop);
 }
 
-int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt) {
+int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt, int host) {
     if (pick_geometry()) return 1;
-    return select_s(nreq, dst_capacity, cvt) < 0;
+    return select_s(nreq, dst_capacity, cvt, host != 0) < 0;
 }
 
 int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, void *dst_dev, int64_t dst_capacity,
@@ -3350,6 +3402,7 @@ int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int6
     }
     ddsk_var_t dummy; // (each variable's window is read from m->vars_dev)
     memset(&dummy, 0, sizeof(dummy));
+    dummy.host = m->host;
     GatherArgs a;
     if (int rc = gather_args(a, &dummy, scr, flags)) return rc;
     PlanSrc p;

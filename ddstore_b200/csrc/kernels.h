@@ -21,7 +21,7 @@ typedef struct ddsk_var {
     int64_t lenlist[DDSK_MAX_RANKS];   /* inclusive cumulative row counts, ddstore.hpp:84-89 */
     int64_t row_bytes;                 /* disp * itemsize, the window's disp_unit, ddstore.hpp:58 */
     int32_t nranks;
-    int32_t pad_;
+    int32_t host;                      /* 1: every shard is mapped host memory (DDS_PLACE_HOST), read over PCIe */
 } ddsk_var_t;
 
 /* status word written by the kernels: 0xFFFF... = ok, else (ordinal << 48) | (first_bad_request << 8) | code, where
@@ -185,8 +185,9 @@ typedef struct ddsk_index {
 int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, void *dst_dev,
                     int64_t dst_capacity, int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags,
                     const ddsk_cvt_t *cvt, void *stream);
-/* (cvt: the conversion the launch will carry, or NULL; its tables take shared memory from the in-launch plan) */
-int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt);
+/* (cvt: the conversion the launch will carry, or NULL; its tables take shared memory from the in-launch plan. host: the
+ * variable's ddsk_var_t.host -- HOST launches always plan in the plan kernels) */
+int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt, int host);
 int64_t ddsk_plan_smem_max(void);
 
 /* Padded batch: request i owns a slot of max_rows rows. The walk runs over the padded SOURCE byte space [0, nreq * slot)
@@ -247,6 +248,7 @@ static inline DDSK_HD ddsk_pad_cut_t ddsk_pad_cut(int64_t i, int64_t payload, in
  * (offsets[v] nullable, nreq+1 entries). */
 typedef struct ddsk_multi {
     int nvars;
+    int host; /* every variable is HOST (a batch never mixes placements) */
     const ddsk_var_t *vars_dev;
     const int64_t *table[DDSK_MAX_MULTI]; /* [nsamples[v]][2] */
     int64_t nsamples[DDSK_MAX_MULTI];
@@ -325,6 +327,9 @@ int ddsk_debug_timing(unsigned long long *host_out, int max_ctas);
 
 /* launch geometry actually used (for bench reporting / DESIGN.md) */
 void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk_bytes, int *smem_bytes);
+
+/* CTAs of a gather launch that reads DDS_PLACE_HOST shards */
+int ddsk_host_gather_ctas(void);
 
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 unsigned long long ddsk_launch_count(void);

@@ -108,6 +108,8 @@ struct PeerRec { // what every rank publishes in add()/init(): the reference's A
     uint64_t alloc_bytes; // mapped size of the shard block
     int32_t vmm;          // 1: CUDA VMM block shared by POSIX fd; 0: cudaMalloc + legacy cudaIpc handle
     int32_t ok;           // 0: this rank failed locally (bad argument, allocation, fill): every rank fails the call
+    int32_t placement;    // DDS_PLACE_*: every rank must pass the same
+    int32_t pad_;
     cudaIpcMemHandle_t handle;
 };
 
@@ -120,7 +122,8 @@ struct Var {
     void *base = nullptr; // local shard (device)
     size_t bytes = 0;
     bool vmm = false;               // shard is a CUDA VMM block (else cudaMalloc)
-    dds_vmm::Block block;           // valid when vmm
+    bool host = false;              // DDS_PLACE_HOST: shard is a mapped host block, shared by memfd (never vmm)
+    dds_vmm::Block block;           // valid when vmm or host
     std::vector<void *> peer_base;  // as mapped here
     std::vector<char> peer_opened;  // 1 = cudaIpcOpenMemHandle'd (must be closed), 2 = VMM import (peer_block)
     bool unprotected_peers = false; // a peer reads this shard through a raw pointer / legacy IPC mapping: the memory
@@ -390,8 +393,8 @@ int renew_plan_tags(dds_store *s) {
 
 // Whether a variable-count launch of nreq requests into cap (source) bytes is planned by the plan kernels rather than
 // in shared memory, and if so their scratch made ready: an overlapped launch plans into a slot of its own.
-int plan_scratch(dds_store *s, int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool ovl, bool *uses_scratch) {
-    *uses_scratch = ddsk_var_uses_scratch(nreq, cap, cvt);
+int plan_scratch(dds_store *s, int64_t nreq, int64_t cap, const ddsk_cvt_t *cvt, bool ovl, bool host, bool *uses_scratch) {
+    *uses_scratch = ddsk_var_uses_scratch(nreq, cap, cvt, host);
     if (!*uses_scratch) return DDS_OK;
     if (int rc = renew_plan_tags(s)) return rc;
     return ovl ? ensure_slots(s, nreq, cap) : ensure_scratch(s, nreq, cap);
@@ -467,13 +470,16 @@ Var *find_var(dds_store *s, const char *name) {
 
 // What the entries do first: clear the error, reset the outputs, resolve the store and the variable, and check
 // the variable's itemsize when the entry takes one (ddstore.hpp:189-190, 202-203; NULL: none, or checked per conversion).
-int entry_var(dds_store *s, const char *name, const int *itemsize, int64_t *total_bytes, int64_t *bad_index, Var **v) {
+// `host_refused` (non-null): the entry does not take DDS_PLACE_HOST variables; the text of its DDS_ERR_ARG.
+int entry_var(dds_store *s, const char *name, const int *itemsize, int64_t *total_bytes, int64_t *bad_index, Var **v,
+              const char *host_refused = nullptr) {
     clear_error();
     if (bad_index) *bad_index = -1;
     if (total_bytes) *total_bytes = 0;
     if (!s) return fail(DDS_ERR_ARG, "null store");
     *v = find_var(s, name);
     if (!*v) return fail(DDS_ERR_UNKNOWN_VAR, name ? name : "(null)");
+    if (host_refused && (*v)->host) return fail(DDS_ERR_ARG, host_refused);
     if (itemsize && (*v)->itemsize != *itemsize) return fail(DDS_ERR_DTYPE);
     return DDS_OK;
 }
@@ -495,7 +501,7 @@ void free_shard(Var &v) {
     if (v.d_norm) cudaFree(v.d_norm);
     v.d_norm = nullptr;
     v.norm_nchan = 0;
-    if (v.vmm)
+    if (v.vmm || v.host)
         dds_vmm::release(&v.block);
     else if (v.base)
         cudaFree(v.base);
@@ -508,7 +514,7 @@ void free_shard(Var &v) {
 // all-gathered record (PeerRec.ok) and makes EVERY rank fail consistently afterwards, instead of leaving the peers
 // stuck in a collective the failing rank never entered.
 int register_var(dds_store *s, const char *name, const void *buffer, int64_t nrows, int disp, int itemsize,
-                 int buffer_on_device, bool zero_fill) {
+                 int buffer_on_device, bool zero_fill, int placement) {
     if (!s || !name) return fail(DDS_ERR_ARG, "null store or name");
     int local_rc = DDS_OK;
     std::string local_err;
@@ -524,6 +530,7 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     if (nrows < 0 || disp < 0 || itemsize <= 0) note(fail(DDS_ERR_ARG, "negative nrows/disp or itemsize <= 0"));
     if (s->size > DDSK_MAX_RANKS) note(fail(DDS_ERR_ARG, "communicator larger than DDSK_MAX_RANKS"));
     if (!zero_fill && !buffer && nrows * (int64_t)disp > 0) note(fail(DDS_ERR_ARG, "null buffer"));
+    if (placement != DDS_PLACE_HBM && placement != DDS_PLACE_HOST) note(fail(DDS_ERR_ARG, "unknown placement"));
     note_cuda(cudaSetDevice(s->device), "cudaSetDevice");
     const bool exists = s->vars.count(name) != 0;
     const unsigned long long seq = s->reg_seq++;
@@ -532,10 +539,17 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     const size_t payload = local_rc ? 0 : (size_t)nrows * (size_t)disp * (size_t)itemsize;
     size_t alloc = ((payload + 16 + 255) / 256) * 256;
     Var v;
-    v.vmm = dds_vmm::available(s->device);
+    v.host = placement == DDS_PLACE_HOST;
+    v.vmm = !v.host && dds_vmm::available(s->device);
     void *base = nullptr;
     if (!local_rc) {
-        if (v.vmm) {
+        if (v.host) { // (a fresh memfd reads as zeros: no fill for zero_fill or the slack)
+            note(dds_vmm::host_alloc(alloc, &v.block));
+            if (!local_rc) {
+                base = v.block.ptr;
+                alloc = v.block.size;
+            }
+        } else if (v.vmm) {
             note(dds_vmm::alloc(s->device, alloc, &v.block));
             if (!local_rc) {
                 base = v.block.ptr;
@@ -548,7 +562,11 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     }
     v.base = base;
     v.bytes = alloc;
-    if (base) {
+    if (base && v.host) {
+        if (!zero_fill && payload > 0)
+            note_cuda(cudaMemcpyAsync(v.block.host, buffer, payload, cudaMemcpyDefault, s->stream), "cudaMemcpyAsync (shard fill)");
+        note_cuda(cudaStreamSynchronize(s->stream), "cudaStreamSynchronize (shard fill)");
+    } else if (base) {
         if (zero_fill || payload == 0) {
             note_cuda(cudaMemsetAsync(base, 0, alloc, s->stream), "cudaMemsetAsync (shard)");
         } else {
@@ -571,7 +589,8 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     mine.host_tag = host_tag();
     mine.alloc_bytes = alloc;
     mine.vmm = v.vmm ? 1 : 0;
-    if (s->size > 1 && !v.vmm && base) note_cuda(cudaIpcGetMemHandle(&mine.handle, base), "cudaIpcGetMemHandle");
+    mine.placement = placement;
+    if (s->size > 1 && !v.vmm && !v.host && base) note_cuda(cudaIpcGetMemHandle(&mine.handle, base), "cudaIpcGetMemHandle");
     mine.ok = local_rc ? 0 : 1;
     std::vector<PeerRec> all((size_t)s->size);
     if (int rc = dds_comm_allgather(s->comm, &mine, all.data(), sizeof(PeerRec))) {
@@ -581,9 +600,10 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
 
     // ddstore.hpp:78-82: every rank must pass the same disp; the ranks that differ from the max throw
     int max_disp = 0;
-    bool bad_item = false, mixed = false, other_host = false, other_proc = false, peer_failed = false;
+    bool bad_item = false, mixed = false, other_host = false, other_proc = false, peer_failed = false, bad_place = false;
     for (auto &p : all) {
         max_disp = std::max(max_disp, (int)p.disp);
+        bad_place |= p.placement != placement;
         bad_item |= p.itemsize != itemsize;
         mixed |= p.vmm != mine.vmm;
         other_host |= p.host_tag != mine.host_tag;
@@ -600,6 +620,7 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
             map_rc = fail(DDS_ERR_COMM, "a peer rank failed to allocate or fill its shard");
         }
     }
+    if (!map_rc && bad_place) map_rc = fail(DDS_ERR_ARG, "ranks disagree on the placement of a variable");
     if (!map_rc && mixed)
         map_rc = fail(DDS_ERR_CUDA, "ranks disagree on the shard allocation mode (set DDS_SHARD_ALLOC on all ranks)");
     if (!map_rc && other_host)
@@ -623,7 +644,7 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     v.peer_opened.assign((size_t)s->size, 0);
     v.peer_block.resize((size_t)s->size);
     std::vector<int> fds;
-    if (!map_rc && v.vmm && other_proc) {
+    if (!map_rc && (v.vmm || v.host) && other_proc) {
         std::vector<char> want((size_t)s->size, 0);
         std::vector<int> pids((size_t)s->size, 0);
         for (int r = 0; r < s->size; r++) {
@@ -648,7 +669,7 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
         } else if (p.pid == mine.pid) {
             // thread-ranks of one process: the raw pointer is already valid here
             v.unprotected_peers = true;
-            if (p.device != s->device && !v.vmm) {
+            if (p.device != s->device && !v.vmm && !v.host) { // (a host block is portable: valid on every device)
                 int can = 0;
                 cudaError_t e = cudaDeviceCanAccessPeer(&can, s->device, p.device);
                 if (e != cudaSuccess) {
@@ -667,13 +688,14 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
                 (void)cudaGetLastError();
             }
             v.peer_base[(size_t)r] = (void *)p.raw_ptr;
-        } else if (v.vmm) {
+        } else if (v.vmm || v.host) {
             int fd = fds.size() > (size_t)r ? fds[(size_t)r] : -1;
             if (fd < 0) {
                 map_rc = fail(DDS_ERR_COMM, "no descriptor received from a peer rank");
                 break;
             }
-            map_rc = dds_vmm::import_fd(s->device, fd, (size_t)p.alloc_bytes, &v.peer_block[(size_t)r]);
+            map_rc = v.host ? dds_vmm::host_import(fd, (size_t)p.alloc_bytes, &v.peer_block[(size_t)r])
+                            : dds_vmm::import_fd(s->device, fd, (size_t)p.alloc_bytes, &v.peer_block[(size_t)r]);
             close(fd);
             fds[(size_t)r] = -1;
             if (map_rc) break;
@@ -706,7 +728,7 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     if (map_rc || bad_disp || bad_item || exists) {
         release_var(v, s->rank);
         if (base) {
-            if (v.vmm)
+            if (v.vmm || v.host)
                 s->zombie_blocks.push_back(v.block); // peers may have mapped it; released in dds_free
             else
                 s->zombies.push_back(base);
@@ -730,6 +752,7 @@ int register_var(dds_store *s, const char *name, const void *buffer, int64_t nro
     }
     v.kv.row_bytes = (int64_t)disp * (int64_t)itemsize;
     v.kv.nranks = s->size;
+    v.kv.host = v.host ? 1 : 0;
     if (s->db_enabled && s->d_vars && s->next_var_id < dds_store::kMaxDbVars) { // window into the doorbell kernel's table
         if (cudaMemcpy(&s->d_vars[s->next_var_id], &v.kv, sizeof(ddsk_var_t), cudaMemcpyHostToDevice) == cudaSuccess)
             v.id = s->next_var_id++;
@@ -1039,13 +1062,30 @@ int dds_size(const dds_store_t *s) { return s ? s->size : -1; }
 
 int dds_add(dds_store_t *s, const char *name, const void *buffer, int64_t nrows, int disp, int itemsize,
             int buffer_on_device) {
-    clear_error();
-    return register_var(s, name, buffer, nrows, disp, itemsize, buffer_on_device, false);
+    return dds_add_placed(s, name, buffer, nrows, disp, itemsize, buffer_on_device, DDS_PLACE_HBM);
 }
 
 int dds_init(dds_store_t *s, const char *name, int64_t nrows, int disp, int itemsize) {
+    return dds_init_placed(s, name, nrows, disp, itemsize, DDS_PLACE_HBM);
+}
+
+int dds_add_placed(dds_store_t *s, const char *name, const void *buffer, int64_t nrows, int disp, int itemsize,
+                   int buffer_on_device, int placement) {
     clear_error();
-    return register_var(s, name, nullptr, nrows, disp, itemsize, 0, true);
+    return register_var(s, name, buffer, nrows, disp, itemsize, buffer_on_device, false, placement);
+}
+
+int dds_init_placed(dds_store_t *s, const char *name, int64_t nrows, int disp, int itemsize, int placement) {
+    clear_error();
+    return register_var(s, name, nullptr, nrows, disp, itemsize, 0, true, placement);
+}
+
+int dds_query_placement(dds_store_t *s, const char *name, int *placement) {
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, nullptr, nullptr, &v)) return rc;
+    if (!placement) return fail(DDS_ERR_ARG, "null placement");
+    *placement = v->host ? DDS_PLACE_HOST : DDS_PLACE_HBM;
+    return DDS_OK;
 }
 
 static int update_impl(dds_store_t *s, const char *name, const void *buffer, int64_t nrows, int64_t offset, int itemsize,
@@ -1057,8 +1097,11 @@ static int update_impl(dds_store_t *s, const char *name, const void *buffer, int
     CU(cudaSetDevice(s->device));
     const size_t row = (size_t)v->disp * (size_t)v->itemsize;
     if (nrows * (int64_t)row > 0) {
-        CU(cudaMemcpyAsync((char *)v->base + (size_t)offset * row, buffer, (size_t)nrows * row,
-                           buffer_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+        if (v->host)
+            CU(cudaMemcpyAsync((char *)v->block.host + (size_t)offset * row, buffer, (size_t)nrows * row, cudaMemcpyDefault, st));
+        else
+            CU(cudaMemcpyAsync((char *)v->base + (size_t)offset * row, buffer, (size_t)nrows * row,
+                               buffer_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
         if (sync) CU(cudaStreamSynchronize(st));
         else if (st != s->stream) s->update_streams.insert(st); // the next fence / free waits for it
     }
@@ -1119,7 +1162,7 @@ int dds_ingest(dds_store_t *s, const char *name, const void *host_rows, int64_t 
     if (int rc = ensure_pool(s)) return rc;
     IngestPool *p = s->ingest;
     const char *src = (const char *)host_rows;
-    char *dst = (char *)v->base + (size_t)offset * row;
+    char *dst = (char *)(v->host ? v->block.host : v->base) + (size_t)offset * row;
     while (total) {
         const size_t n = std::min(total, IngestPool::kStage);
         const int k = p->next;
@@ -1128,7 +1171,7 @@ int dds_ingest(dds_store_t *s, const char *name, const void *host_rows, int64_t 
             p->ev_pending[k] = false;
         }
         p->copy(p->pin[k], src, n);
-        CU(cudaMemcpyAsync(dst, p->pin[k], n, cudaMemcpyHostToDevice, p->stream));
+        CU(cudaMemcpyAsync(dst, p->pin[k], n, v->host ? cudaMemcpyDefault : cudaMemcpyHostToDevice, p->stream));
         CU(cudaEventRecord(p->ev[k], p->stream));
         p->ev_pending[k] = true;
         p->next ^= 1;
@@ -1417,10 +1460,10 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     const int code = cvt ? cvt->code[0] : DDSK_CVT_NONE;
     if (cvt) cap = cvt_cap_to_src(dst_capacity, code);
     if (!d_dst && cap > 0) return fail(DDS_ERR_ARG, "null destination");
-    const bool ovl = no_sync && (flags & DDS_OVERLAP);
+    const bool ovl = no_sync && (flags & DDS_OVERLAP) && !v->host; // (a HOST launch ends an overlap run)
     bool uses_scratch = false;
     if (!fixed)
-        if (int rc = plan_scratch(s, nreq, cap, cvt, ovl, &uses_scratch)) return rc;
+        if (int rc = plan_scratch(s, nreq, cap, cvt, ovl, v->host, &uses_scratch)) return rc;
 
     // ---- launch
     int64_t *d_offsets = dst_dev ? dst_offsets : nullptr;
@@ -1676,7 +1719,7 @@ static int padded_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *st
     if (int rc = stage_indices(s, v, by_sample, starts, counts, nreq, idx_dev, c.st, &ix)) return rc;
     int kflags;
     ddsk_scratch_t scr;
-    if (int rc = launch_flags(s, c, no_sync && (flags & DDS_OVERLAP), false, &kflags, &scr)) return rc;
+    if (int rc = launch_flags(s, c, no_sync && (flags & DDS_OVERLAP) && !v->host, false, &kflags, &scr)) return rc;
     if (ddsk_gather_padded(&v->kv, &ix, nreq, pad->max_rows, pad->pad_bits, out_log2, pad->lengths, dst, &scr, kflags, cvt, c.st))
         return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
     if (total_bytes) *total_bytes = total; // (the padded size, whatever the status says)
@@ -1722,6 +1765,9 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
 // op OP_CAS (acc 0): the compare-and-swap behind dds_compare_and_swap_batch / dds_compare_and_swap_samples, the fetch-op
 // launch whose drain swaps where the shard equals `compare` (the layout of src; DDSK_F_FOP_CAS) on elements of the
 // variable's itemsize. src and compare must be aligned to it too.
+// Device atomics on mapped host memory are not atomic across GPUs over PCIe, so HOST variables take no batched write
+// at all: they are written only by their owner's update / ingest.
+static const char *const kHostWrite = "batched writes do not take DDS_PLACE_HOST variables (write them with update / ingest)";
 static constexpr int OP_CAS = 3; // (put_impl's own op code, beside the DDS_OP_* of the fetch-ops)
 static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
                     int64_t fixed_count, int64_t nreq, const void *src, int64_t src_bytes, unsigned flags,
@@ -1755,7 +1801,7 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     if (int rc = stage_indices(s, v, by_sample, starts, counts, nreq, idx_dev, c.st, &ix)) return rc;
     bool uses_scratch = false;
     if (!fixed)
-        if (int rc = plan_scratch(s, nreq, src_bytes, nullptr, false, &uses_scratch)) return rc;
+        if (int rc = plan_scratch(s, nreq, src_bytes, nullptr, false, false, &uses_scratch)) return rc;
     // (never overlapped: a put ends any overlap run, and the next overlapped batch starts a new one and waits for the grid)
     int kflags;
     ddsk_scratch_t scr;
@@ -1785,7 +1831,7 @@ int dds_put_batch(dds_store_t *s, const char *name, const int64_t *starts, const
                   int64_t nreq, int itemsize, const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream,
                   int64_t *total_bytes, int64_t *bad_index) {
     Var *v;
-    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v, kHostWrite)) return rc;
     return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
                     bad_index);
 }
@@ -1794,7 +1840,7 @@ int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
                     const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                     int64_t *bad_index) {
     Var *v;
-    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v)) return rc;
+    if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v, kHostWrite)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index);
 }
 
@@ -1805,7 +1851,7 @@ static_assert(DDS_ACC_F32 == DDSK_ACC_F32 && DDS_ACC_F64 == DDSK_ACC_F64 && DDS_
 // The accumulates' prologue: entry_var with the dtype in place of the itemsize (an unknown type is an argument error, a
 // size other than the variable's itemsize the reference's "Invalid data type")
 static int acc_entry(dds_store_t *s, const char *name, int dtype, int64_t *total_bytes, int64_t *bad_index, Var **v) {
-    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, v)) return rc;
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, v, kHostWrite)) return rc;
     if (dtype < DDS_ACC_F32 || dtype > DDS_ACC_BF16) return fail(DDS_ERR_ARG, "unknown accumulate dtype");
     if ((*v)->itemsize != 1 << DDSK_ACC_LOG2(dtype)) return fail(DDS_ERR_DTYPE);
     return DDS_OK;
@@ -1887,7 +1933,7 @@ int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *
 // The compare-and-swaps' prologue: entry_var, an itemsize outside {1, 2, 4, 8} (an argument error) and then one other
 // than the variable's (the reference's "Invalid data type")
 static int cas_entry(dds_store_t *s, const char *name, int itemsize, int64_t *total_bytes, int64_t *bad_index, Var **v) {
-    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, v)) return rc;
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, v, kHostWrite)) return rc;
     if (itemsize != 1 && itemsize != 2 && itemsize != 4 && itemsize != 8)
         return fail(DDS_ERR_ARG, "compare-and-swaps take elements of 1, 2, 4 or 8 bytes");
     if ((*v)->itemsize != itemsize) return fail(DDS_ERR_DTYPE);
@@ -1930,6 +1976,7 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
     for (int v = 0; v < nvars; v++) {
         vv[v] = find_var(s, names[v]);
         if (!vv[v]) return fail(DDS_ERR_UNKNOWN_VAR, names[v] ? names[v] : "(null)");
+        if (vv[v]->host != vv[0]->host) return fail(DDS_ERR_ARG, "a multi-array batch takes variables of one placement");
         if (!vv[v]->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
         if (dst_capacities[v] < 0) return fail(DDS_ERR_ARG, "negative capacity");
         key += vv[v]->name;
@@ -1972,9 +2019,10 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
         CU(cudaMemcpyAsync(s->d_starts, sample_ids, (size_t)nreq * 8, cudaMemcpyHostToDevice, c.st));
         d_ids = s->d_starts;
     }
-    const bool ovl = no_sync && (flags & DDS_OVERLAP);
+    const bool host = vv[0]->host;
+    const bool ovl = no_sync && (flags & DDS_OVERLAP) && !host;
     bool uses_scratch;
-    if (int rc = plan_scratch(s, nreq * nvars, cap_total, kcp, ovl, &uses_scratch)) return rc;
+    if (int rc = plan_scratch(s, nreq * nvars, cap_total, kcp, ovl, host, &uses_scratch)) return rc;
     // a synchronous caller wants the per-variable totals: they are the last entries of the per-variable offsets, which
     // go to the caller's arrays or to a staging array of the store
     const bool stage_offs = !no_sync && total_bytes != nullptr;
@@ -1984,6 +2032,7 @@ static int multi_impl(dds_store_t *s, int nvars, const char *const *names, const
     ddsk_multi_t m;
     memset(&m, 0, sizeof(m));
     m.nvars = nvars;
+    m.host = host ? 1 : 0;
     m.vars_dev = s->d_multi_vars;
     for (int v = 0; v < nvars; v++) {
         m.table[v] = vv[v]->d_tab;
@@ -2108,7 +2157,7 @@ int dds_push_setup(dds_store_t *s, int64_t max_requests, int64_t max_bytes) {
     t.dst_off[0] = t.idx_off[1] + up(max_requests * 8);
     t.dst_off[1] = t.dst_off[0] + up(max_bytes);
     const int64_t bytes = t.dst_off[1] + up(max_bytes);
-    if (int rc = register_var(s, kPushWindow, nullptr, bytes, 1, 1, 0, true)) return rc; // collective, zero-filled, mapped
+    if (int rc = register_var(s, kPushWindow, nullptr, bytes, 1, 1, 0, true, DDS_PLACE_HBM)) return rc; // collective, zero-filled, mapped
     Var *w = find_var(s, kPushWindow);
     for (int r = 0; r < s->size; r++) t.win[r] = (unsigned char *)w->kv.bases[r];
     CU(cudaMemset(t.win[t.me] + 24, 0xFF, 8)); // the window's status word starts as "ok"
@@ -2125,7 +2174,8 @@ int dds_get_batch_push(dds_store_t *s, const char *name, const int64_t *starts_d
     if (!s || !dst_out) return fail(DDS_ERR_ARG, "null store or dst_out");
     if (!s->push.ready) return fail(DDS_ERR_ARG, "no push windows (call dds_push_setup on every rank first)");
     Var *v;
-    if (int rc = entry_var(s, name, &itemsize, nullptr, nullptr, &v)) return rc;
+    if (int rc = entry_var(s, name, &itemsize, nullptr, nullptr, &v, "the push fetch does not serve DDS_PLACE_HOST variables"))
+        return rc;
     const int64_t nb = fixed_count * v->kv.row_bytes;
     if (fixed_count <= 0 || nreq < 0 || (nreq > 0 && !starts_dev)) return fail(DDS_ERR_ARG, "push batches fetch count >= 1 rows per request");
     if (nreq > s->push.table.max_requests || nreq * nb > s->push.table.max_bytes)
@@ -2318,6 +2368,7 @@ int dds_test_occupy(int device, int ctas, int smem_bytes, uint64_t nanoseconds, 
 }
 
 unsigned long long dds_kernel_launches(void) { return ddsk_launch_count(); }
+int dds_host_gather_ctas(void) { return ddsk_host_gather_ctas(); }
 void dds_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk_bytes, int *smem_bytes) {
     ddsk_gather_geometry(ctas, warps_per_cta, stages, chunk_bytes, smem_bytes);
 }

@@ -9,9 +9,14 @@
 //
 // The driver entry points are resolved at run time with cudaGetDriverEntryPoint, so the library has no link-time
 // dependency on libcuda and still loads (and fails loudly in dds_create) on a machine without a GPU.
+//
+// A HOST-placed shard (dds_add_placed) is pinned host memory instead: a memfd mapped MAP_SHARED and registered with
+// cudaHostRegister(Mapped | Portable). It travels to the other processes of the box as a file descriptor over the same
+// socket, and needs neither a driver attribute nor /dev/shm.
 #include <cuda.h>
 #include <cuda_runtime_api.h>
 #include <poll.h>
+#include <sys/mman.h>
 #include <sys/socket.h>
 #include <sys/un.h>
 #include <unistd.h>
@@ -225,9 +230,70 @@ int import_fd(int device, int fd, size_t size, Block *out) {
     return DDS_OK;
 }
 
+namespace {
+
+// map `size` bytes of memfd `fd` and register them mapped + portable (valid on every device of the process)
+int host_map(int fd, size_t size, Block *out) {
+    void *h = mmap(nullptr, size, PROT_READ | PROT_WRITE, MAP_SHARED, fd, 0);
+    if (h == MAP_FAILED) return dds_internal::fail(DDS_ERR_CUDA, "host shard: mmap failed");
+    cudaError_t e = cudaHostRegister(h, size, cudaHostRegisterMapped | cudaHostRegisterPortable);
+    void *d = nullptr;
+    if (e == cudaSuccess) {
+        e = cudaHostGetDevicePointer(&d, h, 0);
+        if (e != cudaSuccess) cudaHostUnregister(h);
+    }
+    if (e != cudaSuccess) {
+        (void)cudaGetLastError();
+        munmap(h, size);
+        return dds_internal::fail(DDS_ERR_CUDA, std::string("host shard: cudaHostRegister: ") + cudaGetErrorString(e));
+    }
+    out->ptr = d;
+    out->host = h;
+    out->size = size;
+    out->mapped = true;
+    return DDS_OK;
+}
+
+} // namespace
+
+int host_alloc(size_t bytes, Block *out) {
+    memset(out, 0, sizeof(*out));
+    out->fd = -1;
+    const size_t page = (size_t)sysconf(_SC_PAGESIZE);
+    size_t size = ((bytes + page - 1) / page) * page;
+    if (size == 0) size = page;
+    int fd = memfd_create("dds-host-shard", MFD_CLOEXEC);
+    if (fd < 0) return dds_internal::fail(DDS_ERR_CUDA, "host shard: memfd_create failed");
+    if (ftruncate(fd, (off_t)size) != 0) {
+        close(fd);
+        return dds_internal::fail(DDS_ERR_CUDA, "host shard: ftruncate failed");
+    }
+    if (int rc = host_map(fd, size, out)) {
+        close(fd);
+        return rc;
+    }
+    out->fd = fd;
+    return DDS_OK;
+}
+
+int host_import(int fd, size_t size, Block *out) {
+    memset(out, 0, sizeof(*out));
+    out->fd = -1;
+    return host_map(fd, size, out);
+}
+
 void release(Block *b) {
     if (!b || !b->mapped) return;
     if (b->fd >= 0) close(b->fd);
+    if (b->host) {
+        cudaHostUnregister(b->host);
+        munmap(b->host, b->size);
+        b->host = nullptr;
+        b->mapped = false;
+        b->ptr = nullptr;
+        b->fd = -1;
+        return;
+    }
     g_drv.MemUnmap((CUdeviceptr)b->ptr, b->size);
     g_drv.MemAddressFree((CUdeviceptr)b->ptr, b->size);
     g_drv.MemRelease((CUmemGenericAllocationHandle)b->handle);

@@ -40,8 +40,8 @@ cdef extern from "ddstore_b200.h":
 cdef extern from "ddstore_b200.hpp" nogil:
     cdef cppclass DDStore:
         DDStore(int method, dds_comm_t* comm, int device) except +dds_translate_exception
-        void add[T](string name, T* buffer, long nrows, int disp) except +dds_translate_exception
-        void add_device[T](string name, const T* buffer, long nrows, int disp) except +dds_translate_exception
+        void add[T](string name, T* buffer, long nrows, int disp, int placement) except +dds_translate_exception
+        void add_device[T](string name, const T* buffer, long nrows, int disp, int placement) except +dds_translate_exception
         void get[T](string name, long start, long count, T* buffer) except +dds_translate_exception
         void get_device[T](string name, long start, long count, T* buffer) except +dds_translate_exception
         long get_batch[T](string name, const long* starts, const long* counts, long fixed_count, long nreq, T* dst,
@@ -71,10 +71,22 @@ cdef extern from "ddstore_b200.hpp" nogil:
         void epoch_begin() except +dds_translate_exception
         void epoch_end() except +dds_translate_exception
         void free() except +dds_translate_exception
-        void init(string name, long nrows, int disp, int itemsize) except +dds_translate_exception
+        void init(string name, long nrows, int disp, int itemsize, int placement) except +dds_translate_exception
+        int placement(string name) except +dds_translate_exception
         void update[T](string name, T* buffer, long nrows, long offset) except +dds_translate_exception
         int rank()
         int size()
+
+
+# where a variable's shards live (DDS_PLACE_*), by name
+PLACEMENTS = {"hbm": 0, "host": 1}
+PLACEMENT_NAMES = {v: k for k, v in PLACEMENTS.items()}
+
+
+def _placement(str placement):
+    if placement not in PLACEMENTS:
+        raise ValueError(f"unknown placement {placement!r} (expected 'hbm' or 'host')")
+    return PLACEMENTS[placement]
 
 
 # element types of accumulate_batch (DDS_ACC_*), by dtype name
@@ -110,7 +122,8 @@ cdef class PyDDStore:
     def size(self):
         return self.c_ddstore.size()
 
-    def add(self, str name, arr):
+    def add(self, str name, arr, str placement="hbm"):
+        cdef int pl = _placement(placement)
         b = _Buf(arr)
         cdef long nrows = b.shape[0]
         cdef int disp = (b.size // b.shape[0]) if b.shape[0] else int(np.prod(b.shape[1:], dtype=np.int64))
@@ -119,14 +132,14 @@ cdef class PyDDStore:
         cdef int w = b.itemsize
         if b.on_device:
             with nogil:
-                if w == 1: self.c_ddstore.add_device[char](nm, <const char*> p, nrows, disp)
-                elif w == 4: self.c_ddstore.add_device[int](nm, <const int*> p, nrows, disp)
-                else: self.c_ddstore.add_device[long](nm, <const long*> p, nrows, disp)
+                if w == 1: self.c_ddstore.add_device[char](nm, <const char*> p, nrows, disp, pl)
+                elif w == 4: self.c_ddstore.add_device[int](nm, <const int*> p, nrows, disp, pl)
+                else: self.c_ddstore.add_device[long](nm, <const long*> p, nrows, disp, pl)
         else:
             with nogil:
-                if w == 1: self.c_ddstore.add[char](nm, <char*> p, nrows, disp)
-                elif w == 4: self.c_ddstore.add[int](nm, <int*> p, nrows, disp)
-                else: self.c_ddstore.add[long](nm, <long*> p, nrows, disp)
+                if w == 1: self.c_ddstore.add[char](nm, <char*> p, nrows, disp, pl)
+                elif w == 4: self.c_ddstore.add[int](nm, <int*> p, nrows, disp, pl)
+                else: self.c_ddstore.add[long](nm, <long*> p, nrows, disp, pl)
 
     def get(self, str name, arr, long start=0):
         b = _Buf(arr, writable=True)
@@ -475,10 +488,15 @@ cdef class PyDDStore:
         with nogil:
             self.c_ddstore.free()
 
-    def init(self, str name, long nrows, int disp, int itemsize=1):
+    def init(self, str name, long nrows, int disp, int itemsize=1, str placement="hbm"):
+        cdef int pl = _placement(placement)
         cdef string nm = name.encode()
         with nogil:
-            self.c_ddstore.init(nm, nrows, disp, itemsize)
+            self.c_ddstore.init(nm, nrows, disp, itemsize, pl)
+
+    def placement(self, str name):
+        cdef string nm = name.encode()
+        return PLACEMENT_NAMES[self.c_ddstore.placement(nm)]
 
     def update(self, str name, arr, long offset):
         b = _Buf(arr)

@@ -50,10 +50,12 @@ class DistDataset(Dataset):
     gather (see PyDDStore.set_normalization for the channel rule), as out_dtype (default float32). A uint8 source is
     decoded through `lut` (256 float32 entries, default the plain value: pass torch.arange(256).float().div(255) for
     ToTensor() + Normalize()). The labels are never normalised.
+    placement="host": the samples and labels live in pinned host memory every rank of the box maps instead of HBM (a
+    dataset larger than the HBM the model leaves free); batches are still gathered on the GPU, over PCIe.
     """
 
     def __init__(self, data, label, comm=None, ddstore_width=None, device=None, local_only=False, out_dtype=None, lut=None,
-                 normalize=None):
+                 normalize=None, placement="hbm"):
         super().__init__()
         self.label = label
         self.comm = as_dds_comm(comm)
@@ -94,10 +96,11 @@ class DistDataset(Dataset):
         self.lut = lut
         if self.src_dtype is not None:  # an unsupported pair fails here, not at the first batch
             _conversion(self.src_dtype, self.out_dtype, lut, self.normalize)
-        self.ddstore.add(f"{self.label}data", np.ascontiguousarray(arr))
+        self.ddstore.add(f"{self.label}data", np.ascontiguousarray(arr), placement=placement)
         if self.normalize:
             self.ddstore.set_normalization(f"{self.label}data", *_norm_spec(normalize))
-        self.ddstore.add(f"{self.label}labels", np.ascontiguousarray(np.array(labels, dtype=np.int32).reshape(-1, 1)))
+        self.ddstore.add(f"{self.label}labels", np.ascontiguousarray(np.array(labels, dtype=np.int32).reshape(-1, 1)),
+                         placement=placement)
 
     def _allgather_int(self, v):
         parts = self.ddstore_comm.allgather_bytes(int(v).to_bytes(8, "little"))
@@ -156,7 +159,7 @@ class RaggedDataset(Dataset):
     The (start, count) tables of ALL samples are kept on the device, so a batch needs only the sample ids."""
 
     def __init__(self, local_arrays, local_counts, comm=None, device=None, out_dtypes=None, luts=None, normalize=None,
-                 pad=None):
+                 pad=None, placement="hbm"):
         """local_arrays: {name: 2-D ndarray of this rank's rows}; local_counts: {name: int64[n_local_samples]}
         out_dtypes / luts: {name: dtype} / {name: 256-entry table}: those variables' batches are delivered converted in
         the gather (see DistDataset); their row offsets count rows as always.
@@ -164,7 +167,8 @@ class RaggedDataset(Dataset):
         as out_dtypes[name] (default float32).
         pad: {name: max_rows | (max_rows, pad_value)}: those variables are delivered padded, as (tensor [B, max_rows,
         ...width] in their output dtype, int64 lengths [B]): each sample's first max_rows rows, then pad_value (default
-        0) encoded in the output dtype. The other variables stay packed."""
+        0) encoded in the output dtype. The other variables stay packed.
+        placement="host": every variable lives in pinned host memory instead of HBM (see DistDataset)."""
         out_dtypes, luts, normalize = dict(out_dtypes or {}), dict(luts or {}), dict(normalize or {})
         super().__init__()
         self.comm = as_dds_comm(comm)
@@ -179,7 +183,7 @@ class RaggedDataset(Dataset):
             arr = np.ascontiguousarray(local_arrays[name])
             cnt = np.ascontiguousarray(local_counts[name], dtype=np.int64)
             assert cnt.sum() == arr.shape[0] and len(cnt) == n_local
-            self.ddstore.add(name, arr)
+            self.ddstore.add(name, arr, placement=placement)
             first_row = ([0] + self.ddstore.query(name)["lenlist"])[self.rank]
             local_start = first_row + np.concatenate([[0], np.cumsum(cnt)[:-1]])
             # every rank learns every sample's (start, count): 16 B per sample per variable

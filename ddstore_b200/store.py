@@ -91,6 +91,15 @@ def _norm_tables(mean, std):
     return m, s, nm, dm
 
 
+_PLACEMENT_NAMES = {v: k for k, v in _capi.PLACEMENTS.items()}
+
+
+def _placement(placement):
+    if placement not in _capi.PLACEMENTS:
+        raise ValueError(f"unknown placement {placement!r} (expected 'hbm' or 'host')")
+    return _capi.PLACEMENTS[placement]
+
+
 def _ptr(t):
     return t.ctypes.data if isinstance(t, np.ndarray) else t.data_ptr()
 
@@ -195,12 +204,14 @@ class PyDDStore:
         self.last_bad_index = -1
 
     # ---------------------------------------------------------------- reference surface
-    def add(self, name, arr):
-        # src/pyddstore.pyx:65-82
+    def add(self, name, arr, placement="hbm"):
+        # src/pyddstore.pyx:65-82. placement="host": the shards live in pinned host memory every rank of the box maps
+        # (a dataset larger than free HBM); the gathers still run on the GPU. Batched writes refuse such variables.
+        pl = _placement(placement)
         b = _Buf(arr)
         nrows = b.shape[0]
         disp = b.size // b.shape[0] if b.shape[0] else int(np.prod(b.shape[1:], dtype=np.int64))
-        _capi.raise_for(self._L.dds_add(self._h, name.encode(), b.ptr, nrows, disp, b.itemsize, b.on_device))
+        _capi.raise_for(self._L.dds_add_placed(self._h, name.encode(), b.ptr, nrows, disp, b.itemsize, b.on_device, pl))
 
     def get(self, name, arr, start=0):
         # src/pyddstore.pyx:84-101: count = arr.shape[0]; fills arr in place
@@ -229,8 +240,9 @@ class PyDDStore:
             self._itemsize.clear()
             _capi.raise_for(self._L.dds_free(self._h))  # src/pyddstore.pyx:109-110
 
-    def init(self, name, nrows, disp, itemsize=1):
-        _capi.raise_for(self._L.dds_init(self._h, name.encode(), int(nrows), int(disp), int(itemsize)))  # :112-113
+    def init(self, name, nrows, disp, itemsize=1, placement="hbm"):
+        pl = _placement(placement)
+        _capi.raise_for(self._L.dds_init_placed(self._h, name.encode(), int(nrows), int(disp), int(itemsize), pl))  # :112-113
 
     def update(self, name, arr, offset, stream=None, wait=True):
         # src/pyddstore.pyx:115-131. wait=False: enqueue the copy on `stream` and return (streaming ingest; the
@@ -861,7 +873,9 @@ class PyDDStore:
     def query(self, name):
         vi = _capi.VarInfo()
         _capi.raise_for(self._L.dds_query(self._h, name.encode(), C.byref(vi)))
-        return {"itemsize": vi.itemsize, "disp": vi.disp, "nranks": vi.nranks, "fence_active": bool(vi.fence_active),
+        pl = C.c_int(0)
+        _capi.raise_for(self._L.dds_query_placement(self._h, name.encode(), C.byref(pl)))
+        return {"placement": _PLACEMENT_NAMES[pl.value],"itemsize": vi.itemsize, "disp": vi.disp, "nranks": vi.nranks, "fence_active": bool(vi.fence_active),
                 "local_nrows": vi.local_nrows, "total_nrows": vi.total_nrows,
                 "lenlist": [vi.lenlist[i] for i in range(vi.nranks)], "local_base": vi.local_base}
 

@@ -28,8 +28,9 @@ extern "C" {
                            puts (dds_put_batch, dds_put_samples, DDS_SRC_ON_DEVICE), the batched accumulates
                            (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*), the batched fetch-ops
                            (dds_get_accumulate_batch, dds_get_accumulate_samples, DDS_OP_*), the batched
-                           compare-and-swaps (dds_compare_and_swap_batch, dds_compare_and_swap_samples) and the batched
-                           reductions (dds_accumulate_op_batch, dds_accumulate_op_samples, DDS_OP_MAX & co.). */
+                           compare-and-swaps (dds_compare_and_swap_batch, dds_compare_and_swap_samples), the batched
+                           reductions (dds_accumulate_op_batch, dds_accumulate_op_samples, DDS_OP_MAX & co.) and the
+                           placed variables (dds_add_placed, dds_init_placed, dds_query_placement, DDS_PLACE_*). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -113,6 +114,28 @@ int dds_add(dds_store_t *s, const char *name, const void *buffer, int64_t nrows,
             int buffer_on_device);
 /* void init(string name, long nrows, int disp, int itemsize), ddstore.hpp:110-179. COLLECTIVE, zero-filled. */
 int dds_init(dds_store_t *s, const char *name, int64_t nrows, int disp, int itemsize);
+
+/* ---- placement: where a variable's shards live, chosen when it is created -----------------------------------------
+ * DDS_PLACE_HBM (dds_add / dds_init): each shard in its GPU's HBM. DDS_PLACE_HOST: each shard in pinned host memory that
+ * every rank of the box maps (the reference's host-RAM shards), so a dataset may be larger than the HBM a model leaves
+ * free. The gathers still run on the GPU and read a HOST shard over PCIe, into HBM or a host buffer as usual.
+ * On a HOST variable these work exactly as on an HBM one, byte for byte, errors included: dds_get, dds_get_batch,
+ * dds_get_samples, the converting, normalising and padded entries, dds_get_samples_multi(_convert) when every variable
+ * of the batch is HOST, dds_update(_async), dds_ingest, dds_synth_fill and dds_synth_verify. DDS_OVERLAP is ignored for
+ * HOST batches (a HOST batch ends an overlap run, like a put).
+ * Refused with DDS_ERR_ARG, nothing enqueued, right after the unknown-variable check: every batched write (put,
+ * accumulate, accumulate_op, get_accumulate, compare_and_swap, batch and samples forms), dds_get_batch_push, and a
+ * multi-array batch that mixes placements. Device atomics on mapped host memory are not atomic across GPUs over PCIe,
+ * and one rule is simpler than two: a HOST variable is written only by its owner's update / ingest. Per-sample state
+ * that training writes back belongs in HBM variables.
+ * dds_add_placed / dds_init_placed are dds_add / dds_init with a placement (COLLECTIVE): an unknown placement is
+ * DDS_ERR_ARG, and so is a placement the ranks disagree on (on every rank; nothing is registered). */
+#define DDS_PLACE_HBM 0
+#define DDS_PLACE_HOST 1
+int dds_add_placed(dds_store_t *s, const char *name, const void *buffer, int64_t nrows, int disp, int itemsize,
+                   int buffer_on_device, int placement);
+int dds_init_placed(dds_store_t *s, const char *name, int64_t nrows, int disp, int itemsize, int placement);
+int dds_query_placement(dds_store_t *s, const char *name, int *placement);
 /* template<T> void update(string name, T* buffer, long nrows, long offset), ddstore.hpp:181-195. Local copy
  * into rows [offset, offset+nrows) of this rank's shard. (The reference does not bounds-check; this does:
  * DDS_ERR_ARG.) */
@@ -496,6 +519,8 @@ int dds_test_occupy(int device, int ctas, int smem_bytes, uint64_t nanoseconds, 
 /* kernels launched by this library since load, and the gather launch geometry in use */
 unsigned long long dds_kernel_launches(void);
 void dds_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk_bytes, int *smem_bytes);
+/* CTAs of a gather launch that reads DDS_PLACE_HOST shards (at most 16; 0 without a usable device) */
+int dds_host_gather_ctas(void);
 
 #ifdef __cplusplus
 }

@@ -71,12 +71,18 @@ class DDStore {
     void epoch_end() { check(dds_epoch_end(store_)); }     // ddstore.cxx:65-77
     void free() { check(dds_free(store_)); }               // ddstore.cxx:79-96
 
+    // (placement: DDS_PLACE_HBM, the reference's behaviour, or DDS_PLACE_HOST -- see include/ddstore_b200.h)
     template <typename T>
-    void add(std::string name, T *buffer, long nrows, int disp) { // ddstore.hpp:39-108
-        check(dds_add(store_, name.c_str(), buffer, nrows, disp, (int)sizeof(T), 0));
+    void add(std::string name, T *buffer, long nrows, int disp, int placement = DDS_PLACE_HBM) { // ddstore.hpp:39-108
+        check(dds_add_placed(store_, name.c_str(), buffer, nrows, disp, (int)sizeof(T), 0, placement));
     }
-    void init(std::string name, long nrows, int disp, int itemsize) { // ddstore.hpp:110-179
-        check(dds_init(store_, name.c_str(), nrows, disp, itemsize));
+    void init(std::string name, long nrows, int disp, int itemsize, int placement = DDS_PLACE_HBM) { // ddstore.hpp:110-179
+        check(dds_init_placed(store_, name.c_str(), nrows, disp, itemsize, placement));
+    }
+    int placement(std::string name) {
+        int p = DDS_PLACE_HBM;
+        check(dds_query_placement(store_, name.c_str(), &p));
+        return p;
     }
     template <typename T>
     void update(std::string name, T *buffer, long nrows, long offset = 0) { // ddstore.hpp:181-195
@@ -324,8 +330,8 @@ class DDStore {
     }
     // device-pointer variants of add/get for callers that already hold the data in HBM
     template <typename T>
-    void add_device(std::string name, const T *dev_buffer, long nrows, int disp) {
-        check(dds_add(store_, name.c_str(), dev_buffer, nrows, disp, (int)sizeof(T), 1));
+    void add_device(std::string name, const T *dev_buffer, long nrows, int disp, int placement = DDS_PLACE_HBM) {
+        check(dds_add_placed(store_, name.c_str(), dev_buffer, nrows, disp, (int)sizeof(T), 1, placement));
     }
     template <typename T>
     void get_device(std::string name, long start, long count, T *dev_buffer) {
