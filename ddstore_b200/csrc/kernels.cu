@@ -211,84 +211,8 @@ __device__ __forceinline__ unsigned short lds16h(uint32_t addr) { // (into a 16-
     return v;
 }
 
-// Reductions of the accumulate (ACC), element type t = DDSK_ACC_* (warp-uniform). Every one is atomic per element: the
-// element reductions at .sys scope (a peer's reductions into the same shard must combine with the owner's), the bulk
-// ones at the scope the ISA gives them. The f32 element and vector reductions flush subnormal inputs and results to
-// zero (atomicAdd's rule; the f32 bulk reduction kept them on H100, see DESIGN.md 3.8); f16 / bf16 are .noftz; f64 is
-// exact IEEE, the integer types wrap.
-// shared -> global bulk reduction, dst[e] += staged[e]: tma_store_1d's rules (16-byte aligned addresses and size) and
-// bulk async-group (SASS: UBLKRED)
-__device__ __forceinline__ void tma_red_add_1d(void *dst_gmem, uint32_t src_smem, uint32_t bytes, int t) {
-    switch (t) {
-    case DDSK_ACC_F32:
-        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
-        break;
-    case DDSK_ACC_F64:
-        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f64 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
-        break;
-    case DDSK_ACC_I32:
-        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u32 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
-        break;
-    case DDSK_ACC_I64:
-        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
-        break;
-    case DDSK_ACC_F16:
-        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.noftz.f16 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
-        break;
-    default:
-        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.noftz.bf16 [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), "r"(bytes) : "memory");
-        break;
-    }
-}
-// one element: *d += the element staged at shared address s (both aligned to the element size)
-__device__ __forceinline__ void red_add1(char *d, uint32_t s, int t) {
-    switch (t) {
-    case DDSK_ACC_F32:
-        asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(d), "f"(__uint_as_float(lds32(s))) : "memory");
-        break;
-    case DDSK_ACC_F64:
-        asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__longlong_as_double((long long)lds64(s))) : "memory");
-        break;
-    case DDSK_ACC_I32: asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(lds32(s)) : "memory"); break;
-    case DDSK_ACC_I64: asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"(lds64(s)) : "memory"); break;
-    case DDSK_ACC_F16: asm volatile("red.relaxed.sys.global.add.noftz.f16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
-    default: asm volatile("red.relaxed.sys.global.add.noftz.bf16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
-    }
-}
-// 16 bytes at a 16-byte aligned d: *d += v, element-wise
-__device__ __forceinline__ void red_add16(char *d, uint4 v, int t) {
-    switch (t) {
-    case DDSK_ACC_F32:
-        asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(d), "f"(__uint_as_float(v.x)),
-                     "f"(__uint_as_float(v.y)), "f"(__uint_as_float(v.z)), "f"(__uint_as_float(v.w)) : "memory");
-        break;
-    case DDSK_ACC_F64:
-        asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__hiloint2double((int)v.y, (int)v.x)) : "memory");
-        asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d + 8), "d"(__hiloint2double((int)v.w, (int)v.z)) : "memory");
-        break;
-    case DDSK_ACC_I32:
-        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(v.x) : "memory");
-        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 4), "r"(v.y) : "memory");
-        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 8), "r"(v.z) : "memory");
-        asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 12), "r"(v.w) : "memory");
-        break;
-    case DDSK_ACC_I64:
-        asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"((uint64_t)v.y << 32 | v.x) : "memory");
-        asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d + 8), "l"((uint64_t)v.w << 32 | v.z) : "memory");
-        break;
-    case DDSK_ACC_F16:
-        asm volatile("red.relaxed.sys.global.add.noftz.v4.f16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z),
-                     "r"(v.w) : "memory");
-        break;
-    default:
-        asm volatile("red.relaxed.sys.global.add.noftz.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z),
-                     "r"(v.w) : "memory");
-        break;
-    }
-}
-
-// Fetch-ops (FETCH), element type t = DDSK_ACC_*, swap or add (both warp-uniform): atomics that return the element's
-// previous value, at .sys scope for the accumulate's reason. Adds round and flush exactly as the accumulate's element and
+// Fetch-ops (fetch1 / fetch16 below): atomics that return the element's previous value, at .sys scope for the
+// accumulate's reason. Adds round and flush exactly as the accumulate's element and
 // vector reductions do (f32 flushes, f16 / bf16 are .noftz, f64 is IEEE, integers wrap).
 __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
     asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
@@ -335,87 +259,8 @@ __device__ __forceinline__ uint32_t atom_exch_b16(char *d, uint32_t v) {
     }
     return (cur >> sh) & 0xFFFFu;
 }
-// one element at d: the operand staged at shared address s is replaced by the element's previous value (both aligned to
-// the element size)
-__device__ __forceinline__ void fop1(char *d, uint32_t s, int t, bool swap) {
-    if (swap) {
-        switch (DDSK_ACC_LOG2(t)) {
-        case 3: sts64(s, atom_exch_b64(d, lds64(s))); break;
-        case 2: sts32(s, atom_exch_b32(d, lds32(s))); break;
-        default: sts16(s, atom_exch_b16(d, lds16h(s))); break;
-        }
-        return;
-    }
-    switch (t) {
-    case DDSK_ACC_F32: {
-        float o;
-        asm volatile("atom.relaxed.sys.global.add.f32 %0, [%1], %2;" : "=f"(o) : "l"(d), "f"(__uint_as_float(lds32(s))) : "memory");
-        sts32(s, __float_as_uint(o));
-        break;
-    }
-    case DDSK_ACC_F64: sts64(s, atom_add_f64(d, lds64(s))); break;
-    case DDSK_ACC_I32: sts32(s, atom_add_u32(d, lds32(s))); break;
-    case DDSK_ACC_I64: sts64(s, atom_add_u64(d, lds64(s))); break;
-    case DDSK_ACC_F16: {
-        unsigned short o;
-        asm volatile("atom.relaxed.sys.global.add.noftz.f16 %0, [%1], %2;" : "=h"(o) : "l"(d), "h"(lds16h(s)) : "memory");
-        sts16(s, o);
-        break;
-    }
-    default: {
-        unsigned short o;
-        asm volatile("atom.relaxed.sys.global.add.noftz.bf16 %0, [%1], %2;" : "=h"(o) : "l"(d), "h"(lds16h(s)) : "memory");
-        sts16(s, o);
-        break;
-    }
-    }
-}
-// 16 bytes at a 16-byte aligned d: the operands v, element-wise; returns the previous 16 bytes
-__device__ __forceinline__ uint4 fop16(char *d, uint4 v, int t, bool swap) {
-    uint4 o;
-    if (swap) {
-        if (DDSK_ACC_LOG2(t) == 3) {
-            const uint64_t a = atom_exch_b64(d, (uint64_t)v.y << 32 | v.x), b = atom_exch_b64(d + 8, (uint64_t)v.w << 32 | v.z);
-            o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
-        } else { // (a 32-bit exchange is atomic for each 16-bit element it holds)
-            o = make_uint4(atom_exch_b32(d, v.x), atom_exch_b32(d + 4, v.y), atom_exch_b32(d + 8, v.z), atom_exch_b32(d + 12, v.w));
-        }
-        return o;
-    }
-    switch (t) {
-    case DDSK_ACC_F32:
-        asm volatile("atom.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
-                     : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
-                     : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-        break;
-    case DDSK_ACC_F64: {
-        const uint64_t a = atom_add_f64(d, (uint64_t)v.y << 32 | v.x), b = atom_add_f64(d + 8, (uint64_t)v.w << 32 | v.z);
-        o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
-        break;
-    }
-    case DDSK_ACC_I32:
-        o = make_uint4(atom_add_u32(d, v.x), atom_add_u32(d + 4, v.y), atom_add_u32(d + 8, v.z), atom_add_u32(d + 12, v.w));
-        break;
-    case DDSK_ACC_I64: {
-        const uint64_t a = atom_add_u64(d, (uint64_t)v.y << 32 | v.x), b = atom_add_u64(d + 8, (uint64_t)v.w << 32 | v.z);
-        o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
-        break;
-    }
-    case DDSK_ACC_F16:
-        asm volatile("atom.relaxed.sys.global.add.noftz.v4.f16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
-                     : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
-                     : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-        break;
-    default:
-        asm volatile("atom.relaxed.sys.global.add.noftz.v4.bf16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
-                     : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
-                     : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-        break;
-    }
-    return o;
-}
 
-// Compare-and-swap (FETCH, op kFopCas), element size 1 << el (warp-uniform): the element becomes the operand where it
+// Compare-and-swap (a fetch-op of op DDSK_OP_CAS), element size 1 << el (warp-uniform): the element becomes the operand where it
 // equals the compare operand bit for bit, and its previous value comes back either way. 4- and 8-byte elements take one
 // atom.cas each (no atom.cas.b128: its behaviour towards a peer over NVLink is not established); 1- and 2-byte elements
 // a compare-and-swap loop on the aligned 32-bit word that holds them (cas_word). .sys scope, as the other fetch-ops.
@@ -552,13 +397,17 @@ __device__ __forceinline__ uint4 cas16(char *d, uint4 v, uint4 c, uint32_t el) {
                       cas_word(d + 12, c.w, v.w, ~0u, el));
 }
 
-// Reductions beside the sum (ACC and FETCH, op = DDSK_RED_MAX.., warp-uniform like the element type t). Integers take
-// the hardware's signed min / max and bitwise reductions and atomics. f16 / bf16 take the bulk, vector and vector-atomic
+// The reductions and fetch-ops of the batched writes: op = DDSK_OP_* and element type t = DDSK_ACC_*, both warp-uniform.
+// Every one is atomic per element: the element ops at .sys scope (a peer's ops on the same shard must combine with the
+// owner's), the bulk reductions at the scope the ISA gives them.
+// Sums: the f32 element and vector reductions flush subnormal inputs and results to zero (atomicAdd's rule; the f32 bulk
+// reduction kept them on H100, see DESIGN.md 3.8); f16 / bf16 are .noftz; f64 is exact IEEE; the integer types wrap.
+// Max / min / bitwise: integers take the hardware's signed min / max and bitwise reductions and atomics. f16 / bf16 take the bulk, vector and vector-atomic
 // max / min, whose maximumNumber / minimumNumber semantics (NaN ignored, -0 < +0, nothing flushed) were measured on H100
 // (DESIGN.md 3.11); there is no scalar 16-bit max / min, so their ragged ends take a compare-and-swap loop on the aligned
 // word. f32 and f64 have no max / min atomic in any form: every element takes a compare-and-swap loop, and the bulk
 // reduction's pieces fall back to the cooperative drain (red_bulk).
-__device__ __forceinline__ bool red_bulk(int t, int op) { return op == DDSK_RED_SUM || (t != DDSK_ACC_F32 && t != DDSK_ACC_F64); }
+__device__ __forceinline__ bool red_bulk(int t, int op) { return op == DDSK_OP_SUM || (t != DDSK_ACC_F32 && t != DDSK_ACC_F64); }
 // maximumNumber (mx) / minimumNumber of the element bits c and operand bits o of a W-bit float (inf: its +inf bits):
 // a NaN operand leaves c, a NaN c takes o, else the larger / smaller by the total order of the bits (so -0 < +0, and
 // subnormals compare exactly whatever the ftz mode). The result is always the bits of c or of o.
@@ -614,29 +463,29 @@ __device__ __forceinline__ uint32_t fmm_word(char *w, uint32_t o, uint32_t m, bo
 // integer reductions, without (red) and with (atom) the previous value
 __device__ __forceinline__ void red_i32(char *d, uint32_t v, int op) {
     switch (op) {
-    case DDSK_RED_MAX: asm volatile("red.relaxed.sys.global.max.s32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
-    case DDSK_RED_MIN: asm volatile("red.relaxed.sys.global.min.s32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
-    case DDSK_RED_AND: asm volatile("red.relaxed.sys.global.and.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
-    case DDSK_RED_OR: asm volatile("red.relaxed.sys.global.or.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_MAX: asm volatile("red.relaxed.sys.global.max.s32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_MIN: asm volatile("red.relaxed.sys.global.min.s32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_BAND: asm volatile("red.relaxed.sys.global.and.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_BOR: asm volatile("red.relaxed.sys.global.or.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
     default: asm volatile("red.relaxed.sys.global.xor.b32 [%0], %1;" ::"l"(d), "r"(v) : "memory"); break;
     }
 }
 __device__ __forceinline__ void red_i64(char *d, uint64_t v, int op) {
     switch (op) {
-    case DDSK_RED_MAX: asm volatile("red.relaxed.sys.global.max.s64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
-    case DDSK_RED_MIN: asm volatile("red.relaxed.sys.global.min.s64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
-    case DDSK_RED_AND: asm volatile("red.relaxed.sys.global.and.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
-    case DDSK_RED_OR: asm volatile("red.relaxed.sys.global.or.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_MAX: asm volatile("red.relaxed.sys.global.max.s64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_MIN: asm volatile("red.relaxed.sys.global.min.s64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_BAND: asm volatile("red.relaxed.sys.global.and.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_BOR: asm volatile("red.relaxed.sys.global.or.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
     default: asm volatile("red.relaxed.sys.global.xor.b64 [%0], %1;" ::"l"(d), "l"(v) : "memory"); break;
     }
 }
 __device__ __forceinline__ uint32_t atom_i32(char *d, uint32_t v, int op) {
     uint32_t o;
     switch (op) {
-    case DDSK_RED_MAX: asm volatile("atom.relaxed.sys.global.max.s32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
-    case DDSK_RED_MIN: asm volatile("atom.relaxed.sys.global.min.s32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
-    case DDSK_RED_AND: asm volatile("atom.relaxed.sys.global.and.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
-    case DDSK_RED_OR: asm volatile("atom.relaxed.sys.global.or.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_MAX: asm volatile("atom.relaxed.sys.global.max.s32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_MIN: asm volatile("atom.relaxed.sys.global.min.s32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_BAND: asm volatile("atom.relaxed.sys.global.and.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
+    case DDSK_OP_BOR: asm volatile("atom.relaxed.sys.global.or.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
     default: asm volatile("atom.relaxed.sys.global.xor.b32 %0, [%1], %2;" : "=r"(o) : "l"(d), "r"(v) : "memory"); break;
     }
     return o;
@@ -644,15 +493,16 @@ __device__ __forceinline__ uint32_t atom_i32(char *d, uint32_t v, int op) {
 __device__ __forceinline__ uint64_t atom_i64(char *d, uint64_t v, int op) {
     uint64_t o;
     switch (op) {
-    case DDSK_RED_MAX: asm volatile("atom.relaxed.sys.global.max.s64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
-    case DDSK_RED_MIN: asm volatile("atom.relaxed.sys.global.min.s64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
-    case DDSK_RED_AND: asm volatile("atom.relaxed.sys.global.and.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
-    case DDSK_RED_OR: asm volatile("atom.relaxed.sys.global.or.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_MAX: asm volatile("atom.relaxed.sys.global.max.s64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_MIN: asm volatile("atom.relaxed.sys.global.min.s64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_BAND: asm volatile("atom.relaxed.sys.global.and.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
+    case DDSK_OP_BOR: asm volatile("atom.relaxed.sys.global.or.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
     default: asm volatile("atom.relaxed.sys.global.xor.b64 %0, [%1], %2;" : "=l"(o) : "l"(d), "l"(v) : "memory"); break;
     }
     return o;
 }
-// the bulk reduction (tma_red_add_1d's rules) of op; red_bulk(t, op) holds
+// shared -> global bulk reduction of op, dst[e] = op(dst[e], staged[e]): tma_store_1d's rules (16-byte aligned addresses
+// and size) and bulk async-group (SASS: UBLKRED); red_bulk(t, op) holds
 __device__ __forceinline__ void tma_red_1d(void *dst_gmem, uint32_t src_smem, uint32_t bytes, int t, int op) {
 #define DDSK_BULK_RED(OPT)                                                                                                     \
     asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group." OPT " [%0], [%1], %2;" ::"l"(dst_gmem), "r"(src_smem), \
@@ -660,24 +510,33 @@ __device__ __forceinline__ void tma_red_1d(void *dst_gmem, uint32_t src_smem, ui
                  : "memory")
     const bool w64 = t == DDSK_ACC_I64;
     switch (op) {
-    case DDSK_RED_SUM: tma_red_add_1d(dst_gmem, src_smem, bytes, t); break;
-    case DDSK_RED_MAX:
+    case DDSK_OP_SUM:
+        switch (t) {
+        case DDSK_ACC_F32: DDSK_BULK_RED("add.f32"); break;
+        case DDSK_ACC_F64: DDSK_BULK_RED("add.f64"); break;
+        case DDSK_ACC_I32: DDSK_BULK_RED("add.u32"); break;
+        case DDSK_ACC_I64: DDSK_BULK_RED("add.u64"); break;
+        case DDSK_ACC_F16: DDSK_BULK_RED("add.noftz.f16"); break;
+        default: DDSK_BULK_RED("add.noftz.bf16"); break;
+        }
+        break;
+    case DDSK_OP_MAX:
         if (t == DDSK_ACC_I32) DDSK_BULK_RED("max.s32");
         else if (t == DDSK_ACC_I64) DDSK_BULK_RED("max.s64");
         else if (t == DDSK_ACC_F16) DDSK_BULK_RED("max.f16");
         else DDSK_BULK_RED("max.bf16");
         break;
-    case DDSK_RED_MIN:
+    case DDSK_OP_MIN:
         if (t == DDSK_ACC_I32) DDSK_BULK_RED("min.s32");
         else if (t == DDSK_ACC_I64) DDSK_BULK_RED("min.s64");
         else if (t == DDSK_ACC_F16) DDSK_BULK_RED("min.f16");
         else DDSK_BULK_RED("min.bf16");
         break;
-    case DDSK_RED_AND:
+    case DDSK_OP_BAND:
         if (w64) DDSK_BULK_RED("and.b64");
         else DDSK_BULK_RED("and.b32");
         break;
-    case DDSK_RED_OR:
+    case DDSK_OP_BOR:
         if (w64) DDSK_BULK_RED("or.b64");
         else DDSK_BULK_RED("or.b32");
         break;
@@ -688,10 +547,24 @@ __device__ __forceinline__ void tma_red_1d(void *dst_gmem, uint32_t src_smem, ui
     }
 #undef DDSK_BULK_RED
 }
-// one element at d (red_add1's rules) of op
+// one element at d: *d = op(*d, the element staged at shared address s) (both aligned to the element size)
 __device__ __forceinline__ void red1(char *d, uint32_t s, int t, int op) {
-    if (op == DDSK_RED_SUM) return red_add1(d, s, t);
-    const bool mx = op == DDSK_RED_MAX;
+    if (op == DDSK_OP_SUM) {
+        switch (t) {
+        case DDSK_ACC_F32:
+            asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(d), "f"(__uint_as_float(lds32(s))) : "memory");
+            break;
+        case DDSK_ACC_F64:
+            asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__longlong_as_double((long long)lds64(s))) : "memory");
+            break;
+        case DDSK_ACC_I32: asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(lds32(s)) : "memory"); break;
+        case DDSK_ACC_I64: asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"(lds64(s)) : "memory"); break;
+        case DDSK_ACC_F16: asm volatile("red.relaxed.sys.global.add.noftz.f16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
+        default: asm volatile("red.relaxed.sys.global.add.noftz.bf16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
+        }
+        return;
+    }
+    const bool mx = op == DDSK_OP_MAX;
     switch (t) {
     case DDSK_ACC_I32: red_i32(d, lds32(s), op); break;
     case DDSK_ACC_I64: red_i64(d, lds64(s), op); break;
@@ -704,10 +577,40 @@ __device__ __forceinline__ void red1(char *d, uint32_t s, int t, int op) {
     }
     }
 }
-// 16 bytes at a 16-byte aligned d (red_add16's rules) of op
+// 16 bytes at a 16-byte aligned d, element-wise: *d = op(*d, v)
 __device__ __forceinline__ void red16(char *d, uint4 v, int t, int op) {
-    if (op == DDSK_RED_SUM) return red_add16(d, v, t);
-    const bool mx = op == DDSK_RED_MAX;
+    if (op == DDSK_OP_SUM) {
+        switch (t) {
+        case DDSK_ACC_F32:
+            asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(d), "f"(__uint_as_float(v.x)),
+                         "f"(__uint_as_float(v.y)), "f"(__uint_as_float(v.z)), "f"(__uint_as_float(v.w)) : "memory");
+            break;
+        case DDSK_ACC_F64:
+            asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__hiloint2double((int)v.y, (int)v.x)) : "memory");
+            asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d + 8), "d"(__hiloint2double((int)v.w, (int)v.z)) : "memory");
+            break;
+        case DDSK_ACC_I32:
+            asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(v.x) : "memory");
+            asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 4), "r"(v.y) : "memory");
+            asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 8), "r"(v.z) : "memory");
+            asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d + 12), "r"(v.w) : "memory");
+            break;
+        case DDSK_ACC_I64:
+            asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"((uint64_t)v.y << 32 | v.x) : "memory");
+            asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d + 8), "l"((uint64_t)v.w << 32 | v.z) : "memory");
+            break;
+        case DDSK_ACC_F16:
+            asm volatile("red.relaxed.sys.global.add.noftz.v4.f16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z),
+                         "r"(v.w) : "memory");
+            break;
+        default:
+            asm volatile("red.relaxed.sys.global.add.noftz.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(v.x), "r"(v.y), "r"(v.z),
+                         "r"(v.w) : "memory");
+            break;
+        }
+        return;
+    }
+    const bool mx = op == DDSK_OP_MAX;
     switch (t) {
     case DDSK_ACC_I32:
         red_i32(d, v.x, op);
@@ -739,9 +642,45 @@ __device__ __forceinline__ void red16(char *d, uint4 v, int t, int op) {
         break;
     }
 }
-// the fetch forms: fop1's and fop16's contracts, of op
-__device__ __forceinline__ void rfop1(char *d, uint32_t s, int t, int op) {
-    const bool mx = op == DDSK_RED_MAX;
+// The fetch forms of red1 and red16, and the swap (DDSK_OP_REPLACE: shard = operand, on elements of 1 << el bytes).
+// One element at d: the operand staged at shared address s is replaced by the element's previous value (both aligned to
+// the element size).
+__device__ __forceinline__ void fetch1(char *d, uint32_t s, int t, int op, uint32_t el) {
+    if (op == DDSK_OP_REPLACE) {
+        switch (el) {
+        case 3: sts64(s, atom_exch_b64(d, lds64(s))); break;
+        case 2: sts32(s, atom_exch_b32(d, lds32(s))); break;
+        default: sts16(s, atom_exch_b16(d, lds16h(s))); break;
+        }
+        return;
+    }
+    if (op == DDSK_OP_SUM) {
+        switch (t) {
+        case DDSK_ACC_F32: {
+            float o;
+            asm volatile("atom.relaxed.sys.global.add.f32 %0, [%1], %2;" : "=f"(o) : "l"(d), "f"(__uint_as_float(lds32(s))) : "memory");
+            sts32(s, __float_as_uint(o));
+            break;
+        }
+        case DDSK_ACC_F64: sts64(s, atom_add_f64(d, lds64(s))); break;
+        case DDSK_ACC_I32: sts32(s, atom_add_u32(d, lds32(s))); break;
+        case DDSK_ACC_I64: sts64(s, atom_add_u64(d, lds64(s))); break;
+        case DDSK_ACC_F16: {
+            unsigned short o;
+            asm volatile("atom.relaxed.sys.global.add.noftz.f16 %0, [%1], %2;" : "=h"(o) : "l"(d), "h"(lds16h(s)) : "memory");
+            sts16(s, o);
+            break;
+        }
+        default: {
+            unsigned short o;
+            asm volatile("atom.relaxed.sys.global.add.noftz.bf16 %0, [%1], %2;" : "=h"(o) : "l"(d), "h"(lds16h(s)) : "memory");
+            sts16(s, o);
+            break;
+        }
+        }
+        return;
+    }
+    const bool mx = op == DDSK_OP_MAX;
     switch (t) {
     case DDSK_ACC_I32: sts32(s, atom_i32(d, lds32(s), op)); break;
     case DDSK_ACC_I64: sts64(s, atom_i64(d, lds64(s), op)); break;
@@ -755,9 +694,52 @@ __device__ __forceinline__ void rfop1(char *d, uint32_t s, int t, int op) {
     }
     }
 }
-__device__ __forceinline__ uint4 rfop16(char *d, uint4 v, int t, int op) {
-    const bool mx = op == DDSK_RED_MAX;
+// 16 bytes at a 16-byte aligned d: the operands v, element-wise; returns the previous 16 bytes
+__device__ __forceinline__ uint4 fetch16(char *d, uint4 v, int t, int op, uint32_t el) {
     uint4 o;
+    if (op == DDSK_OP_REPLACE) {
+        if (el == 3) {
+            const uint64_t a = atom_exch_b64(d, (uint64_t)v.y << 32 | v.x), b = atom_exch_b64(d + 8, (uint64_t)v.w << 32 | v.z);
+            o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+        } else { // (a 32-bit exchange is atomic for each 16-bit element it holds)
+            o = make_uint4(atom_exch_b32(d, v.x), atom_exch_b32(d + 4, v.y), atom_exch_b32(d + 8, v.z), atom_exch_b32(d + 12, v.w));
+        }
+        return o;
+    }
+    if (op == DDSK_OP_SUM) {
+        switch (t) {
+        case DDSK_ACC_F32:
+            asm volatile("atom.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                         : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                         : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+            break;
+        case DDSK_ACC_F64: {
+            const uint64_t a = atom_add_f64(d, (uint64_t)v.y << 32 | v.x), b = atom_add_f64(d + 8, (uint64_t)v.w << 32 | v.z);
+            o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+            break;
+        }
+        case DDSK_ACC_I32:
+            o = make_uint4(atom_add_u32(d, v.x), atom_add_u32(d + 4, v.y), atom_add_u32(d + 8, v.z), atom_add_u32(d + 12, v.w));
+            break;
+        case DDSK_ACC_I64: {
+            const uint64_t a = atom_add_u64(d, (uint64_t)v.y << 32 | v.x), b = atom_add_u64(d + 8, (uint64_t)v.w << 32 | v.z);
+            o = make_uint4((uint32_t)a, (uint32_t)(a >> 32), (uint32_t)b, (uint32_t)(b >> 32));
+            break;
+        }
+        case DDSK_ACC_F16:
+            asm volatile("atom.relaxed.sys.global.add.noftz.v4.f16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                         : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                         : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+            break;
+        default:
+            asm volatile("atom.relaxed.sys.global.add.noftz.v4.bf16x2 {%0,%1,%2,%3}, [%4], {%5,%6,%7,%8};"
+                         : "=r"(o.x), "=r"(o.y), "=r"(o.z), "=r"(o.w)
+                         : "l"(d), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+            break;
+        }
+        return o;
+    }
+    const bool mx = op == DDSK_OP_MAX;
     switch (t) {
     case DDSK_ACC_I32:
         o = make_uint4(atom_i32(d, v.x, op), atom_i32(d + 4, v.y, op), atom_i32(d + 8, v.z, op), atom_i32(d + 12, v.w, op));
@@ -938,8 +920,10 @@ __device__ __forceinline__ int64_t warp_sum(int64_t v) {
     return v;
 }
 
-// the ops of a fetch-op launch (GatherArgs::fop_op)
-constexpr int kFopAdd = 0, kFopSwap = 1, kFopCas = 2;
+// What a gather launch does with its pieces (dds_gather_kernel's WR): a get, or a batched write (GatherArgs::wr) that
+// stores them (a put), reduces them into the shard (an accumulate) or applies a returning atomic (a fetch-op, the
+// compare-and-swap included)
+constexpr int kWrNone = 0, kWrPut = 1, kWrReduce = 2, kWrFetch = 3;
 
 struct GatherArgs {
     ddsk_var_t var;
@@ -972,14 +956,7 @@ struct GatherArgs {
             int pad_log2, pad_in_log2, pad_out_log2; // output element size; source -> output position shifts
             int64_t *pad_lengths;                    // optional [nreq] delivered row counts
         };
-        struct { // accumulates (ACC) and fetch-ops (FETCH), puts: neither padded nor multi-array
-            int acc_type;            // DDSK_ACC_*: the element type of the sum (or swap)
-            int fop_op;              // FETCH: kFopAdd, kFopSwap or kFopCas (warp-uniform)
-            char *fop_result;        // FETCH: the previous values, at the operands' positions (the layout of dst)
-            const char *fop_compare; // kFopCas: the compare operands, at the operands' positions
-            int fop_el;              // kFopCas: log2 of the element size (0..3; acc_type does not apply)
-            int acc_op;              // ACC, and FETCH's kFopAdd: DDSK_RED_SUM or another reduction (warp-uniform)
-        };
+        ddsk_write_t wr; // batched writes (WR != kWrNone): neither padded nor multi-array. op and type are warp-uniform.
     };
     int min_seg_chunks;                // smallest segment, in chunks (claims cost more when the plan is in global memory)
     // ---- overlap protocol (DDS_OVERLAP: a batch declared independent of the ONE batch queued right before it)
@@ -1355,10 +1332,8 @@ struct ChunkWalker {
 // Re-phase loop: output vector j = staged bytes [q16 + 16j + 4*WS + bs, +16). Specialised on the word shift WS
 // (and on whether a sub-word byte shift is needed at all) so the loop body is branch-free: two aligned 128-bit
 // shared loads, at most four funnel shifts, one aligned 128-bit global store.
-// ACC: the vector is reduced into the destination's (red16 of element type acc_t and reduction acc_op) instead of stored.
-template <int WS, bool BYTES, bool ACC = false>
-__device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t nv, uint32_t bs8, int lane, int acc_t = 0,
-                                             int acc_op = 0) {
+template <int WS, bool BYTES>
+__device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t nv, uint32_t bs8, int lane) {
 #pragma unroll 4
     for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
         const uint4 lo = lds128(sbase + (j << 4));
@@ -1376,48 +1351,7 @@ __device__ __forceinline__ void rephase_loop(uint32_t sbase, char *dv, uint32_t 
             out.z = w[WS + 2];
             out.w = w[WS + 3];
         }
-        if constexpr (ACC) red16(dv + ((size_t)j << 4), out, acc_t, acc_op);
-        else stg128(dv + ((size_t)j << 4), out);
-    }
-}
-
-// The fetch-op's re-phase loop: operand vector j (rephase_loop's shift), applied to the shard's 16 bytes at dv + 16j
-// (fop16), and the previous 16 bytes written back over the operand's staged bytes at s + 16j. Those are element-aligned
-// (2-byte elements: s may be 2 mod 4), and the stores touch exactly them: the neighbouring vectors are other lanes'.
-// (rephase_loop is not shared: the existing instantiations' register allocation changed when it was.)
-template <int WS, bool BYTES>
-__device__ __forceinline__ void fop_rephase_loop(uint32_t sbase, uint32_t s, char *dv, uint32_t nv, uint32_t bs8, int lane, int t,
-                                                 bool swap, int op) {
-#pragma unroll 4
-    for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
-        const uint4 lo = lds128(sbase + (j << 4));
-        const uint4 hi = lds128(sbase + (j << 4) + 16);
-        const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-        uint4 v;
-        if (BYTES) {
-            v.x = __funnelshift_r(w[WS + 0], w[WS + 1], bs8);
-            v.y = __funnelshift_r(w[WS + 1], w[WS + 2], bs8);
-            v.z = __funnelshift_r(w[WS + 2], w[WS + 3], bs8);
-            v.w = __funnelshift_r(w[WS + 3], w[WS + 4], bs8);
-        } else {
-            v = make_uint4(w[WS + 0], w[WS + 1], w[WS + 2], w[WS + 3]);
-        }
-        const uint4 o = op == DDSK_RED_SUM ? fop16(dv + ((size_t)j << 4), v, t, swap) : rfop16(dv + ((size_t)j << 4), v, t, op);
-        const uint32_t p = s + (j << 4);
-        if (!BYTES && WS == 0) {
-            sts128(p, o);
-        } else if (!BYTES) {
-            sts32(p, o.x);
-            sts32(p + 4, o.y);
-            sts32(p + 8, o.z);
-            sts32(p + 12, o.w);
-        } else {
-            sts16(p, o.x);
-            sts32(p + 2, __funnelshift_r(o.x, o.y, 16));
-            sts32(p + 6, __funnelshift_r(o.y, o.z, 16));
-            sts32(p + 10, __funnelshift_r(o.z, o.w, 16));
-            sts16(p + 14, o.w >> 16);
-        }
+        stg128(dv + ((size_t)j << 4), out);
     }
 }
 
@@ -1460,21 +1394,97 @@ __device__ __forceinline__ void drain_chunk(uint32_t sb, uint32_t a, char *d, ui
     }
 }
 
-// The accumulate's drain_chunk: the same three cases with every store an atomic reduction op (DDSK_RED_*: the add, or
-// another) of element type t (DDSK_ACC_*). Same phase: lane 0 bulk-reduces the body, if the op has a bulk form for t
-// (red_bulk). Different phase, or no bulk form: re-phased vectors, each reduced (red16). The head and tail, below 16
-// bytes, are reduced element by element by the first lanes (red1). A piece never cuts an element and the caller's rows
-// are element-aligned (see cvt_in_log2), so head, body and tail are whole, aligned elements.
-__device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t, int op) {
-    const uint32_t el = (uint32_t)DDSK_ACC_LOG2(t);
+// The batched writes' drain: what write_chunk does to each element and each re-phased 16-byte vector of a piece.
+// kActReduce: combine it with the shard's (red1 / red16; tma_red_1d for a same-phase body). kActFetch: combine it by a
+// returning atomic (fetch1 / fetch16) and put the previous value back in the stage, over the operand. kActCas: the same
+// with cas1 / cas16 and the piece's compare operands.
+constexpr int kActReduce = 0, kActFetch = 1, kActCas = 2;
+
+// Operand vector j of a piece's body: rephase_loop's shift of the staged bytes. (rephase_loop keeps its own copy: the
+// get instantiations' register allocation changed when a loop was shared with the writes.)
+template <int WS, bool BYTES>
+__device__ __forceinline__ uint4 rephased(uint32_t sbase, uint32_t j, uint32_t bs8) {
+    const uint4 lo = lds128(sbase + (j << 4));
+    const uint4 hi = lds128(sbase + (j << 4) + 16);
+    const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    uint4 v;
+    if (BYTES) {
+        v.x = __funnelshift_r(w[WS + 0], w[WS + 1], bs8);
+        v.y = __funnelshift_r(w[WS + 1], w[WS + 2], bs8);
+        v.z = __funnelshift_r(w[WS + 2], w[WS + 3], bs8);
+        v.w = __funnelshift_r(w[WS + 3], w[WS + 4], bs8);
+    } else {
+        v = make_uint4(w[WS + 0], w[WS + 1], w[WS + 2], w[WS + 3]);
+    }
+    return v;
+}
+
+// ACT applied to operand vector j, for j = lane, lane + 32, .. < nv: the shard's 16 bytes at dv + 16j. The fetch forms
+// write the previous 16 bytes back over the operand's staged bytes at s + 16j with stores that touch exactly them (the
+// neighbouring vectors are other lanes'): a fetch-op's elements are 2, 4 or 8 bytes (s is then 0 or 2 mod 4), a
+// compare-and-swap's may be single bytes (any phase). A compare-and-swap reads compare vector j at cv + 16j, in the
+// compare buffer's own phase.
+template <int ACT, int WS, bool BYTES>
+__device__ __forceinline__ void write_loop(uint32_t sbase, uint32_t s, char *dv, const char *cv, uint32_t nv, uint32_t bs8,
+                                           int lane, int t, int op, uint32_t el) {
+#pragma unroll(ACT == kActCas ? 2 : 4)
+    for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
+        const uint4 v = rephased<WS, BYTES>(sbase, j, bs8);
+        char *const d = dv + ((size_t)j << 4);
+        const uint32_t p = s + (j << 4);
+        if constexpr (ACT == kActReduce) {
+            red16(d, v, t, op);
+        } else if constexpr (ACT == kActFetch) {
+            const uint4 o = fetch16(d, v, t, op, el);
+            if (!BYTES && WS == 0) {
+                sts128(p, o);
+            } else if (!BYTES) {
+                sts32(p, o.x);
+                sts32(p + 4, o.y);
+                sts32(p + 8, o.z);
+                sts32(p + 12, o.w);
+            } else {
+                sts16(p, o.x);
+                sts32(p + 2, __funnelshift_r(o.x, o.y, 16));
+                sts32(p + 6, __funnelshift_r(o.y, o.z, 16));
+                sts32(p + 10, __funnelshift_r(o.z, o.w, 16));
+                sts16(p + 14, o.w >> 16);
+            }
+        } else {
+            const uint4 o = cas16(d, v, ldg16_any(cv + ((size_t)j << 4)), el);
+            if (!BYTES && WS == 0) sts128(p, o);
+            else sts16_any(p, o);
+        }
+    }
+}
+
+// ACT applied to the element of 1 << el bytes at d + k, its operand staged at shared address s + k (and its compare
+// operand at c + k)
+template <int ACT>
+__device__ __forceinline__ void write1(char *d, uint32_t s, const char *c, uint32_t k, int t, int op, uint32_t el) {
+    if constexpr (ACT == kActReduce) red1(d + k, s + k, t, op);
+    else if constexpr (ACT == kActFetch) fetch1(d + k, s + k, t, op, el);
+    else cas1(d + k, s + k, c + k, el);
+}
+
+// A batched write's drain of one staged piece (payload byte k at shared address sb + a + k, shard byte d[k], compare
+// operand c[k] for kActCas), drain_chunk's cut in the shard's 16-byte phase: the head and tail, below 16 bytes, element
+// by element on the first lanes (write1), the body as 16-byte vectors re-phased from the stage (write_loop). A reduction
+// whose body shares the stage's phase, and whose op has a bulk form for t (red_bulk), bulk-reduces it from lane 0
+// instead; no bulk form returns the old values. A piece never cuts an element and the caller's rows are element-aligned
+// (see cvt_in_log2), so head, body and tail are whole, aligned elements. After a fetch form the caller drains the stage,
+// now the previous values, to the result with the raw drain.
+template <int ACT>
+__device__ __forceinline__ void write_chunk(uint32_t sb, uint32_t a, char *d, const char *c, uint32_t n, int lane, int t,
+                                            int op, uint32_t el) {
     uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
     if (head > n) head = n;
-    uint32_t nv = (n - head) >> 4;
-    uint32_t tail = n - head - (nv << 4);
-    uint32_t s = a + head;
-    uint32_t sh = s & 15u;
+    const uint32_t nv = (n - head) >> 4;
+    const uint32_t tail = n - head - (nv << 4);
+    const uint32_t s = a + head;
+    const uint32_t sh = s & 15u;
     if (nv) {
-        if (sh == 0 && red_bulk(t, op)) {
+        if (ACT == kActReduce && sh == 0 && red_bulk(t, op)) {
             if (lane == 0) {
                 fence_proxy_async();
                 tma_red_1d(d + head, sb + s, nv << 4, t, op);
@@ -1483,124 +1493,24 @@ __device__ __forceinline__ void acc_drain_chunk(uint32_t sb, uint32_t a, char *d
             const uint32_t sbase = sb + (s & ~15u);
             const uint32_t bs8 = (sh & 3u) * 8u;
             char *dv = d + head;
+            const char *cv = ACT == kActCas ? c + head : nullptr;
             switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform (2-byte elements: bs8 is 0 or 16)
-            case 0: rephase_loop<0, false, true>(sbase, dv, nv, bs8, lane, t, op); break; // (no bulk form)
-            case 1: rephase_loop<0, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
-            case 2: rephase_loop<1, false, true>(sbase, dv, nv, bs8, lane, t, op); break;
-            case 3: rephase_loop<1, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
-            case 4: rephase_loop<2, false, true>(sbase, dv, nv, bs8, lane, t, op); break;
-            case 5: rephase_loop<2, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
-            case 6: rephase_loop<3, false, true>(sbase, dv, nv, bs8, lane, t, op); break;
-            default: rephase_loop<3, true, true>(sbase, dv, nv, bs8, lane, t, op); break;
+            case 0: write_loop<ACT, 0, false>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
+            case 1: write_loop<ACT, 0, true>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
+            case 2: write_loop<ACT, 1, false>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
+            case 3: write_loop<ACT, 1, true>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
+            case 4: write_loop<ACT, 2, false>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
+            case 5: write_loop<ACT, 2, true>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
+            case 6: write_loop<ACT, 3, false>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
+            default: write_loop<ACT, 3, true>(sbase, sb + s, dv, cv, nv, bs8, lane, t, op, el); break;
             }
         }
     }
-    if ((uint32_t)lane < (head >> el)) red1(d + ((uint32_t)lane << el), sb + a + ((uint32_t)lane << el), t, op);
-    if ((uint32_t)lane < (tail >> el)) {
-        const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
-        red1(d + k, sb + a + k, t, op);
-    }
-}
-
-// The fetch-op's first pass over one staged piece (payload byte k at shared address sb + a + k, shard byte d[k]): every
-// element is combined with the shard's by a returning atomic (fop1 / fop16) in the shard's 16-byte phase -- the head and
-// tail element by element, the body as 16-byte vectors re-phased like acc_drain_chunk's -- and its previous value replaces
-// the operand in the stage. (No bulk form returns the old values.) The caller then drains the stage to the result with
-// the raw drain. Head, body and tail are whole, aligned elements, as in acc_drain_chunk. op: DDSK_RED_SUM for the add
-// and the swap, else the reduction (rfop1 / rfop16).
-__device__ __forceinline__ void fop_chunk(uint32_t sb, uint32_t a, char *d, uint32_t n, int lane, int t, bool swap, int op) {
-    const uint32_t el = (uint32_t)DDSK_ACC_LOG2(t);
-    uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
-    if (head > n) head = n;
-    const uint32_t nv = (n - head) >> 4;
-    const uint32_t tail = n - head - (nv << 4);
-    const uint32_t s = a + head;
-    const uint32_t sh = s & 15u;
-    if (nv) {
-        const uint32_t sbase = sb + (s & ~15u);
-        const uint32_t bs8 = (sh & 3u) * 8u;
-        char *dv = d + head;
-        switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform (2-byte elements: bs8 is 0 or 16)
-        case 0: fop_rephase_loop<0, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        case 1: fop_rephase_loop<0, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        case 2: fop_rephase_loop<1, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        case 3: fop_rephase_loop<1, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        case 4: fop_rephase_loop<2, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        case 5: fop_rephase_loop<2, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        case 6: fop_rephase_loop<3, false>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        default: fop_rephase_loop<3, true>(sbase, sb + s, dv, nv, bs8, lane, t, swap, op); break;
-        }
-    }
     if ((uint32_t)lane < (head >> el)) {
-        const uint32_t k = (uint32_t)lane << el;
-        if (op == DDSK_RED_SUM) fop1(d + k, sb + a + k, t, swap);
-        else rfop1(d + k, sb + a + k, t, op);
+        write1<ACT>(d, sb + a, c, (uint32_t)lane << el, t, op, el);
     }
     if ((uint32_t)lane < (tail >> el)) {
-        const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
-        if (op == DDSK_RED_SUM) fop1(d + k, sb + a + k, t, swap);
-        else rfop1(d + k, sb + a + k, t, op);
-    }
-}
-
-// The compare-and-swap's fop_rephase_loop: operand vector j re-phased from the stage, compare vector j read from global
-// memory at cv + 16j in its own phase (the compare buffer's, not the shard's), cas16 on the shard's 16 bytes at dv + 16j,
-// and the previous 16 bytes written back over the operand's staged bytes at s + 16j (any phase: 1-byte elements).
-template <int WS, bool BYTES>
-__device__ __forceinline__ void cas_rephase_loop(uint32_t sbase, uint32_t s, char *dv, const char *cv, uint32_t nv,
-                                                 uint32_t bs8, int lane, uint32_t el) {
-#pragma unroll 2
-    for (uint32_t j = (uint32_t)lane; j < nv; j += 32) {
-        const uint4 lo = lds128(sbase + (j << 4));
-        const uint4 hi = lds128(sbase + (j << 4) + 16);
-        const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-        uint4 v;
-        if (BYTES) {
-            v.x = __funnelshift_r(w[WS + 0], w[WS + 1], bs8);
-            v.y = __funnelshift_r(w[WS + 1], w[WS + 2], bs8);
-            v.z = __funnelshift_r(w[WS + 2], w[WS + 3], bs8);
-            v.w = __funnelshift_r(w[WS + 3], w[WS + 4], bs8);
-        } else {
-            v = make_uint4(w[WS + 0], w[WS + 1], w[WS + 2], w[WS + 3]);
-        }
-        const uint4 o = cas16(dv + ((size_t)j << 4), v, ldg16_any(cv + ((size_t)j << 4)), el);
-        if (!BYTES && WS == 0) sts128(s + (j << 4), o);
-        else sts16_any(s + (j << 4), o);
-    }
-}
-
-// The compare-and-swap's first pass over one staged piece: fop_chunk's cuts and phases, with the piece's compare
-// operands at c[k] (payload byte k) and elements of 1 << el bytes. Only the piece's own compare bytes are read.
-__device__ __forceinline__ void cas_chunk(uint32_t sb, uint32_t a, char *d, const char *c, uint32_t n, int lane, uint32_t el) {
-    uint32_t head = (16u - (uint32_t)((uint64_t)d & 15u)) & 15u;
-    if (head > n) head = n;
-    const uint32_t nv = (n - head) >> 4;
-    const uint32_t tail = n - head - (nv << 4);
-    const uint32_t s = a + head;
-    const uint32_t sh = s & 15u;
-    if (nv) {
-        const uint32_t sbase = sb + (s & ~15u);
-        const uint32_t bs8 = (sh & 3u) * 8u;
-        char *dv = d + head;
-        const char *cv = c + head;
-        switch ((sh >> 2) * 2u + (bs8 ? 1u : 0u)) { // warp-uniform
-        case 0: cas_rephase_loop<0, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        case 1: cas_rephase_loop<0, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        case 2: cas_rephase_loop<1, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        case 3: cas_rephase_loop<1, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        case 4: cas_rephase_loop<2, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        case 5: cas_rephase_loop<2, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        case 6: cas_rephase_loop<3, false>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        default: cas_rephase_loop<3, true>(sbase, sb + s, dv, cv, nv, bs8, lane, el); break;
-        }
-    }
-    if ((uint32_t)lane < (head >> el)) {
-        const uint32_t k = (uint32_t)lane << el;
-        cas1(d + k, sb + a + k, c + k, el);
-    }
-    if ((uint32_t)lane < (tail >> el)) {
-        const uint32_t k = head + (nv << 4) + ((uint32_t)lane << el);
-        cas1(d + k, sb + a + k, c + k, el);
+        write1<ACT>(d, sb + a, c, head + (nv << 4) + ((uint32_t)lane << el), t, op, el);
     }
 }
 
@@ -2019,7 +1929,7 @@ struct PieceDesc {
     int64_t dpos;
     uint32_t n, pack; // pack = stage offset | (source misalignment << 16)
 };
-// FETCH: the shared address of a piece's result address, [NW][S][32] in dynamic shared memory behind the rings and the
+// kWrFetch: the shared address of a piece's result address, [NW][S][32] in dynamic shared memory behind the rings and the
 // plan. (A function: a constant of the kernel itself changed the other instantiations' register allocation.)
 template <int NW, int S, int STAGE, int PCAP>
 __device__ __forceinline__ uint32_t fop_rdst(const unsigned char *smem_dyn, int warp, uint32_t st, int lane) {
@@ -2047,7 +1957,8 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // since a multi-array launch may mix normalised, plainly converted and raw variables.
 // PAD (with FIXED): a padded batch -- a fixed-stride walk over slots of a.pad_slot source bytes (see ChunkWalker), the
 // padding filled by the warps that claim it, the lengths written after the walk. No plan, no offsets, no push fetch.
-// PUT: a batched put (DDSK_F_PUT) -- the raw walk with every copy reversed. Lookup, checks, plan, segment claims and
+// WR: a get (kWrNone) or a batched write (a.wr). kWrPut, a batched put (DDSK_OP_PUT) -- the raw walk with every copy
+// reversed. Lookup, checks, plan, segment claims and
 // status reports are the gather's; a piece's TMA load reads its packed position in a.dst (the caller's rows, a.dst_cap
 // bytes) and the drain writes its shard address, through the same drain paths, which store exactly the piece's bytes
 // (plain byte / 16-byte stores and bulk stores, never a read-modify-write of a neighbouring byte: other warps and other
@@ -2055,27 +1966,25 @@ __device__ __forceinline__ void spin_until_done(const unsigned int *ovl, unsigne
 // zero. The load reads the 16-byte-aligned superset of the piece's range in the caller's buffer: up to 15 bytes on
 // either side that belong to no request, in the same 16-byte block (which never crosses a page), whose values are
 // discarded. Never overlapped, no offsets, no conversion, no push.
-// ACC (with PUT): a batched accumulate (DDSK_F_ACC) -- the put whose drain adds (or reduces by a.acc_op) instead of
-// storing, in the element type a.acc_type: bulk reductions where the put bulk-stores (and the op has a bulk form),
-// element reductions for the ragged ends, vector reductions of the re-phased body. Each is atomic per element, so
-// requests of any batch or rank that hit the same element combine.
-// FETCH (with PUT): a batched fetch-op (DDSK_F_FOP) -- the put whose drain applies a returning atomic (add, swap or
-// compare-and-swap, a.fop_op; add and swap in the element type a.acc_type, compare-and-swap on 1 << a.fop_el bytes) to
-// every element and sends the previous values to a.fop_result, at the operands' positions. Every piece is drained
-// cooperatively in two passes: fop_chunk (cas_chunk) replaces the staged operands by the previous values, then the raw
-// drain (bulk stores where the phases allow) writes the stage to the result. The result address of each piece is kept beside its descriptor, in dynamic shared memory behind the rings and the plan.
-template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
-          bool ACC = false, bool FETCH = false, bool HOST = false>
+// kWrReduce: a batched accumulate -- the put whose drain reduces by a.wr.op (the sum or another) instead of storing, in
+// the element type a.wr.type: bulk reductions where the put bulk-stores (and the op has a bulk form), element reductions
+// for the ragged ends, vector reductions of the re-phased body (write_chunk). Each is atomic per element, so requests of
+// any batch or rank that hit the same element combine.
+// kWrFetch: a batched fetch-op -- the put whose drain applies a returning atomic (a.wr.op, in the element type a.wr.type;
+// a compare-and-swap on 1 << a.wr.el_log2 bytes) to every element and sends the previous values to a.wr.result, at the
+// operands' positions. Every piece is drained cooperatively in two passes: write_chunk replaces the staged operands by
+// the previous values, then the raw drain (bulk stores where the phases allow) writes the stage to the result. The result
+// address of each piece is kept beside its descriptor, in dynamic shared memory behind the rings and the plan.
+template <bool FIXED, int NW, int S, int CH, int PCAP, bool CVT = false, bool NORM = false, bool PAD = false,
+          int WR = kWrNone, bool HOST = false>
 __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_constant__ GatherArgs a,
                                                                 const __grid_constant__ CvtParam<CVT> c) {
     static_assert(CVT || !NORM, "a normalising launch is a converting one");
     static_assert(FIXED || !PAD, "a padded batch is a fixed-stride walk");
-    static_assert(!PUT || (!CVT && !PAD), "a put writes raw rows");
-    static_assert(PUT || !ACC, "an accumulate is a put that adds");
-    static_assert((PUT && !ACC) || !FETCH, "a fetch-op is a put that returns the previous rows");
-    static_assert(!HOST || !PUT, "HOST shards take no batched writes");
+    static_assert(WR == kWrNone || (!CVT && !PAD), "a write writes raw rows");
+    static_assert(!HOST || WR == kWrNone, "HOST shards take no batched writes");
     constexpr int STAGE = CH + 32; // room for the aligned superset of a misaligned CH-byte range
-    constexpr bool PUSH = FIXED && !CVT && !PAD && !PUT;
+    constexpr bool PUSH = FIXED && !CVT && !PAD && WR == kWrNone;
     extern __shared__ __align__(128) unsigned char smem_dyn[];
     __shared__ __align__(8) uint64_t full_bar[NW][S];
     __shared__ __align__(16) PieceDesc desc[NW][S][32];
@@ -2126,14 +2035,14 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
     };
 
     // ---- the plan (variable counts) ------------------------------------------------------------
-    ChunkWalker<FIXED, CH, PCAP, CVT, PAD, PUT> w;
+    ChunkWalker<FIXED, CH, PCAP, CVT, PAD, WR != kWrNone> w; // (every write walks, plans and checks as a put)
     if (!FIXED) {
         if constexpr (PCAP > 0) {
             w.pv.src_s = smem_u32(smem_dyn) + (uint32_t)(NW * S * STAGE);
             w.pv.dst_s = w.pv.src_s + (uint32_t)PCAP * 8u;
             const bool writer = blockIdx.x == 0;
             if (writer) pass_gate(); // CTA 0 writes the offsets / the total for the caller
-            w.T = plan_in_smem<NW, PCAP, CVT, NORM, PUT>(a, w.pv, wtot, warp, lane, writer, code0);
+            w.T = plan_in_smem<NW, PCAP, CVT, NORM, WR != kWrNone>(a, w.pv, wtot, warp, lane, writer, code0);
         } else {
             w.pv.src = a.req_src;
             w.pv.dst = a.req_dst;
@@ -2372,9 +2281,9 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
             desc[warp][st][lane].dpos = pc.dpos;
             desc[warp][st][lane].n = pc.n;
             desc[warp][st][lane].pack = pc.off | (al << 16);
-            if constexpr (FETCH) // the piece's result address: its source position, in the result buffer
+            if constexpr (WR == kWrFetch) // the piece's result address: its source position, in the result buffer
                 sts64(fop_rdst<NW, S, STAGE, PCAP>(smem_dyn, warp, st, lane),
-                      pc.n ? (uint64_t)a.fop_result + (pc.src - (uint64_t)a.dst) : 0);
+                      pc.n ? (uint64_t)a.wr.result + (pc.src - (uint64_t)a.dst) : 0);
             if constexpr (HOST) {
                 // A source in mapped host memory never goes to the TMA unit. The lanes copy each piece's 16-byte-aligned
                 // superset window together, 16 bytes per cp.async, and every lane's arrival completes the stage.
@@ -2420,9 +2329,9 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         const int64_t my_dpos = desc[warp][st][lane].dpos;
         const uint32_t my_n = desc[warp][st][lane].n;
         const uint32_t my_pack = desc[warp][st][lane].pack;
-        if constexpr (FETCH) {
+        if constexpr (WR == kWrFetch) {
             // fetch-op: pass 1, the atomics, every piece cooperatively; pass 2, the previous values to the result. A
-            // compare-and-swap finds a piece's compare operands at its result address's position in a.fop_compare; pass 1
+            // compare-and-swap finds a piece's compare operands at its result address's position in a.wr.compare; pass 1
             // has read them all before pass 2 writes a result byte (result == compare is allowed).
             char *const my_res = (char *)lds64(fop_rdst<NW, S, STAGE, PCAP>(smem_dyn, warp, st, lane));
             unsigned todo = __ballot_sync(0xffffffffu, my_n != 0);
@@ -2431,13 +2340,14 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
                 const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
                 const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
-                if (a.fop_op == kFopCas) {
+                if (a.wr.op == DDSK_OP_CAS) {
                     const uint64_t r = __shfl_sync(0xffffffffu, (uint64_t)my_res, j);
-                    cas_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos,
-                              a.fop_compare + (r - (uint64_t)a.fop_result), n, lane, (uint32_t)a.fop_el);
+                    write_chunk<kActCas>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos,
+                                         (const char *)a.wr.compare + (r - (uint64_t)a.wr.result), n, lane, a.wr.type,
+                                         a.wr.op, (uint32_t)a.wr.el_log2);
                 } else {
-                    fop_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type,
-                              a.fop_op == kFopSwap, a.acc_op);
+                    write_chunk<kActFetch>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, nullptr, n, lane,
+                                           a.wr.type, a.wr.op, (uint32_t)a.wr.el_log2);
                 }
             }
             fence_proxy_async(); // (every lane: its stage writes, before any lane's bulk store reads them)
@@ -2453,14 +2363,14 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
                 drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, d, n, lane);
             }
-        } else if constexpr (PUT) {
+        } else if constexpr (WR != kWrNone) {
             // put: the raw drain (the last branch) into the shard address the descriptor carries -- a branch of its own,
             // so that the raw instantiations compile exactly as they did
             char *const my_dst = (char *)my_dpos;
             bool direct = my_n != 0 && (((uint32_t)(uint64_t)my_dst | my_n | (my_pack >> 16)) & 15u) == 0;
-            if constexpr (ACC) {
-                direct = direct && red_bulk(a.acc_type, a.acc_op);
-                if (direct) tma_red_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n, a.acc_type, a.acc_op);
+            if constexpr (WR == kWrReduce) {
+                direct = direct && red_bulk(a.wr.type, a.wr.op);
+                if (direct) tma_red_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n, a.wr.type, a.wr.op);
             } else {
                 if (direct) tma_store_1d(my_dst, ring + st * STAGE + (my_pack & 0xffffu), my_n);
             }
@@ -2471,8 +2381,10 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
                 const int64_t dpos = __shfl_sync(0xffffffffu, my_dpos, j);
                 const uint32_t n = __shfl_sync(0xffffffffu, my_n, j);
                 const uint32_t pk = __shfl_sync(0xffffffffu, my_pack, j);
-                if constexpr (ACC)
-                    acc_drain_chunk(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane, a.acc_type, a.acc_op);
+                if constexpr (WR == kWrReduce) // (the element size from the type: read from the record, it cost the
+                                                // fixed-count form two registers)
+                    write_chunk<kActReduce>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, nullptr, n, lane,
+                                            a.wr.type, a.wr.op, (uint32_t)DDSK_ACC_LOG2(a.wr.type));
                 else drain_chunk<CH>(ring + st * STAGE + (pk & 0xffffu), pk >> 16, (char *)dpos, n, lane);
             }
         } else if constexpr (CVT) {
@@ -2530,7 +2442,7 @@ __global__ void __launch_bounds__(NW * 32, 1) dds_gather_kernel(const __grid_con
         __syncwarp();  // all lanes are done reading the stage before it is refilled
         consumed++;
     }
-    if (PUT || a.overlap || (FIXED && push)) {
+    if (WR != kWrNone || a.overlap || (FIXED && push)) {
         // every lane: its bulk stores have been performed (the done / arrive word below promises that; a put's rows are
         // complete when its last warp finishes)
         bulk_wait_all<0>();
@@ -3045,14 +2957,14 @@ bool cvt_has_norm(const ddsk_cvt_t *cvt) {
     return false;
 }
 
-template <bool FIXED, const Geometry &G, bool CVT = false, bool NORM = false, bool PAD = false, bool PUT = false,
-          bool ACC = false, bool FETCH = false, bool HOST = false>
+template <bool FIXED, const Geometry &G, bool CVT = false, bool NORM = false, bool PAD = false, int WR = kWrNone,
+          bool HOST = false>
 int launch_gather_t(const GatherArgs &args_in, cudaStream_t stream, const ddsk_cvt_t *cvt = nullptr) {
     // (a converting launch also holds its tables in dynamic shared memory, behind the rings and the plan; a fetch-op its
     //  pieces' result addresses)
-    const int smem = smem_bytes_of(G) + (CVT ? cvt->lut_bytes : 0) + (FETCH ? G.nw * G.stages * 32 * 8 : 0);
+    const int smem = smem_bytes_of(G) + (CVT ? cvt->lut_bytes : 0) + (WR == kWrFetch ? G.nw * G.stages * 32 * 8 : 0);
     static std::atomic<unsigned long long> configured{0}; // bit d: attribute set on device d (it is per device)
-    auto kern = dds_gather_kernel<FIXED, G.nw, G.stages, G.ch, G.pcap, CVT, NORM, PAD, PUT, ACC, FETCH, HOST>;
+    auto kern = dds_gather_kernel<FIXED, G.nw, G.stages, G.ch, G.pcap, CVT, NORM, PAD, WR, HOST>;
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (CVT) { // the most a converting launch can ask for: every table at its widest
@@ -3139,13 +3051,13 @@ int launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, A
     return 0;
 }
 
-// One launch of the kind the flags ask for: a fetch-op at geometry GF, every other kind (accumulate, put, normalising,
-// converting, raw) at G.
+// One launch of the kind asked for (wr: kWr*; cvt): a fetch-op at geometry GF, every other kind (accumulate, put,
+// normalising, converting, raw) at G.
 template <bool FIXED, const Geometry &G, const Geometry &GF>
-int launch_kind(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put, bool acc, bool fop) {
-    if (fop) return launch_gather_t<FIXED, GF, false, false, false, true, false, true>(args, stream);
-    if (acc) return launch_gather_t<FIXED, G, false, false, false, true, true>(args, stream);
-    if (put) return launch_gather_t<FIXED, G, false, false, false, true>(args, stream);
+int launch_kind(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, int wr) {
+    if (wr == kWrFetch) return launch_gather_t<FIXED, GF, false, false, false, kWrFetch>(args, stream);
+    if (wr == kWrReduce) return launch_gather_t<FIXED, G, false, false, false, kWrReduce>(args, stream);
+    if (wr == kWrPut) return launch_gather_t<FIXED, G, false, false, false, kWrPut>(args, stream);
     if (cvt) return cvt_has_norm(cvt) ? launch_gather_t<FIXED, G, true, true>(args, stream, cvt)
                                       : launch_gather_t<FIXED, G, true>(args, stream, cvt);
     return launch_gather_t<FIXED, G>(args, stream);
@@ -3154,22 +3066,21 @@ int launch_kind(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *c
 // a read of HOST shards (never a write: the store refuses those), raw, converting or normalising
 template <bool FIXED, bool PAD = false>
 int launch_host(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt) {
-    if (!cvt) return launch_gather_t<FIXED, kLargeRows, false, false, PAD, false, false, false, true>(args, stream);
-    return cvt_has_norm(cvt) ? launch_gather_t<FIXED, kLargeRows, true, true, PAD, false, false, false, true>(args, stream, cvt)
-                             : launch_gather_t<FIXED, kLargeRows, true, false, PAD, false, false, false, true>(args, stream, cvt);
+    if (!cvt) return launch_gather_t<FIXED, kLargeRows, false, false, PAD, kWrNone, true>(args, stream);
+    return cvt_has_norm(cvt) ? launch_gather_t<FIXED, kLargeRows, true, true, PAD, kWrNone, true>(args, stream, cvt)
+                             : launch_gather_t<FIXED, kLargeRows, true, false, PAD, kWrNone, true>(args, stream, cvt);
 }
 
 // plan in global memory (or none): small rows for fixed-count raw gets of requests under 2 KiB, large rows otherwise
 template <bool FIXED>
-int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, bool put = false, bool acc = false,
-                  bool fop = false) {
+int launch_gather(const GatherArgs &args, cudaStream_t stream, const ddsk_cvt_t *cvt, int wr = kWrNone) {
     if (args.var.host) return launch_host<FIXED>(args, stream, cvt);
     if constexpr (FIXED) {
         // (a count too large to multiply safely counts as large)
         const int64_t request_bytes = args.count < ((int64_t)1 << 20) ? args.count * args.var.row_bytes : INT64_MAX;
-        if (!put && !acc && !fop && !cvt && request_bytes < 2048) return launch_gather_t<true, kSmallRows>(args, stream);
+        if (wr == kWrNone && !cvt && request_bytes < 2048) return launch_gather_t<true, kSmallRows>(args, stream);
     }
-    return launch_kind<FIXED, kLargeRows, kFetch>(args, stream, cvt, put, acc, fop);
+    return launch_kind<FIXED, kLargeRows, kFetch>(args, stream, cvt, wr);
 }
 
 // The shared-memory plan for a batch of nreq requests into cap bytes: 0 = kPlan4K, 1 = kPlan8K (-1: the plan kernels).
@@ -3202,17 +3113,15 @@ int gather_args(GatherArgs &a, const ddsk_var_t *var, const ddsk_scratch_t *scr,
     // GPU either); the variable-count entries set the slot's own word below (their CTAs
     // may start late, behind the plan kernel, and must not keep a fixed share of the work).
     a.tickets = a.overlap ? nullptr : scr->counters;
-    if (flags & (DDSK_F_ACC | DDSK_F_FOP)) {
-        a.acc_type = DDSK_F_ACC_TYPE(flags);
-        a.acc_op = DDSK_F_RED_OP(flags);
-    }
-    if (flags & DDSK_F_FOP) {
-        a.fop_op = (flags & DDSK_F_FOP_CAS) ? kFopCas : (flags & DDSK_F_FOP_SWAP) ? kFopSwap : kFopAdd;
-        a.fop_result = (char *)scr->fop_result;
-        a.fop_compare = (const char *)scr->fop_compare;
-        a.fop_el = DDSK_F_ACC_TYPE(flags); // (a compare-and-swap's log2 element size, in the element type's bits)
-    }
     return 0;
+}
+
+// The kernel form of a launch that carries the write record wr (NULL for a get), which then goes into a.wr: op 0 is a
+// put, a record without a result a reduction, one with a result a fetch-op
+int write_form(GatherArgs &a, const ddsk_write_t *wr) {
+    if (!wr) return kWrNone;
+    a.wr = *wr;
+    return wr->op == DDSK_OP_PUT ? kWrPut : wr->result ? kWrFetch : kWrReduce;
 }
 
 } // namespace
@@ -3248,18 +3157,18 @@ void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk
 
 int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t count, int64_t nreq, void *dst_dev,
                       int64_t dst_capacity, int64_t *offsets_dev_or_null, const ddsk_scratch_t *scr, int flags,
-                      const ddsk_cvt_t *cvt, void *stream) {
+                      const ddsk_cvt_t *cvt, const ddsk_write_t *wr, void *stream) {
     if (nreq <= 0) return 0;
     GatherArgs a;
     if (int rc = gather_args(a, var, scr, flags)) return rc;
+    const int form = write_form(a, wr);
     a.starts = starts_dev;
     a.count = count;
     a.nreq = nreq;
     a.dst = (char *)dst_dev;
     a.dst_cap = dst_capacity;
     a.offsets_out = offsets_dev_or_null;
-    return launch_gather<true>(a, (cudaStream_t)stream, cvt, (flags & DDSK_F_PUT) != 0, (flags & DDSK_F_ACC) != 0,
-                               (flags & DDSK_F_FOP) != 0);
+    return launch_gather<true>(a, (cudaStream_t)stream, cvt, form);
 }
 
 int ddsk_gather_push(const ddsk_var_t *var, const ddsk_push_t *push_host, const ddsk_push_t *push_dev,
@@ -3309,22 +3218,21 @@ int ddsk_gather_padded(const ddsk_var_t *var, const ddsk_index_t *index, int64_t
 }
 
 // shared by ddsk_gather_var / ddsk_gather_multi: plan (in the launch, or by the two plan kernels) + gather. `a` comes
-// from gather_args.
+// from gather_args; form is write_form's.
 static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq, int64_t cap_total, GatherArgs &a,
-                           int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt,
+                           int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt, int form,
                            cudaStream_t st) {
     a.nreq = nreq;
     a.plan = p; // the gather needs nvars / per_var even when the plan ran in its own kernels
     a.total_out = scr->total;
-    const bool put = (flags & DDSK_F_PUT) != 0, acc = (flags & DDSK_F_ACC) != 0, fop = (flags & DDSK_F_FOP) != 0;
     const int gs = select_s(nreq, cap_total, cvt, a.var.host != 0);
     if (gs >= 0) {
         a.offsets_out = offsets_dev_or_null;
         a.min_seg_chunks = g_min_seg_s;
         // (no scratch is shared between launches: independent batches may overlap)
         if (a.overlap) a.tickets = scr->ovl + 8 + (a.seq & 3u);
-        return gs ? launch_kind<false, kPlan8K, kPlan8KFetch>(a, st, cvt, put, acc, fop)
-                  : launch_kind<false, kPlan4K, kPlan4K>(a, st, cvt, put, acc, fop);
+        return gs ? launch_kind<false, kPlan8K, kPlan8KFetch>(a, st, cvt, form)
+                  : launch_kind<false, kPlan4K, kPlan4K>(a, st, cvt, form);
     }
     if (nreq > scr->cap_req || cap_total / SEG_GRAIN + 2 > scr->seg_cap) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_gather_var: scratch too small (%lld requests > %lld, or %lld segments > %lld)",
@@ -3352,7 +3260,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
         g_l2_base = p.tab ? (const void *)p.tab : (const void *)p.mtab[0];
         g_l2_bytes = (size_t)(p.tab ? p.nsamples : p.mnsamples[0]) * 16;
     }
-    if (int rc = launch_pdl(put ? dds_plan_kernel<true> : dds_plan_kernel<false>, dim3(tiles), dim3(PLAN_THREADS), st, *var, p, nreq, scr->req_src, scr->req_dst,
+    if (int rc = launch_pdl(form != kWrNone ? dds_plan_kernel<true> : dds_plan_kernel<false>, dim3(tiles), dim3(PLAN_THREADS), st, *var, p, nreq, scr->req_src, scr->req_dst,
                             (unsigned long long *)scr->tile_sums, scr->plan_tag, offsets_dev_or_null, scr->seg_tab, scr->seg_cap,
                             scr->status, scr->status_tag, pr, cvt && p.nvars <= 1 ? (int)cvt->code[0] : 0))
         return rc;
@@ -3368,7 +3276,7 @@ static int plan_and_gather(const ddsk_var_t *var, const PlanSrc &p, int64_t nreq
         a.plan_word = scr->plan_word;
         a.plan_tiles = tiles;
     }
-    return launch_gather<false>(a, st, cvt, put, acc, fop);
+    return launch_gather<false>(a, st, cvt, form);
 }
 
 int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt, int host) {
@@ -3377,10 +3285,12 @@ int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *
 }
 
 int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, void *dst_dev, int64_t dst_capacity,
-                    int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt, void *stream) {
+                    int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags, const ddsk_cvt_t *cvt,
+                    const ddsk_write_t *wr, void *stream) {
     if (nreq <= 0) return 0;
     GatherArgs a;
     if (int rc = gather_args(a, var, scr, flags)) return rc;
+    const int form = write_form(a, wr);
     PlanSrc p;
     memset(&p, 0, sizeof(p));
     p.starts = index->starts;
@@ -3390,7 +3300,7 @@ int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nr
     p.nsamples = index->nsamples;
     a.dst = (char *)dst_dev;
     a.dst_cap = dst_capacity;
-    return plan_and_gather(var, p, nreq, dst_capacity, a, offsets_dev_or_null, scr, flags, cvt, (cudaStream_t)stream);
+    return plan_and_gather(var, p, nreq, dst_capacity, a, offsets_dev_or_null, scr, flags, cvt, form, (cudaStream_t)stream);
 }
 
 int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int64_t nreq, ddsk_scratch_t *scr, int flags,
@@ -3424,7 +3334,7 @@ int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int6
         a.mcap[v] = m->cap[v];
         a.moffsets[v] = m->offsets[v];
     }
-    return plan_and_gather(&dummy, p, nreq * m->nvars, cap_total, a, nullptr, scr, flags, cvt, (cudaStream_t)stream);
+    return plan_and_gather(&dummy, p, nreq * m->nvars, cap_total, a, nullptr, scr, flags, cvt, kWrNone, (cudaStream_t)stream);
 }
 
 int ddsk_small_get(const ddsk_var_t *var, int64_t start, int64_t count, void *dst, int64_t dst_capacity,

@@ -60,10 +60,6 @@ typedef struct ddsk_scratch {
     int64_t seg_cap;
     unsigned long long *host_mirror; /* device alias of pinned host words: [0] status, [1] packed total (written by the
                                         last warp of a gather launch that asks for it), [2] ticket of dds_small_get */
-    void *fop_result;           /* host side, set by the caller of a DDSK_F_FOP launch: the caller's result buffer (device
-                                   memory, the layout of the source rows) */
-    const void *fop_compare;    /* host side, set by the caller of a DDSK_F_FOP_CAS launch: the caller's compare operands
-                                   (device memory, the layout of the source rows) */
 } ddsk_scratch_t;
 
 /* `flags` of the launchers */
@@ -74,38 +70,38 @@ typedef struct ddsk_scratch {
 #define DDSK_F_PREV1 32     /* overlap launch ovl_seq-1 belongs to the same run (retire after it) */
 #define DDSK_F_PREV2 64     /* overlap launch ovl_seq-2 belongs to the same run (do not write before it retired) */
 #define DDSK_F_PREV4 128    /* overlap launch ovl_seq-4 belongs to the same run (it used the same plan scratch slot) */
-#define DDSK_F_PUT 256      /* a batched put (ddsk_gather_fixed / ddsk_gather_var, raw, never with DDSK_F_OVERLAP): the same
-                               walk with every copy reversed. dst_dev is the caller's packed SOURCE rows and dst_capacity
-                               its size; request i's bytes are taken from its packed position and written to its rows in
-                               the owner's shard. The layout keeps an invalid request's bytes (count * row_bytes when
-                               0 < count <= the variable's rows, else 0; 0 for a sample id outside the index); it writes
-                               nothing, like a layout above dst_capacity. No offsets. */
-#define DDSK_F_ACC 512      /* with DDSK_F_PUT: a batched accumulate -- the put's walk, layout and checks, whose drain adds
-                               every staged element to the shard's (atomically) instead of storing it. The element type
-                               is DDSK_F_ACC_TYPE(flags); the caller's rows are aligned to its size. */
-#define DDSK_F_ACC_SHIFT 10 /* bits 10..12 of the flags: the accumulate's element type (DDSK_ACC_*) */
-#define DDSK_F_ACC_TYPE(f) (((f) >> DDSK_F_ACC_SHIFT) & 7)
-#define DDSK_F_FOP 8192     /* with DDSK_F_PUT: a batched fetch-op -- the put's walk, layout and checks, whose drain applies
-                               an atomic that returns each element's previous value and writes that value to the same
-                               position of scr->fop_result as the operand's in the caller's rows. The element type is
-                               DDSK_F_ACC_TYPE(flags); the caller's rows and fop_result are aligned to its size. */
-#define DDSK_F_FOP_SWAP 16384 /* with DDSK_F_FOP: the op is a swap (shard = src); else an add (shard = shard + src) */
-#define DDSK_F_FOP_CAS 32768  /* with DDSK_F_FOP: the op is a compare-and-swap (shard = src where shard == compare, bit for
-                                 bit, at the same position of scr->fop_compare). Bits 10..12 of the flags then hold log2 of
-                                 the element size (0..3), not an element type; src, compare and result are aligned to it. */
-#define DDSK_F_RED_SHIFT 16   /* bits 16..19 of the flags, with DDSK_F_ACC or DDSK_F_FOP (not swap, not compare-and-swap):
-                                 the reduction (DDSK_RED_*); 0 is the sum */
-#define DDSK_F_RED_OP(f) (((f) >> DDSK_F_RED_SHIFT) & 15)
 
-/* reductions of an accumulate or a fetch-op beside the sum (same values as DDS_OP_MAX.. in include/ddstore_b200.h). Max
- * and min compare integers as signed and floats by IEEE 754-2019 maximumNumber / minimumNumber with -0 < +0; the bitwise
- * ops take the integer types only. */
-#define DDSK_RED_SUM 0
-#define DDSK_RED_MAX 4
-#define DDSK_RED_MIN 5
-#define DDSK_RED_AND 6
-#define DDSK_RED_OR 7
-#define DDSK_RED_XOR 8
+/* ops of a batched write (same values as DDS_OP_* in include/ddstore_b200.h; DDSK_OP_PUT and DDSK_OP_CAS have no public
+ * op code). Max and min compare integers as signed and floats by IEEE 754-2019 maximumNumber / minimumNumber with
+ * -0 < +0; the bitwise ops take the integer types only. */
+#define DDSK_OP_PUT 0     /* shard = src */
+#define DDSK_OP_SUM 1     /* shard = shard + src */
+#define DDSK_OP_REPLACE 2 /* shard = src (a fetch-op only: the swap) */
+#define DDSK_OP_CAS 3     /* shard = src where shard == compare, bit for bit (a fetch-op only) */
+#define DDSK_OP_MAX 4
+#define DDSK_OP_MIN 5
+#define DDSK_OP_BAND 6
+#define DDSK_OP_BOR 7
+#define DDSK_OP_BXOR 8
+
+/* A batched write (ddsk_gather_fixed / ddsk_gather_var, raw, never with DDSK_F_OVERLAP): the get's walk with every copy
+ * reversed. dst_dev is the caller's packed SOURCE rows and dst_capacity its size; request i's bytes are taken from its
+ * packed position and written to its rows in the owner's shard, by `op`. The layout keeps an invalid request's bytes
+ * (count * row_bytes when 0 < count <= the variable's rows, else 0; 0 for a sample id outside the index); it writes
+ * nothing, like a layout above dst_capacity. No offsets.
+ * - a put (DDSK_OP_PUT) stores the bytes;
+ * - a reduction (any other op, result NULL: an accumulate) combines every element with the shard's atomically;
+ * - a fetch-op (result set) applies an atomic that returns each element's previous value and writes that value to the
+ *   same position of result as the operand's in the caller's rows. DDSK_OP_CAS is a fetch-op whose operands are compared
+ *   with the compare operands at the same position of `compare`.
+ * The caller's rows, result and compare are aligned to the element size. */
+typedef struct ddsk_write {
+    int32_t op;          /* DDSK_OP_* */
+    int32_t type;        /* the element type (DDSK_ACC_*) of a sum or reduction (a fetch-op's too), else 0 */
+    int32_t el_log2;     /* log2 of the element size (the type's, or the variable's itemsize) */
+    void *result;        /* a fetch-op's previous values (device memory, the layout of the source rows), else NULL */
+    const void *compare; /* DDSK_OP_CAS: the compare operands (device memory, the layout of the source rows), else NULL */
+} ddsk_write_t;
 
 /* element types of an accumulate (same values as DDS_ACC_* in include/ddstore_b200.h) */
 #define DDSK_ACC_F32 1
@@ -164,10 +160,11 @@ typedef struct ddsk_cvt {
  * One launch: validate + owner lookup + gather + pack.
  * cvt (nullable): convert the elements on the way; dst_capacity is then in SOURCE bytes (the caller's output capacity
  * rounded down to whole elements, scaled), while offsets_dev_or_null receives OUTPUT byte offsets. The same holds for
- * ddsk_gather_var and ddsk_gather_multi (per variable). */
+ * ddsk_gather_var and ddsk_gather_multi (per variable).
+ * wr (nullable): a batched write (see ddsk_write_t) instead of a get, here and in ddsk_gather_var; cvt is then NULL. */
 int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t count, int64_t nreq, void *dst_dev,
                       int64_t dst_capacity, int64_t *offsets_dev_or_null, const ddsk_scratch_t *scr, int flags,
-                      const ddsk_cvt_t *cvt, void *stream);
+                      const ddsk_cvt_t *cvt, const ddsk_write_t *wr, void *stream);
 
 /* Where the (start row, row count) of request i comes from (all device pointers): explicit arrays, or -- when
  * sample_ids is set -- the per-sample table of the variable: {start, count} = table[sample_ids[i]] (int64 pairs). */
@@ -184,7 +181,7 @@ typedef struct ddsk_index {
  * of the launch's own (slot = ovl_seq & 3): the plan then runs under the previous batch's gather. */
 int ddsk_gather_var(const ddsk_var_t *var, const ddsk_index_t *index, int64_t nreq, void *dst_dev,
                     int64_t dst_capacity, int64_t *offsets_dev_or_null, ddsk_scratch_t *scr, int flags,
-                    const ddsk_cvt_t *cvt, void *stream);
+                    const ddsk_cvt_t *cvt, const ddsk_write_t *wr, void *stream);
 /* (cvt: the conversion the launch will carry, or NULL; its tables take shared memory from the in-launch plan. host: the
  * variable's ddsk_var_t.host -- HOST launches always plan in the plan kernels) */
 int ddsk_var_uses_scratch(int64_t nreq, int64_t dst_capacity, const ddsk_cvt_t *cvt, int host);

@@ -1475,8 +1475,9 @@ static int batch_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *sta
     int kflags;
     ddsk_scratch_t scr;
     if (int rc = launch_flags(s, c, ovl, uses_scratch, &kflags, &scr)) return rc;
-    const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, c.st)
-                          : ddsk_gather_var(&v->kv, &ix, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, c.st);
+    const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt,
+                                              nullptr, c.st)
+                          : ddsk_gather_var(&v->kv, &ix, nreq, d_dst, cap, d_offsets, &scr, kflags, cvt, nullptr, c.st);
     s->scr.plan_tag = scr.plan_tag;
     if (krc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
 
@@ -1750,29 +1751,22 @@ int dds_get_samples_padded(dds_store_t *s, const char *name, const int64_t *samp
                        cuda_stream, total_bytes, bad_index);
 }
 
-// The batched put behind dds_put_batch / dds_put_samples (by_sample: starts = sample ids): the gather's launch with every
-// copy reversed (DDSK_F_PUT). Request i's rows come from src bytes [o_i, o_i + n_i), n_i = req_bytes(count_i) even for
-// an invalid request, o_i the exclusive scan. Like batch_impl, the host knows the layout of a fixed count or of host
-// indices and leaves capacity and validation to the kernel. A put is never overlapped and never takes the
-// single-request kernels.
-// acc: 0 for a put; a DDS_ACC_* element type for the accumulate behind dds_accumulate_batch / dds_accumulate_samples,
-// the same launch whose drain adds (DDSK_F_ACC). Its src must be aligned to the element size.
-// op: 0, or a DDS_OP_* for the fetch-op behind dds_get_accumulate_batch / dds_get_accumulate_samples (with acc its element
-// type): the same launch whose drain applies a returning atomic and writes the previous rows to `result`, in the layout
-// of src (DDSK_F_FOP). result must be aligned to the element size too.
-// red: DDSK_RED_SUM, or the reduction (DDS_OP_MAX..) of an accumulate (result null: dds_accumulate_op_*) or of a fetch-op
-// (op == red), carried in the launch flags' DDSK_F_RED bits.
-// op OP_CAS (acc 0): the compare-and-swap behind dds_compare_and_swap_batch / dds_compare_and_swap_samples, the fetch-op
-// launch whose drain swaps where the shard equals `compare` (the layout of src; DDSK_F_FOP_CAS) on elements of the
-// variable's itemsize. src and compare must be aligned to it too.
+// The batched writes behind dds_put_*, dds_accumulate_*, dds_get_accumulate_* and dds_compare_and_swap_* (by_sample:
+// starts = sample ids): the gather's launch with every copy reversed, whose drain does what the write record `w` (see
+// ddsk_write_t) says. Request i's rows come from src bytes [o_i, o_i + n_i), n_i = req_bytes(count_i) even for an
+// invalid request, o_i the exclusive scan. Like batch_impl, the host knows the layout of a fixed count or of host indices
+// and leaves capacity and validation to the kernel. A write is never overlapped and never takes the single-request
+// kernels.
+// w.type is set for a sum or reduction (an accumulate or a fetch-op): src must be aligned to that element type. fetch:
+// the entry returns the previous rows in w.result (a fetch-op or a compare-and-swap), which must be aligned to the
+// element size too; it may be NULL only when there is nothing to write, and the launch then writes nothing either way.
+// A compare-and-swap (DDSK_OP_CAS) takes src and compare aligned to the variable's itemsize.
 // Device atomics on mapped host memory are not atomic across GPUs over PCIe, so HOST variables take no batched write
 // at all: they are written only by their owner's update / ingest.
 static const char *const kHostWrite = "batched writes do not take DDS_PLACE_HOST variables (write them with update / ingest)";
-static constexpr int OP_CAS = 3; // (put_impl's own op code, beside the DDS_OP_* of the fetch-ops)
 static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts,
                     int64_t fixed_count, int64_t nreq, const void *src, int64_t src_bytes, unsigned flags,
-                    void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, int acc = 0, int op = 0,
-                    void *result = nullptr, const void *compare = nullptr, int red = DDSK_RED_SUM) {
+                    void *cuda_stream, int64_t *total_bytes, int64_t *bad_index, const ddsk_write_t &w, bool fetch = false) {
     if (!(flags & DDS_SRC_ON_DEVICE)) return fail(DDS_ERR_ARG, "puts take their rows from device memory (DDS_SRC_ON_DEVICE)");
     if (nreq < 0 || src_bytes < 0) return fail(DDS_ERR_ARG, "negative nreq or src_bytes");
     if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
@@ -1782,13 +1776,13 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     const bool fixed = !by_sample && counts == nullptr;
     const int64_t layout = host_layout(v, by_sample, starts, counts, fixed_count, nreq, idx_dev);
     if (!src && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null src");
-    if (acc && (uintptr_t)src % (uintptr_t)v->itemsize)
+    if (w.type && (uintptr_t)src % (uintptr_t)v->itemsize)
         return fail(DDS_ERR_ARG, "accumulates take src aligned to the element size");
-    if (op && !result && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null result");
-    if (op && (uintptr_t)result % (uintptr_t)v->itemsize)
+    if (fetch && !w.result && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null result");
+    if (fetch && (uintptr_t)w.result % (uintptr_t)v->itemsize)
         return fail(DDS_ERR_ARG, "fetch-ops take result aligned to the element size");
-    if (op == OP_CAS && !compare && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null compare");
-    if (op == OP_CAS && ((uintptr_t)src % (uintptr_t)v->itemsize || (uintptr_t)compare % (uintptr_t)v->itemsize))
+    if (w.op == DDSK_OP_CAS && !w.compare && (src_bytes > 0 || layout > 0)) return fail(DDS_ERR_ARG, "null compare");
+    if (w.op == DDSK_OP_CAS && ((uintptr_t)src % (uintptr_t)v->itemsize || (uintptr_t)w.compare % (uintptr_t)v->itemsize))
         return fail(DDS_ERR_ARG, "compare-and-swaps take src and compare aligned to the element size");
 
     Call c;
@@ -1807,24 +1801,20 @@ static int put_impl(dds_store_t *s, Var *v, bool by_sample, const int64_t *start
     ddsk_scratch_t scr;
     if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
     void *d_src = const_cast<void *>(src);
-    if (op == OP_CAS) {
-        const int el = v->itemsize == 8 ? 3 : v->itemsize == 4 ? 2 : v->itemsize == 2 ? 1 : 0;
-        kflags |= DDSK_F_PUT | DDSK_F_FOP | DDSK_F_FOP_CAS | el << DDSK_F_ACC_SHIFT;
-        scr.fop_result = result;
-        scr.fop_compare = compare;
-    } else if (op) {
-        kflags |= DDSK_F_PUT | DDSK_F_FOP | acc << DDSK_F_ACC_SHIFT | (op == DDS_OP_REPLACE ? DDSK_F_FOP_SWAP : 0) |
-                  red << DDSK_F_RED_SHIFT;
-        scr.fop_result = result;
-    } else {
-        kflags |= DDSK_F_PUT | (acc ? DDSK_F_ACC | acc << DDSK_F_ACC_SHIFT | red << DDSK_F_RED_SHIFT : 0);
-    }
-    const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st)
-                          : ddsk_gather_var(&v->kv, &ix, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, c.st);
+    const int krc = fixed ? ddsk_gather_fixed(&v->kv, ix.starts, fixed_count, nreq, d_src, src_bytes, nullptr, &scr, kflags,
+                                              nullptr, &w, c.st)
+                          : ddsk_gather_var(&v->kv, &ix, nreq, d_src, src_bytes, nullptr, &scr, kflags, nullptr, &w, c.st);
     s->scr.plan_tag = scr.plan_tag;
     if (krc) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
     return end_launch(s, c, fixed ? layout : -1, uses_scratch ? &scr.req_dst[nreq] : scr.total, DDSK_CVT_NONE, true,
                       total_bytes, bad_index);
+}
+
+// The write record of op on variable v: type the element type of a sum or reduction (0 for a put or a compare-and-swap),
+// result and compare the fetch forms' buffers. Every element is the variable's itemsize (an accumulate's type has it).
+static ddsk_write_t write_rec(const Var *v, int op, int type = 0, void *result = nullptr, const void *compare = nullptr) {
+    const int el = v->itemsize == 8 ? 3 : v->itemsize == 4 ? 2 : v->itemsize == 2 ? 1 : 0;
+    return ddsk_write_t{op, type, el, result, compare};
 }
 
 int dds_put_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts, int64_t fixed_count,
@@ -1833,7 +1823,7 @@ int dds_put_batch(dds_store_t *s, const char *name, const int64_t *starts, const
     Var *v;
     if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v, kHostWrite)) return rc;
     return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
-                    bad_index);
+                    bad_index, write_rec(v, DDSK_OP_PUT));
 }
 
 int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
@@ -1841,7 +1831,8 @@ int dds_put_samples(dds_store_t *s, const char *name, const int64_t *sample_ids,
                     int64_t *bad_index) {
     Var *v;
     if (int rc = entry_var(s, name, &itemsize, total_bytes, bad_index, &v, kHostWrite)) return rc;
-    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index);
+    return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
+                    write_rec(v, DDSK_OP_PUT));
 }
 
 static_assert(DDS_ACC_F32 == DDSK_ACC_F32 && DDS_ACC_F64 == DDSK_ACC_F64 && DDS_ACC_I32 == DDSK_ACC_I32 &&
@@ -1857,21 +1848,20 @@ static int acc_entry(dds_store_t *s, const char *name, int dtype, int64_t *total
     return DDS_OK;
 }
 
-static_assert(DDS_OP_MAX == DDSK_RED_MAX && DDS_OP_MIN == DDSK_RED_MIN && DDS_OP_BAND == DDSK_RED_AND &&
-                  DDS_OP_BOR == DDSK_RED_OR && DDS_OP_BXOR == DDSK_RED_XOR,
-              "the kernels' reductions are the public ops");
+static_assert(DDS_OP_SUM == DDSK_OP_SUM && DDS_OP_REPLACE == DDSK_OP_REPLACE && DDS_OP_MAX == DDSK_OP_MAX &&
+                  DDS_OP_MIN == DDSK_OP_MIN && DDS_OP_BAND == DDSK_OP_BAND && DDS_OP_BOR == DDSK_OP_BOR &&
+                  DDS_OP_BXOR == DDSK_OP_BXOR,
+              "the kernels' ops are the public ones");
 
 // The reductions' and fetch-ops' prologue: the accumulates', then an unknown op (fetch: DDS_OP_REPLACE is an op; not
-// fetch: it is not, a put writes rows), then a bitwise op on a float dtype. *red: the kernels' reduction (DDSK_RED_SUM for
-// the sum and the swap).
+// fetch: it is not, a put writes rows), then a bitwise op on a float dtype.
 static int fop_entry(dds_store_t *s, const char *name, int op, int dtype, int64_t *total_bytes, int64_t *bad_index,
-                     Var **v, bool fetch = true, int *red = nullptr) {
+                     Var **v, bool fetch = true) {
     if (int rc = acc_entry(s, name, dtype, total_bytes, bad_index, v)) return rc;
     if (!(op == DDS_OP_SUM || (fetch && op == DDS_OP_REPLACE) || (op >= DDS_OP_MAX && op <= DDS_OP_BXOR)))
         return fail(DDS_ERR_ARG, fetch ? "unknown fetch-op" : "unknown accumulate op");
     if (op >= DDS_OP_BAND && dtype != DDS_ACC_I32 && dtype != DDS_ACC_I64)
         return fail(DDS_ERR_ARG, "bitwise ops take DDS_ACC_I32 or DDS_ACC_I64");
-    if (red) *red = op >= DDS_OP_MAX ? op : DDSK_RED_SUM;
     return DDS_OK;
 }
 
@@ -1879,20 +1869,18 @@ int dds_accumulate_op_batch(dds_store_t *s, const char *name, const int64_t *sta
                             int64_t fixed_count, int64_t nreq, int op, int dtype, const void *src, int64_t src_bytes,
                             unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
     Var *v;
-    int red;
-    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, false, &red)) return rc;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, false)) return rc;
     return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
-                    bad_index, dtype, 0, nullptr, nullptr, red);
+                    bad_index, write_rec(v, op, dtype));
 }
 
 int dds_accumulate_op_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
                               int dtype, const void *src, int64_t src_bytes, unsigned flags, void *cuda_stream,
                               int64_t *total_bytes, int64_t *bad_index) {
     Var *v;
-    int red;
-    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, false, &red)) return rc;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, false)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
-                    dtype, 0, nullptr, nullptr, red);
+                    write_rec(v, op, dtype));
 }
 
 int dds_accumulate_batch(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
@@ -1914,20 +1902,18 @@ int dds_get_accumulate_batch(dds_store_t *s, const char *name, const int64_t *st
                              int64_t src_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes,
                              int64_t *bad_index) {
     Var *v;
-    int red;
-    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, true, &red)) return rc;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
-                    bad_index, dtype, op, result, nullptr, red);
+                    bad_index, write_rec(v, op, dtype, result), true);
 }
 
 int dds_get_accumulate_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int op,
                                int dtype, const void *src, void *result, int64_t src_bytes, unsigned flags,
                                void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
     Var *v;
-    int red;
-    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v, true, &red)) return rc;
+    if (int rc = fop_entry(s, name, op, dtype, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
-                    dtype, op, result, nullptr, red);
+                    write_rec(v, op, dtype, result), true);
 }
 
 // The compare-and-swaps' prologue: entry_var, an itemsize outside {1, 2, 4, 8} (an argument error) and then one other
@@ -1947,7 +1933,7 @@ int dds_compare_and_swap_batch(dds_store_t *s, const char *name, const int64_t *
     Var *v;
     if (int rc = cas_entry(s, name, itemsize, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, false, starts, counts, fixed_count, nreq, src, src_bytes, flags, cuda_stream, total_bytes,
-                    bad_index, 0, OP_CAS, result, compare);
+                    bad_index, write_rec(v, DDSK_OP_CAS, 0, result, compare), true);
 }
 
 int dds_compare_and_swap_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
@@ -1956,7 +1942,7 @@ int dds_compare_and_swap_samples(dds_store_t *s, const char *name, const int64_t
     Var *v;
     if (int rc = cas_entry(s, name, itemsize, total_bytes, bad_index, &v)) return rc;
     return put_impl(s, v, true, sample_ids, nullptr, 0, nreq, src, src_bytes, flags, cuda_stream, total_bytes, bad_index,
-                    0, OP_CAS, result, compare);
+                    write_rec(v, DDSK_OP_CAS, 0, result, compare), true);
 }
 
 // The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,

@@ -331,7 +331,7 @@ def _nan_bits(t, q):
 
 # ------------------------------------------------------------------------------------------------ paths and verdicts
 def drain_path(dst_phase, src_phase, nbytes, k):
-    """which reduction the kernel's drain (acc_drain_chunk) uses for byte k of ONE staged piece of nbytes bytes whose
+    """which reduction the kernel's drain (write_chunk<kActReduce>) uses for byte k of ONE staged piece of nbytes bytes whose
     destination starts dst_phase bytes and whose staged source starts src_phase bytes past a 16-byte boundary: the
     head before the destination's first 16-byte boundary and the tail after its last are element reductions; the body
     between is one bulk reduction when source and destination share the phase, re-phased vector reductions otherwise.

@@ -472,10 +472,10 @@ def once_verdict(got_prev, got_new, start, x, t, op, where=None, paths=None, wha
 
 # ------------------------------------------------------------------------------------------------ paths
 def fop_path(dst_phase, src_phase, nbytes, k, res_phase=0):
-    """which atomic the fetch drain (fop_chunk) applies to byte k of ONE staged piece of nbytes bytes whose shard
-    bytes start dst_phase and whose staged operands start src_phase bytes past a 16-byte boundary: "element" (fop1)
+    """which atomic the fetch drain (write_chunk<kActFetch>) applies to byte k of ONE staged piece of nbytes bytes whose shard
+    bytes start dst_phase and whose staged operands start src_phase bytes past a 16-byte boundary: "element" (fetch1)
     for the head before the shard's first 16-byte boundary and the tail after its last; for the body between,
-    "vector WS/B", fop_rephase_loop<WS, BYTES> with the word shift WS and BYTES (0 / 1) of the staged phase
+    "vector WS/B", write_loop<kActFetch, WS, BYTES> with the word shift WS and BYTES (0 / 1) of the staged phase
     (src_phase + head) % 16. k may be an array. Also returns how the previous values reach the result whose bytes start
     res_phase past a boundary: "bulk" (one bulk store) when result, size and staged phase are all 16-byte aligned,
     else "drain_chunk" (the raw drain's head / body / tail)."""
@@ -488,7 +488,7 @@ def fop_path(dst_phase, src_phase, nbytes, k, res_phase=0):
 
 
 def vector_paths(t):
-    """the fop_rephase_loop variants elements of type t can take: 8 for 2-byte types, 4 for 4-byte, 2 for 8-byte"""
+    """the write_loop<kActFetch> variants elements of type t can take: 8 for 2-byte types, 4 for 4-byte, 2 for 8-byte"""
     E = np.dtype(ao.STORAGE[t]).itemsize
     return [f"vector {sh >> 2}/{int(sh % 4 != 0)}" for sh in range(0, 16, E)]
 

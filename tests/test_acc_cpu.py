@@ -427,7 +427,7 @@ def test_bf16_nan_encoding():
 
 
 def test_drain_path():
-    """acc_drain_chunk's cases, element by element: head and tail elements, a same-phase body in bulk, a re-phased body
+    """write_chunk<kActReduce>'s cases, element by element: head and tail elements, a same-phase body in bulk, a re-phased body
     in vectors"""
     lab = lambda dp, sp, n: "".join(x[0] for x in ao.drain_path(dp, sp, n, np.arange(0, n, 4)))  # noqa: E731
     assert lab(0, 0, 64) == "b" * 16

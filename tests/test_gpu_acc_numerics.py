@@ -4,7 +4,7 @@ the drain's three reductions (bulk, re-phased vector, element), with one contrib
 bit: `admissible`), two or three (every order admitted, nothing else) and many (`sum_bound`), then read back.
 
 Which reduction an element takes depends only on where its destination and its staged source bytes sit relative to
-16-byte boundaries (acc_drain_chunk). A one-request call whose rows fit in one chunk is one staged piece, so there
+16-byte boundaries (write_chunk<kActReduce>). A one-request call whose rows fit in one chunk is one staged piece, so there
 `acc_oracle.drain_path` names the path of every element; the coverage of every (type, path, value family) cell is
 asserted. The verdict on an element does not depend on its path, except that f32 may flush subnormals.
 """

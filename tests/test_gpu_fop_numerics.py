@@ -1,8 +1,8 @@
 """The batched fetch-ops' arithmetic and returned values on the GPU against the correctly rounded oracle of
 tests/fop_oracle.py (built on tests/acc_oracle.py): inexact floats, subnormals, the min-normal boundary, overflow,
 signed zeros, inf and NaN payloads and integer wraparound, through each atomic of the fetch drain -- the element
-atomics of the head and tail (fop1: returning atom.add / exch, the 2-byte swap's CAS loop, the f16 / bf16 element adds
-ptxas makes CAS loops) and the eight re-phased vector forms of the body (fop_rephase_loop, fop16) -- and both writes of
+atomics of the head and tail (fetch1: returning atom.add / exch, the 2-byte swap's CAS loop, the f16 / bf16 element adds
+ptxas makes CAS loops) and the eight re-phased vector forms of the body (write_loop<kActFetch, WS, BYTES>, fetch16) -- and both writes of
 the previous values to the result (one bulk store, or drain_chunk).
 
   (a) one fetch-op per element, every path: previous values bit for bit, new values by one rounded addition (f32 IEEE
