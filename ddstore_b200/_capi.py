@@ -56,6 +56,16 @@ class Pad(C.Structure):  # dds_pad_t
     _fields_ = [("max_rows", C.c_int64), ("pad_bits", C.c_uint64), ("lengths", C.c_void_p)]
 
 
+# pooling modes of the pooled batches (DDS_POOL_*), by torch's embedding_bag names
+POOL_SUM, POOL_MEAN, POOL_MAX = 1, 2, 3
+POOL_MODES = {"sum": POOL_SUM, "mean": POOL_MEAN, "max": POOL_MAX}
+
+
+class Pool(C.Structure):  # dds_pool_t
+    _fields_ = [("mode", C.c_int32), ("dtype", C.c_int32), ("bags", C.c_void_p), ("nbags", C.c_int64),
+                ("weights", C.c_void_p)]
+
+
 # every symbol include/ddstore_b200.h declares: name -> (restype, argtypes)
 I64P = C.POINTER(C.c_int64)
 SIGNATURES = {
@@ -125,6 +135,10 @@ SIGNATURES = {
                                              C.c_void_p, I64P, I64P]),
     "dds_compare_and_swap_samples": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_get_batch_pooled": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                       C.POINTER(Pool), C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_get_samples_pooled": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(Pool), C.c_void_p,
+                                         C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

@@ -47,6 +47,8 @@
 // bench / test helpers (payload generator, on-device verifier, SM occupier).
 //
 // Nothing here calls a library kernel; everything is launched from the ddsk_* functions at the end.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -2886,6 +2888,224 @@ __global__ void dds_occupy_kernel(unsigned long long ns, int smem_bytes) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// pooled batches (dds_get_batch_pooled / dds_get_samples_pooled): each bag of requests folded into one output row
+// ------------------------------------------------------------------------------------------------
+// One warp per (bag, column slice), grid-striding over them. A lane owns one VB-byte vector of the slice (VB = 16, or one
+// element when the row or the destination is not 16-byte aligned) and folds it over the bag's rows in request order, then
+// row order: every output element is the sequential fold the contract defines, whatever the grid or the slicing. A bag's
+// requests are read 32 at a time (one coalesced load of starts / counts / ids / weights, located lane-parallel); the rows
+// of that window are then walked kPoolRows at a time, their loads in flight together before any of them is folded.
+// Slices need no synchronisation with each other; the launcher narrows them (down to kPoolMinSlice bytes) until a few long
+// bags still give every SM warps.
+constexpr int kPoolThreads = 256;
+constexpr int kPoolMinBlocks = 2; // CTAs per SM the registers must allow (__launch_bounds__)
+constexpr int kPoolRows = 4;      // rows in flight per warp
+constexpr int64_t kPoolMinSlice = 128;
+
+struct PoolArgs {
+    ddsk_var_t var;
+    const int64_t *starts, *counts; // explicit requests (counts NULL: `count` rows each), or
+    int64_t count;
+    const int64_t *ids;             // sample ids looked up in the variable's sample index
+    const longlong2 *tab;
+    int64_t nsamples;
+    const int64_t *bags; // [nbags + 1] request offsets, NULL: bag k = request k
+    int64_t nbags, nreq;
+    const void *weights; // [nreq] in the element type, NULL: unweighted
+    int mode;            // DDSK_POOL_*
+    char *dst;
+    int64_t slice, nslices; // bytes per column slice (a multiple of VB, at most 32 * VB) and slices per row
+    unsigned long long *status;
+    unsigned long long status_tag;
+};
+
+// element bits (U) and accumulator (A) of each element type
+template <int DT>
+struct PoolType {
+    using U = uint32_t;
+    using A = float;
+};
+template <>
+struct PoolType<DDSK_ACC_F64> {
+    using U = uint64_t;
+    using A = double;
+};
+template <>
+struct PoolType<DDSK_ACC_F16> {
+    using U = uint16_t;
+    using A = float;
+};
+template <>
+struct PoolType<DDSK_ACC_BF16> {
+    using U = uint16_t;
+    using A = float;
+};
+
+template <int DT>
+__device__ __forceinline__ typename PoolType<DT>::A pool_dec(typename PoolType<DT>::U b) {
+    if constexpr (DT == DDSK_ACC_F64) return __longlong_as_double((long long)b);
+    else if constexpr (DT == DDSK_ACC_F16) return __half2float(__ushort_as_half(b));
+    else if constexpr (DT == DDSK_ACC_BF16) return __bfloat162float(__ushort_as_bfloat16(b));
+    else return __uint_as_float(b);
+}
+// one round-to-nearest conversion; a NaN becomes the type's canonical NaN (all ones but the sign)
+template <int DT>
+__device__ __forceinline__ typename PoolType<DT>::U pool_enc(typename PoolType<DT>::A v) {
+    if constexpr (DT == DDSK_ACC_F64) return v != v ? 0x7FFFFFFFFFFFFFFFull : (uint64_t)__double_as_longlong(v);
+    else if constexpr (DT == DDSK_ACC_F16) return v != v ? (uint16_t)0x7FFF : __half_as_ushort(__float2half_rn(v));
+    else if constexpr (DT == DDSK_ACC_BF16) return v != v ? (uint16_t)0x7FFF : __bfloat16_as_ushort(__float2bfloat16_rn(v));
+    else return v != v ? 0x7FFFFFFFu : __float_as_uint(v);
+}
+// IEEE round-to-nearest arithmetic, never contracted
+__device__ __forceinline__ float pool_add(float a, float x) { return __fadd_rn(a, x); }
+__device__ __forceinline__ double pool_add(double a, double x) { return __dadd_rn(a, x); }
+__device__ __forceinline__ float pool_fma(float w, float x, float a) { return __fmaf_rn(w, x, a); }
+__device__ __forceinline__ double pool_fma(double w, double x, double a) { return __fma_rn(w, x, a); }
+__device__ __forceinline__ float pool_div(float a, int64_t n) { return __fdiv_rn(a, (float)n); }
+__device__ __forceinline__ double pool_div(double a, int64_t n) { return __ddiv_rn(a, (double)n); }
+
+// element e of a lane's vector RW (uint4, or one element)
+template <typename U, typename RW>
+__device__ __forceinline__ U pool_elem(const RW &r, int e) {
+    if constexpr (std::is_same<RW, uint4>::value) {
+        const uint32_t w[4] = {r.x, r.y, r.z, r.w};
+        if constexpr (sizeof(U) == 2) return (U)(w[e >> 1] >> ((e & 1) * 16));
+        else if constexpr (sizeof(U) == 4) return (U)w[e];
+        else return (U)w[2 * e] | ((U)w[2 * e + 1] << 32);
+    } else {
+        return r;
+    }
+}
+template <typename RW>
+__device__ __forceinline__ RW pool_load(uint64_t p) {
+    if constexpr (std::is_same<RW, uint4>::value) return __ldcg((const uint4 *)p);
+    else if constexpr (sizeof(RW) == 2) return (RW)__ldcg((const unsigned short *)p);
+    else if constexpr (sizeof(RW) == 4) return (RW)__ldcg((const unsigned int *)p);
+    else return (RW)__ldcg((const unsigned long long *)p);
+}
+template <typename U, int E>
+__device__ __forceinline__ void pool_store(char *p, const U (&o)[E]) {
+    if constexpr (E * sizeof(U) == 16) {
+        uint32_t w[4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            if constexpr (sizeof(U) == 2) w[i] = (uint32_t)o[2 * i] | ((uint32_t)o[2 * i + 1] << 16);
+            else if constexpr (sizeof(U) == 4) w[i] = (uint32_t)o[i];
+            else w[i] = (uint32_t)(o[i >> 1] >> ((i & 1) * 32));
+        }
+        stg128(p, make_uint4(w[0], w[1], w[2], w[3]));
+    } else {
+        *(U *)p = o[0];
+    }
+}
+
+template <int DT, int VB>
+__global__ void __launch_bounds__(kPoolThreads, kPoolMinBlocks) dds_pool_kernel(const __grid_constant__ PoolArgs a) {
+    using U = typename PoolType<DT>::U;
+    using A = typename PoolType<DT>::A;
+    using RW = typename std::conditional<VB == 16, uint4, U>::type;
+    constexpr int E = VB / (int)sizeof(U);
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = (int64_t)gridDim.x * (kPoolThreads / 32);
+    const int64_t row_bytes = a.var.row_bytes;
+    for (int64_t w = (int64_t)blockIdx.x * (kPoolThreads / 32) + (threadIdx.x >> 5); w < a.nbags * a.nslices; w += nwarps) {
+        const int64_t k = w / a.nslices, sl = w - k * a.nslices;
+        const int64_t col = sl * a.slice + (int64_t)lane * VB;
+        const bool mine = (int64_t)lane * VB < a.slice && col < row_bytes; // (everything below is warp-uniform but the loads)
+        int64_t b0 = k, b1 = k + 1;
+        if (a.bags) {
+            b0 = a.bags[k];
+            b1 = a.bags[k + 1];
+        }
+        if (b0 < 0 || b1 < b0 || b1 > a.nreq) { // malformed: the row is written as zeros
+            if (lane == 0 && sl == 0) report(a.status, a.status_tag, k, DDSK_CODE_BAG);
+            b0 = b1 = 0;
+        }
+        A acc[E];
+        U mx[E];
+#pragma unroll
+        for (int e = 0; e < E; e++) {
+            acc[e] = A(0);
+            mx[e] = U(0);
+        }
+        int64_t rows = 0; // rows folded so far
+        for (int64_t base = b0; base < b1; base += 32) {
+            const int64_t i = base + lane;
+            uint64_t src = 0;
+            int64_t n = 0;
+            A wt = A(1);
+            if (i < b1) {
+                int64_t start = 0, count = 0;
+                int code = 0;
+                if (a.ids) {
+                    const int64_t id = a.ids[i];
+                    if (id < 0 || id >= a.nsamples) {
+                        code = DDSK_CODE_SAMPLE;
+                    } else {
+                        const longlong2 e = ldg_pair(&a.tab[id]);
+                        start = e.x;
+                        count = e.y;
+                    }
+                } else {
+                    start = a.starts[i];
+                    count = a.counts ? a.counts[i] : a.count;
+                }
+                if (!code) code = dev_locate(a.var, start, count, &src);
+                if (code) report(a.status, a.status_tag, (int64_t)(DDSK_STATUS_LATE | (uint64_t)i), code);
+                else n = count;
+                if (a.weights) wt = pool_dec<DT>(((const U *)a.weights)[i]);
+            }
+            // the window's rows, in order: row r belongs to the request whose inclusive row scan first exceeds r
+            const int64_t incl = warp_incl_scan(n, lane), excl = incl - n;
+            const int64_t total = __shfl_sync(0xffffffffu, incl, 31);
+            for (int64_t g = 0; g < total; g += kPoolRows) {
+                RW x[kPoolRows];
+                A wr[kPoolRows];
+#pragma unroll
+                for (int u = 0; u < kPoolRows; u++) {
+                    const int64_t r = g + u;
+                    const int j = __popc(__ballot_sync(0xffffffffu, incl <= r)) & 31;
+                    const uint64_t s = __shfl_sync(0xffffffffu, src, j);
+                    const int64_t e0 = __shfl_sync(0xffffffffu, excl, j);
+                    wr[u] = __shfl_sync(0xffffffffu, wt, j);
+                    x[u] = RW{};
+                    if (mine && r < total) x[u] = pool_load<RW>(s + (uint64_t)(r - e0) * (uint64_t)row_bytes + (uint64_t)col);
+                }
+#pragma unroll
+                for (int u = 0; u < kPoolRows; u++) {
+                    if (g + u >= total) break;
+#pragma unroll
+                    for (int e = 0; e < E; e++) {
+                        const U xb = pool_elem<U>(x[u], e);
+                        if (a.mode == DDSK_POOL_MAX) {
+                            if (rows + g + u == 0 || pool_dec<DT>(xb) > pool_dec<DT>(mx[e])) mx[e] = xb;
+                        } else if (a.weights) {
+                            acc[e] = pool_fma(wr[u], pool_dec<DT>(xb), acc[e]);
+                        } else {
+                            acc[e] = pool_add(acc[e], pool_dec<DT>(xb));
+                        }
+                    }
+                }
+            }
+            rows += total;
+        }
+        if (mine) {
+            U o[E];
+#pragma unroll
+            for (int e = 0; e < E; e++) {
+                if (a.mode == DDSK_POOL_MAX) {
+                    o[e] = mx[e];
+                } else {
+                    const A v = a.mode == DDSK_POOL_MEAN && rows > 0 ? pool_div(acc[e], rows) : acc[e];
+                    o[e] = pool_enc<DT>(v);
+                }
+            }
+            pool_store<U, E>(a.dst + k * row_bytes + col, o);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // launch geometry
 // ------------------------------------------------------------------------------------------------
 // Every geometry dds_gather_kernel is launched with: warps per CTA, ring stages per warp, chunk bytes, and the capacity of
@@ -3124,6 +3344,15 @@ int write_form(GatherArgs &a, const ddsk_write_t *wr) {
     return wr->op == DDSK_OP_PUT ? kWrPut : wr->result ? kWrFetch : kWrReduce;
 }
 
+template <int DT>
+int launch_pool_t(const PoolArgs &a, int vb, int blocks, cudaStream_t st) {
+    if (vb == 16) dds_pool_kernel<DT, 16><<<blocks, kPoolThreads, 0, st>>>(a);
+    else dds_pool_kernel<DT, (int)sizeof(typename PoolType<DT>::U)><<<blocks, kPoolThreads, 0, st>>>(a);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
 } // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -3335,6 +3564,57 @@ int ddsk_gather_multi(const ddsk_multi_t *m, const int64_t *sample_ids_dev, int6
         a.moffsets[v] = m->offsets[v];
     }
     return plan_and_gather(&dummy, p, nreq * m->nvars, cap_total, a, nullptr, scr, flags, cvt, kWrNone, (cudaStream_t)stream);
+}
+
+int ddsk_pool(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_count, int64_t nreq, const ddsk_pool_t *pool,
+              void *dst, const ddsk_scratch_t *scr, int flags, void *stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (pool->nbags <= 0 || var->row_bytes <= 0) return 0;
+    if (int rc = pick_geometry()) return rc;
+    PoolArgs a;
+    memset(&a, 0, sizeof(a));
+    a.var = *var;
+    a.starts = index->starts;
+    a.counts = index->counts;
+    a.count = fixed_count;
+    a.ids = index->sample_ids;
+    a.tab = (const longlong2 *)index->table;
+    a.nsamples = index->nsamples;
+    a.bags = pool->bags;
+    a.nbags = pool->nbags;
+    a.nreq = nreq;
+    a.weights = pool->weights;
+    a.mode = pool->mode;
+    a.dst = (char *)dst;
+    a.status = scr->status;
+    a.status_tag = scr->status_tag;
+    const int64_t R = var->row_bytes;
+    const int vb = (R % 16 == 0 && (uint64_t)dst % 16 == 0) ? 16 : 1 << DDSK_ACC_LOG2(pool->type);
+    // slices: whole warps of vectors, halved while the bags leave resident warps idle (a few long bags then still spread)
+    const int64_t resident = (int64_t)g_sms * kPoolMinBlocks * (kPoolThreads / 32);
+    a.slice = 32 * vb;
+    a.nslices = (R + a.slice - 1) / a.slice;
+    while (a.slice / 2 >= kPoolMinSlice && a.nbags * a.nslices < resident) {
+        a.slice /= 2;
+        a.nslices = (R + a.slice - 1) / a.slice;
+    }
+    const int64_t units = a.nbags * a.nslices, per_cta = kPoolThreads / 32;
+    const int64_t most = var->host ? std::min(g_sms, g_host_ctas) : (int64_t)g_sms * kPoolMinBlocks;
+    const int blocks = (int)std::min((units + per_cta - 1) / per_cta, most);
+    int rc = 0;
+    switch (pool->type) {
+    case DDSK_ACC_F32: rc = launch_pool_t<DDSK_ACC_F32>(a, vb, blocks, st); break;
+    case DDSK_ACC_F64: rc = launch_pool_t<DDSK_ACC_F64>(a, vb, blocks, st); break;
+    case DDSK_ACC_F16: rc = launch_pool_t<DDSK_ACC_F16>(a, vb, blocks, st); break;
+    case DDSK_ACC_BF16: rc = launch_pool_t<DDSK_ACC_BF16>(a, vb, blocks, st); break;
+    default:
+        snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_pool: unsupported element type %d", (int)pool->type);
+        return -2;
+    }
+    if (rc) return rc;
+    if (flags & DDSK_F_MIRROR) // (a synchronous call reads the status from the pinned mirror word)
+        CUDA_TRY(cudaMemcpyAsync(scr->host_mirror, scr->status, 8, cudaMemcpyDefault, st));
+    return 0;
 }
 
 int ddsk_small_get(const ddsk_var_t *var, int64_t start, int64_t count, void *dst, int64_t dst_capacity,

@@ -27,15 +27,18 @@ typedef struct ddsk_var {
 /* status word written by the kernels: 0xFFFF... = ok, else (ordinal << 48) | (first_bad_request << 8) | code, where
  * ordinal is the launch's position in its queue of DDS_NO_SYNC batches (0 for a synchronous call; saturates at 0xFFFF).
  * Kernels only atomicMin into it, so the word holds the first error in queue order, and inside that batch the
- * lowest-index one. Request indices stay below 2^40. */
+ * lowest-index one. Request indices stay below 2^39: a pooled launch sets bit 39 of the index field (DDSK_STATUS_LATE) in
+ * its request reports, so that its malformed-bag reports (DDSK_CODE_BAG, index = the bag) come first. */
 #define DDSK_STATUS_OK 0xFFFFFFFFFFFFFFFFull
 #define DDSK_STATUS_ORD_SHIFT 48
-#define DDSK_STATUS_REQ_MASK 0xFFFFFFFFFFull /* (word >> 8) & this = request index */
+#define DDSK_STATUS_REQ_MASK 0x7FFFFFFFFFull /* (word >> 8) & this = request index */
+#define DDSK_STATUS_LATE (1ull << 39)        /* in the index field: a report ordered after every bag report */
 #define DDSK_CODE_START 2
 #define DDSK_CODE_COUNT 3
 #define DDSK_CODE_CAPACITY 12
 #define DDSK_CODE_WATCHDOG 14
 #define DDSK_CODE_SAMPLE 15
+#define DDSK_CODE_BAG 16 /* a pooled launch's malformed bag offsets (index = the bag) */
 
 /* scratch a store owns for the batched path (all device memory) */
 typedef struct ddsk_scratch {
@@ -239,6 +242,22 @@ static inline DDSK_HD ddsk_pad_cut_t ddsk_pad_cut(int64_t i, int64_t payload, in
     c.pad_len = qs < hi ? ((hi - qs) >> in_log2) << out_log2 : 0;
     return c;
 }
+
+/* Pooled batch (dds_get_batch_pooled): bag k folds the rows of requests [bags[k], bags[k+1]) (bags NULL: request k) into
+ * output row k of dst, by `mode` in element type `type` (the public DDS_POOL_* / DDS_ACC_* codes). index: explicit starts
+ * (counts NULL: fixed_count rows each) or sample ids. bags and weights are device memory; the kernel checks the bags and
+ * reports a malformed one as DDSK_CODE_BAG. The host has checked everything else (dst holds nbags rows, alignment). */
+#define DDSK_POOL_SUM 1
+#define DDSK_POOL_MEAN 2
+#define DDSK_POOL_MAX 3
+typedef struct ddsk_pool {
+    int32_t mode, type;
+    const int64_t *bags;
+    int64_t nbags;
+    const void *weights;
+} ddsk_pool_t;
+int ddsk_pool(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_count, int64_t nreq, const ddsk_pool_t *pool,
+              void *dst, const ddsk_scratch_t *scr, int flags, void *stream);
 
 /* Multi-array batch: the rows of the SAME nreq sample ids in nvars (<= DDSK_MAX_MULTI) variables, one launch. vars_dev =
  * device array of the variables' windows; table[v] = sample index of variable v; dst[v]/cap[v]/offsets[v] per variable

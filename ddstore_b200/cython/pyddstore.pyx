@@ -65,6 +65,9 @@ cdef extern from "ddstore_b200.hpp" nogil:
         long get_accumulate_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                                   int op, int dtype, const void* src, void* result, long src_bytes, cbool idx_on_device,
                                   void* stream) except +dds_translate_exception
+        long get_batch_pooled(string name, const long* starts, const long* counts, long fixed_count, long nreq,
+                              int mode, int dtype, const long* bags, long nbags, const void* weights, void* dst,
+                              long dst_capacity_bytes, cbool idx_on_device, void* stream) except +dds_translate_exception
         long compare_and_swap_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                                     int itemsize, const void* src, const void* compare, void* result, long src_bytes,
                                     cbool idx_on_device, void* stream) except +dds_translate_exception
@@ -95,6 +98,8 @@ _ACC_TYPES = {"float32": 1, "float64": 2, "int32": 3, "int64": 4, "float16": 5, 
 _FOP_OPS = {"sum": 1, "replace": 2}
 # reductions of accumulate_batch and get_accumulate_batch beside the sum (DDS_OP_MAX..), by torch's names
 _RED_OPS = {"amax": 4, "amin": 5, "bitwise_and": 6, "bitwise_or": 7, "bitwise_xor": 8}
+# pooling modes of get_batch_pooled (DDS_POOL_*), by torch's embedding_bag names
+_POOL_MODES = {"sum": 1, "mean": 2, "max": 3}
 
 cdef class PyDDStore:
     cdef DDStore* c_ddstore
@@ -365,6 +370,48 @@ cdef class PyDDStore:
             total = self.c_ddstore.accumulate_op_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, opc, code,
                                                        <const void*> dp, nbytes, idx_dev, <void*> st)
         del keep
+        return total
+
+    def get_batch_pooled(self, str name, starts, counts=None, count=None, out=None, bags=None, mode="sum",
+                         weights=None, stream=None):
+        """one kernel launch folding bags of requests into the rows of the CUDA tensor `out` (float32, float64, float16
+        or bfloat16); see ddstore_b200.store.PyDDStore.get_batch_pooled (this binding's call is synchronous). bags and
+        weights are converted to where starts lives. Returns the bytes written."""
+        import torch
+        if mode not in _POOL_MODES:
+            raise ValueError(f"pooled batch of {name!r}: mode {mode!r} is not one of {', '.join(_POOL_MODES)}")
+        if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)) or not out.is_contiguous():
+            raise ValueError("out must be a C-contiguous CUDA tensor")
+        dt = str(out.dtype).replace("torch.", "")
+        if dt not in ("float32", "float64", "float16", "bfloat16"):
+            raise ValueError(f"pooled batch of {name!r}: out dtype {dt} is not float32, float64, float16 or bfloat16")
+        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        dev = out.device if s_dev else "cpu"
+        sa = torch.as_tensor(_i64(starts) if not s_dev else starts, dtype=torch.int64, device=dev).contiguous()
+        ca = torch.as_tensor(_i64(counts) if not s_dev else counts, dtype=torch.int64, device=dev).contiguous() \
+            if counts is not None else None
+        ba = torch.as_tensor(_i64(bags) if not s_dev else bags, dtype=torch.int64, device=dev).contiguous() \
+            if bags is not None else None
+        wa = torch.as_tensor(weights, dtype=out.dtype, device=dev).contiguous() if weights is not None else None
+        cdef long nreq = sa.numel()
+        cdef long nbags = ba.numel() - 1 if ba is not None else nreq
+        cdef size_t sp = sa.data_ptr(), cp = ca.data_ptr() if ca is not None else 0
+        cdef size_t bp = ba.data_ptr() if ba is not None else 0, wp = wa.data_ptr() if wa is not None else 0
+        cdef size_t dp = out.data_ptr()
+        cdef long cap = out.numel() * out.element_size()
+        cdef long fixed = 1 if count is None else int(count)
+        cdef int modec = _POOL_MODES[mode], code = _ACC_TYPES[dt]
+        cdef size_t st = 0
+        if stream is not None:
+            st = int(stream) if int(stream) != 0 else 1
+        cdef string nm = name.encode()
+        cdef cbool idx_dev = bool(s_dev)
+        cdef long total
+        with nogil:
+            total = self.c_ddstore.get_batch_pooled(nm, <const long*> sp, <const long*> cp, fixed, nreq, modec, code,
+                                                    <const long*> bp, nbags, <const void*> wp, <void*> dp, cap, idx_dev,
+                                                    <void*> st)
+        del sa, ca, ba, wa
         return total
 
     def get_accumulate_batch(self, str name, starts, counts=None, src=None, out=None, op="sum", count=None,

@@ -658,6 +658,71 @@ class PyDDStore:
             raise ValueError(f"put into {name!r}: src must be device memory (copy host rows to the device first)")
         return sb, src
 
+    # ---------------------------------------------------------------- pooled batches (embedding_bag)
+    def get_batch_pooled(self, name, starts, counts=None, count=None, out=None, bags=None, mode="sum", weights=None,
+                         stream=None, wait=True):
+        """Fold bags of requests into one row each, in ONE kernel launch: torch's embedding_bag over a sharded variable.
+        Bag k is requests [bags[k], bags[k+1]) (torch's include_last_offset offsets, nbags + 1 of them; None: one bag
+        per request) and goes to out row k -- out (a CUDA float32, float64, float16 or bfloat16 tensor of the variable's
+        itemsize) holds nbags rows of disp elements. mode "sum", "mean" or "max"; weights (mode "sum" only): one per
+        request, torch's per_sample_weights. Requests are located and validated as in get_batch: an invalid one
+        contributes nothing, every valid one is applied, the first invalid one raises with last_bad_index its index; a
+        malformed bag raises ValueError("malformed bag offsets") with last_bad_index the bag, before any request error.
+        Each element is the sequential fold of its bag's rows in float32 (float64 for float64 rows) -- a weighted sum
+        with one fma per row, a mean divided once at the end -- rounded once to out.dtype; max keeps the first row and
+        replaces it by any later row that compares greater. bags and weights live where starts lives (a CUDA tensor:
+        device; else they are staged from the host). Returns the bytes written (None with wait=False)."""
+        return self._pooled(name, False, starts, counts, count, out, bags, mode, weights, stream, wait)
+
+    def get_samples_pooled(self, name, sample_ids, out, bags=None, mode="sum", weights=None, stream=None, wait=True):
+        """get_batch_pooled by SAMPLE ID: request i = the rows of sample sample_ids[i] in the index registered with
+        set_sample_index (e.g. a variable-length sample mean-pooled to one vector)."""
+        return self._pooled(name, True, sample_ids, None, None, out, bags, mode, weights, stream, wait)
+
+    def _pooled(self, name, by_sample, starts, counts, count, out, bags, mode, weights, stream, wait):
+        import torch
+        if mode not in _capi.POOL_MODES:
+            raise ValueError(f"pooled batch of {name!r}: mode {mode!r} is not one of {', '.join(_capi.POOL_MODES)}")
+        if not (isinstance(out, torch.Tensor) and out.is_cuda and out.is_contiguous()):
+            raise ValueError("out must be a C-contiguous CUDA tensor")
+        dt = _dtype_name(out.dtype)
+        if dt not in ("float32", "float64", "float16", "bfloat16"):
+            raise ValueError(f"pooled batch of {name!r}: out dtype {dt} is not float32, float64, float16 or bfloat16")
+        s_dev = isinstance(starts, torch.Tensor) and starts.is_cuda
+        if s_dev:
+            sa = starts.to(torch.int64).contiguous()
+            ca = counts.to(torch.int64).contiguous() if counts is not None else None
+            nreq, sp, cp = sa.numel(), sa.data_ptr(), ca.data_ptr() if ca is not None else None
+            ba = torch.as_tensor(bags, dtype=torch.int64, device=out.device).contiguous() if bags is not None else None
+            wa = torch.as_tensor(weights, dtype=out.dtype, device=out.device).contiguous() if weights is not None else None
+            if not wait and any(t is not None and t is not u for t, u in ((sa, starts), (ca, counts), (ba, bags),
+                                                                          (wa, weights))):
+                raise ValueError("wait=False takes contiguous CUDA tensors: int64 starts, counts and bags, weights of "
+                                 "out.dtype (a converted copy could be freed before the queued launch reads it)")
+        else:
+            sa = _i64(starts)
+            ca = _i64(counts) if counts is not None else None
+            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
+            ba = torch.as_tensor(_i64(bags)) if bags is not None else None
+            wa = torch.as_tensor(weights, dtype=out.dtype, device="cpu").contiguous() if weights is not None else None
+        nbags = ba.numel() - 1 if ba is not None else nreq
+        pool = _capi.Pool(_capi.POOL_MODES[mode], _capi.ACC_TYPES[dt], ba.data_ptr() if ba is not None else None, nbags,
+                          wa.data_ptr() if wa is not None else None)
+        flags = _capi.DST_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
+        total, bad = C.c_int64(0), C.c_int64(-1)
+        cap = out.numel() * out.element_size()
+        if by_sample:
+            rc = self._L.dds_get_samples_pooled(self._h, name.encode(), sp, nreq, C.byref(pool), out.data_ptr(), cap,
+                                                flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
+        else:
+            rc = self._L.dds_get_batch_pooled(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
+                                              C.byref(pool), out.data_ptr(), cap, flags, self._stream_arg(stream),
+                                              C.byref(total), C.byref(bad))
+        del sa, ca, ba, wa
+        self.last_bad_index = bad.value
+        _capi.raise_for(rc)
+        return total.value if wait else None
+
     # ---------------------------------------------------------------- collective owner-push fetch
     def push_setup(self, max_requests, max_bytes):
         """COLLECTIVE: allocate and peer-map the windows of the push fetch (see dds_push_setup)."""

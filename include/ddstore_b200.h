@@ -29,8 +29,9 @@ extern "C" {
                            (dds_accumulate_batch, dds_accumulate_samples, DDS_ACC_*), the batched fetch-ops
                            (dds_get_accumulate_batch, dds_get_accumulate_samples, DDS_OP_*), the batched
                            compare-and-swaps (dds_compare_and_swap_batch, dds_compare_and_swap_samples), the batched
-                           reductions (dds_accumulate_op_batch, dds_accumulate_op_samples, DDS_OP_MAX & co.) and the
-                           placed variables (dds_add_placed, dds_init_placed, dds_query_placement, DDS_PLACE_*). */
+                           reductions (dds_accumulate_op_batch, dds_accumulate_op_samples, DDS_OP_MAX & co.), the
+                           placed variables (dds_add_placed, dds_init_placed, dds_query_placement, DDS_PLACE_*) and the
+                           pooled batches (dds_get_batch_pooled, dds_get_samples_pooled, DDS_POOL_*). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -463,6 +464,55 @@ int dds_compare_and_swap_batch(dds_store_t *s, const char *name, const int64_t *
 int dds_compare_and_swap_samples(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq, int itemsize,
                                  const void *src, const void *compare, void *result, int64_t src_bytes, unsigned flags,
                                  void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+
+/* ---- pooled batches: bags of rows from any rank's shard reduced to one row each (torch's embedding_bag over a sharded
+ * variable, in one launch)
+ * Requests are located and validated exactly as in dds_get_batch / dds_get_samples, with the same codes, texts and
+ * divergences; a sample id outside the index is DDS_ERR_ARG, "sample id outside the variable's sample index".
+ * Bag k folds the rows of requests [bags[k], bags[k+1]) -- in request order, within a request in row order -- into output
+ * row k: dst bytes [k * R, (k + 1) * R), R = disp * itemsize, in `dtype`. *total_bytes = nbags * R. bags == NULL: bag i is
+ * request i (nbags must equal nreq). Requests no bag covers are neither read nor validated.
+ * An invalid request contributes nothing and every valid request is still applied (the padded entries' rule); the first
+ * (lowest-index) invalid request is reported.
+ * Numerics, per output element -- the sequential fold torch's CUDA embedding_bag forward computes:
+ *   acc is f32 for f32, f16 and bf16 rows and f64 for f64 rows, starting at +0;
+ *   DDS_POOL_SUM   acc = acc + x, or with weights acc = fma(w, x, acc) (one rounding);
+ *   DDS_POOL_MEAN  acc = acc + x, then acc / (rows folded) (IEEE division; a bag with no rows stays 0);
+ *   then one round-to-nearest conversion to dtype;
+ *   DDS_POOL_MAX   in dtype: the bag's first row as it is, then acc = (x > acc) ? x : acc -- so a leading NaN stays,
+ *                  later NaNs are ignored, and of -0 and +0 the earlier one is kept.
+ * An empty bag, or one whose requests are all invalid, is +0 in every mode. Nothing flushes subnormals. NaN results of the
+ * arithmetic are the canonical NaN. The result is bitwise deterministic: it does not depend on the grid, the ranks, the
+ * stream or the queue.
+ * Argument errors, DDS_ERR_ARG with nothing enqueued: an unknown mode; a dtype that is not DDS_ACC_F32, F64, F16 or BF16;
+ * weights with a mode other than DDS_POOL_SUM; flags without DDS_DST_ON_DEVICE; nbags < 0; bags == NULL with nbags !=
+ * nreq; dst_capacity < nbags * R or nbags * R overflowing; dst or weights not aligned to the element size;
+ * dds_get_samples_pooled on a variable without a sample index; DDS_NO_SYNC with host indices. A dtype whose size is not
+ * the variable's itemsize is DDS_ERR_DTYPE.
+ * Malformed bags: bag k is malformed when bags[k] < 0, bags[k + 1] < bags[k] or bags[k + 1] > nreq. Host bags are checked
+ * before anything is enqueued; device bags by the kernel, which writes a malformed bag's row as zeros. Either way the call
+ * returns DDS_ERR_ARG, "malformed bag offsets", with *bad_index = the lowest such k; a malformed bag takes precedence over
+ * any invalid request.
+ * Flags: DDS_IDX_ON_DEVICE covers starts, counts, sample ids, bags and weights alike; host ones are staged as in the get
+ * entries. DDS_NO_SYNC queues the call (dds_batch_wait reports it like a queued get, its total nbags * R). DDS_OVERLAP is
+ * ignored: a pooled launch ends an overlap run, like a put. DDS_PLACE_HOST variables are read over PCIe on the host
+ * gather's small grid, with the same results. */
+#define DDS_POOL_SUM 1
+#define DDS_POOL_MEAN 2
+#define DDS_POOL_MAX 3
+typedef struct {
+    int32_t mode;        /* DDS_POOL_* */
+    int32_t dtype;       /* DDS_ACC_F32, DDS_ACC_F64, DDS_ACC_F16 or DDS_ACC_BF16: element type of rows and output */
+    const int64_t *bags; /* nbags + 1 request offsets (torch's include_last_offset form); NULL: bag i = request i */
+    int64_t nbags;
+    const void *weights; /* nullable, one per REQUEST, in `dtype`; DDS_POOL_SUM only (torch's per_sample_weights) */
+} dds_pool_t;
+int dds_get_batch_pooled(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                         int64_t fixed_count, int64_t nreq, const dds_pool_t *pool, void *dst, int64_t dst_capacity,
+                         unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
+int dds_get_samples_pooled(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq,
+                           const dds_pool_t *pool, void *dst, int64_t dst_capacity, unsigned flags, void *cuda_stream,
+                           int64_t *total_bytes, int64_t *bad_index);
 
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite

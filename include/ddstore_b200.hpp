@@ -213,6 +213,30 @@ class DDStore {
                             bool idx_on_device = true, void *cuda_stream = nullptr) {
         return accumulate_samples(name, sample_ids, nreq, acc_type<T>(), src, src_bytes, idx_on_device, cuda_stream);
     }
+    // Pooled batch (dds_get_batch_pooled): bag k = requests [bags[k], bags[k+1]) (bags NULL: one bag per request) folded
+    // into row k of dst by `mode` (DDS_POOL_*) in `dtype` (DDS_ACC_F32, F64, F16 or BF16); weights nullable, one per
+    // request, DDS_POOL_SUM only. dst is device memory; bags and weights live where the indices do. Returns nbags * R.
+    long get_batch_pooled(std::string name, const long *starts, const long *counts, long fixed_count, long nreq, int mode,
+                          int dtype, const long *bags, long nbags, const void *weights, void *dst, long dst_capacity_bytes,
+                          bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        dds_pool_t p{mode, dtype, (const int64_t *)bags, nbags, weights};
+        const unsigned flags = DDS_DST_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_get_batch_pooled(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts, fixed_count, nreq,
+                                   &p, dst, dst_capacity_bytes, flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    // The same by sample id (dds_get_samples_pooled).
+    long get_samples_pooled(std::string name, const long *sample_ids, long nreq, int mode, int dtype, const long *bags,
+                            long nbags, const void *weights, void *dst, long dst_capacity_bytes, bool idx_on_device = true,
+                            void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        dds_pool_t p{mode, dtype, (const int64_t *)bags, nbags, weights};
+        const unsigned flags = DDS_DST_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_get_samples_pooled(store_, name.c_str(), (const int64_t *)sample_ids, nreq, &p, dst, dst_capacity_bytes,
+                                     flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
     // Batched reduction (dds_accumulate_op_batch): accumulate_batch with each element becoming op(shard, src), op one of
     // DDS_OP_SUM, DDS_OP_MAX, DDS_OP_MIN, DDS_OP_BAND, DDS_OP_BOR, DDS_OP_BXOR (the bitwise ops on integer types only).
     long accumulate_op_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq, int op,
