@@ -17,8 +17,11 @@ from libc.stdint cimport uint64_t
 
 import numpy as np
 
+from ddstore_b200._capi import PLACEMENTS
 from ddstore_b200.comm import as_dds_comm
-from ddstore_b200.store import _Buf, _conversion, _dtype_name, _i64, _norm_tables, _pad_bits, _ptr
+from ddstore_b200.store import (_PLACEMENT_NAMES as PLACEMENT_NAMES, _Buf, _acc_type, _cas_args, _dtype_name, _fop_args,
+                                _get_args, _norm_tables, _offsets, _pad, _pad_rows, _placement, _pool_args,
+                                _pool_requests, _ptr, _put_src, _red_op, _requests, _stream_handle)
 
 cdef extern from *:
     """
@@ -80,26 +83,6 @@ cdef extern from "ddstore_b200.hpp" nogil:
         int rank()
         int size()
 
-
-# where a variable's shards live (DDS_PLACE_*), by name
-PLACEMENTS = {"hbm": 0, "host": 1}
-PLACEMENT_NAMES = {v: k for k, v in PLACEMENTS.items()}
-
-
-def _placement(str placement):
-    if placement not in PLACEMENTS:
-        raise ValueError(f"unknown placement {placement!r} (expected 'hbm' or 'host')")
-    return PLACEMENTS[placement]
-
-
-# element types of accumulate_batch (DDS_ACC_*), by dtype name
-_ACC_TYPES = {"float32": 1, "float64": 2, "int32": 3, "int64": 4, "float16": 5, "bfloat16": 6}
-# ops of get_accumulate_batch (DDS_OP_*), by name
-_FOP_OPS = {"sum": 1, "replace": 2}
-# reductions of accumulate_batch and get_accumulate_batch beside the sum (DDS_OP_MAX..), by torch's names
-_RED_OPS = {"amax": 4, "amin": 5, "bitwise_and": 6, "bitwise_or": 7, "bitwise_xor": 8}
-# pooling modes of get_batch_pooled (DDS_POOL_*), by torch's embedding_bag names
-_POOL_MODES = {"sum": 1, "mean": 2, "max": 3}
 
 cdef class PyDDStore:
     cdef DDStore* c_ddstore
@@ -170,116 +153,48 @@ cdef class PyDDStore:
         src_dtype / lut: deliver the rows converted to out.dtype (a CUDA tensor), as in ddstore_b200's get_batch;
         normalize=True: normalised with the tables of set_normalization, as there.
         pad_rows / pad_value / lengths (with counts and a CUDA tensor `out`): a padded batch, as there."""
-        if out is None:
-            raise ValueError("get_batch needs an `out` buffer")
-        cv = lut_keep = None
-        if normalize and src_dtype is None:
-            raise ValueError("normalize=True needs src_dtype")
-        if pad_rows is not None and (counts is None or count is not None or offsets is not None):
-            raise ValueError("pad_rows needs counts, and takes neither `count` nor `offsets`")
-        if src_dtype is not None:
-            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
+        cv, lut_keep = _get_args(False, counts, count, out, offsets, src_dtype, lut, normalize, pad_rows)
         ob = _Buf(out, writable=True, half_ok=cv is not None or pad_rows is not None)
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
+        py_nreq, py_sp, py_cp, s_dev, keep = _requests(starts, counts)
         if pad_rows is not None:
-            return self._get_batch_padded(name, starts, counts, out, ob, stream, src_dtype, cv, lut_keep, bool(s_dev),
-                                          pad_rows, pad_value, lengths)
-        if cv is not None:
-            return self._get_batch_convert(name, starts, counts, ob, count, offsets, stream, cv, lut_keep, bool(s_dev))
-        if bool(s_dev) != bool(ob.on_device):
+            return self._get_batch_padded(name, py_sp, py_cp, py_nreq, s_dev, out, ob, stream, src_dtype, cv, pad_rows,
+                                          pad_value, lengths)
+        if cv is None and s_dev != bool(ob.on_device):
             raise ValueError("the Cython get_batch wants indices and out on the same side (both host or both device)")
-        cdef size_t sp, cp = 0, op = 0, dp = ob.ptr
-        cdef long nreq
-        if s_dev:
-            nreq = starts.numel(); sp = starts.data_ptr()
-            if counts is not None: cp = counts.data_ptr()
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
-            ca = _i64(counts) if counts is not None else None
-            if ca is not None: cp = ca.ctypes.data
-            keep = (sa, ca)
-        if offsets is not None:
-            fb = _Buf(offsets, writable=True)
-            op = fb.ptr
-        cdef long fixed = 1 if count is None else int(count)
-        cdef long cap = ob.nbytes
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
+        if cv is not None and not ob.on_device:
+            raise ValueError("converting batches deliver into device memory")
+        cdef size_t op = _offsets(offsets, ob, py_nreq, False) or 0
+        cdef size_t sp = py_sp, cp = py_cp or 0, dp = ob.ptr, lp = (cv.lut or 0) if cv is not None else 0
+        cdef long nreq = py_nreq, fixed = 1 if count is None else int(count), cap = ob.nbytes
+        cdef size_t st = _stream_handle(stream)
         cdef string nm = name.encode()
-        cdef int w = ob.itemsize
-        cdef cbool dev = bool(ob.on_device)
+        cdef int w = ob.itemsize, code = cv.code if cv is not None else 0
+        cdef cbool dev = s_dev
         cdef long total
         with nogil:
-          if w == 1:
+          if code:
+            total = self.c_ddstore.get_batch_convert(nm, <const long*> sp, <const long*> cp, fixed, nreq, <void*> dp, cap,
+                                                     code, <const void*> lp, <long*> op, dev, <void*> st)
+          elif w == 1:
             total = self.c_ddstore.get_batch[char](nm, <const long*> sp, <const long*> cp, fixed, nreq, <char*> dp, cap, <long*> op, dev, <void*> st)
           elif w == 4:
             total = self.c_ddstore.get_batch[int](nm, <const long*> sp, <const long*> cp, fixed, nreq, <int*> dp, cap, <long*> op, dev, <void*> st)
           else:
             total = self.c_ddstore.get_batch[long](nm, <const long*> sp, <const long*> cp, fixed, nreq, <long*> dp, cap, <long*> op, dev, <void*> st)
-        del keep
-        return total
-
-    def _get_batch_convert(self, str name, starts, counts, ob, count, offsets, stream, cv, lut_keep, s_dev):
-        cdef size_t sp, cp = 0, op = 0, dp = ob.ptr, lp = cv.lut or 0
-        cdef long nreq
-        if s_dev:
-            nreq = starts.numel(); sp = starts.data_ptr()
-            if counts is not None: cp = counts.data_ptr()
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
-            ca = _i64(counts) if counts is not None else None
-            if ca is not None: cp = ca.ctypes.data
-            keep = (sa, ca)
-        if offsets is not None:
-            op = _Buf(offsets, writable=True).ptr
-        cdef long fixed = 1 if count is None else int(count)
-        cdef long cap = ob.nbytes
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
-        cdef string nm = name.encode()
-        cdef int code = cv.code
-        cdef cbool idx_dev = s_dev
-        cdef long total
-        if not ob.on_device:
-            raise ValueError("converting batches deliver into device memory")
-        with nogil:
-            total = self.c_ddstore.get_batch_convert(nm, <const long*> sp, <const long*> cp, fixed, nreq, <void*> dp, cap,
-                                                     code, <const void*> lp, <long*> op, idx_dev, <void*> st)
         del keep, lut_keep
         return total
 
-    def _get_batch_padded(self, str name, starts, counts, out, ob, stream, src_dtype, cv, lut_keep, s_dev, pad_rows,
+    def _get_batch_padded(self, str name, py_sp, py_cp, py_nreq, s_dev, out, ob, stream, src_dtype, cv, pad_rows,
                           pad_value, lengths):
-        if not (ob.on_device and str(getattr(out, "dtype", "")).startswith("torch.")):
-            raise ValueError("a padded batch delivers into a CUDA tensor")
-        cdef size_t sp, cp, dp = ob.ptr, lp = (cv.lut or 0) if cv is not None else 0, lnp = 0
-        cdef long nreq
-        if s_dev:
-            nreq = starts.numel(); sp = starts.data_ptr(); cp = counts.data_ptr()
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
-            ca = _i64(counts); cp = ca.ctypes.data
-            keep = (sa, ca)
-        if lengths is not None:
-            lb = _Buf(lengths, writable=True)
-            if not lb.on_device or lb.itemsize != 8 or lb.size < nreq:
-                raise ValueError("lengths must be an int64 CUDA tensor of len(starts)")
-            lnp = lb.ptr
+        cdef long max_rows = _pad_rows(pad_rows, out, ob)
+        pad = _pad(max_rows, pad_value, lengths, out, py_nreq)
+        cdef size_t sp = py_sp, cp = py_cp, dp = ob.ptr, lp = (cv.lut or 0) if cv is not None else 0
+        cdef size_t lnp = pad.lengths or 0
         cdef int itemsize = ob.itemsize if cv is None else np.dtype(_dtype_name(src_dtype)).itemsize
         cdef int code = 0 if cv is None else cv.code
-        cdef long max_rows = int(pad_rows)
-        if max_rows < 0:
-            raise ValueError("pad_rows must be >= 0")
-        cdef uint64_t bits = _pad_bits(pad_value, out.dtype)
-        cdef long cap = ob.nbytes
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
+        cdef uint64_t bits = pad.pad_bits
+        cdef long nreq = py_nreq, cap = ob.nbytes
+        cdef size_t st = _stream_handle(stream)
         cdef string nm = name.encode()
         cdef cbool idx_dev = s_dev
         cdef long total
@@ -287,38 +202,18 @@ cdef class PyDDStore:
             total = self.c_ddstore.get_batch_padded_convert(nm, <const long*> sp, <const long*> cp, nreq, itemsize, code,
                                                             <const void*> lp, max_rows, bits, <void*> dp, cap,
                                                             <long*> lnp, idx_dev, <void*> st)
-        del keep, lut_keep
         return total
 
     def put_batch(self, str name, starts, counts=None, src=None, count=None, stream=None):
         """one kernel launch writing len(starts) requests from the CUDA tensor `src` into the owners' shards; see
         ddstore_b200.store.PyDDStore.put_batch (this binding's put is synchronous). Returns the layout's bytes."""
-        if src is None:
-            raise ValueError("a put needs `src` rows")
-        if not (hasattr(src, "data_ptr") and getattr(src, "is_cuda", False)):
-            raise ValueError(f"put into {name!r}: src must be a CUDA tensor (copy host rows to the device first)")
-        if not src.is_contiguous():
-            raise ValueError("src must be C-contiguous")
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        cdef size_t sp, cp = 0, dp = src.data_ptr()
-        cdef long nreq
-        if s_dev:
-            nreq = starts.numel(); sp = starts.data_ptr()
-            if counts is not None: cp = counts.data_ptr()
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
-            ca = _i64(counts) if counts is not None else None
-            if ca is not None: cp = ca.ctypes.data
-            keep = (sa, ca)
-        cdef long fixed = 1 if count is None else int(count)
-        cdef int w = src.element_size()
-        cdef long nbytes = src.numel() * w
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
+        sb = _put_src(name, src)
+        py_nreq, py_sp, py_cp, s_dev, keep = _requests(starts, counts)
+        cdef size_t sp = py_sp, cp = py_cp or 0, dp = sb.ptr, st = _stream_handle(stream)
+        cdef long nreq = py_nreq, fixed = 1 if count is None else int(count), nbytes = sb.nbytes
+        cdef int w = sb.itemsize
         cdef string nm = name.encode()
-        cdef cbool idx_dev = bool(s_dev)
+        cdef cbool idx_dev = s_dev
         cdef long total
         with nogil:
             if w == 1: total = self.c_ddstore.put_batch[char](nm, <const long*> sp, <const long*> cp, fixed, nreq, <const char*> dp, nbytes, idx_dev, <void*> st)
@@ -333,38 +228,13 @@ cdef class PyDDStore:
         len(starts) requests of the CUDA tensor `src` into the owners' shards, in src's dtype (float32, float64, int32,
         int64, float16 or bfloat16); see ddstore_b200.store.PyDDStore.accumulate_batch (this binding's accumulate is
         synchronous). Returns the layout's bytes."""
-        if src is None:
-            raise ValueError("an accumulate needs `src` rows")
-        if not (hasattr(src, "data_ptr") and getattr(src, "is_cuda", False)):
-            raise ValueError(f"accumulate into {name!r}: src must be a CUDA tensor (copy host rows to the device first)")
-        if not src.is_contiguous():
-            raise ValueError("src must be C-contiguous")
-        dt = str(src.dtype).replace("torch.", "")
-        if dt not in _ACC_TYPES:
-            raise ValueError(f"accumulate into {name!r}: src dtype {dt} is not one of {', '.join(_ACC_TYPES)}")
-        ops = {"sum": 1, **_RED_OPS}
-        if op not in ops:
-            raise ValueError(f"accumulate into {name!r}: op {op!r} is not one of {', '.join(ops)}")
-        cdef int code = _ACC_TYPES[dt], opc = ops[op]
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        cdef size_t sp, cp = 0, dp = src.data_ptr()
-        cdef long nreq
-        if s_dev:
-            nreq = starts.numel(); sp = starts.data_ptr()
-            if counts is not None: cp = counts.data_ptr()
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
-            ca = _i64(counts) if counts is not None else None
-            if ca is not None: cp = ca.ctypes.data
-            keep = (sa, ca)
-        cdef long fixed = 1 if count is None else int(count)
-        cdef long nbytes = src.numel() * src.element_size()
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
+        sb = _put_src(name, src)
+        cdef int code = _acc_type(name, src), opc = _red_op(name, op)
+        py_nreq, py_sp, py_cp, s_dev, keep = _requests(starts, counts)
+        cdef size_t sp = py_sp, cp = py_cp or 0, dp = sb.ptr, st = _stream_handle(stream)
+        cdef long nreq = py_nreq, fixed = 1 if count is None else int(count), nbytes = sb.nbytes
         cdef string nm = name.encode()
-        cdef cbool idx_dev = bool(s_dev)
+        cdef cbool idx_dev = s_dev
         cdef long total
         with nogil:
             total = self.c_ddstore.accumulate_op_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, opc, code,
@@ -377,35 +247,17 @@ cdef class PyDDStore:
         """one kernel launch folding bags of requests into the rows of the CUDA tensor `out` (float32, float64, float16
         or bfloat16); see ddstore_b200.store.PyDDStore.get_batch_pooled (this binding's call is synchronous). bags and
         weights are converted to where starts lives. Returns the bytes written."""
-        import torch
-        if mode not in _POOL_MODES:
-            raise ValueError(f"pooled batch of {name!r}: mode {mode!r} is not one of {', '.join(_POOL_MODES)}")
-        if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)) or not out.is_contiguous():
-            raise ValueError("out must be a C-contiguous CUDA tensor")
-        dt = str(out.dtype).replace("torch.", "")
-        if dt not in ("float32", "float64", "float16", "bfloat16"):
-            raise ValueError(f"pooled batch of {name!r}: out dtype {dt} is not float32, float64, float16 or bfloat16")
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        dev = out.device if s_dev else "cpu"
-        sa = torch.as_tensor(_i64(starts) if not s_dev else starts, dtype=torch.int64, device=dev).contiguous()
-        ca = torch.as_tensor(_i64(counts) if not s_dev else counts, dtype=torch.int64, device=dev).contiguous() \
-            if counts is not None else None
-        ba = torch.as_tensor(_i64(bags) if not s_dev else bags, dtype=torch.int64, device=dev).contiguous() \
-            if bags is not None else None
-        wa = torch.as_tensor(weights, dtype=out.dtype, device=dev).contiguous() if weights is not None else None
+        modes_types = _pool_args(name, mode, out)
+        cdef int modec = modes_types[0], code = modes_types[1]
+        sa, ca, ba, wa, s_dev = _pool_requests(starts, counts, bags, weights, out, True)
         cdef long nreq = sa.numel()
         cdef long nbags = ba.numel() - 1 if ba is not None else nreq
         cdef size_t sp = sa.data_ptr(), cp = ca.data_ptr() if ca is not None else 0
         cdef size_t bp = ba.data_ptr() if ba is not None else 0, wp = wa.data_ptr() if wa is not None else 0
-        cdef size_t dp = out.data_ptr()
-        cdef long cap = out.numel() * out.element_size()
-        cdef long fixed = 1 if count is None else int(count)
-        cdef int modec = _POOL_MODES[mode], code = _ACC_TYPES[dt]
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
+        cdef size_t dp = out.data_ptr(), st = _stream_handle(stream)
+        cdef long cap = out.numel() * out.element_size(), fixed = 1 if count is None else int(count)
         cdef string nm = name.encode()
-        cdef cbool idx_dev = bool(s_dev)
+        cdef cbool idx_dev = s_dev
         cdef long total
         with nogil:
             total = self.c_ddstore.get_batch_pooled(nm, <const long*> sp, <const long*> cp, fixed, nreq, modec, code,
@@ -420,42 +272,15 @@ cdef class PyDDStore:
         requests of the CUDA tensor `src` into the owners' shards and writing the previous rows to the CUDA tensor `out` (src's layout, at least its
         bytes; it may be src); see ddstore_b200.store.PyDDStore.get_accumulate_batch (this binding's fetch-op is
         synchronous). Returns the layout's bytes."""
-        if src is None:
-            raise ValueError("a fetch-op needs `src` rows")
-        if not (hasattr(src, "data_ptr") and getattr(src, "is_cuda", False)):
-            raise ValueError(f"fetch-op on {name!r}: src must be a CUDA tensor (copy host rows to the device first)")
-        if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)):
-            raise ValueError(f"fetch-op on {name!r}: out must be a CUDA tensor")
-        if not src.is_contiguous() or not out.is_contiguous():
-            raise ValueError("src and out must be C-contiguous")
-        dt = str(src.dtype).replace("torch.", "")
-        if dt not in _ACC_TYPES:
-            raise ValueError(f"fetch-op on {name!r}: src dtype {dt} is not one of {', '.join(_ACC_TYPES)}")
-        ops = {**_FOP_OPS, **_RED_OPS}
-        if op not in ops:
-            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(ops)}")
-        cdef long nbytes = src.numel() * src.element_size()
-        if out.numel() * out.element_size() < nbytes:
-            raise ValueError(f"fetch-op on {name!r}: out holds {out.numel() * out.element_size()} bytes, src {nbytes}")
-        cdef int code = _ACC_TYPES[dt], opc = ops[op]
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        cdef size_t sp, cp = 0, dp = src.data_ptr(), rp = out.data_ptr()
-        cdef long nreq
-        if s_dev:
-            nreq = starts.numel(); sp = starts.data_ptr()
-            if counts is not None: cp = counts.data_ptr()
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
-            ca = _i64(counts) if counts is not None else None
-            if ca is not None: cp = ca.ctypes.data
-            keep = (sa, ca)
-        cdef long fixed = 1 if count is None else int(count)
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
+        sb = _put_src(name, src)
+        cdef int code = _acc_type(name, src)
+        opc_res = _fop_args(name, op, out, sb)
+        cdef int opc = opc_res[0]
+        py_nreq, py_sp, py_cp, s_dev, keep = _requests(starts, counts)
+        cdef size_t sp = py_sp, cp = py_cp or 0, dp = sb.ptr, rp = opc_res[1], st = _stream_handle(stream)
+        cdef long nreq = py_nreq, fixed = 1 if count is None else int(count), nbytes = sb.nbytes
         cdef string nm = name.encode()
-        cdef cbool idx_dev = bool(s_dev)
+        cdef cbool idx_dev = s_dev
         cdef long total
         with nogil:
             total = self.c_ddstore.get_accumulate_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, opc, code,
@@ -470,40 +295,15 @@ cdef class PyDDStore:
         src's element size and at least its bytes, src's layout; out may be src or compare); see
         ddstore_b200.store.PyDDStore.compare_and_swap_batch (this binding's compare-and-swap is synchronous). Returns the
         layout's bytes."""
-        if src is None:
-            raise ValueError("a compare-and-swap needs `src` rows")
-        for what, t in (("src", src), ("compare", compare), ("out", out)):
-            if not (hasattr(t, "data_ptr") and getattr(t, "is_cuda", False)):
-                raise ValueError(f"compare-and-swap on {name!r}: {what} must be a CUDA tensor")
-            if not t.is_contiguous():
-                raise ValueError(f"{what} must be C-contiguous")
-            if t.element_size() != src.element_size():
-                raise ValueError(f"compare-and-swap on {name!r}: {what} has {t.element_size()}-byte elements, src "
-                                 f"{src.element_size()}-byte ones")
-        cdef long nbytes = src.numel() * src.element_size()
-        for what, t in (("compare", compare), ("out", out)):
-            if t.numel() * t.element_size() < nbytes:
-                raise ValueError(f"compare-and-swap on {name!r}: {what} holds {t.numel() * t.element_size()} bytes, "
-                                 f"src {nbytes}")
-        cdef int itemsize = src.element_size()
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        cdef size_t sp, cp = 0, dp = src.data_ptr(), qp = compare.data_ptr(), rp = out.data_ptr()
-        cdef long nreq
-        if s_dev:
-            nreq = starts.numel(); sp = starts.data_ptr()
-            if counts is not None: cp = counts.data_ptr()
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts); nreq = sa.size; sp = sa.ctypes.data
-            ca = _i64(counts) if counts is not None else None
-            if ca is not None: cp = ca.ctypes.data
-            keep = (sa, ca)
-        cdef long fixed = 1 if count is None else int(count)
-        cdef size_t st = 0
-        if stream is not None:
-            st = int(stream) if int(stream) != 0 else 1
+        sb = _put_src(name, src)
+        cmp_res = _cas_args(name, compare, out, sb)
+        py_nreq, py_sp, py_cp, s_dev, keep = _requests(starts, counts)
+        cdef size_t sp = py_sp, cp = py_cp or 0, dp = sb.ptr, qp = cmp_res[0], rp = cmp_res[1]
+        cdef size_t st = _stream_handle(stream)
+        cdef long nreq = py_nreq, fixed = 1 if count is None else int(count), nbytes = sb.nbytes
+        cdef int itemsize = sb.itemsize
         cdef string nm = name.encode()
-        cdef cbool idx_dev = bool(s_dev)
+        cdef cbool idx_dev = s_dev
         cdef long total
         with nogil:
             total = self.c_ddstore.compare_and_swap_batch(nm, <const long*> sp, <const long*> cp, fixed, nreq, itemsize,

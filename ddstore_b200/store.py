@@ -188,7 +188,198 @@ def _i64(x):
     return np.ascontiguousarray(x, dtype=np.int64)
 
 
+def _requests(starts, counts=None):
+    """-> (nreq, starts_ptr, counts_ptr, on_device, keep) of a batch's index arrays: CUDA tensors are passed as they
+    are, anything else as host int64 arrays (counts None: a null counts pointer). `keep` holds what the pointers
+    point into; the caller keeps it until the call has returned."""
+    if hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False):
+        return starts.numel(), starts.data_ptr(), counts.data_ptr() if counts is not None else None, True, \
+            (starts, counts)
+    sa = _i64(starts)
+    ca = _i64(counts) if counts is not None else None
+    return sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None, False, (sa, ca)
+
+
+def _stream_handle(stream):
+    """the raw cudaStream_t of a `stream` argument: None -> 0, the store's own stream; otherwise the handle (e.g.
+    torch.cuda.current_stream().cuda_stream). Handle 0 is CUDA's legacy default stream, which the C-ABI spells
+    cudaStreamLegacy (0x1) because NULL there means "the store's stream"."""
+    if stream is None:
+        return 0
+    h = int(stream)
+    return h if h != 0 else 1
+
+
+# ---------------------------------------------------------------- argument checks of the batched gets
+def _get_args(by_sample, counts, count, out, offsets, src_dtype, lut, normalize, pad_rows):
+    """the argument rules of get_batch / get_samples (by_sample) that precede the `out` buffer's -> (dds_convert_t,
+    keepalive) of a converting batch, (None, None) of a raw one"""
+    if by_sample:
+        if pad_rows is not None and offsets is not None:
+            raise ValueError("a padded batch takes no `offsets`")
+    else:
+        if out is None:
+            raise ValueError("get_batch needs an `out` buffer (like get(), it never allocates)")
+        if pad_rows is not None:
+            if counts is None:
+                raise ValueError("pad_rows needs counts (there is no fixed-count padded batch)")
+            if count is not None or offsets is not None:
+                raise ValueError("a padded batch takes neither `count` nor `offsets`")
+    if normalize and src_dtype is None:
+        raise ValueError("normalize=True needs src_dtype")
+    if src_dtype is None:
+        return None, None
+    return _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
+
+
+def _offsets(offsets, ob, nreq, by_sample):
+    """the address of a batch's `offsets` (None: no offsets); ValueError unless it is int64[nreq + 1] on out's side"""
+    if offsets is None:
+        return None
+    fb = _Buf(offsets, writable=True)
+    if fb.on_device != ob.on_device or fb.itemsize != 8 or fb.size < nreq + 1:
+        raise ValueError(f"offsets must be int64[len({'sample_ids' if by_sample else 'starts'})+1] with the same "
+                         f"residency as out")
+    return fb.ptr
+
+
+def _pad_rows(pad_rows, out, ob):
+    """pad_rows of a padded batch into `out` (ob: its _Buf) as an int; ValueError unless it is >= 0 and out is a CUDA
+    tensor"""
+    pad_rows = int(pad_rows)
+    if pad_rows < 0:
+        raise ValueError("pad_rows must be >= 0")
+    if not (ob.on_device and hasattr(out, "dtype") and str(out.dtype).startswith("torch.")):
+        raise ValueError("a padded batch delivers into a CUDA tensor")
+    return pad_rows
+
+
+def _pad(pad_rows, pad_value, lengths, out, nreq):
+    """the dds_pad_t of a padded batch of nreq requests into `out`"""
+    pad = _capi.Pad(pad_rows, _pad_bits(pad_value, out.dtype), None)
+    if lengths is not None:
+        lb = _Buf(lengths, writable=True)
+        if not lb.on_device or lb.itemsize != 8 or lb.size < nreq:
+            raise ValueError("lengths must be an int64 CUDA tensor of len(starts)")
+        pad.lengths = lb.ptr
+    return pad
+
+
+# ---------------------------------------------------------------- argument checks of the batched writes and pools
+def _put_src(name, src):
+    """the _Buf of a put's source rows (a CUDA tensor or CAI object; ValueError for host memory)"""
+    if src is None:
+        raise ValueError("a put needs `src` rows")
+    if hasattr(src, "data_ptr") and hasattr(src, "element_size"):  # any torch dtype: only its element size matters
+        if not src.is_contiguous():
+            raise ValueError("src must be C-contiguous")
+        sb = _Buf.__new__(_Buf)
+        sb.ptr, sb.on_device, sb.itemsize = src.data_ptr(), 1 if src.is_cuda else 0, src.element_size()
+        sb.nbytes = src.numel() * sb.itemsize
+    else:
+        sb = _Buf(src)
+    if not sb.on_device:
+        raise ValueError(f"put into {name!r}: src must be device memory (copy host rows to the device first)")
+    return sb
+
+
+def _acc_type(name, src):
+    """the DDS_ACC_* element type of an accumulate's src, from its dtype (ValueError for any other)"""
+    dt = str(getattr(src, "dtype", "")).replace("torch.", "")
+    if dt not in _capi.ACC_TYPES:
+        raise ValueError(f"accumulate into {name!r}: src dtype {dt or type(src).__name__} is not one of "
+                         f"{', '.join(_capi.ACC_TYPES)}")
+    return _capi.ACC_TYPES[dt]
+
+
+def _red_op(name, op):
+    """the DDS_OP_* code of an accumulate's reduction (ValueError for an unknown one)"""
+    ops = {"sum": _capi.OP_SUM, **_capi.RED_OPS}
+    if op not in ops:
+        raise ValueError(f"accumulate into {name!r}: op {op!r} is not one of {', '.join(ops)}")
+    return ops[op]
+
+
+def _fop_args(name, op, out, sb):
+    """the DDS_OP_* code of a fetch-op and the address of its `out` tensor (ValueError for an unknown op, or an out
+    that is not a contiguous CUDA tensor of at least src's bytes)"""
+    ops = {**_capi.FOP_OPS, **_capi.RED_OPS}
+    if op not in ops:
+        raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(ops)}")
+    if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)):
+        raise ValueError(f"fetch-op on {name!r}: out must be a CUDA tensor")
+    if not out.is_contiguous():
+        raise ValueError("out must be C-contiguous")
+    if out.numel() * out.element_size() < sb.nbytes:
+        raise ValueError(f"fetch-op on {name!r}: out holds {out.numel() * out.element_size()} bytes, src "
+                         f"{sb.nbytes}")
+    return ops[op], out.data_ptr()
+
+
+def _cas_args(name, compare, out, sb):
+    """the addresses of a compare-and-swap's `compare` and `out` tensors (ValueError unless each is a C-contiguous
+    CUDA tensor of src's element size and at least src's bytes)"""
+    ptrs = []
+    for what, t in (("compare", compare), ("out", out)):
+        if not (hasattr(t, "data_ptr") and getattr(t, "is_cuda", False)):
+            raise ValueError(f"compare-and-swap on {name!r}: {what} must be a CUDA tensor")
+        if not t.is_contiguous():
+            raise ValueError(f"{what} must be C-contiguous")
+        if t.element_size() != sb.itemsize:
+            raise ValueError(f"compare-and-swap on {name!r}: {what} has {t.element_size()}-byte elements, src "
+                             f"{sb.itemsize}-byte ones")
+        if t.numel() * t.element_size() < sb.nbytes:
+            raise ValueError(f"compare-and-swap on {name!r}: {what} holds {t.numel() * t.element_size()} bytes, "
+                             f"src {sb.nbytes}")
+        ptrs.append(t.data_ptr())
+    return ptrs[0], ptrs[1]
+
+
+def _pool_args(name, mode, out):
+    """the DDS_POOL_* mode and the DDS_ACC_* element type of a pooled batch into `out` (ValueError for an unknown
+    mode, or an out that is not a C-contiguous CUDA float32, float64, float16 or bfloat16 tensor)"""
+    import torch
+    if mode not in _capi.POOL_MODES:
+        raise ValueError(f"pooled batch of {name!r}: mode {mode!r} is not one of {', '.join(_capi.POOL_MODES)}")
+    if not (isinstance(out, torch.Tensor) and out.is_cuda and out.is_contiguous()):
+        raise ValueError("out must be a C-contiguous CUDA tensor")
+    dt = _dtype_name(out.dtype)
+    if dt not in ("float32", "float64", "float16", "bfloat16"):
+        raise ValueError(f"pooled batch of {name!r}: out dtype {dt} is not float32, float64, float16 or bfloat16")
+    return _capi.POOL_MODES[mode], _capi.ACC_TYPES[dt]
+
+
+def _pool_requests(starts, counts, bags, weights, out, wait):
+    """-> (sa, ca, ba, wa, on_device) of a pooled batch: int64 starts, counts and bags and weights of out.dtype as
+    contiguous tensors (None where not given) on the side starts lives. Unlike _requests this converts dtypes, so a
+    queued batch (wait=False) must not be handed a converted copy the queued launch could outlive."""
+    import torch
+    if isinstance(starts, torch.Tensor) and starts.is_cuda:
+        sa = starts.to(torch.int64).contiguous()
+        ca = counts.to(torch.int64).contiguous() if counts is not None else None
+        ba = torch.as_tensor(bags, dtype=torch.int64, device=out.device).contiguous() if bags is not None else None
+        wa = torch.as_tensor(weights, dtype=out.dtype, device=out.device).contiguous() if weights is not None else None
+        if not wait and any(t is not None and t is not u for t, u in ((sa, starts), (ca, counts), (ba, bags),
+                                                                      (wa, weights))):
+            raise ValueError("wait=False takes contiguous CUDA tensors: int64 starts, counts and bags, weights of "
+                             "out.dtype (a converted copy could be freed before the queued launch reads it)")
+        return sa, ca, ba, wa, True
+    sa = torch.as_tensor(_i64(starts))
+    ca = torch.as_tensor(_i64(counts)) if counts is not None else None
+    ba = torch.as_tensor(_i64(bags)) if bags is not None else None
+    wa = torch.as_tensor(weights, dtype=out.dtype, device="cpu").contiguous() if weights is not None else None
+    return sa, ca, ba, wa, False
+
+
 class PyDDStore:
+    # the argument checks of the batched writes, also reachable from the class (the Cython binding calls the
+    # module-level functions)
+    _put_src = staticmethod(_put_src)
+    _acc_type = staticmethod(_acc_type)
+    _red_op = staticmethod(_red_op)
+    _fop_args = staticmethod(_fop_args)
+    _cas_args = staticmethod(_cas_args)
+
     def __init__(self, comm=None, method=0, device=None):
         # src/pyddstore.pyx:61-63. `comm`: see ddstore_b200.comm.as_dds_comm; `device`: CUDA ordinal
         # for this rank's shards (default: the current device).
@@ -252,7 +443,7 @@ class PyDDStore:
             rc = self._L.dds_update(self._h, name.encode(), b.ptr, b.shape[0], int(offset), b.itemsize, b.on_device)
         else:
             rc = self._L.dds_update_async(self._h, name.encode(), b.ptr, b.shape[0], int(offset), b.itemsize,
-                                          b.on_device, self._stream_arg(stream))
+                                          b.on_device, _stream_handle(stream))
         _capi.raise_for(rc)
 
     def ingest(self, name, arr, offset):
@@ -302,61 +493,8 @@ class PyDDStore:
         lengths (optional int64 CUDA tensor of len(starts)) receives the delivered row counts. Returns out's padded
         size in bytes, len(starts) * M * row elements * out.element_size().
         """
-        if out is None:
-            raise ValueError("get_batch needs an `out` buffer (like get(), it never allocates)")
-        if pad_rows is not None:
-            if counts is None:
-                raise ValueError("pad_rows needs counts (there is no fixed-count padded batch)")
-            if count is not None or offsets is not None:
-                raise ValueError("a padded batch takes neither `count` nor `offsets`")
-        cv = lut_keep = None
-        if normalize and src_dtype is None:
-            raise ValueError("normalize=True needs src_dtype")
-        if src_dtype is not None:
-            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
-        else:
-            itemsize = self._itemsize.get(name)
-            if itemsize is None:
-                itemsize = self._itemsize[name] = self.query(name)["itemsize"]
-        ob = _Buf(out, writable=True, half_ok=cv is not None or pad_rows is not None)
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        if s_dev:
-            nreq = starts.numel()
-            sp = starts.data_ptr()
-            cp = counts.data_ptr() if counts is not None else None
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts)
-            nreq = sa.size
-            sp = sa.ctypes.data
-            ca = _i64(counts) if counts is not None else None
-            cp = ca.ctypes.data if ca is not None else None
-            keep = (sa, ca)
-        flags = (_capi.IDX_ON_DEVICE if s_dev else 0) | (_capi.DST_ON_DEVICE if ob.on_device else 0)
-        if not wait:
-            flags |= _capi.NO_SYNC | (_capi.OVERLAP if overlap else 0)
-        if pad_rows is not None:
-            return self._padded(name, False, sp, cp, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream,
-                                (keep, lut_keep))
-        op = None
-        if offsets is not None:
-            fb = _Buf(offsets, writable=True)
-            if fb.on_device != ob.on_device or fb.itemsize != 8 or fb.size < nreq + 1:
-                raise ValueError("offsets must be int64[len(starts)+1] with the same residency as out")
-            op = fb.ptr
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        if cv is None:
-            rc = self._L.dds_get_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
-                                       itemsize, ob.ptr, ob.nbytes, op, flags,
-                                       self._stream_arg(stream), C.byref(total), C.byref(bad))
-        else:
-            rc = self._L.dds_get_batch_convert(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
-                                               ob.ptr, ob.nbytes, op, flags, self._stream_arg(stream), C.byref(cv),
-                                               C.byref(total), C.byref(bad))
-        del keep, lut_keep
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._get(name, False, starts, counts, count, out, offsets, stream, wait, overlap, src_dtype, lut,
+                         normalize, pad_rows, pad_value, lengths)
 
     # ---------------------------------------------------------------- batched puts (update<T> from any rank)
     def put_batch(self, name, starts, counts=None, src=None, count=None, stream=None, wait=True):
@@ -373,45 +511,13 @@ class PyDDStore:
         sides have passed (epoch_begin / epoch_end complete queued puts); later work on the same stream sees them at
         once. Two writes to the same bytes in one epoch leave one writer's byte; reading rows being put in the same
         epoch is undefined."""
-        sb, keep_src = self._put_src(name, src)
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        if s_dev:
-            nreq, sp = starts.numel(), starts.data_ptr()
-            cp = counts.data_ptr() if counts is not None else None
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts)
-            ca = _i64(counts) if counts is not None else None
-            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
-            keep = (sa, ca)
-        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_put_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq, sb.itemsize,
-                                   sb.ptr, sb.nbytes, flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._write("put", name, False, starts, counts, count, src, stream, wait)
 
     def put_samples(self, name, sample_ids, src, stream=None, wait=True):
         """put_batch by SAMPLE ID: request i writes the rows of sample sample_ids[i] in the index registered with
         set_sample_index. Same layout, error behaviour (every valid request is still written), ordering and
         visibility as put_batch; a sample id outside the index keeps 0 bytes of the layout."""
-        sb, keep_src = self._put_src(name, src)
-        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
-        if s_dev:
-            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
-        else:
-            sa = _i64(sample_ids)
-            nreq, sp, keep = sa.size, sa.ctypes.data, sa
-        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_put_samples(self._h, name.encode(), sp, nreq, sb.itemsize, sb.ptr, sb.nbytes, flags,
-                                     self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._write("put", name, True, sample_ids, None, None, src, stream, wait)
 
     # ---------------------------------------------------------------- batched accumulates (MPI_Accumulate)
     def accumulate_batch(self, name, starts, counts=None, src=None, count=None, stream=None, wait=True, op="sum"):
@@ -428,49 +534,12 @@ class PyDDStore:
         "bitwise_and" / "bitwise_or" / "bitwise_xor" (int32 and int64 src only) its bitwise combination with src[e].
         Reductions with the same op and dtype on one element in one epoch combine atomically, also with
         get_accumulate_batch's; mixing different ops on one element in one epoch is undefined."""
-        sb, keep_src = self._put_src(name, src)
-        code = self._acc_type(name, src)
-        opc = self._red_op(name, op)
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        if s_dev:
-            nreq, sp = starts.numel(), starts.data_ptr()
-            cp = counts.data_ptr() if counts is not None else None
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts)
-            ca = _i64(counts) if counts is not None else None
-            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
-            keep = (sa, ca)
-        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_accumulate_op_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
-                                             opc, code, sb.ptr, sb.nbytes, flags, self._stream_arg(stream),
-                                             C.byref(total), C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._write("accumulate_op", name, False, starts, counts, count, src, stream, wait, op=op)
 
     def accumulate_samples(self, name, sample_ids, src, stream=None, wait=True, op="sum"):
         """accumulate_batch by SAMPLE ID: request i adds into (or reduces by op into) the rows of sample sample_ids[i]
         in the index registered with set_sample_index. Layout and errors as put_samples, ops as accumulate_batch."""
-        sb, keep_src = self._put_src(name, src)
-        code = self._acc_type(name, src)
-        opc = self._red_op(name, op)
-        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
-        if s_dev:
-            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
-        else:
-            sa = _i64(sample_ids)
-            nreq, sp, keep = sa.size, sa.ctypes.data, sa
-        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_accumulate_op_samples(self._h, name.encode(), sp, nreq, opc, code, sb.ptr, sb.nbytes, flags,
-                                               self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._write("accumulate_op", name, True, sample_ids, None, None, src, stream, wait, op=op)
 
     # ---------------------------------------------------------------- batched fetch-ops (MPI_Get_accumulate)
     def get_accumulate_batch(self, name, starts, counts=None, src=None, out=None, op="sum", count=None, stream=None,
@@ -487,49 +556,12 @@ class PyDDStore:
         accumulates on one element in one epoch is undefined. op may also be one of accumulate_batch's reductions
         ("amax", "amin", "bitwise_and", "bitwise_or", "bitwise_xor"), which combine atomically with accumulate_batch's
         of the same op. Returns the layout's size in bytes."""
-        sb, keep_src = self._put_src(name, src)
-        code = self._acc_type(name, src)
-        opc, res = self._fop_args(name, op, out, sb)
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        if s_dev:
-            nreq, sp = starts.numel(), starts.data_ptr()
-            cp = counts.data_ptr() if counts is not None else None
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts)
-            ca = _i64(counts) if counts is not None else None
-            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
-            keep = (sa, ca)
-        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_get_accumulate_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
-                                              opc, code, sb.ptr, res, sb.nbytes, flags, self._stream_arg(stream),
-                                              C.byref(total), C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._write("get_accumulate", name, False, starts, counts, count, src, stream, wait, op=op, out=out)
 
     def get_accumulate_samples(self, name, sample_ids, src, out, op="sum", stream=None, wait=True):
         """get_accumulate_batch by SAMPLE ID: request i adds into (or swaps) the rows of sample sample_ids[i] in the
         index registered with set_sample_index. Layout and errors as put_samples, ops as get_accumulate_batch."""
-        sb, keep_src = self._put_src(name, src)
-        code = self._acc_type(name, src)
-        opc, res = self._fop_args(name, op, out, sb)
-        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
-        if s_dev:
-            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
-        else:
-            sa = _i64(sample_ids)
-            nreq, sp, keep = sa.size, sa.ctypes.data, sa
-        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_get_accumulate_samples(self._h, name.encode(), sp, nreq, opc, code, sb.ptr, res, sb.nbytes,
-                                                flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._write("get_accumulate", name, True, sample_ids, None, None, src, stream, wait, op=op, out=out)
 
     # ---------------------------------------------------------------- batched compare-and-swaps (MPI_Compare_and_swap)
     def compare_and_swap_batch(self, name, starts, counts=None, src=None, compare=None, out=None, count=None,
@@ -545,118 +577,39 @@ class PyDDStore:
         epoch are linearisable, from any batch, rank or duplicate request: of N that expect the same value exactly one
         wins. Mixing them with puts, accumulates or fetch-ops on one element in one epoch is undefined. Returns the
         layout's size in bytes."""
-        sb, keep_src = self._put_src(name, src)
-        cmp, res = self._cas_args(name, compare, out, sb)
-        s_dev = hasattr(starts, "data_ptr") and getattr(starts, "is_cuda", False)
-        if s_dev:
-            nreq, sp = starts.numel(), starts.data_ptr()
-            cp = counts.data_ptr() if counts is not None else None
-            keep = (starts, counts)
-        else:
-            sa = _i64(starts)
-            ca = _i64(counts) if counts is not None else None
-            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
-            keep = (sa, ca)
-        flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_compare_and_swap_batch(self._h, name.encode(), sp, cp, 1 if count is None else int(count),
-                                                nreq, sb.itemsize, sb.ptr, cmp, res, sb.nbytes, flags,
-                                                self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        return self._write("compare_and_swap", name, False, starts, counts, count, src, stream, wait,
+                           compare=compare, out=out)
 
     def compare_and_swap_samples(self, name, sample_ids, src, compare, out, stream=None, wait=True):
         """compare_and_swap_batch by SAMPLE ID: request i compares and swaps the rows of sample sample_ids[i] in the
         index registered with set_sample_index. Layout and errors as put_samples, semantics as
         compare_and_swap_batch."""
-        sb, keep_src = self._put_src(name, src)
-        cmp, res = self._cas_args(name, compare, out, sb)
-        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
-        if s_dev:
-            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
+        return self._write("compare_and_swap", name, True, sample_ids, None, None, src, stream, wait,
+                           compare=compare, out=out)
+
+    def _write(self, entry, name, by_sample, starts, counts, count, src, stream, wait, op="sum", compare=None,
+               out=None):
+        """the batched writes: `entry` ("put", "accumulate_op", "get_accumulate" or "compare_and_swap") names the
+        C entries dds_<entry>_batch / dds_<entry>_samples; every argument is checked before the requests are staged"""
+        sb = _put_src(name, src)
+        if entry == "put":
+            operands = (sb.itemsize, sb.ptr)
+        elif entry == "compare_and_swap":
+            operands = (sb.itemsize, sb.ptr, *_cas_args(name, compare, out, sb))
         else:
-            sa = _i64(sample_ids)
-            nreq, sp, keep = sa.size, sa.ctypes.data, sa
+            code = _acc_type(name, src)
+            if entry == "accumulate_op":
+                operands = (_red_op(name, op), code, sb.ptr)
+            else:
+                opc, res = _fop_args(name, op, out, sb)
+                operands = (opc, code, sb.ptr, res)
+        nreq, sp, cp, s_dev, keep = _requests(starts, counts)
         flags = _capi.SRC_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_compare_and_swap_samples(self._h, name.encode(), sp, nreq, sb.itemsize, sb.ptr, cmp, res,
-                                                  sb.nbytes, flags, self._stream_arg(stream), C.byref(total),
-                                                  C.byref(bad))
-        del keep, keep_src
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
-
-    @staticmethod
-    def _cas_args(name, compare, out, sb):
-        """the addresses of a compare-and-swap's `compare` and `out` tensors (ValueError unless each is a C-contiguous
-        CUDA tensor of src's element size and at least src's bytes)"""
-        ptrs = []
-        for what, t in (("compare", compare), ("out", out)):
-            if not (hasattr(t, "data_ptr") and getattr(t, "is_cuda", False)):
-                raise ValueError(f"compare-and-swap on {name!r}: {what} must be a CUDA tensor")
-            if not t.is_contiguous():
-                raise ValueError(f"{what} must be C-contiguous")
-            if t.element_size() != sb.itemsize:
-                raise ValueError(f"compare-and-swap on {name!r}: {what} has {t.element_size()}-byte elements, src "
-                                 f"{sb.itemsize}-byte ones")
-            if t.numel() * t.element_size() < sb.nbytes:
-                raise ValueError(f"compare-and-swap on {name!r}: {what} holds {t.numel() * t.element_size()} bytes, "
-                                 f"src {sb.nbytes}")
-            ptrs.append(t.data_ptr())
-        return ptrs[0], ptrs[1]
-
-    @staticmethod
-    def _fop_args(name, op, out, sb):
-        """the DDS_OP_* code of a fetch-op and the address of its `out` tensor (ValueError for an unknown op, or an out
-        that is not a contiguous CUDA tensor of at least src's bytes)"""
-        ops = {**_capi.FOP_OPS, **_capi.RED_OPS}
-        if op not in ops:
-            raise ValueError(f"fetch-op on {name!r}: op {op!r} is not one of {', '.join(ops)}")
-        if not (hasattr(out, "data_ptr") and getattr(out, "is_cuda", False)):
-            raise ValueError(f"fetch-op on {name!r}: out must be a CUDA tensor")
-        if not out.is_contiguous():
-            raise ValueError("out must be C-contiguous")
-        if out.numel() * out.element_size() < sb.nbytes:
-            raise ValueError(f"fetch-op on {name!r}: out holds {out.numel() * out.element_size()} bytes, src "
-                             f"{sb.nbytes}")
-        return ops[op], out.data_ptr()
-
-    @staticmethod
-    def _red_op(name, op):
-        """the DDS_OP_* code of an accumulate's reduction (ValueError for an unknown one)"""
-        ops = {"sum": _capi.OP_SUM, **_capi.RED_OPS}
-        if op not in ops:
-            raise ValueError(f"accumulate into {name!r}: op {op!r} is not one of {', '.join(ops)}")
-        return ops[op]
-
-    @staticmethod
-    def _acc_type(name, src):
-        """the DDS_ACC_* element type of an accumulate's src, from its dtype (ValueError for any other)"""
-        dt = str(getattr(src, "dtype", "")).replace("torch.", "")
-        if dt not in _capi.ACC_TYPES:
-            raise ValueError(f"accumulate into {name!r}: src dtype {dt or type(src).__name__} is not one of "
-                             f"{', '.join(_capi.ACC_TYPES)}")
-        return _capi.ACC_TYPES[dt]
-
-    @staticmethod
-    def _put_src(name, src):
-        """the _Buf of a put's source rows (a CUDA tensor or CAI object; ValueError for host memory)"""
-        if src is None:
-            raise ValueError("a put needs `src` rows")
-        if hasattr(src, "data_ptr") and hasattr(src, "element_size"):  # any torch dtype: only its element size matters
-            if not src.is_contiguous():
-                raise ValueError("src must be C-contiguous")
-            sb = _Buf.__new__(_Buf)
-            sb.ptr, sb.on_device, sb.itemsize = src.data_ptr(), 1 if src.is_cuda else 0, src.element_size()
-            sb.nbytes = src.numel() * sb.itemsize
-        else:
-            sb = _Buf(src)
-        if not sb.on_device:
-            raise ValueError(f"put into {name!r}: src must be device memory (copy host rows to the device first)")
-        return sb, src
+        if by_sample:
+            return self._call(getattr(self._L, f"dds_{entry}_samples"), self._h, name.encode(), sp, nreq, *operands,
+                              sb.nbytes, flags, _stream_handle(stream))
+        return self._call(getattr(self._L, f"dds_{entry}_batch"), self._h, name.encode(), sp, cp,
+                          1 if count is None else int(count), nreq, *operands, sb.nbytes, flags, _stream_handle(stream))
 
     # ---------------------------------------------------------------- pooled batches (embedding_bag)
     def get_batch_pooled(self, name, starts, counts=None, count=None, out=None, bags=None, mode="sum", weights=None,
@@ -680,48 +633,22 @@ class PyDDStore:
         return self._pooled(name, True, sample_ids, None, None, out, bags, mode, weights, stream, wait)
 
     def _pooled(self, name, by_sample, starts, counts, count, out, bags, mode, weights, stream, wait):
-        import torch
-        if mode not in _capi.POOL_MODES:
-            raise ValueError(f"pooled batch of {name!r}: mode {mode!r} is not one of {', '.join(_capi.POOL_MODES)}")
-        if not (isinstance(out, torch.Tensor) and out.is_cuda and out.is_contiguous()):
-            raise ValueError("out must be a C-contiguous CUDA tensor")
-        dt = _dtype_name(out.dtype)
-        if dt not in ("float32", "float64", "float16", "bfloat16"):
-            raise ValueError(f"pooled batch of {name!r}: out dtype {dt} is not float32, float64, float16 or bfloat16")
-        s_dev = isinstance(starts, torch.Tensor) and starts.is_cuda
-        if s_dev:
-            sa = starts.to(torch.int64).contiguous()
-            ca = counts.to(torch.int64).contiguous() if counts is not None else None
-            nreq, sp, cp = sa.numel(), sa.data_ptr(), ca.data_ptr() if ca is not None else None
-            ba = torch.as_tensor(bags, dtype=torch.int64, device=out.device).contiguous() if bags is not None else None
-            wa = torch.as_tensor(weights, dtype=out.dtype, device=out.device).contiguous() if weights is not None else None
-            if not wait and any(t is not None and t is not u for t, u in ((sa, starts), (ca, counts), (ba, bags),
-                                                                          (wa, weights))):
-                raise ValueError("wait=False takes contiguous CUDA tensors: int64 starts, counts and bags, weights of "
-                                 "out.dtype (a converted copy could be freed before the queued launch reads it)")
-        else:
-            sa = _i64(starts)
-            ca = _i64(counts) if counts is not None else None
-            nreq, sp, cp = sa.size, sa.ctypes.data, ca.ctypes.data if ca is not None else None
-            ba = torch.as_tensor(_i64(bags)) if bags is not None else None
-            wa = torch.as_tensor(weights, dtype=out.dtype, device="cpu").contiguous() if weights is not None else None
+        modec, dtc = _pool_args(name, mode, out)
+        sa, ca, ba, wa, s_dev = _pool_requests(starts, counts, bags, weights, out, wait)
+        nreq = sa.numel()
         nbags = ba.numel() - 1 if ba is not None else nreq
-        pool = _capi.Pool(_capi.POOL_MODES[mode], _capi.ACC_TYPES[dt], ba.data_ptr() if ba is not None else None, nbags,
+        pool = _capi.Pool(modec, dtc, ba.data_ptr() if ba is not None else None, nbags,
                           wa.data_ptr() if wa is not None else None)
         flags = _capi.DST_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        total, bad = C.c_int64(0), C.c_int64(-1)
         cap = out.numel() * out.element_size()
         if by_sample:
-            rc = self._L.dds_get_samples_pooled(self._h, name.encode(), sp, nreq, C.byref(pool), out.data_ptr(), cap,
-                                                flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
+            total = self._call(self._L.dds_get_samples_pooled, self._h, name.encode(), sa.data_ptr(), nreq,
+                               C.byref(pool), out.data_ptr(), cap, flags, _stream_handle(stream))
         else:
-            rc = self._L.dds_get_batch_pooled(self._h, name.encode(), sp, cp, 1 if count is None else int(count), nreq,
-                                              C.byref(pool), out.data_ptr(), cap, flags, self._stream_arg(stream),
-                                              C.byref(total), C.byref(bad))
-        del sa, ca, ba, wa
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value if wait else None
+            total = self._call(self._L.dds_get_batch_pooled, self._h, name.encode(), sa.data_ptr(),
+                               ca.data_ptr() if ca is not None else None, 1 if count is None else int(count), nreq,
+                               C.byref(pool), out.data_ptr(), cap, flags, _stream_handle(stream))
+        return total if wait else None
 
     # ---------------------------------------------------------------- collective owner-push fetch
     def push_setup(self, max_requests, max_bytes):
@@ -733,14 +660,12 @@ class PyDDStore:
         uint8 CUDA tensor VIEW of the packed rows inside this rank's window (valid until the next-but-one push step);
         the step is enqueued on `stream`, wait() reports errors."""
         import torch
-        itemsize = self._itemsize.get(name)
-        if itemsize is None:
-            itemsize = self._itemsize[name] = self.query(name)["itemsize"]
+        itemsize = self._var_itemsize(name)
         if not (hasattr(starts, "data_ptr") and starts.is_cuda):
             raise ValueError("get_batch_push takes a CUDA int64 tensor of start rows")
         out = C.c_void_p()
         _capi.raise_for(self._L.dds_get_batch_push(self._h, name.encode(), starts.data_ptr(), int(count), starts.numel(), itemsize,
-                                                   C.byref(out), self._stream_arg(stream)))
+                                                   C.byref(out), _stream_handle(stream)))
         rb = self._rowbytes.get(name)
         if rb is None:
             rb = self._rowbytes[name] = self.query(name)["disp"] * itemsize
@@ -751,12 +676,7 @@ class PyDDStore:
     def set_sample_index(self, name, row_start, row_count):
         """Register, for variable `name`, which GLOBAL rows every sample owns: sample i = rows
         [row_start[i], row_start[i] + row_count[i]). Tables: int64 host arrays or CUDA tensors; copied once."""
-        dev = hasattr(row_start, "data_ptr") and getattr(row_start, "is_cuda", False)
-        if dev:
-            n, sp, cp, keep = row_start.numel(), row_start.data_ptr(), row_count.data_ptr(), (row_start, row_count)
-        else:
-            sa, ca = _i64(row_start), _i64(row_count)
-            n, sp, cp, keep = sa.size, sa.ctypes.data, ca.ctypes.data, (sa, ca)
+        n, sp, cp, dev, keep = _requests(row_start, row_count)
         _capi.raise_for(self._L.dds_set_sample_index(self._h, name.encode(), sp, cp, n, 1 if dev else 0))
         del keep
 
@@ -775,78 +695,43 @@ class PyDDStore:
         """get_batch by SAMPLE ID: the id -> (start, count) lookup runs inside the launch, against the index
         registered with set_sample_index. Same packing / offsets / error behaviour, conversions and padding (pad_rows,
         pad_value, lengths) as get_batch."""
-        if pad_rows is not None and offsets is not None:
-            raise ValueError("a padded batch takes no `offsets`")
-        cv = lut_keep = None
-        if normalize and src_dtype is None:
-            raise ValueError("normalize=True needs src_dtype")
-        if src_dtype is not None:
-            cv, lut_keep = _conversion(src_dtype, getattr(out, "dtype", None), lut, normalize)
-        else:
-            itemsize = self._itemsize.get(name)
-            if itemsize is None:
-                itemsize = self._itemsize[name] = self.query(name)["itemsize"]
+        return self._get(name, True, sample_ids, None, None, out, offsets, stream, wait, overlap, src_dtype, lut,
+                         normalize, pad_rows, pad_value, lengths)
+
+    def _get(self, name, by_sample, starts, counts, count, out, offsets, stream, wait, overlap, src_dtype, lut,
+             normalize, pad_rows, pad_value, lengths):
+        """get_batch, and get_samples (by_sample: starts are sample ids, counts and count are None)"""
+        cv, lut_keep = _get_args(by_sample, counts, count, out, offsets, src_dtype, lut, normalize, pad_rows)
+        if cv is None:
+            itemsize = self._var_itemsize(name)
         ob = _Buf(out, writable=True, half_ok=cv is not None or pad_rows is not None)
-        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
-        if s_dev:
-            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
-        else:
-            sa = _i64(sample_ids)
-            nreq, sp, keep = sa.size, sa.ctypes.data, sa
+        nreq, sp, cp, s_dev, keep = _requests(starts, counts)
         flags = (_capi.IDX_ON_DEVICE if s_dev else 0) | (_capi.DST_ON_DEVICE if ob.on_device else 0)
         if not wait:
             flags |= _capi.NO_SYNC | (_capi.OVERLAP if overlap else 0)
         if pad_rows is not None:
-            return self._padded(name, True, sp, None, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream,
-                                (keep, lut_keep))
-        op = None
-        if offsets is not None:
-            fb = _Buf(offsets, writable=True)
-            if fb.on_device != ob.on_device or fb.itemsize != 8 or fb.size < nreq + 1:
-                raise ValueError("offsets must be int64[len(sample_ids)+1] with the same residency as out")
-            op = fb.ptr
-        total, bad = C.c_int64(0), C.c_int64(-1)
+            return self._padded(name, by_sample, sp, cp, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream)
+        op = _offsets(offsets, ob, nreq, by_sample)
+        reqs = (sp, nreq) if by_sample else (sp, cp, 1 if count is None else int(count), nreq)
         if cv is None:
-            rc = self._L.dds_get_samples(self._h, name.encode(), sp, nreq, itemsize, ob.ptr, ob.nbytes, op, flags,
-                                         self._stream_arg(stream), C.byref(total), C.byref(bad))
-        else:
-            rc = self._L.dds_get_samples_convert(self._h, name.encode(), sp, nreq, ob.ptr, ob.nbytes, op, flags,
-                                                 self._stream_arg(stream), C.byref(cv), C.byref(total), C.byref(bad))
-        del keep, lut_keep
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+            fn = self._L.dds_get_samples if by_sample else self._L.dds_get_batch
+            return self._call(fn, self._h, name.encode(), *reqs, itemsize, ob.ptr, ob.nbytes, op, flags,
+                              _stream_handle(stream))
+        fn = self._L.dds_get_samples_convert if by_sample else self._L.dds_get_batch_convert
+        return self._call(fn, self._h, name.encode(), *reqs, ob.ptr, ob.nbytes, op, flags, _stream_handle(stream),
+                          C.byref(cv))
 
-    def _padded(self, name, by_sample, sp, cp, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream, keep):
-        """the padded form of get_batch / get_samples (arguments already converted by them)"""
-        pad_rows = int(pad_rows)
-        if pad_rows < 0:
-            raise ValueError("pad_rows must be >= 0")
-        if not (ob.on_device and hasattr(out, "dtype") and str(out.dtype).startswith("torch.")):
-            raise ValueError("a padded batch delivers into a CUDA tensor")
-        itemsize = self._itemsize.get(name)
-        if itemsize is None:
-            itemsize = self._itemsize[name] = self.query(name)["itemsize"]
+    def _padded(self, name, by_sample, sp, cp, nreq, out, ob, cv, pad_rows, pad_value, lengths, flags, stream):
+        """the padded form of get_batch / get_samples (arguments already converted by _get)"""
+        pad_rows = _pad_rows(pad_rows, out, ob)
+        itemsize = self._var_itemsize(name)
         if cv is None and ob.itemsize != itemsize:
             raise ValueError(f"out.dtype {out.dtype} does not have the variable's itemsize ({itemsize})")
-        pad = _capi.Pad(pad_rows, _pad_bits(pad_value, out.dtype), None)
-        if lengths is not None:
-            lb = _Buf(lengths, writable=True)
-            if not lb.on_device or lb.itemsize != 8 or lb.size < nreq:
-                raise ValueError("lengths must be an int64 CUDA tensor of len(starts)")
-            pad.lengths = lb.ptr
-        total, bad = C.c_int64(0), C.c_int64(-1)
-        cvp = C.byref(cv) if cv is not None else None
-        if by_sample:
-            rc = self._L.dds_get_samples_padded(self._h, name.encode(), sp, nreq, itemsize, cvp, C.byref(pad), ob.ptr,
-                                                ob.nbytes, flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
-        else:
-            rc = self._L.dds_get_batch_padded(self._h, name.encode(), sp, cp, nreq, itemsize, cvp, C.byref(pad), ob.ptr,
-                                              ob.nbytes, flags, self._stream_arg(stream), C.byref(total), C.byref(bad))
-        del keep
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
-        return total.value
+        pad = _pad(pad_rows, pad_value, lengths, out, nreq)
+        reqs = (sp, nreq) if by_sample else (sp, cp, nreq)
+        fn = self._L.dds_get_samples_padded if by_sample else self._L.dds_get_batch_padded
+        return self._call(fn, self._h, name.encode(), *reqs, itemsize, C.byref(cv) if cv is not None else None,
+                          C.byref(pad), ob.ptr, ob.nbytes, flags, _stream_handle(stream))
 
     def get_samples_multi(self, names, sample_ids, outs, offsets=None, stream=None, wait=True, overlap=False,
                           src_dtypes=None, luts=None, normalize=None):
@@ -877,12 +762,7 @@ class PyDDStore:
         obs = [_Buf(o, writable=True, half_ok=cvs is not None and src_dtypes[v] is not None) for v, o in enumerate(outs)]
         if not all(o.on_device for o in obs):
             raise ValueError("get_samples_multi delivers into device buffers")
-        s_dev = hasattr(sample_ids, "data_ptr") and getattr(sample_ids, "is_cuda", False)
-        if s_dev:
-            nreq, sp, keep = sample_ids.numel(), sample_ids.data_ptr(), sample_ids
-        else:
-            sa = _i64(sample_ids)
-            nreq, sp, keep = sa.size, sa.ctypes.data, sa
+        nreq, sp, _, s_dev, keep = _requests(sample_ids)
         flags = (_capi.IDX_ON_DEVICE if s_dev else 0) | _capi.DST_ON_DEVICE | (0 if wait else _capi.NO_SYNC)
         if overlap and not wait:
             flags |= _capi.OVERLAP
@@ -894,28 +774,13 @@ class PyDDStore:
             fbs = [_Buf(f, writable=True) for f in offsets]
             c_offs = (C.c_void_p * nv)(*[f.ptr for f in fbs])
         totals = (C.c_int64 * nv)()
-        bad = C.c_int64(-1)
         if cvs is None:
-            rc = self._L.dds_get_samples_multi(self._h, nv, c_names, sp, nreq, c_dsts, c_caps, c_offs, flags,
-                                               self._stream_arg(stream), totals, C.byref(bad))
+            self._call(self._L.dds_get_samples_multi, self._h, nv, c_names, sp, nreq, c_dsts, c_caps, c_offs, flags,
+                       _stream_handle(stream), totals=totals)
         else:
-            rc = self._L.dds_get_samples_multi_convert(self._h, nv, c_names, sp, nreq, c_dsts, c_caps, c_offs, flags,
-                                                       self._stream_arg(stream), cvs, totals, C.byref(bad))
-            del lut_keep
-        del keep
-        self.last_bad_index = bad.value
-        _capi.raise_for(rc)
+            self._call(self._L.dds_get_samples_multi_convert, self._h, nv, c_names, sp, nreq, c_dsts, c_caps, c_offs,
+                       flags, _stream_handle(stream), cvs, totals=totals)
         return [totals[v] for v in range(nv)] if wait else None
-
-    @staticmethod
-    def _stream_arg(stream):
-        """None -> the store's own stream; a cudaStream_t handle (e.g. torch.cuda.current_stream().cuda_stream)
-        otherwise. Handle 0 is CUDA's legacy default stream, which the C-ABI spells cudaStreamLegacy (0x1)
-        because NULL there means "the store's stream"."""
-        if stream is None:
-            return None
-        h = int(stream)
-        return C.c_void_p(h if h != 0 else 1)
 
     def wait(self):
         """Complete the batches queued with wait=False; raises like get_batch for the earliest failing batch in queue
@@ -928,11 +793,23 @@ class PyDDStore:
         epoch_begin when the queue holds a put, an accumulate, a fetch-op or a compare-and-swap, free) completes it, keeps its first failure for the next wait(), and raises only
         for its own requests. A failure kept from earlier wins over later ones; after wait() has raised it, the next
         wait() is clean. close() drops an outcome no wait() has reported."""
+        return self._call(self._L.dds_batch_wait, self._h)
+
+    def _call(self, fn, *args, totals=None):
+        """fn(*args, &total, &bad) -- a batched C entry, or totals (an int64 array) in place of &total -> total. Sets
+        last_bad_index and raises the reference's exception for a failed call."""
         total, bad = C.c_int64(0), C.c_int64(-1)
-        rc = self._L.dds_batch_wait(self._h, C.byref(total), C.byref(bad))
+        rc = fn(*args, C.byref(total) if totals is None else totals, C.byref(bad))
         self.last_bad_index = bad.value
-        _capi.raise_for(rc)
+        if rc:
+            _capi.raise_for(rc)
         return total.value
+
+    def _var_itemsize(self, name):
+        itemsize = self._itemsize.get(name)
+        if itemsize is None:
+            itemsize = self._itemsize[name] = self.query(name)["itemsize"]
+        return itemsize
 
     # ---------------------------------------------------------------- extras
     def query(self, name):
@@ -954,7 +831,7 @@ class PyDDStore:
         _capi.raise_for(self._L.dds_synth_verify(
             self._h, name.encode(), packed.data_ptr(), starts.data_ptr(), counts.data_ptr() if counts is not None else None,
             int(count), offsets.data_ptr() if offsets is not None else None, starts.numel(), int(seed),
-            self._stream_arg(stream), res))
+            _stream_handle(stream), res))
         return int(res[0]), int(res[1]), [int(res[2 + r]) for r in range(self.size)]
 
     def close(self):

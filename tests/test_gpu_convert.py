@@ -538,3 +538,42 @@ def test_plan_in_shared_memory_up_to_8192_requests():
             % (ROOT, os.path.join(ROOT, "tests", "test_gpu_convert.py")))
     r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=900, cwd=ROOT)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
+
+
+@pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
+def test_cython_binding(case):
+    """pyddstore.PyDDStore.get_batch converting without padding: fixed and explicit counts, host and device indices,
+    with offsets"""
+    cydir = os.path.join(ROOT, "ddstore_b200", "cython")
+    if cydir not in sys.path:
+        sys.path.insert(0, cydir)
+    pyd = pytest.importorskip("pyddstore", reason="Cython binding not built")
+    _, var, sdt, odt, lut, code = case
+    dt, disp = VARS[var]
+    rng = np.random.default_rng(CASE_IDS.index(case[0]))
+    nrows, n = 500, 300
+    if dt is np.uint8:
+        rows = rng.integers(0, 256, (nrows, disp)).astype(dt)
+    else:
+        rows = (rng.standard_normal((nrows, disp)) * np.exp2(rng.integers(-20, 20, (nrows, disp)))).astype(dt)
+    row = disp * np.dtype(dt).itemsize
+    starts = rng.integers(0, nrows - 3, n).astype(np.int64)
+    store = pyd.PyDDStore(None, device=0)
+    try:
+        store.add(var, rows)
+        for counts in (None, rng.integers(0, 4, n).astype(np.int64)):
+            c = np.full(n, 3) if counts is None else counts
+            packed = np.concatenate([rows[a:a + k].reshape(-1) for a, k in zip(starts, c)])
+            raw = torch.from_numpy(packed.view(np.uint8).copy()).to(DEV)
+            raw_offs = np.concatenate([[0], np.cumsum(c * row)])
+            nb = co.out_bytes(raw.numel(), code)
+            for dev in (False, True):
+                whole, view = _dest(nb, 0)
+                offs = torch.full((n + 1,), -7, dtype=torch.int64, device=DEV)
+                t = store.get_batch(var, _idx(starts, dev), None if counts is None else _idx(counts, dev),
+                                    out=view.view(odt), count=3 if counts is None else None, offsets=offs,
+                                    src_dtype=sdt, lut=lut)
+                _check(case, whole, 0, t, offs.cpu().numpy(), raw, raw_offs,
+                       f"cython {case[0]} counts={counts is not None} dev={dev}")
+    finally:
+        store.free()

@@ -596,3 +596,47 @@ def test_configurations(config):
             % (ROOT, os.path.join(ROOT, "tests", "test_gpu_normalize.py")))
     r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=900, cwd=ROOT)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
+
+
+@pytest.mark.parametrize("case", CASES, ids=CASE_IDS)
+def test_cython_binding(case):
+    """pyddstore.PyDDStore.set_normalization (host and CUDA tables) and get_batch(normalize=True), fixed and explicit
+    counts, host and device indices"""
+    cydir = os.path.join(ROOT, "ddstore_b200", "cython")
+    if cydir not in sys.path:
+        sys.path.insert(0, cydir)
+    pyd = pytest.importorskip("pyddstore", reason="Cython binding not built")
+    _, var, sdt, odt, lut, code = case
+    dt, disp, nchan, inner = VARS[var]
+    rng = np.random.default_rng(CASE_IDS.index(case[0]))
+    nrows, n = 300, 200
+    if dt is np.uint8:
+        rows = rng.integers(0, 256, (nrows, disp)).astype(dt)
+    else:
+        rows = (rng.standard_normal((nrows, disp)) * 4).astype(dt)
+    mean, std = _tables(var)
+    tabs = {var: (mean, std)}
+    row = disp * np.dtype(dt).itemsize
+    starts = rng.integers(0, nrows - 3, n).astype(np.int64)
+    store = pyd.PyDDStore(None, device=0)
+    try:
+        store.add(var, rows)
+        for counts, dev in ((None, False), (rng.integers(0, 4, n).astype(np.int64), True)):
+            if dev:
+                store.set_normalization(var, torch.from_numpy(mean).to(DEV), torch.from_numpy(std).to(DEV), inner)
+            else:
+                store.set_normalization(var, mean, std, inner)
+            c = np.full(n, 3) if counts is None else counts
+            packed = np.concatenate([rows[a:a + k].reshape(-1) for a, k in zip(starts, c)])
+            raw = torch.from_numpy(packed.view(np.uint8).copy()).to(DEV)
+            raw_offs = np.concatenate([[0], np.cumsum(c * row)])
+            nb = no.out_bytes(raw.numel(), code)
+            whole, view = _dest(nb, 0)
+            offs = torch.full((n + 1,), -7, dtype=torch.int64, device=DEV)
+            t = store.get_batch(var, _idx(starts, dev), None if counts is None else _idx(counts, dev),
+                                out=view.view(odt), count=3 if counts is None else None, offsets=offs, src_dtype=sdt,
+                                lut=lut, normalize=True)
+            _check(case, tabs, whole, 0, t, offs.cpu().numpy(), raw, raw_offs,
+                   f"cython {case[0]} counts={counts is not None} dev={dev}")
+    finally:
+        store.free()

@@ -4,6 +4,8 @@ element to 16 KiB, bags of 0 to 20000 rows, every request form with host and dev
 subnormals, NaNs and signed zeros, thread-rank worlds with an empty shard, invalid requests, malformed bags, every
 argument error, queues, HOST placement -- and torch's CUDA embedding_bag on a local copy of the table."""
 import ctypes as C
+import os
+import sys
 
 import numpy as np
 import pytest
@@ -472,3 +474,40 @@ def test_matches_torch_embedding_bag(t, mode):
     got = run_world(3, body)
     check(got[0], bits_of(ref, t), f"type {t} {mode} against torch.nn.functional.embedding_bag")
     check(got[2], got[0], "ranks agree")
+
+
+# ----------------------------------------------------------------------------------------- the Cython binding
+@pytest.mark.parametrize("dev", [False, True])
+@pytest.mark.parametrize("t,mode", [(pl.ACC_F32, "weighted"), (pl.ACC_F64, "mean")])
+def test_cython_binding(dev, t, mode):
+    """pyddstore.PyDDStore.get_batch_pooled: a weighted sum and a mean over bags, host and device indices"""
+    cydir = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "ddstore_b200", "cython")
+    if cydir not in sys.path:
+        sys.path.insert(0, cydir)
+    pyd = pytest.importorskip("pyddstore", reason="Cython binding not built")
+    rng = np.random.default_rng(17 + dev + t)
+    nrows, disp = 600, 24
+    shard = data_bits(rng, t, nrows * disp).reshape(nrows, disp)
+    sizes = rng.integers(0, 20, 12)
+    sizes[2] = 0
+    nreq = int(sizes.sum())
+    bags = bag_offsets(rng, sizes)
+    starts = rng.integers(0, nrows - 3, nreq).astype(np.int64)
+    counts = rng.integers(0, 4, nreq).astype(np.int64)
+    w = data_bits(rng, t, nreq, special=False) if mode == "weighted" else None
+    wt = None if w is None else (to_torch(w, t).cuda() if dev else to_torch(w, t))
+    out = torch.full((len(sizes), disp), 7, dtype=TORCH_DT[t], device="cuda")
+
+    def idx(a):
+        return torch.from_numpy(a).cuda() if dev else a
+    s = pyd.PyDDStore(None, device=0)
+    try:
+        s.add("x", shard)
+        total = s.get_batch_pooled("x", idx(starts), idx(counts), out=out, bags=idx(bags),
+                                   mode="sum" if mode == "weighted" else mode, weights=wt)
+        assert total == out.numel() * out.element_size()
+        exp, _, eerr = oracle([shard], t, MODES[mode], {"starts": starts, "counts": counts}, bags, w)
+        assert eerr == (0, -1)
+        check(bits_of(out, t), exp, f"cython {mode} dev={dev}")
+    finally:
+        s.free()
