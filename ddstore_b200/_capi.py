@@ -139,6 +139,11 @@ SIGNATURES = {
                                        C.POINTER(Pool), C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_get_samples_pooled": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(Pool), C.c_void_p,
                                          C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
+    "dds_accumulate_batch_pooled": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,
+                                              C.POINTER(Pool), C.c_double, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p,
+                                              I64P, I64P]),
+    "dds_accumulate_samples_pooled": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(Pool),
+                                                C.c_double, C.c_void_p, C.c_int64, C.c_uint, C.c_void_p, I64P, I64P]),
     "dds_batch_wait": (C.c_int, [C.c_void_p, I64P, I64P]),
     "dds_set_sample_index": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int]),
     "dds_set_normalization": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64,

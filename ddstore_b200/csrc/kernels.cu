@@ -549,36 +549,53 @@ __device__ __forceinline__ void tma_red_1d(void *dst_gmem, uint32_t src_smem, ui
     }
 #undef DDSK_BULK_RED
 }
-// one element at d: *d = op(*d, the element staged at shared address s) (both aligned to the element size)
-__device__ __forceinline__ void red1(char *d, uint32_t s, int t, int op) {
+// The operand of red1v: the element staged at a shared address (red1), or its bits held in a register (Held). Each
+// accessor reads it at one width (16, 32, 64 bits), at the point the reduction takes it.
+struct Staged {
+    uint32_t s;
+    __device__ __forceinline__ unsigned short h() const { return lds16h(s); }
+    __device__ __forceinline__ uint32_t w() const { return lds32(s); }
+    __device__ __forceinline__ uint64_t l() const { return lds64(s); }
+};
+struct Held {
+    uint64_t v;
+    __device__ __forceinline__ unsigned short h() const { return (unsigned short)v; }
+    __device__ __forceinline__ uint32_t w() const { return (uint32_t)v; }
+    __device__ __forceinline__ uint64_t l() const { return v; }
+};
+// one element at d: *d = op(*d, o) (d aligned to the element size)
+template <typename O>
+__device__ __forceinline__ void red1v(char *d, O o, int t, int op) {
     if (op == DDSK_OP_SUM) {
         switch (t) {
         case DDSK_ACC_F32:
-            asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(d), "f"(__uint_as_float(lds32(s))) : "memory");
+            asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(d), "f"(__uint_as_float(o.w())) : "memory");
             break;
         case DDSK_ACC_F64:
-            asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__longlong_as_double((long long)lds64(s))) : "memory");
+            asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(d), "d"(__longlong_as_double((long long)o.l())) : "memory");
             break;
-        case DDSK_ACC_I32: asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(lds32(s)) : "memory"); break;
-        case DDSK_ACC_I64: asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"(lds64(s)) : "memory"); break;
-        case DDSK_ACC_F16: asm volatile("red.relaxed.sys.global.add.noftz.f16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
-        default: asm volatile("red.relaxed.sys.global.add.noftz.bf16 [%0], %1;" ::"l"(d), "h"(lds16h(s)) : "memory"); break;
+        case DDSK_ACC_I32: asm volatile("red.relaxed.sys.global.add.u32 [%0], %1;" ::"l"(d), "r"(o.w()) : "memory"); break;
+        case DDSK_ACC_I64: asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(d), "l"(o.l()) : "memory"); break;
+        case DDSK_ACC_F16: asm volatile("red.relaxed.sys.global.add.noftz.f16 [%0], %1;" ::"l"(d), "h"(o.h()) : "memory"); break;
+        default: asm volatile("red.relaxed.sys.global.add.noftz.bf16 [%0], %1;" ::"l"(d), "h"(o.h()) : "memory"); break;
         }
         return;
     }
     const bool mx = op == DDSK_OP_MAX;
     switch (t) {
-    case DDSK_ACC_I32: red_i32(d, lds32(s), op); break;
-    case DDSK_ACC_I64: red_i64(d, lds64(s), op); break;
-    case DDSK_ACC_F32: fmm32(d, lds32(s), mx); break;
-    case DDSK_ACC_F64: fmm64(d, lds64(s), mx); break;
+    case DDSK_ACC_I32: red_i32(d, o.w(), op); break;
+    case DDSK_ACC_I64: red_i64(d, o.l(), op); break;
+    case DDSK_ACC_F32: fmm32(d, o.w(), mx); break;
+    case DDSK_ACC_F64: fmm64(d, o.l(), mx); break;
     default: {
         const uint32_t sh = ((uint32_t)(uint64_t)d & 2u) * 8u;
-        fmm_word((char *)((uint64_t)d & ~(uint64_t)3), (uint32_t)lds16h(s) << sh, 0xFFFFu << sh, t == DDSK_ACC_BF16, mx);
+        fmm_word((char *)((uint64_t)d & ~(uint64_t)3), (uint32_t)o.h() << sh, 0xFFFFu << sh, t == DDSK_ACC_BF16, mx);
         break;
     }
     }
 }
+// one element at d: *d = op(*d, the element staged at shared address s) (both aligned to the element size)
+__device__ __forceinline__ void red1(char *d, uint32_t s, int t, int op) { red1v(d, Staged{s}, t, op); }
 // 16 bytes at a 16-byte aligned d, element-wise: *d = op(*d, v)
 __device__ __forceinline__ void red16(char *d, uint4 v, int t, int op) {
     if (op == DDSK_OP_SUM) {
@@ -2983,19 +3000,46 @@ __device__ __forceinline__ RW pool_load(uint64_t p) {
     else if constexpr (sizeof(RW) == 4) return (RW)__ldcg((const unsigned int *)p);
     else return (RW)__ldcg((const unsigned long long *)p);
 }
+// the 16 bytes of E elements
+template <typename U, int E>
+__device__ __forceinline__ uint4 pool_pack(const U (&o)[E]) {
+    uint32_t w[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        if constexpr (sizeof(U) == 2) w[i] = (uint32_t)o[2 * i] | ((uint32_t)o[2 * i + 1] << 16);
+        else if constexpr (sizeof(U) == 4) w[i] = (uint32_t)o[i];
+        else w[i] = (uint32_t)(o[i >> 1] >> ((i & 1) * 32));
+    }
+    return make_uint4(w[0], w[1], w[2], w[3]);
+}
 template <typename U, int E>
 __device__ __forceinline__ void pool_store(char *p, const U (&o)[E]) {
-    if constexpr (E * sizeof(U) == 16) {
-        uint32_t w[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            if constexpr (sizeof(U) == 2) w[i] = (uint32_t)o[2 * i] | ((uint32_t)o[2 * i + 1] << 16);
-            else if constexpr (sizeof(U) == 4) w[i] = (uint32_t)o[i];
-            else w[i] = (uint32_t)(o[i >> 1] >> ((i & 1) * 32));
+    if constexpr (E * sizeof(U) == 16) stg128(p, pool_pack<U, E>(o));
+    else *(U *)p = o[0];
+}
+// Request i of a pooled batch: its first row's address in *src and its row count in *n; an invalid request leaves *n and
+// is reported when `rep` (ordered after every bag report)
+__device__ __forceinline__ void pool_req(const PoolArgs &a, int64_t i, uint64_t *src, int64_t *n, bool rep) {
+    int64_t start = 0, count = 0;
+    int code = 0;
+    if (a.ids) {
+        const int64_t id = a.ids[i];
+        if (id < 0 || id >= a.nsamples) {
+            code = DDSK_CODE_SAMPLE;
+        } else {
+            const longlong2 e = ldg_pair(&a.tab[id]);
+            start = e.x;
+            count = e.y;
         }
-        stg128(p, make_uint4(w[0], w[1], w[2], w[3]));
     } else {
-        *(U *)p = o[0];
+        start = a.starts[i];
+        count = a.counts ? a.counts[i] : a.count;
+    }
+    if (!code) code = dev_locate(a.var, start, count, src);
+    if (code) {
+        if (rep) report(a.status, a.status_tag, (int64_t)(DDSK_STATUS_LATE | (uint64_t)i), code);
+    } else {
+        *n = count;
     }
 }
 
@@ -3034,7 +3078,7 @@ __global__ void __launch_bounds__(kPoolThreads, kPoolMinBlocks) dds_pool_kernel(
             uint64_t src = 0;
             int64_t n = 0;
             A wt = A(1);
-            if (i < b1) {
+            if (i < b1) { // (pool_req's locate, kept inline here: calling it changes this kernel's register allocation)
                 int64_t start = 0, count = 0;
                 int code = 0;
                 if (a.ids) {
@@ -3101,6 +3145,130 @@ __global__ void __launch_bounds__(kPoolThreads, kPoolMinBlocks) dds_pool_kernel(
                 }
             }
             pool_store<U, E>(a.dst + k * row_bytes + col, o);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// pooled accumulates (dds_accumulate_batch_pooled / dds_accumulate_samples_pooled): the pooled batch's adjoint
+// ------------------------------------------------------------------------------------------------
+// One warp per (bag, row window, column slice). A lane loads its vector of grad[k] once; every row of the bag's valid
+// requests then takes one atomic of the contribution (grad, times the request's weight, over the bag's row count for a
+// mean, times alpha; each step rounded once, then rounded to the element type): red16 per 16-byte vector, else one red1v
+// per element. The contributions are independent atomics, so there is no order to keep: window j of a bag's `windows`
+// takes the bag's valid rows j, j + windows, ... The requests are read and located 32 at a time as in the pooled get, and
+// every window walks all of them (it needs each row's place in the bag). A mean needs the bag's row count before its first
+// atomic: for bags of at most 32 requests it is the first window of requests' row total, longer bags count in a first pass.
+// An unweighted bag's contribution is the same for every row and is computed once.
+struct PoolAccArgs {
+    PoolArgs p;       // requests, bags, weights, mode and slices as in the pooled get (p.dst unused)
+    const char *grad; // [nbags] rows of row_bytes in the element type
+    double alpha;
+    int64_t windows; // row windows per bag
+};
+constexpr int64_t kPoolAccFill = 4;        // warps per resident warp the launcher aims for
+constexpr int64_t kPoolAccMaxWindows = 32; // row windows per bag at most
+
+__device__ __forceinline__ float pool_mul(float a, float x) { return __fmul_rn(a, x); }
+__device__ __forceinline__ double pool_mul(double a, double x) { return __dmul_rn(a, x); }
+template <typename RW>
+__device__ __forceinline__ RW pool_ldg(const char *p) {
+    if constexpr (std::is_same<RW, uint4>::value) return __ldg((const uint4 *)p);
+    else if constexpr (sizeof(RW) == 2) return (RW)__ldg((const unsigned short *)p);
+    else if constexpr (sizeof(RW) == 4) return (RW)__ldg((const unsigned int *)p);
+    else return (RW)__ldg((const unsigned long long *)p);
+}
+// a lane's contribution vector: g (weighted by w), over n (mean, n > 0), times alpha, each step rounded; then encoded
+template <int DT, int E>
+__device__ __forceinline__ void pool_contrib(typename PoolType<DT>::U (&c)[E], const typename PoolType<DT>::A (&g)[E],
+                                             bool weighted, typename PoolType<DT>::A w, int64_t n,
+                                             typename PoolType<DT>::A alpha) {
+#pragma unroll
+    for (int e = 0; e < E; e++) {
+        typename PoolType<DT>::A v = g[e];
+        if (weighted) v = pool_mul(v, w);
+        if (n > 0) v = pool_div(v, n);
+        c[e] = pool_enc<DT>(pool_mul(v, alpha));
+    }
+}
+template <int DT, int E>
+__device__ __forceinline__ void pool_red(char *d, const typename PoolType<DT>::U (&c)[E]) {
+    if constexpr (E * sizeof(typename PoolType<DT>::U) == 16) red16(d, pool_pack(c), DT, DDSK_OP_SUM);
+    else red1v(d, Held{(uint64_t)c[0]}, DT, DDSK_OP_SUM);
+}
+
+template <int DT, int VB>
+__global__ void __launch_bounds__(kPoolThreads, kPoolMinBlocks) dds_pool_acc_kernel(const __grid_constant__ PoolAccArgs aa) {
+    using U = typename PoolType<DT>::U;
+    using A = typename PoolType<DT>::A;
+    using RW = typename std::conditional<VB == 16, uint4, U>::type;
+    constexpr int E = VB / (int)sizeof(U);
+    const PoolArgs &a = aa.p;
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = (int64_t)gridDim.x * (kPoolThreads / 32);
+    const int64_t row_bytes = a.var.row_bytes, W = aa.windows, per_bag = a.nslices * W;
+    const bool mean = a.mode == DDSK_POOL_MEAN, weighted = a.weights != nullptr;
+    const A alpha = (A)aa.alpha;
+    for (int64_t w = (int64_t)blockIdx.x * (kPoolThreads / 32) + (threadIdx.x >> 5); w < a.nbags * per_bag; w += nwarps) {
+        const int64_t k = w / per_bag, rem = w - k * per_bag, j = rem / a.nslices, sl = rem - j * a.nslices;
+        const int64_t col = sl * a.slice + (int64_t)lane * VB;
+        const bool mine = (int64_t)lane * VB < a.slice && col < row_bytes; // (everything below is warp-uniform but the loads)
+        int64_t b0 = k, b1 = k + 1;
+        if (a.bags) {
+            b0 = a.bags[k];
+            b1 = a.bags[k + 1];
+        }
+        if (b0 < 0 || b1 < b0 || b1 > a.nreq) { // malformed: nothing is written
+            if (lane == 0 && sl == 0 && j == 0) report(a.status, a.status_tag, k, DDSK_CODE_BAG);
+            continue;
+        }
+        A g[E];
+        {
+            const RW x = mine ? pool_ldg<RW>(aa.grad + k * row_bytes + col) : RW{};
+#pragma unroll
+            for (int e = 0; e < E; e++) g[e] = pool_dec<DT>(pool_elem<U>(x, e));
+        }
+        int64_t nk = 0; // a mean bag's rows (0: no division)
+        if (mean && b1 - b0 > 32)
+            for (int64_t base = b0; base < b1; base += 32) {
+                uint64_t src;
+                int64_t n = 0;
+                if (base + lane < b1) pool_req(a, base + lane, &src, &n, false);
+                nk += warp_sum(n);
+            }
+        U cu[E]; // the unweighted contribution, once the bag's row count is known
+        int64_t rows = 0; // the bag's valid rows before this window of requests
+        for (int64_t base = b0; base < b1; base += 32) {
+            const int64_t i = base + lane;
+            uint64_t src = 0;
+            int64_t n = 0;
+            A wt = A(1);
+            if (i < b1) {
+                pool_req(a, i, &src, &n, j == 0);
+                if (weighted) wt = pool_dec<DT>(((const U *)a.weights)[i]);
+            }
+            const int64_t incl = warp_incl_scan(n, lane), excl = incl - n;
+            const int64_t total = __shfl_sync(0xffffffffu, incl, 31);
+            if (base == b0 && !weighted) {
+                if (mean && b1 - b0 <= 32) nk = total;
+                pool_contrib<DT, E>(cu, g, false, A(1), nk, alpha);
+            }
+            // this window's rows r of the requests: (rows + r) % W == j
+            for (int64_t r = ((j - rows) % W + W) % W; r < total; r += W) {
+                const int q = __popc(__ballot_sync(0xffffffffu, incl <= r)) & 31;
+                const uint64_t s = __shfl_sync(0xffffffffu, src, q);
+                const int64_t e0 = __shfl_sync(0xffffffffu, excl, q);
+                char *d = (char *)(s + (uint64_t)(r - e0) * (uint64_t)row_bytes + (uint64_t)col);
+                if (weighted) {
+                    const A wr = __shfl_sync(0xffffffffu, wt, q);
+                    U c[E];
+                    pool_contrib<DT, E>(c, g, true, wr, 0, alpha);
+                    if (mine) pool_red<DT, E>(d, c);
+                } else if (mine) {
+                    pool_red<DT, E>(d, cu);
+                }
+            }
+            rows += total;
         }
     }
 }
@@ -3352,6 +3520,34 @@ int launch_pool_t(const PoolArgs &a, int vb, int blocks, cudaStream_t st) {
     CUDA_TRY(cudaGetLastError());
     return 0;
 }
+template <int DT>
+int launch_pool_acc_t(const PoolAccArgs &a, int vb, int blocks, cudaStream_t st) {
+    if (vb == 16) dds_pool_acc_kernel<DT, 16><<<blocks, kPoolThreads, 0, st>>>(a);
+    else dds_pool_acc_kernel<DT, (int)sizeof(typename PoolType<DT>::U)><<<blocks, kPoolThreads, 0, st>>>(a);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+// A pooled launch's arguments but its slices and output
+void pool_args(PoolArgs &a, const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_count, int64_t nreq,
+               const ddsk_pool_t *pool, const ddsk_scratch_t *scr) {
+    memset(&a, 0, sizeof(a));
+    a.var = *var;
+    a.starts = index->starts;
+    a.counts = index->counts;
+    a.count = fixed_count;
+    a.ids = index->sample_ids;
+    a.tab = (const longlong2 *)index->table;
+    a.nsamples = index->nsamples;
+    a.bags = pool->bags;
+    a.nbags = pool->nbags;
+    a.nreq = nreq;
+    a.weights = pool->weights;
+    a.mode = pool->mode;
+    a.status = scr->status;
+    a.status_tag = scr->status_tag;
+}
 
 } // namespace
 
@@ -3572,22 +3768,8 @@ int ddsk_pool(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_co
     if (pool->nbags <= 0 || var->row_bytes <= 0) return 0;
     if (int rc = pick_geometry()) return rc;
     PoolArgs a;
-    memset(&a, 0, sizeof(a));
-    a.var = *var;
-    a.starts = index->starts;
-    a.counts = index->counts;
-    a.count = fixed_count;
-    a.ids = index->sample_ids;
-    a.tab = (const longlong2 *)index->table;
-    a.nsamples = index->nsamples;
-    a.bags = pool->bags;
-    a.nbags = pool->nbags;
-    a.nreq = nreq;
-    a.weights = pool->weights;
-    a.mode = pool->mode;
+    pool_args(a, var, index, fixed_count, nreq, pool, scr);
     a.dst = (char *)dst;
-    a.status = scr->status;
-    a.status_tag = scr->status_tag;
     const int64_t R = var->row_bytes;
     const int vb = (R % 16 == 0 && (uint64_t)dst % 16 == 0) ? 16 : 1 << DDSK_ACC_LOG2(pool->type);
     // slices: whole warps of vectors, halved while the bags leave resident warps idle (a few long bags then still spread)
@@ -3609,6 +3791,42 @@ int ddsk_pool(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_co
     case DDSK_ACC_BF16: rc = launch_pool_t<DDSK_ACC_BF16>(a, vb, blocks, st); break;
     default:
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_pool: unsupported element type %d", (int)pool->type);
+        return -2;
+    }
+    if (rc) return rc;
+    if (flags & DDSK_F_MIRROR) // (a synchronous call reads the status from the pinned mirror word)
+        CUDA_TRY(cudaMemcpyAsync(scr->host_mirror, scr->status, 8, cudaMemcpyDefault, st));
+    return 0;
+}
+
+int ddsk_pool_acc(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_count, int64_t nreq,
+                  const ddsk_pool_t *pool, double alpha, const void *grad, const ddsk_scratch_t *scr, int flags,
+                  void *stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (pool->nbags <= 0 || var->row_bytes <= 0) return 0;
+    if (int rc = pick_geometry()) return rc;
+    PoolAccArgs a;
+    pool_args(a.p, var, index, fixed_count, nreq, pool, scr);
+    a.grad = (const char *)grad;
+    a.alpha = alpha;
+    const int64_t R = var->row_bytes;
+    const int vb = (R % 16 == 0 && (uint64_t)grad % 16 == 0) ? 16 : 1 << DDSK_ACC_LOG2(pool->type);
+    // whole-warp slices; then each bag's rows are dealt to row windows until there are kPoolAccFill warps per resident one
+    // (a few long bags, such as mean-pooled frames, then still spread over the machine)
+    const int64_t resident = (int64_t)g_sms * kPoolMinBlocks * (kPoolThreads / 32);
+    a.p.slice = 32 * vb;
+    a.p.nslices = (R + a.p.slice - 1) / a.p.slice;
+    const int64_t units = a.p.nbags * a.p.nslices, per_cta = kPoolThreads / 32;
+    a.windows = std::max<int64_t>(1, std::min<int64_t>(kPoolAccMaxWindows, (kPoolAccFill * resident + units - 1) / units));
+    const int blocks = (int)std::min((units * a.windows + per_cta - 1) / per_cta, (int64_t)g_sms * kPoolMinBlocks);
+    int rc = 0;
+    switch (pool->type) {
+    case DDSK_ACC_F32: rc = launch_pool_acc_t<DDSK_ACC_F32>(a, vb, blocks, st); break;
+    case DDSK_ACC_F64: rc = launch_pool_acc_t<DDSK_ACC_F64>(a, vb, blocks, st); break;
+    case DDSK_ACC_F16: rc = launch_pool_acc_t<DDSK_ACC_F16>(a, vb, blocks, st); break;
+    case DDSK_ACC_BF16: rc = launch_pool_acc_t<DDSK_ACC_BF16>(a, vb, blocks, st); break;
+    default:
+        snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_pool_acc: unsupported element type %d", (int)pool->type);
         return -2;
     }
     if (rc) return rc;

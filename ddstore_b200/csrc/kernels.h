@@ -258,6 +258,12 @@ typedef struct ddsk_pool {
 } ddsk_pool_t;
 int ddsk_pool(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_count, int64_t nreq, const ddsk_pool_t *pool,
               void *dst, const ddsk_scratch_t *scr, int flags, void *stream);
+/* Pooled accumulate (dds_accumulate_batch_pooled), the adjoint of ddsk_pool with the same requests and pool (mode SUM or
+ * MEAN): every row of bag k's valid requests gets grad row k (times the request's weight, over the bag's valid rows for
+ * a mean, times alpha) added atomically. grad is device memory holding nbags rows, aligned to the element size. */
+int ddsk_pool_acc(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_count, int64_t nreq,
+                  const ddsk_pool_t *pool, double alpha, const void *grad, const ddsk_scratch_t *scr, int flags,
+                  void *stream);
 
 /* Multi-array batch: the rows of the SAME nreq sample ids in nvars (<= DDSK_MAX_MULTI) variables, one launch. vars_dev =
  * device array of the variables' windows; table[v] = sample index of variable v; dst[v]/cap[v]/offsets[v] per variable

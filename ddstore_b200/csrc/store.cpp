@@ -19,6 +19,7 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <cmath>
 #include <atomic>
 #include <condition_variable>
 #include <mutex>
@@ -1946,71 +1947,126 @@ int dds_compare_and_swap_samples(dds_store_t *s, const char *name, const int64_t
                     write_rec(v, DDSK_OP_CAS, 0, result, compare), true);
 }
 
-// The pooled path behind dds_get_batch_pooled / dds_get_samples_pooled (by_sample: starts = sample ids, counts unused).
-// Every argument, and host bags, are checked before anything is enqueued; device bags are checked by the kernel. Host
-// bags and weights are staged in the store's offsets buffer, behind each other. A pooled launch is never overlapped.
 static_assert(DDS_POOL_SUM == DDSK_POOL_SUM && DDS_POOL_MEAN == DDSK_POOL_MEAN && DDS_POOL_MAX == DDSK_POOL_MAX,
               "the kernels' pooling modes are the public ones");
-static int pool_impl(dds_store_t *s, const char *name, bool by_sample, const int64_t *starts, const int64_t *counts,
-                     int64_t fixed_count, int64_t nreq, const dds_pool_t *pool, void *dst, int64_t dst_capacity,
-                     unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
-    Var *v;
-    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, &v)) return rc;
+// The argument checks of both pooled paths, in one order. buf is the get's destination (`acc` false) or the
+// accumulate's grad (`acc`: no max mode, a device source, "grad" in the texts), holding buf_bytes; it must hold
+// *total = nbags * R. Host bags are checked last, before anything is enqueued.
+static int pool_check(Var *v, bool by_sample, const int64_t *starts, int64_t nreq, const dds_pool_t *pool, const void *buf,
+                      int64_t buf_bytes, bool acc, unsigned flags, int64_t *bad_index, int64_t *total) {
     if (!pool) return fail(DDS_ERR_ARG, "null pooling");
     if (pool->mode < DDS_POOL_SUM || pool->mode > DDS_POOL_MAX) return fail(DDS_ERR_ARG, "unknown pooling mode");
+    if (acc && pool->mode == DDS_POOL_MAX)
+        return fail(DDS_ERR_ARG, "pooled accumulates take DDS_POOL_SUM or DDS_POOL_MEAN (max has no adjoint without its argmax)");
     const int dt = pool->dtype;
     if (dt != DDS_ACC_F32 && dt != DDS_ACC_F64 && dt != DDS_ACC_F16 && dt != DDS_ACC_BF16)
         return fail(DDS_ERR_ARG, "pooled batches take DDS_ACC_F32, F64, F16 or BF16");
     const int64_t el = (int64_t)1 << DDSK_ACC_LOG2(dt);
     if (v->itemsize != el) return fail(DDS_ERR_DTYPE);
     if (pool->weights && pool->mode != DDS_POOL_SUM) return fail(DDS_ERR_ARG, "weights apply to DDS_POOL_SUM only");
-    if (!(flags & DDS_DST_ON_DEVICE)) return fail(DDS_ERR_ARG, "pooled batches deliver into device memory");
-    if (nreq < 0 || dst_capacity < 0) return fail(DDS_ERR_ARG, "negative nreq or capacity");
+    if (!acc && !(flags & DDS_DST_ON_DEVICE)) return fail(DDS_ERR_ARG, "pooled batches deliver into device memory");
+    if (acc && !(flags & DDS_SRC_ON_DEVICE))
+        return fail(DDS_ERR_ARG, "pooled accumulates take grad from device memory (DDS_SRC_ON_DEVICE)");
+    if (nreq < 0 || buf_bytes < 0) return fail(DDS_ERR_ARG, acc ? "negative nreq or grad_bytes" : "negative nreq or capacity");
     if (pool->nbags < 0) return fail(DDS_ERR_ARG, "nbags < 0");
     if (!pool->bags && pool->nbags != nreq) return fail(DDS_ERR_ARG, "without bag offsets, nbags must equal nreq");
-    int64_t total = 0;
-    if (__builtin_mul_overflow(pool->nbags, v->kv.row_bytes, &total)) return fail(DDS_ERR_ARG, "the pooled batch's size overflows");
-    if (dst_capacity < total)
-        return fail(DDS_ERR_ARG, "destination holds " + std::to_string(dst_capacity) + " bytes, the pooled batch " +
-                                     std::to_string(total));
-    if ((uint64_t)dst % (uint64_t)el || (uint64_t)pool->weights % (uint64_t)el)
-        return fail(DDS_ERR_ARG, "destination or weights not aligned to the element size");
-    if (total > 0 && !dst) return fail(DDS_ERR_ARG, "null destination");
+    if (__builtin_mul_overflow(pool->nbags, v->kv.row_bytes, total)) return fail(DDS_ERR_ARG, "the pooled batch's size overflows");
+    const char *what = acc ? "grad" : "destination";
+    if (buf_bytes < *total)
+        return fail(DDS_ERR_ARG, std::string(what) + " holds " + std::to_string(buf_bytes) + " bytes, the pooled batch " +
+                                     std::to_string(*total));
+    if ((uint64_t)buf % (uint64_t)el || (uint64_t)pool->weights % (uint64_t)el)
+        return fail(DDS_ERR_ARG, std::string(what) + " or weights not aligned to the element size");
+    if (*total > 0 && !buf) return fail(DDS_ERR_ARG, std::string("null ") + what);
     if (nreq > 0 && !starts) return fail(DDS_ERR_ARG, "null starts / sample ids");
     if (by_sample && !v->d_tab) return fail(DDS_ERR_ARG, "variable has no sample index (call dds_set_sample_index first)");
-    const bool idx_dev = flags & DDS_IDX_ON_DEVICE, no_sync = flags & DDS_NO_SYNC;
-    if (no_sync && !idx_dev) return fail(DDS_ERR_ARG, "async batches need device indices and a device destination");
+    const bool idx_dev = flags & DDS_IDX_ON_DEVICE;
+    if ((flags & DDS_NO_SYNC) && !idx_dev)
+        return fail(DDS_ERR_ARG, acc ? "async pooled accumulates need device indices, bags and weights"
+                                     : "async batches need device indices and a device destination");
     if (pool->bags && !idx_dev) // host bags: checked here, before anything is enqueued
         for (int64_t k = 0; k < pool->nbags; k++)
             if (pool->bags[k] < 0 || pool->bags[k + 1] < pool->bags[k] || pool->bags[k + 1] > nreq) {
                 if (bad_index) *bad_index = k;
                 return fail(DDS_ERR_ARG, "malformed bag offsets");
             }
+    return DDS_OK;
+}
+
+// A pooled call's requests, bags and weights on the device: host ones are staged (bags and weights in the store's
+// offsets buffer, behind each other)
+static int pool_stage(dds_store_t *s, Var *v, bool by_sample, const int64_t *starts, const int64_t *counts, int64_t nreq,
+                      const dds_pool_t *pool, bool idx_dev, cudaStream_t st, ddsk_index_t *ix, ddsk_pool_t *kp) {
+    if (int rc = stage_indices(s, v, by_sample, starts, counts, nreq, idx_dev, st, ix)) return rc;
+    *kp = ddsk_pool_t{pool->mode, pool->dtype, pool->bags, pool->nbags, pool->weights};
+    if (!idx_dev && (pool->bags || pool->weights)) {
+        const int64_t nb = pool->bags ? pool->nbags + 1 : 0;
+        if (int rc = ensure_offs(s, nb + nreq)) return rc;
+        if (pool->bags) CU(cudaMemcpyAsync(s->d_offs, pool->bags, (size_t)nb * 8, cudaMemcpyHostToDevice, st));
+        if (pool->weights && nreq > 0)
+            CU(cudaMemcpyAsync(s->d_offs + nb, pool->weights, (size_t)(nreq * v->itemsize), cudaMemcpyHostToDevice, st));
+        kp->bags = pool->bags ? s->d_offs : nullptr;
+        kp->weights = pool->weights ? (const void *)(s->d_offs + nb) : nullptr;
+    }
+    return DDS_OK;
+}
+
+// The pooled path behind dds_get_batch_pooled / dds_get_samples_pooled (by_sample: starts = sample ids, counts unused).
+// Every argument, and host bags, are checked before anything is enqueued; device bags are checked by the kernel. A pooled
+// launch is never overlapped.
+static int pool_impl(dds_store_t *s, const char *name, bool by_sample, const int64_t *starts, const int64_t *counts,
+                     int64_t fixed_count, int64_t nreq, const dds_pool_t *pool, void *dst, int64_t dst_capacity,
+                     unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, &v)) return rc;
+    int64_t total = 0;
+    if (int rc = pool_check(v, by_sample, starts, nreq, pool, dst, dst_capacity, false, flags, bad_index, &total)) return rc;
 
     Call c;
-    if (int rc = begin_call(s, cuda_stream, no_sync, &c)) return rc;
+    if (int rc = begin_call(s, cuda_stream, flags & DDS_NO_SYNC, &c)) return rc;
     if (pool->nbags == 0) {
         note_empty_async(s, c);
         return DDS_OK;
     }
     ddsk_index_t ix;
-    if (int rc = stage_indices(s, v, by_sample, starts, counts, nreq, idx_dev, c.st, &ix)) return rc;
-    ddsk_pool_t kp{pool->mode, dt, pool->bags, pool->nbags, pool->weights};
-    if (!idx_dev && (pool->bags || pool->weights)) {
-        const int64_t nb = pool->bags ? pool->nbags + 1 : 0;
-        if (int rc = ensure_offs(s, nb + nreq)) return rc;
-        if (pool->bags) CU(cudaMemcpyAsync(s->d_offs, pool->bags, (size_t)nb * 8, cudaMemcpyHostToDevice, c.st));
-        if (pool->weights && nreq > 0)
-            CU(cudaMemcpyAsync(s->d_offs + nb, pool->weights, (size_t)(nreq * el), cudaMemcpyHostToDevice, c.st));
-        kp.bags = pool->bags ? s->d_offs : nullptr;
-        kp.weights = pool->weights ? (const void *)(s->d_offs + nb) : nullptr;
-    }
+    ddsk_pool_t kp;
+    if (int rc = pool_stage(s, v, by_sample, starts, counts, nreq, pool, flags & DDS_IDX_ON_DEVICE, c.st, &ix, &kp)) return rc;
     int kflags;
     ddsk_scratch_t scr;
     if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
     if (ddsk_pool(&v->kv, &ix, fixed_count, nreq, &kp, dst, &scr, kflags, c.st)) return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
     if (total_bytes) *total_bytes = total;
     return end_launch(s, c, total, nullptr, DDSK_CVT_NONE, false, nullptr, bad_index);
+}
+
+// The pooled accumulates behind dds_accumulate_batch_pooled / dds_accumulate_samples_pooled: the pooled get's checks
+// and staging, with grad in place of the destination, then the same lifecycle (a write: it ends any overlap run).
+static int pool_acc_impl(dds_store_t *s, const char *name, bool by_sample, const int64_t *starts, const int64_t *counts,
+                         int64_t fixed_count, int64_t nreq, const dds_pool_t *pool, double alpha, const void *grad,
+                         int64_t grad_bytes, unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    Var *v;
+    if (int rc = entry_var(s, name, nullptr, total_bytes, bad_index, &v, kHostWrite)) return rc;
+    int64_t total = 0;
+    if (int rc = pool_check(v, by_sample, starts, nreq, pool, grad, grad_bytes, true, flags, bad_index, &total)) return rc;
+    if (!std::isfinite(alpha)) return fail(DDS_ERR_ARG, "alpha must be finite");
+
+    Call c;
+    if (int rc = begin_call(s, cuda_stream, flags & DDS_NO_SYNC, &c)) return rc;
+    if (pool->nbags == 0) {
+        note_empty_async(s, c);
+        return DDS_OK;
+    }
+    ddsk_index_t ix;
+    ddsk_pool_t kp;
+    if (int rc = pool_stage(s, v, by_sample, starts, counts, nreq, pool, flags & DDS_IDX_ON_DEVICE, c.st, &ix, &kp)) return rc;
+    int kflags;
+    ddsk_scratch_t scr;
+    if (int rc = launch_flags(s, c, false, false, &kflags, &scr)) return rc;
+    if (ddsk_pool_acc(&v->kv, &ix, fixed_count, nreq, &kp, alpha, grad, &scr, kflags, c.st))
+        return fail(DDS_ERR_CUDA, ddsk_last_cuda_error());
+    if (total_bytes) *total_bytes = total;
+    // (a write: queued, it is completed by the next dds_epoch_begin, as every batched write is)
+    return end_launch(s, c, total, nullptr, DDSK_CVT_NONE, true, nullptr, bad_index);
 }
 
 int dds_get_batch_pooled(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
@@ -2025,6 +2081,21 @@ int dds_get_samples_pooled(dds_store_t *s, const char *name, const int64_t *samp
                            int64_t *total_bytes, int64_t *bad_index) {
     return pool_impl(s, name, true, sample_ids, nullptr, 0, nreq, pool, dst, dst_capacity, flags, cuda_stream, total_bytes,
                      bad_index);
+}
+
+int dds_accumulate_batch_pooled(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                                int64_t fixed_count, int64_t nreq, const dds_pool_t *pool, double alpha,
+                                const void *grad, int64_t grad_bytes, unsigned flags, void *cuda_stream,
+                                int64_t *total_bytes, int64_t *bad_index) {
+    return pool_acc_impl(s, name, false, starts, counts, fixed_count, nreq, pool, alpha, grad, grad_bytes, flags,
+                         cuda_stream, total_bytes, bad_index);
+}
+
+int dds_accumulate_samples_pooled(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq,
+                                  const dds_pool_t *pool, double alpha, const void *grad, int64_t grad_bytes,
+                                  unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index) {
+    return pool_acc_impl(s, name, true, sample_ids, nullptr, 0, nreq, pool, alpha, grad, grad_bytes, flags, cuda_stream,
+                         total_bytes, bad_index);
 }
 
 // The multi-array path behind dds_get_samples_multi / dds_get_samples_multi_convert (cvts: one conversion per variable,

@@ -20,7 +20,7 @@ import numpy as np
 from ddstore_b200._capi import PLACEMENTS
 from ddstore_b200.comm import as_dds_comm
 from ddstore_b200.store import (_PLACEMENT_NAMES as PLACEMENT_NAMES, _Buf, _acc_type, _cas_args, _dtype_name, _fop_args,
-                                _get_args, _norm_tables, _offsets, _pad, _pad_rows, _placement, _pool_args,
+                                _get_args, _norm_tables, _offsets, _pad, _pad_rows, _placement, _pool_acc_args, _pool_args,
                                 _pool_requests, _ptr, _put_src, _red_op, _requests, _stream_handle)
 
 cdef extern from *:
@@ -71,6 +71,10 @@ cdef extern from "ddstore_b200.hpp" nogil:
         long get_batch_pooled(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                               int mode, int dtype, const long* bags, long nbags, const void* weights, void* dst,
                               long dst_capacity_bytes, cbool idx_on_device, void* stream) except +dds_translate_exception
+        long accumulate_batch_pooled(string name, const long* starts, const long* counts, long fixed_count, long nreq,
+                                     int mode, int dtype, const long* bags, long nbags, const void* weights,
+                                     double alpha, const void* grad, long grad_bytes, cbool idx_on_device,
+                                     void* stream) except +dds_translate_exception
         long compare_and_swap_batch(string name, const long* starts, const long* counts, long fixed_count, long nreq,
                                     int itemsize, const void* src, const void* compare, void* result, long src_bytes,
                                     cbool idx_on_device, void* stream) except +dds_translate_exception
@@ -263,6 +267,31 @@ cdef class PyDDStore:
             total = self.c_ddstore.get_batch_pooled(nm, <const long*> sp, <const long*> cp, fixed, nreq, modec, code,
                                                     <const long*> bp, nbags, <const void*> wp, <void*> dp, cap, idx_dev,
                                                     <void*> st)
+        del sa, ca, ba, wa
+        return total
+
+    def accumulate_batch_pooled(self, str name, starts, counts=None, count=None, grad=None, bags=None, mode="sum",
+                                weights=None, alpha=1.0, stream=None):
+        """one kernel launch scattering each bag's row of the CUDA tensor `grad` (float32, float64, float16 or bfloat16)
+        into the rows of its requests, the adjoint of get_batch_pooled; see
+        ddstore_b200.store.PyDDStore.accumulate_batch_pooled (this binding's call is synchronous). Returns nbags * R."""
+        modes_types = _pool_acc_args(name, mode, alpha, grad)
+        cdef int modec = modes_types[0], code = modes_types[1]
+        sa, ca, ba, wa, s_dev = _pool_requests(starts, counts, bags, weights, grad, True)
+        cdef long nreq = sa.numel()
+        cdef long nbags = ba.numel() - 1 if ba is not None else nreq
+        cdef size_t sp = sa.data_ptr(), cp = ca.data_ptr() if ca is not None else 0
+        cdef size_t bp = ba.data_ptr() if ba is not None else 0, wp = wa.data_ptr() if wa is not None else 0
+        cdef size_t gp = grad.data_ptr(), st = _stream_handle(stream)
+        cdef long nbytes = grad.numel() * grad.element_size(), fixed = 1 if count is None else int(count)
+        cdef double a = alpha
+        cdef string nm = name.encode()
+        cdef cbool idx_dev = s_dev
+        cdef long total
+        with nogil:
+            total = self.c_ddstore.accumulate_batch_pooled(nm, <const long*> sp, <const long*> cp, fixed, nreq, modec,
+                                                           code, <const long*> bp, nbags, <const void*> wp, a,
+                                                           <const void*> gp, nbytes, idx_dev, <void*> st)
         del sa, ca, ba, wa
         return total
 

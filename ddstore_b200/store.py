@@ -6,6 +6,7 @@ meaning, same exception types/texts): add / get / epoch_begin / epoch_end / free
 (host) or CUDA tensors / __cuda_array_interface__ objects (device; fetched bytes then never leave HBM).
 """
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -335,18 +336,28 @@ def _cas_args(name, compare, out, sb):
     return ptrs[0], ptrs[1]
 
 
-def _pool_args(name, mode, out):
-    """the DDS_POOL_* mode and the DDS_ACC_* element type of a pooled batch into `out` (ValueError for an unknown
-    mode, or an out that is not a C-contiguous CUDA float32, float64, float16 or bfloat16 tensor)"""
+def _pool_args(name, mode, t, what="out"):
+    """the DDS_POOL_* mode and the DDS_ACC_* element type of a pooled batch's tensor t, its `out` or its `grad` (ValueError
+    for an unknown mode, or a t that is not a C-contiguous CUDA float32, float64, float16 or bfloat16 tensor)"""
     import torch
     if mode not in _capi.POOL_MODES:
         raise ValueError(f"pooled batch of {name!r}: mode {mode!r} is not one of {', '.join(_capi.POOL_MODES)}")
-    if not (isinstance(out, torch.Tensor) and out.is_cuda and out.is_contiguous()):
-        raise ValueError("out must be a C-contiguous CUDA tensor")
-    dt = _dtype_name(out.dtype)
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.is_contiguous()):
+        raise ValueError(f"{what} must be a C-contiguous CUDA tensor")
+    dt = _dtype_name(t.dtype)
     if dt not in ("float32", "float64", "float16", "bfloat16"):
-        raise ValueError(f"pooled batch of {name!r}: out dtype {dt} is not float32, float64, float16 or bfloat16")
+        raise ValueError(f"pooled batch of {name!r}: {what} dtype {dt} is not float32, float64, float16 or bfloat16")
     return _capi.POOL_MODES[mode], _capi.ACC_TYPES[dt]
+
+
+def _pool_acc_args(name, mode, alpha, grad):
+    """_pool_args of a pooled accumulate's `grad`, refusing first mode "max" (its adjoint needs the forward's argmax)
+    and a non-finite alpha (one NaN step would poison the whole table)"""
+    if mode == "max":
+        raise ValueError(f"pooled accumulate into {name!r}: mode 'max' has no adjoint here (use 'sum' or 'mean')")
+    if alpha is None or not math.isfinite(alpha):
+        raise ValueError(f"pooled accumulate into {name!r}: alpha must be finite, not {alpha!r}")
+    return _pool_args(name, mode, grad, "grad")
 
 
 def _pool_requests(starts, counts, bags, weights, out, wait):
@@ -632,22 +643,47 @@ class PyDDStore:
         set_sample_index (e.g. a variable-length sample mean-pooled to one vector)."""
         return self._pooled(name, True, sample_ids, None, None, out, bags, mode, weights, stream, wait)
 
-    def _pooled(self, name, by_sample, starts, counts, count, out, bags, mode, weights, stream, wait):
-        modec, dtc = _pool_args(name, mode, out)
-        sa, ca, ba, wa, s_dev = _pool_requests(starts, counts, bags, weights, out, wait)
+    # ---------------------------------------------------------------- pooled accumulates (embedding_bag backward)
+    def accumulate_batch_pooled(self, name, starts, counts=None, count=None, grad=None, bags=None, mode="sum",
+                                weights=None, alpha=1.0, stream=None, wait=True):
+        """Scatter each bag's gradient into its rows, in ONE kernel launch: the adjoint of get_batch_pooled with the same
+        requests, bags, mode ("sum" or "mean") and weights -- torch's embedding_bag backward fused with the SGD step
+        p.add_(g, alpha=alpha) over a sharded variable. grad (a C-contiguous CUDA float32, float64, float16 or bfloat16
+        tensor of the variable's itemsize) holds nbags rows of disp elements. Every row of every valid request i of bag
+        k gets grad[k] * weights[i] (weighted sum), / n_k (mean: n_k the rows the pooled get folds for bag k), * alpha,
+        each step rounded once in float32 (float64 for float64 rows), then rounded to grad.dtype and added atomically
+        into the shard as accumulate_batch adds (atomic across ranks and duplicate ids, in no fixed order). Requests,
+        bags, errors and wait=False are get_batch_pooled's: an invalid request adds nothing and is left out of n_k, a
+        malformed bag adds nothing and raises before any request error. alpha must be finite. The rows are visible at
+        the next fence. Returns nbags * R bytes (None with wait=False)."""
+        return self._pooled(name, False, starts, counts, count, grad, bags, mode, weights, stream, wait, True, alpha)
+
+    def accumulate_samples_pooled(self, name, sample_ids, grad, bags=None, mode="sum", weights=None, alpha=1.0,
+                                  stream=None, wait=True):
+        """accumulate_batch_pooled by SAMPLE ID: request i = the rows of sample sample_ids[i] in the index registered
+        with set_sample_index (the backward of get_samples_pooled)."""
+        return self._pooled(name, True, sample_ids, None, None, grad, bags, mode, weights, stream, wait, True, alpha)
+
+    def _pooled(self, name, by_sample, starts, counts, count, buf, bags, mode, weights, stream, wait, acc=False,
+                alpha=1.0):
+        """the pooled batches into `buf` = out, or (acc) the pooled accumulates from `buf` = grad"""
+        modec, dtc = _pool_acc_args(name, mode, alpha, buf) if acc else _pool_args(name, mode, buf)
+        sa, ca, ba, wa, s_dev = _pool_requests(starts, counts, bags, weights, buf, wait)
         nreq = sa.numel()
         nbags = ba.numel() - 1 if ba is not None else nreq
         pool = _capi.Pool(modec, dtc, ba.data_ptr() if ba is not None else None, nbags,
                           wa.data_ptr() if wa is not None else None)
-        flags = _capi.DST_ON_DEVICE | (_capi.IDX_ON_DEVICE if s_dev else 0) | (0 if wait else _capi.NO_SYNC)
-        cap = out.numel() * out.element_size()
+        flags = ((_capi.SRC_ON_DEVICE if acc else _capi.DST_ON_DEVICE) | (_capi.IDX_ON_DEVICE if s_dev else 0)
+                 | (0 if wait else _capi.NO_SYNC))
+        operands = (C.byref(pool), *((float(alpha),) if acc else ()), buf.data_ptr(), buf.numel() * buf.element_size())
+        entry = f"dds_{'accumulate' if acc else 'get'}_{'samples' if by_sample else 'batch'}_pooled"
         if by_sample:
-            total = self._call(self._L.dds_get_samples_pooled, self._h, name.encode(), sa.data_ptr(), nreq,
-                               C.byref(pool), out.data_ptr(), cap, flags, _stream_handle(stream))
+            total = self._call(getattr(self._L, entry), self._h, name.encode(), sa.data_ptr(), nreq, *operands, flags,
+                               _stream_handle(stream))
         else:
-            total = self._call(self._L.dds_get_batch_pooled, self._h, name.encode(), sa.data_ptr(),
+            total = self._call(getattr(self._L, entry), self._h, name.encode(), sa.data_ptr(),
                                ca.data_ptr() if ca is not None else None, 1 if count is None else int(count), nreq,
-                               C.byref(pool), out.data_ptr(), cap, flags, _stream_handle(stream))
+                               *operands, flags, _stream_handle(stream))
         return total if wait else None
 
     # ---------------------------------------------------------------- collective owner-push fetch

@@ -31,7 +31,8 @@ extern "C" {
                            compare-and-swaps (dds_compare_and_swap_batch, dds_compare_and_swap_samples), the batched
                            reductions (dds_accumulate_op_batch, dds_accumulate_op_samples, DDS_OP_MAX & co.), the
                            placed variables (dds_add_placed, dds_init_placed, dds_query_placement, DDS_PLACE_*) and the
-                           pooled batches (dds_get_batch_pooled, dds_get_samples_pooled, DDS_POOL_*). */
+                           pooled batches (dds_get_batch_pooled, dds_get_samples_pooled, DDS_POOL_*) and the pooled
+                           accumulates (dds_accumulate_batch_pooled, dds_accumulate_samples_pooled). */
 
 /* ---- status codes. 1-6 carry the reference's exception texts verbatim ------------------------- */
 #define DDS_OK 0
@@ -513,6 +514,37 @@ int dds_get_batch_pooled(dds_store_t *s, const char *name, const int64_t *starts
 int dds_get_samples_pooled(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq,
                            const dds_pool_t *pool, void *dst, int64_t dst_capacity, unsigned flags, void *cuda_stream,
                            int64_t *total_bytes, int64_t *bad_index);
+
+/* ---- pooled accumulates: each bag's gradient scattered into its rows of any rank's shard (the backward of the pooled
+ * batches: torch's embedding_bag backward plus the SGD step over a sharded variable, in one launch)
+ * The exact adjoint of dds_get_batch_pooled / dds_get_samples_pooled with the same requests and dds_pool_t (bags,
+ * weights, DDS_POOL_SUM or DDS_POOL_MEAN). grad holds nbags rows of R = disp * itemsize bytes in pool->dtype. Every
+ * element e of every row of every valid request i in bag k gets one contribution c, computed in the forward's
+ * accumulator type A (f32 for f32, f16 and bf16; f64 for f64), each step one round-to-nearest operation, none contracted:
+ *   c = grad[k][e];  c = c * w_i (weights);  c = c / n_k (DDS_POOL_MEAN);  c = c * (A)alpha;
+ * n_k = the rows the pooled get folds for bag k (the rows of its valid requests). c is then rounded once to dtype (a NaN
+ * becomes the canonical NaN) and added into the shard by dds_accumulate_batch's rule: atomic across batches, ranks and
+ * duplicate ids, one rounding per addition in an unspecified order; f32 may flush subnormals (atomicAdd's rule), f16 and
+ * bf16 do not, f64 is IEEE. It combines atomically with dds_accumulate_* and DDS_OP_SUM fetch-ops of the same dtype on the
+ * same elements. alpha is torch's alpha in p.add_(g, alpha=-lr); 1.0 gives the plain adjoint. *total_bytes = nbags * R.
+ * Errors follow the pooled get's rules: an invalid request contributes nothing and is left out of n_k, every valid one is
+ * still applied and the first invalid one is reported; a malformed bag writes nothing and is reported as DDS_ERR_ARG,
+ * "malformed bag offsets", with *bad_index = the bag, ahead of any invalid request (host bags are checked before anything
+ * is enqueued); requests no bag covers are neither read nor validated.
+ * Argument errors, DDS_ERR_ARG with nothing enqueued: any of the pooled get's; DDS_POOL_MAX (its adjoint needs the
+ * forward's argmax); flags without DDS_SRC_ON_DEVICE; grad_bytes < nbags * R, or grad == NULL with nbags * R > 0; grad or
+ * weights not aligned to the element size; a non-finite alpha. DDS_PLACE_HOST variables are refused as by every batched
+ * write. A dtype whose size is not the variable's itemsize is DDS_ERR_DTYPE.
+ * Flags: DDS_IDX_ON_DEVICE covers indices, bags and weights alike (host ones are staged). DDS_NO_SYNC queues the call
+ * (dds_batch_wait reports it with total nbags * R). DDS_OVERLAP is ignored: the call ends an overlap run, like a put. The
+ * rows are visible at the next fence, as for dds_accumulate_batch. */
+int dds_accumulate_batch_pooled(dds_store_t *s, const char *name, const int64_t *starts, const int64_t *counts,
+                                int64_t fixed_count, int64_t nreq, const dds_pool_t *pool, double alpha,
+                                const void *grad, int64_t grad_bytes, unsigned flags, void *cuda_stream,
+                                int64_t *total_bytes, int64_t *bad_index);
+int dds_accumulate_samples_pooled(dds_store_t *s, const char *name, const int64_t *sample_ids, int64_t nreq,
+                                  const dds_pool_t *pool, double alpha, const void *grad, int64_t grad_bytes,
+                                  unsigned flags, void *cuda_stream, int64_t *total_bytes, int64_t *bad_index);
 
 /* COLLECTIVE fetch by owner-PUSH (every rank calls, every rank on a GPU of its own; fixed-count batches). A one-sided
  * get() pulls: every NVLink direction then carries payload + response headers + the read requests of the opposite

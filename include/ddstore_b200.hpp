@@ -237,6 +237,30 @@ class DDStore {
                                      flags, cuda_stream, &total, &bad));
         return (long)total;
     }
+    // Pooled accumulate (dds_accumulate_batch_pooled), the adjoint of get_batch_pooled: grad row k (nbags rows of R bytes
+    // in `dtype`, device memory) times the request's weight, over the bag's rows for DDS_POOL_MEAN, times alpha, added into
+    // every row of bag k. mode is DDS_POOL_SUM or DDS_POOL_MEAN. Returns nbags * R.
+    long accumulate_batch_pooled(std::string name, const long *starts, const long *counts, long fixed_count, long nreq,
+                                 int mode, int dtype, const long *bags, long nbags, const void *weights, double alpha,
+                                 const void *grad, long grad_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        dds_pool_t p{mode, dtype, (const int64_t *)bags, nbags, weights};
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_accumulate_batch_pooled(store_, name.c_str(), (const int64_t *)starts, (const int64_t *)counts,
+                                          fixed_count, nreq, &p, alpha, grad, grad_bytes, flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
+    // The same by sample id (dds_accumulate_samples_pooled).
+    long accumulate_samples_pooled(std::string name, const long *sample_ids, long nreq, int mode, int dtype,
+                                   const long *bags, long nbags, const void *weights, double alpha, const void *grad,
+                                   long grad_bytes, bool idx_on_device = true, void *cuda_stream = nullptr) {
+        int64_t total = 0, bad = -1;
+        dds_pool_t p{mode, dtype, (const int64_t *)bags, nbags, weights};
+        const unsigned flags = DDS_SRC_ON_DEVICE | (idx_on_device ? DDS_IDX_ON_DEVICE : 0u);
+        check(dds_accumulate_samples_pooled(store_, name.c_str(), (const int64_t *)sample_ids, nreq, &p, alpha, grad,
+                                            grad_bytes, flags, cuda_stream, &total, &bad));
+        return (long)total;
+    }
     // Batched reduction (dds_accumulate_op_batch): accumulate_batch with each element becoming op(shard, src), op one of
     // DDS_OP_SUM, DDS_OP_MAX, DDS_OP_MIN, DDS_OP_BAND, DDS_OP_BOR, DDS_OP_BXOR (the bitwise ops on integer types only).
     long accumulate_op_batch(std::string name, const long *starts, const long *counts, long fixed_count, long nreq, int op,
