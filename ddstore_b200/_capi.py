@@ -165,6 +165,8 @@ SIGNATURES = {
     "dds_test_occupy": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p]),
     "dds_kernel_launches": (C.c_ulonglong, []),
     "dds_gather_geometry": (None, [C.POINTER(C.c_int)] * 5),
+    "dds_pool_geometry": (None, [C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_int), I64P, I64P,
+                                 I64P, C.POINTER(C.c_int)]),
     "dds_host_gather_ctas": (C.c_int, []),
 }
 

@@ -3549,6 +3549,38 @@ void pool_args(PoolArgs &a, const ddsk_var_t *var, const ddsk_index_t *index, in
     a.status_tag = scr->status_tag;
 }
 
+// The launch geometry of a pooled get (adjoint false) or of its adjoint, the one place its rule is written: rows of
+// row_bytes of element type `type`, nbags bags (both > 0), a destination / grad that is 16-byte aligned or not, HOST
+// shards or not. pick_geometry() must have succeeded.
+struct PoolGeometry {
+    int vb;                          // bytes per lane vector: 16, or one element
+    int64_t slice, nslices, windows; // bytes per column slice and slices per row; row windows per bag (1 for the get)
+    int blocks;                      // CTAs of kPoolThreads
+};
+PoolGeometry pool_geometry(bool adjoint, int64_t row_bytes, int type, int64_t nbags, bool aligned16, bool host) {
+    PoolGeometry g;
+    g.vb = (row_bytes % 16 == 0 && aligned16) ? 16 : 1 << DDSK_ACC_LOG2(type);
+    const int64_t resident = (int64_t)g_sms * kPoolMinBlocks * (kPoolThreads / 32), per_cta = kPoolThreads / 32;
+    g.slice = 32 * g.vb;
+    g.nslices = (row_bytes + g.slice - 1) / g.slice;
+    g.windows = 1;
+    if (!adjoint) {
+        // get: slices halved while the bags leave resident warps idle (a few long bags then still spread)
+        while (g.slice / 2 >= kPoolMinSlice && nbags * g.nslices < resident) {
+            g.slice /= 2;
+            g.nslices = (row_bytes + g.slice - 1) / g.slice;
+        }
+    } else {
+        // adjoint: whole-warp slices; then each bag's rows are dealt to row windows until there are kPoolAccFill warps
+        // per resident one (a few long bags, such as mean-pooled frames, then still spread over the machine)
+        const int64_t units = nbags * g.nslices;
+        g.windows = std::max<int64_t>(1, std::min<int64_t>(kPoolAccMaxWindows, (kPoolAccFill * resident + units - 1) / units));
+    }
+    const int64_t most = host ? std::min(g_sms, g_host_ctas) : (int64_t)g_sms * kPoolMinBlocks;
+    g.blocks = (int)std::min((nbags * g.nslices * g.windows + per_cta - 1) / per_cta, most);
+    return g;
+}
+
 } // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -3578,6 +3610,22 @@ void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk
     *stages = kLargeRows.stages;
     *chunk_bytes = kLargeRows.ch;
     *smem_bytes = smem_bytes_of(kLargeRows);
+}
+
+void ddsk_pool_geometry(int adjoint, int64_t row_bytes, int type, int64_t nbags, int aligned16, int host, int *vb,
+                        int64_t *slice, int64_t *nslices, int64_t *windows, int *blocks) {
+    const bool ok = type == DDSK_ACC_F32 || type == DDSK_ACC_F64 || type == DDSK_ACC_F16 || type == DDSK_ACC_BF16;
+    if (!ok || nbags <= 0 || row_bytes <= 0 || pick_geometry()) {
+        *vb = *blocks = 0;
+        *slice = *nslices = *windows = 0;
+        return;
+    }
+    const PoolGeometry g = pool_geometry(adjoint != 0, row_bytes, type, nbags, aligned16 != 0, host != 0);
+    *vb = g.vb;
+    *slice = g.slice;
+    *nslices = g.nslices;
+    *windows = g.windows;
+    *blocks = g.blocks;
 }
 
 int ddsk_gather_fixed(const ddsk_var_t *var, const int64_t *starts_dev, int64_t count, int64_t nreq, void *dst_dev,
@@ -3770,25 +3818,15 @@ int ddsk_pool(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixed_co
     PoolArgs a;
     pool_args(a, var, index, fixed_count, nreq, pool, scr);
     a.dst = (char *)dst;
-    const int64_t R = var->row_bytes;
-    const int vb = (R % 16 == 0 && (uint64_t)dst % 16 == 0) ? 16 : 1 << DDSK_ACC_LOG2(pool->type);
-    // slices: whole warps of vectors, halved while the bags leave resident warps idle (a few long bags then still spread)
-    const int64_t resident = (int64_t)g_sms * kPoolMinBlocks * (kPoolThreads / 32);
-    a.slice = 32 * vb;
-    a.nslices = (R + a.slice - 1) / a.slice;
-    while (a.slice / 2 >= kPoolMinSlice && a.nbags * a.nslices < resident) {
-        a.slice /= 2;
-        a.nslices = (R + a.slice - 1) / a.slice;
-    }
-    const int64_t units = a.nbags * a.nslices, per_cta = kPoolThreads / 32;
-    const int64_t most = var->host ? std::min(g_sms, g_host_ctas) : (int64_t)g_sms * kPoolMinBlocks;
-    const int blocks = (int)std::min((units + per_cta - 1) / per_cta, most);
+    const PoolGeometry g = pool_geometry(false, var->row_bytes, pool->type, pool->nbags, (uint64_t)dst % 16 == 0, var->host);
+    a.slice = g.slice;
+    a.nslices = g.nslices;
     int rc = 0;
     switch (pool->type) {
-    case DDSK_ACC_F32: rc = launch_pool_t<DDSK_ACC_F32>(a, vb, blocks, st); break;
-    case DDSK_ACC_F64: rc = launch_pool_t<DDSK_ACC_F64>(a, vb, blocks, st); break;
-    case DDSK_ACC_F16: rc = launch_pool_t<DDSK_ACC_F16>(a, vb, blocks, st); break;
-    case DDSK_ACC_BF16: rc = launch_pool_t<DDSK_ACC_BF16>(a, vb, blocks, st); break;
+    case DDSK_ACC_F32: rc = launch_pool_t<DDSK_ACC_F32>(a, g.vb, g.blocks, st); break;
+    case DDSK_ACC_F64: rc = launch_pool_t<DDSK_ACC_F64>(a, g.vb, g.blocks, st); break;
+    case DDSK_ACC_F16: rc = launch_pool_t<DDSK_ACC_F16>(a, g.vb, g.blocks, st); break;
+    case DDSK_ACC_BF16: rc = launch_pool_t<DDSK_ACC_BF16>(a, g.vb, g.blocks, st); break;
     default:
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_pool: unsupported element type %d", (int)pool->type);
         return -2;
@@ -3809,22 +3847,17 @@ int ddsk_pool_acc(const ddsk_var_t *var, const ddsk_index_t *index, int64_t fixe
     pool_args(a.p, var, index, fixed_count, nreq, pool, scr);
     a.grad = (const char *)grad;
     a.alpha = alpha;
-    const int64_t R = var->row_bytes;
-    const int vb = (R % 16 == 0 && (uint64_t)grad % 16 == 0) ? 16 : 1 << DDSK_ACC_LOG2(pool->type);
-    // whole-warp slices; then each bag's rows are dealt to row windows until there are kPoolAccFill warps per resident one
-    // (a few long bags, such as mean-pooled frames, then still spread over the machine)
-    const int64_t resident = (int64_t)g_sms * kPoolMinBlocks * (kPoolThreads / 32);
-    a.p.slice = 32 * vb;
-    a.p.nslices = (R + a.p.slice - 1) / a.p.slice;
-    const int64_t units = a.p.nbags * a.p.nslices, per_cta = kPoolThreads / 32;
-    a.windows = std::max<int64_t>(1, std::min<int64_t>(kPoolAccMaxWindows, (kPoolAccFill * resident + units - 1) / units));
-    const int blocks = (int)std::min((units * a.windows + per_cta - 1) / per_cta, (int64_t)g_sms * kPoolMinBlocks);
+    // (the store refuses DDS_PLACE_HOST variables for every batched write: var->host is false here)
+    const PoolGeometry g = pool_geometry(true, var->row_bytes, pool->type, pool->nbags, (uint64_t)grad % 16 == 0, var->host);
+    a.p.slice = g.slice;
+    a.p.nslices = g.nslices;
+    a.windows = g.windows;
     int rc = 0;
     switch (pool->type) {
-    case DDSK_ACC_F32: rc = launch_pool_acc_t<DDSK_ACC_F32>(a, vb, blocks, st); break;
-    case DDSK_ACC_F64: rc = launch_pool_acc_t<DDSK_ACC_F64>(a, vb, blocks, st); break;
-    case DDSK_ACC_F16: rc = launch_pool_acc_t<DDSK_ACC_F16>(a, vb, blocks, st); break;
-    case DDSK_ACC_BF16: rc = launch_pool_acc_t<DDSK_ACC_BF16>(a, vb, blocks, st); break;
+    case DDSK_ACC_F32: rc = launch_pool_acc_t<DDSK_ACC_F32>(a, g.vb, g.blocks, st); break;
+    case DDSK_ACC_F64: rc = launch_pool_acc_t<DDSK_ACC_F64>(a, g.vb, g.blocks, st); break;
+    case DDSK_ACC_F16: rc = launch_pool_acc_t<DDSK_ACC_F16>(a, g.vb, g.blocks, st); break;
+    case DDSK_ACC_BF16: rc = launch_pool_acc_t<DDSK_ACC_BF16>(a, g.vb, g.blocks, st); break;
     default:
         snprintf(g_cuda_err, sizeof(g_cuda_err), "ddsk_pool_acc: unsupported element type %d", (int)pool->type);
         return -2;

@@ -350,6 +350,11 @@ int ddsk_debug_timing(unsigned long long *host_out, int max_ctas);
 /* launch geometry actually used (for bench reporting / DESIGN.md) */
 void ddsk_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk_bytes, int *smem_bytes);
 
+/* launch geometry of a pooled get (adjoint 0) or pooled accumulate (adjoint 1); all zeros without a usable device or for
+ * arguments no pooled launch takes */
+void ddsk_pool_geometry(int adjoint, int64_t row_bytes, int type, int64_t nbags, int aligned16, int host, int *vb,
+                        int64_t *slice, int64_t *nslices, int64_t *windows, int *blocks);
+
 /* CTAs of a gather launch that reads DDS_PLACE_HOST shards */
 int ddsk_host_gather_ctas(void);
 

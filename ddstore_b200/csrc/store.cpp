@@ -2511,5 +2511,9 @@ int dds_host_gather_ctas(void) { return ddsk_host_gather_ctas(); }
 void dds_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk_bytes, int *smem_bytes) {
     ddsk_gather_geometry(ctas, warps_per_cta, stages, chunk_bytes, smem_bytes);
 }
+void dds_pool_geometry(int adjoint, int64_t row_bytes, int dtype, int64_t nbags, int aligned16, int host, int *vb,
+                       int64_t *slice, int64_t *nslices, int64_t *windows, int *ctas) {
+    ddsk_pool_geometry(adjoint, row_bytes, dtype, nbags, aligned16, host, vb, slice, nslices, windows, ctas);
+}
 
 } // extern "C"

@@ -601,6 +601,13 @@ int dds_test_occupy(int device, int ctas, int smem_bytes, uint64_t nanoseconds, 
 /* kernels launched by this library since load, and the gather launch geometry in use */
 unsigned long long dds_kernel_launches(void);
 void dds_gather_geometry(int *ctas, int *warps_per_cta, int *stages, int *chunk_bytes, int *smem_bytes);
+/* Test helper: the launch geometry a pooled get (adjoint 0) or pooled accumulate (adjoint 1) of `nbags` bags over rows of
+ * `row_bytes` of element type `dtype` (DDS_ACC_F32 / F64 / F16 / BF16) is launched with, its destination / grad
+ * 16-byte aligned or not, on a DDS_PLACE_HOST variable or not: bytes per lane vector (16 or one element), bytes per column
+ * slice, slices per row, row windows per bag (1 for a get) and CTAs of 256 threads. All zeros without a usable device,
+ * for nbags or row_bytes <= 0, or for another dtype. */
+void dds_pool_geometry(int adjoint, int64_t row_bytes, int dtype, int64_t nbags, int aligned16, int host, int *vb,
+                       int64_t *slice, int64_t *nslices, int64_t *windows, int *ctas);
 /* CTAs of a gather launch that reads DDS_PLACE_HOST shards (at most 16; 0 without a usable device) */
 int dds_host_gather_ctas(void);
 

@@ -77,7 +77,7 @@ def check(got, exp, what):
                              f"got {int(got[k, e]):#x}, oracle {int(exp[k, e]):#x}")
 
 
-def run_pool(store, name, t, mode, form, dev, rng, nrows, bag_sizes, weighted=False, ids=None):
+def run_pool(store, name, t, mode, form, dev, rng, nrows, bag_sizes, weighted=False, ids=None, out=None):
     """one pooled call on variable `name` (nrows global rows) with bags of bag_sizes requests; returns (got, exp, err)"""
     nreq = int(sum(bag_sizes))
     bags = bag_offsets(rng, bag_sizes)
@@ -91,7 +91,7 @@ def run_pool(store, name, t, mode, form, dev, rng, nrows, bag_sizes, weighted=Fa
         c = 1 if form == "fixed1" else 2
         req = {"starts": rng.integers(0, max(1, nrows - c + 1), nreq), "fixed_count": c}
     w = data_bits(rng, t, nreq, special=False) if weighted else None
-    return call(store, name, t, mode, dev, req, bags, w)
+    return call(store, name, t, mode, dev, req, bags, w, out=out)
 
 
 def call(store, name, t, mode, dev, req, bags, w, out=None):
@@ -138,11 +138,16 @@ def test_types_modes_rows(t, mode, row_bytes):
     store = PyDDStore(device=0)
     try:
         add_var(store, "x", shard, t)
-        out, req, w, err = run_pool(store, "x", t, MODES[mode], "counts", True, rng, nrows, sizes, mode == "weighted")
-        assert err is None, err
-        exp, _, eerr = oracle([shard], t, MODES[mode], req, bag_offsets(rng, sizes), w)
-        assert eerr == (0, -1)
-        check(bits_of(out, t), exp, f"type {t} {mode} disp {disp}")
+        for off in (0, 1):  # out 16-byte aligned (vector path where rows allow), then one element past it
+            buf = torch.full((len(sizes) * disp + 16 // SIZE[t],), 7, dtype=TORCH_DT[t], device="cuda")
+            out = buf[off:off + len(sizes) * disp].view(len(sizes), disp)
+            assert (out.data_ptr() % 16 == 0) == (off == 0)
+            out, req, w, err = run_pool(store, "x", t, MODES[mode], "counts", True, rng, nrows, sizes, mode == "weighted",
+                                        out=out)
+            assert err is None, err
+            exp, _, eerr = oracle([shard], t, MODES[mode], req, bag_offsets(rng, sizes), w)
+            assert eerr == (0, -1)
+            check(bits_of(out, t), exp, f"type {t} {mode} disp {disp} off {off}")
     finally:
         store.free()
         store.close()

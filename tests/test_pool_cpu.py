@@ -203,3 +203,17 @@ def test_header_and_bindings_declare_the_entries():
     assert "get_batch_pooled" in hpp and "get_samples_pooled" in hpp
     pyx = open(os.path.join(ROOT, "ddstore_b200", "cython", "pyddstore.pyx")).read()
     assert "def get_batch_pooled" in pyx
+
+
+def test_geometry_helper_reports_zeros_without_a_device():
+    """dds_pool_geometry, as dds_gather_geometry: no usable device, no geometry"""
+    import ctypes as C
+    torch = pytest.importorskip("torch")
+    if torch.cuda.is_available():
+        pytest.skip("a GPU is present")
+    vb, ctas = C.c_int(-1), C.c_int(-1)
+    sl, ns, w = C.c_int64(-1), C.c_int64(-1), C.c_int64(-1)
+    for adjoint in (0, 1):
+        _capi.lib().dds_pool_geometry(adjoint, 512, pl.ACC_F32, 100, 1, 0, C.byref(vb), C.byref(sl), C.byref(ns),
+                                      C.byref(w), C.byref(ctas))
+        assert (vb.value, sl.value, ns.value, w.value, ctas.value) == (0, 0, 0, 0, 0)
